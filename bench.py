@@ -83,7 +83,7 @@ def bench_config(desc, n, world, scene_info, extra=None):
     """The `config` object of the JSON line: identical for this repo's arm and the reference arm."""
     c = {"workload": desc, "poses_per_step_per_gpu": n, "segs": int(scene_info.n_segs), "subsectors": int(scene_info.n_ssectors),
          "parallelism": "pose-sharded x%d" % world,
-         "l2": "frames written per step >> 126 MB L2 (2.07 MB per 1080p frame); the scene (~0.3 MB) is legitimately cache-resident"}
+         "l2": "frames written per step >> 50 MB L2 (2.07 MB per 1080p frame); the scene (~0.3 MB) is legitimately cache-resident"}
     if extra:
         c.update(extra)
     return c
@@ -103,16 +103,7 @@ def measured_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic():
-    """dram bytes per raster launch from the committed ncu capture (profiles/roofline.json), or None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline.json")) as f:
-            return json.load(f).get("raster_dram_bytes_per_launch")
-    except Exception:  # noqa: BLE001
-        return None
+        return 3350.0, "nominal (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -292,6 +283,35 @@ def verify_maps(result, scenes, poses, width, height, probes_per_map=1):
 
 
 # ---------------------------------------------------------------------------------------------- helpers (GPU arm)
+DUMP_BYTES = 64_000_000
+
+
+def dump_outputs(out_dir, index, rgba=None):
+    """What the caller of the timed path receives, for comparing two builds output for output: the per-frame sum of the
+    palette indices of every frame (float64) and whole frames of a fixed, seeded sample (float32; RGBA8 as 4 channels),
+    at most DUMP_BYTES in all.  index: (n, H, W) uint8 device tensor; rgba: (n, H, W) int32 device tensor or None."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n, h, w = index.shape
+    sums = index.reshape(n, -1).sum(dim=1, dtype=torch.float64).cpu().numpy()
+    budget = DUMP_BYTES - sums.nbytes - (1 << 16)
+    arrays = {"index_frame_sums": sums}
+    parts = [("index", index, 1)] + ([("rgba", rgba, 4)] if rgba is not None else [])
+    for name, t, ch in parts:
+        k = max(1, min(n, budget // len(parts) // (h * w * ch * 4)))
+        ids = np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+        sel = t[torch.from_numpy(ids).to(t.device)].cpu().numpy()
+        if ch == 4:
+            sel = sel.view(np.uint8).reshape(k, h, w, 4)
+        arrays[name + "_frames"] = sel.astype(np.float32)
+        arrays[name + "_frame_ids"] = ids.astype(np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_BYTES:
+        raise SystemExit("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_BYTES))
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def roofline_of(raster_ms_per_launch_set, alg_bytes, walk_ms, note, kernel="b2d_raster_kernel<index>", traffic=None):
     peak, peak_src = measured_peak()
     achieved = alg_bytes / (raster_ms_per_launch_set / 1e3) / 1e9 if raster_ms_per_launch_set > 0 else 0.0
@@ -324,7 +344,12 @@ def main():
                          "first CTAs of batch k+1 fill the SMs that the last CTAs of batch k leave idle (1 = one stream, one buffer)")
     ap.add_argument("--rgba", action="store_true", help="c2: also materialise RGBA8 frames in HBM (5 B/pixel; not the headline config)")
     ap.add_argument("--gather-frames", type=int, default=0, help="c2, N>1: frames per rank in a separate all-gather timing (0 = off; see --config c5)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="c2: after the timed steps, write what the last step computed to DIR/<name>.npy (float32 / float64, "
+                         "<= 64 MB: every frame's index sum and a fixed, seeded sample of whole frames)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config != "c2" or args.impl != "b2d"):
+        raise SystemExit("--dump-outputs is available for --config c2 with --impl b2d")
     args.warmup = max(args.warmup, 0)
     cfg = args.config
     # stdout carries the one JSON line: NCCL's version banner / debug output (NCCL_DEBUG may be set by the box) goes to stderr
@@ -389,7 +414,7 @@ def main():
                 os.environ.pop(k, None)
             os.environ.update(env_of[tname])
             comm = jobs.make_comm(local_rank) if world > 1 else jobs.single_comm(local_rank)
-            r1 = jobs.run_c5(scene, poses, width, height, local_rank, comm, chunk=args.chunk, reps=max(1, min(args.steps, 3)))
+            r1 = jobs.run_c5(scene, poses, width, height, local_rank, comm, chunk=args.chunk, reps=max(1, args.steps))
             v1 = verify_c5(b2d, jobs, r1, scene, poses, width, height, rank, world)
             if not v1["all_ranks_identical"] or v1["oracle_mismatches"] or r1["status_bits"]:
                 raise SystemExit("c5 validation failed (%s): %r status %d" % (tname, v1, r1["status_bits"]))
@@ -404,9 +429,9 @@ def main():
                 "render_only_fps", "gather_only_fps", "joint_fps", "joint_checked_fps", "gather_gbs_received_per_rank",
                 "joint_gbs_received_per_rank", "registration", "nccl_version")
         if rank == 0:
-            nvl = 900.0
+            nvl = 450.0
             print(json.dumps({
-                "metric": METRIC, "value": res["joint_fps"], "unit": UNIT, "n_gpus": world, "steps": 1, "warmup": 1,
+                "metric": METRIC, "value": res["joint_fps"], "unit": UNIT, "n_gpus": world, "steps": max(1, args.steps), "warmup": 1,
                 "ms_per_step": res["joint_ms"], "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
                 "dtype": "u8", "data": "synthetic",
                 "config": bench_config(desc, res["per_rank"], world, scene.info,
@@ -422,7 +447,7 @@ def main():
                 "validation": ver,
                 "roofline": {"bound": "nvlink", "achieved": res["joint_gbs_received_per_rank"], "peak": nvl, "unit": "GB/s",
                              "frac": res["joint_gbs_received_per_rank"] / nvl if world > 1 else None, "traffic": None,
-                             "note": "bytes received per rank per second in the joint run vs one NVLink-5 direction (SURVEY.md 0.5); "
+                             "note": "bytes received per rank per second in the joint run vs one NVLink-4 direction (H100 SXM: 450 GB/s); "
                                      "render-only throughput is the HBM-bound number of --config c2"}}))
         if world > 1:
             dist.destroy_process_group()
@@ -431,7 +456,7 @@ def main():
     # ================================================================== c3 / c4 / 4k / rich: several maps or other shapes
     if cfg in ("c3", "c4", "4k", "rich"):
         mine = jobs.map_assignment(len(maps), world)[rank] if cfg == "c4" else list(range(len(maps)))
-        # frames per launch: the BSP walk is one latency-bound wave (~0.1 ms whatever the batch), so batches are large;
+        # frames per launch: the BSP walk is one latency-bound wave whatever the batch, so batches are large;
         # c3 still interleaves the nine renderers batch by batch
         batch = args.batch or min(n, 500)
         scenes, poses = [], []
@@ -441,7 +466,7 @@ def main():
             scenes.append(sc)
             ps = make_poses(sc, kind, n, pseed)
             poses.append(np.roll(ps, -(rank * n // max(world, 1))) if cfg != "c4" else ps)
-        steps = max(1, args.steps if cfg != "c4" else min(args.steps, 5))
+        steps = max(1, args.steps)
         sampler = ClockSampler(local_rank)
         if rank == 0:
             sampler.start()
@@ -570,6 +595,9 @@ def main():
     join()
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:        # before the trailing raster below writes into buffer 0
+        last = (turn[0] - 1) % nbuf if pipelined else 0
+        dump_outputs(args.dump_outputs, d_index_all[last], d_rgba_all[last])
     if pipelined:                              # the walk issued by the last step belongs to a step that never comes
         r.raster_device(pending[0], d_index.data_ptr(), d_rgba.data_ptr() if args.rgba else 0, stream)
         torch.cuda.synchronize()
@@ -590,11 +618,10 @@ def main():
     # one launch also spans its wait for SMs: the kernel's duration in the timed region is then the region over its launches
     per_launch = ms_total / args.steps if overlapped else raster_ms / max(batches, 1)
     roofline = roofline_of(per_launch, alg_bytes, walk_ms / max(batches, 1),
-                           "index-only output (no RGBA materialised); the raster kernel is instruction-issue / L1 bound, not HBM bound "
-                           "(DESIGN.md 5-6, profiles/README.md)" +
+                           "index-only output (no RGBA materialised)" +
                            ("; avg_launch_ms = timed region / raster launches: the rasters run back to back on two streams, overlapping by "
                             "their tails, with the next batch's BSP walk co-resident" if overlapped else ""),
-                           "b2d_raster_kernel<%s>" % ("rgba" if args.rgba else "index"), None if args.rgba else ncu_traffic())
+                           "b2d_raster_kernel<%s>" % ("rgba" if args.rgba else "index"))
     if pipelined:        # the same kernel timed alone, outside the timed region: one stream, walk first, nothing co-resident
         r.profile(True)
         r.profile_read()
@@ -627,7 +654,7 @@ def main():
                "steps": e2e_steps, "d2h_gbs_per_gpu": e2e_n * e2e_steps * npix / dt / 1e9,
                "api": "b2d_render (pinned host poses in, pinned host frames out, double-buffered D2H on two copy streams)",
                "numa": numa,
-               "note": "PCIe-bound: one 1080p index frame is 2.07 MB over a ~57 GB/s Gen5 x16 link = ~27.5 k frames/s per GPU"}
+               "note": "bound by the host link: every step copies 2.07 MB per 1080p index frame to host memory"}
         if rank == 0 and not np.array_equal(h_index[n // 2].numpy(), d_index[n // 2].cpu().numpy()):
             raise SystemExit("e2e path disagrees with the device path")
         del r2

@@ -1,5 +1,5 @@
 /*
- * b2d.h -- C ABI of the B200-native Doom-WAD software renderer (libb2d.so).
+ * b2d.h -- C ABI of the H100-native Doom-WAD software renderer (libb2d.so).
  *
  * The reference (cristicbz/rust-doom) has no FFI or plugin ABI (100% safe Rust, README.md:39).
  * Its renderer-facing seams are Rust-level only; each entry point below names the reference
@@ -228,7 +228,7 @@ int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_
  * one of the renderer's two worklist slots and returns a ticket; b2d_raster_device enqueues the raster of that ticket on
  * its own `cuda_stream`.  The two calls are ordered through events, not by the streams: with two streams the walk of
  * batch k+1 overlaps the raster of batch k.  b2d_walk_device launches the walk as a background grid (one CTA per SM
- * looping over the frames): it then takes several frame latencies instead of one (~0.7 ms for 1000 frames) but leaves
+ * looping over the frames): it then takes several frame latencies instead of one but leaves
  * 7/8 of the registers to the raster it runs under.  Rasters of consecutive batches may go to two alternating
  * streams (and output buffers): the first CTAs of batch k+1 then fill the SMs the last CTAs of batch k leave idle.  At
  * most two batches can be walked and not yet rastered; tickets are rastered once.  d_poses is read by the walk

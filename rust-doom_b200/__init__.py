@@ -1,4 +1,4 @@
-"""b2d -- B200-native software renderer for the Doom-WAD visibility-and-raster hot path.
+"""b2d -- H100-native software renderer for the Doom-WAD visibility-and-raster hot path.
 
 Host-side mirror of the reference's renderer-facing surface over the C-ABI shared library
 `libb2d.so` (include/b2d.h):
@@ -9,7 +9,7 @@ Host-side mirror of the reference's renderer-facing surface over the C-ABI share
     Renderer     ~ engine::Renderer         (engine/src/renderer.rs:62-175)
 
 Errors surface as B2dError carrying the library's code + message (wad::ErrorKind analogue).
-All rendering runs in hand-written sm_100a CUDA kernels; there is no CPU fallback.
+All rendering runs in hand-written sm_90a CUDA kernels; there is no CPU fallback.
 """
 from __future__ import annotations
 

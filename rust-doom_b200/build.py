@@ -1,4 +1,4 @@
-"""Build recipe for libb2d.so: nvcc, sm_100a only, in-tree output (rust-doom_b200/libb2d.so).
+"""Build recipe for libb2d.so: nvcc, sm_90a only, in-tree output (rust-doom_b200/libb2d.so).
 
 `python -m rust_doom_b200.build` (or __graft_entry__.build()).  nvcc cross-compiles without a GPU.
 """
@@ -12,7 +12,7 @@ OUT = os.path.join(HERE, "libb2d.so")
 SOURCES = ["b2d_api.cu", "b2d_kernels.cu", "b2d_sharded.cu", "b2d_wad.cpp", "b2d_scene.cpp"]
 HEADERS = ["b2d_cli.cpp", "b2d_math.cuh", "b2d_kernels.cuh", "b2d_internal.hpp", "b2d_scene.hpp", "b2d_wad.hpp", "../../include/b2d.h"]
 
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-Wall,-Wextra,-Wno-unused-parameter", "-shared",
               "-Xptxas", "-v" if os.environ.get("B2D_PTXAS_V") else "-warn-spills", "-ldl"]
 

@@ -1,6 +1,6 @@
 // C-ABI of libb2d.so (declared in include/b2d.h).  Thin, exception-free boundary over the C++ host
 // side (WAD loader, scene compiler) and the CUDA kernels.  There is deliberately no CPU rendering
-// path here: every render entry point launches the sm_100a kernels or fails with B2D_ERR_CUDA.
+// path here: every render entry point launches the sm_90a kernels or fails with B2D_ERR_CUDA.
 #include <cmath>
 #include <cstdlib>
 #include <cstring>

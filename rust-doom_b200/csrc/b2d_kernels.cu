@@ -1,4 +1,4 @@
-// sm_100a kernels of the Doom-WAD software renderer.
+// sm_90a kernels of the Doom-WAD software renderer.
 //
 //   b2d_walk_kernel    : one CTA per frame.  Thread-parallel view transform of all vertices, per-seg
 //                        projection setup and per-node-child bounding-box ranges into shared memory,
@@ -11,7 +11,7 @@
 //   b2d_prelight_*     : build those planes once per renderer (32 light rows x texels / flats).
 //   b2d_palette_kernel : index -> RGBA8 with the 256-entry palette in shared memory, 128-bit I/O.
 //
-// There is no dense contraction anywhere on this path, so no tensor-core (tcgen05) work: the
+// There is no dense contraction anywhere on this path, so no tensor-core (wgmma) work: the
 // kernels are integer/LSU/latency bound and are tuned against the HBM write roofline (DESIGN.md).
 #include "b2d_kernels.cuh"
 
@@ -23,7 +23,7 @@ namespace {
 
 constexpr unsigned kFull = 0xFFFFFFFFu;
 
-// texel / table loads of the raster: read-only path; B2D_LOAD_EL (A/B, profiles/README.md) asks L1 to keep them
+// texel / table loads of the raster: read-only path; B2D_LOAD_EL (A/B build variant) asks L1 to keep them
 #if defined(B2D_LOAD_L2EL)
 // A/B: ask L2 to keep the pre-lit planes (a 2 GB/ms write stream passes through the same L2)
 __device__ __forceinline__ uint64_t l2_keep_policy() {
@@ -131,7 +131,7 @@ __host__ __device__ inline WalkSmem walk_layout(int nverts, int nsegs, int nnode
 }
 
 // 1-D bulk copy global -> shared memory through the TMA unit (cp.async.bulk, SASS UBLKCP), completion on an mbarrier.
-// B2D_WALK_NO_BULK (build variant, A/B in profiles/README.md) stages the same bytes with a thread loop instead.
+// B2D_WALK_NO_BULK (A/B build variant) stages the same bytes with a thread loop instead.
 __device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t arrivals) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(arrivals));
@@ -155,7 +155,7 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity) {     
 // ------------------------------------------------------------------------------------------------
 // Kernel 1: BSP walk -> worklist
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 7)     // 7 CTAs/SM (72 registers): 1036 frames resident on 148 SMs
+__global__ void __launch_bounds__(128, 7)     // 7 CTAs/SM (72 registers): 924 frames resident on an H100's 132 SMs
 b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const Pose *__restrict__ poses, int n,
                 FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride) {
     // One CTA per frame.  The per-frame setup (steps 1-3) and the worklist records (step 5) are data-parallel and
@@ -407,7 +407,7 @@ template <bool kRgba>
 __device__ __forceinline__ void put_px(const RasterCtx &c, uint8_t *p8, uint32_t *p32, bool on, uint32_t v) {
     if (on) {
 #if defined(B2D_STORE_CS)
-        __stcs(p8, (uint8_t)v);       // A/B (profiles/README.md): streaming store, keeps frame bytes from displacing texels
+        __stcs(p8, (uint8_t)v);       // A/B: streaming store, keeps frame bytes from displacing texels
 #elif defined(B2D_STORE_WT)
         __stwt(p8, (uint8_t)v);
 #else
@@ -990,6 +990,14 @@ b2d_palette_kernel(const uint32_t *__restrict__ palette, const uint8_t *__restri
 // ------------------------------------------------------------------------------------------------
 size_t walk_smem_per_warp(const DeviceScene &sc) { return walk_layout(sc.nverts, sc.nsegs, sc.nnodes, sc.nss, sc.nsprites).total; }
 
+// SMs of the current device (132 on an H100 SXM): the persistent and capped grids below are sized per SM
+static int device_sms() {
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms > 0 ? sms : 1;
+}
+
 cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
                         FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background) {
     if (n <= 0) return cudaSuccess;
@@ -1000,10 +1008,11 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
         if (e != cudaSuccess) return e;
     }
     // background (b2d_walk_device: the walk of the NEXT batch, meant to run under another batch's raster): a persistent grid
-    // of one CTA per SM.  It takes n/148 frame latencies instead of one, but holds 1/8 of the register file instead of
-    // 7/8, so the raster keeps 28 of its 32 warps per SM while the walk hides behind it (measured: profiles/README.md).
+    // of one CTA per SM.  It takes n/SMs frame latencies instead of one, but holds 1/8 of the register file instead of
+    // 7/8, so the raster keeps 22 of its 24 warps per SM while the walk hides behind it.
     // B2D_TUNE bit 2 (4) turns it off for A/B.
-    const int blocks = (background && !(sc.tune & 4u) && n > 148) ? 148 : n, warps = 4;
+    const int sms = device_sms();
+    const int blocks = (background && !(sc.tune & 4u) && n > sms) ? sms : n, warps = 4;
     b2d_walk_kernel<<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride);
     return cudaGetLastError();
 }
@@ -1013,18 +1022,19 @@ cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameCons
                           uint32_t *d_rgba, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
-    // Launch shape (tuned on B200, profiles/README.md): ONE warp per CTA and 64 registers/thread, i.e. 32 CTAs =
-    // 32 warps resident per SM.  Strips differ a lot in cost; with several warps per CTA the finished warps' slots
-    // stay empty until the slowest warp of the CTA is done (1-warp CTAs: +10 % over 2 or 4, 8 and 16 lose more).
+    // Launch shape: ONE warp per CTA and 80 registers/thread, i.e. 24 CTAs = 24 warps resident per SM.  On sm_90a the
+    // kernel spills at a 64-register cap (32 warps/SM); the 80-register cap keeps most of it in registers and measured
+    // 14 % more frames/s on an H100 SXM (bench.py c2).  Strips differ a lot in cost; with several warps per CTA the finished warps' slots
+    // stay empty until the slowest warp of the CTA is done.
     // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
 #if defined(B2D_RASTER_WARPS)         // A/B: more resident warps per SM at fewer registers per thread
     constexpr int kWarps = B2D_RASTER_WARPS, kMinBlocks = B2D_RASTER_MINBLOCKS;
 #else
-    constexpr int kWarps = 1, kMinBlocks = 32;
+    constexpr int kWarps = 1, kMinBlocks = 24;
 #endif
     const long long total_warps = (long long)n * strips;
     const int nblocks = (int)((total_warps + kWarps - 1) / kWarps);
-    static const bool generic_w = getenv("B2D_RASTER_GENERIC_W") != nullptr;   // A/B knob for profiles/README.md
+    static const bool generic_w = getenv("B2D_RASTER_GENERIC_W") != nullptr;   // A/B knob
     const bool w1920 = vw.W == 1920 && !generic_w;
     // B2D_CARVEOUT=<percent of the SM's L1/shared array given to shared memory> (A/B): the raster uses ~300 B of it per warp
     static const int carve = getenv("B2D_CARVEOUT") ? atoi(getenv("B2D_CARVEOUT")) : -1;
@@ -1091,7 +1101,8 @@ b2d_prelight_tex_kernel(const uint8_t *__restrict__ colormap, const uint8_t *__r
 cudaError_t launch_prelight_textures(const uint8_t *d_colormap, const uint8_t *d_texels, const TexRec *d_tex, int ntex,
                                      uint8_t *d_dst, size_t stride, cudaStream_t stream) {
     if (ntex <= 0) return cudaSuccess;
-    b2d_prelight_tex_kernel<<<ntex < 148 * 8 ? ntex : 148 * 8, 256, 0, stream>>>(d_colormap, d_texels, d_tex, ntex, d_dst, stride);
+    const int cap = device_sms() * 8;
+    b2d_prelight_tex_kernel<<<ntex < cap ? ntex : cap, 256, 0, stream>>>(d_colormap, d_texels, d_tex, ntex, d_dst, stride);
     return cudaGetLastError();
 }
 
@@ -1099,7 +1110,7 @@ cudaError_t launch_prelight(const uint8_t *d_colormap, const uint8_t *d_src, uin
                             cudaStream_t stream) {
     if (n == 0) return cudaSuccess;
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > device_sms() * 8) blocks = device_sms() * 8;
     b2d_prelight_kernel<<<blocks, 256, 0, stream>>>(d_colormap, d_src, d_dst, n, stride);
     return cudaGetLastError();
 }
@@ -1109,7 +1120,7 @@ cudaError_t launch_palette(const uint32_t *d_palette, const uint8_t *d_index, ui
     if (n_pixels == 0) return cudaSuccess;
     size_t nvec = n_pixels / 16 + 1;
     int blocks = (int)((nvec + 255) / 256);
-    const int cap = 148 * 16;
+    const int cap = device_sms() * 16;
     if (blocks > cap) blocks = cap;
     b2d_palette_kernel<<<blocks, 256, 0, stream>>>(d_palette, d_index, d_rgba, n_pixels);
     return cudaGetLastError();

@@ -41,7 +41,7 @@ struct DeviceScene {
     uint32_t *masked_counter;    // chunks handed out by the current raster launch (reset before every launch)
     uint32_t masked_chunks;      // arena capacity in chunks (exhausted -> status bit 8)
     int32_t masked_cap;          // entries one 32-column strip can defer per frame (more -> status bit 8)
-    uint32_t tune;               // A/B switches for profiles/ (env B2D_TUNE, default 0): 1 no incremental wall path,
+    uint32_t tune;               // A/B switches (env B2D_TUNE, default 0): 1 no incremental wall path,
                                  // 2 no 16-row batches, 4 no persistent grid for background walks
 };
 

@@ -183,9 +183,8 @@ int ensure_buffers(b2d_comm *c, size_t bytes) {
     if (c->buf_bytes >= bytes) return B2D_OK;
     Nccl &n = nccl();
     release_buffers(c);
-    // exchange transport: the copy engines over CUDA-IPC peer mappings unless B2D_GATHER=nccl asks for ncclAllGather
-    // (measured on 8 B200: 746 GB/s received per rank against 620-655 with NCCL's kernels, profiles/README.md); if any
-    // rank cannot map a peer's buffer, all ranks agree to fall back to NCCL below
+    // exchange transport: the copy engines over CUDA-IPC peer mappings (no SM or L2 taken from the raster beside it)
+    // unless B2D_GATHER=nccl asks for ncclAllGather; if any rank cannot map a peer's buffer, all ranks agree to fall back to NCCL below
     const char *tr = getenv("B2D_GATHER");
     c->ce = !(tr && std::strcmp(tr, "nccl") == 0) && c->world > 1 && n.AllReduce;
     const bool want_reg = !getenv("B2D_NCCL_NO_REGISTER") && !c->ce;      // IPC needs plain cudaMalloc memory

@@ -51,7 +51,7 @@ def _parse_cpulist(text: str) -> List[int]:
 
 def bind_to_gpu_numa(device_index: int) -> Dict[str, object]:
     """Pin this process to the CPUs of the GPU's NUMA node so that the pinned host buffers it allocates afterwards are
-    first-touched on the memory next to the GPU's PCIe root (SCALE_r01: e2e scaled 58 % at 8 GPUs with unbound buffers).
+    first-touched on the memory next to the GPU's PCIe root.
     Returns what was done (for the bench line)."""
     node = gpu_numa_node(device_index)
     info: Dict[str, object] = {"numa_node": node, "bound": False}
@@ -206,7 +206,7 @@ def run_maps(scenes: Sequence[Scene], poses: Sequence[np.ndarray], width: int, h
     outs = [torch.empty((len(p), height, width), dtype=torch.uint8, device=dev) for p in poses]
     main_stream = torch.cuda.current_stream()
     # rasters that defer masked entries (two-sided middle textures, sprites) share one arena per renderer and are ordered by
-    # an event whatever streams they are on: a second stream buys nothing there (measured: -2 %)
+    # an event whatever streams they are on: a second stream buys nothing there
     masked = any(s.info.n_masked_mids + s.info.n_sprites > 0 for s in scenes)
     side = [torch.cuda.Stream(device=dev) for _ in range(2)] if raster_streams > 1 and not masked else None
 

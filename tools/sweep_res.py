@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Device-resident frames/s of the walk+raster step at several resolutions (CUDA events, 3 warm-ups, inputs and
-outputs in HBM).  Informational table for profiles/README.md; the headline number is bench.py's.
+outputs in HBM).  Informational table; the headline number is bench.py's.
 usage: python tools/sweep_res.py [n_poses]"""
 import json
 import os
