@@ -80,17 +80,6 @@ def build(force: bool = False, verbose: bool = False) -> str:
     return OUT
 
 
-def build_variant(name: str, defines, verbose: bool = False) -> str:
-    """An A/B build of the library with extra -D flags: rust-doom_b200/libb2d_<name>.so (select it with B2D_LIB=<path>)."""
-    out = os.path.join(HERE, "libb2d_%s.so" % name)
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + ["-D" + d for d in defines] + ["-o", out] + [os.path.join(CSRC, s) for s in SOURCES]
-    if verbose:
-        print(" ".join(cmd))
-    subprocess.check_call(cmd)
-    return out
-
-
 CLI_OUT = os.path.join(HERE, "b2d")
 
 

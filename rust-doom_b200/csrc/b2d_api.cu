@@ -231,21 +231,7 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
         for (auto &e : ev) CU(cudaEventCreate(&e));
         CU(cudaEventRecord(ev[0], stream));
     }
-    if (r->l2_window_bytes) {      // B2D_L2PERSIST (A/B): the pre-lit planes are a persisting L2 window for the raster's loads
-        cudaStreamAttrValue av{};
-        av.accessPolicyWindow.base_ptr = r->d_lit;
-        av.accessPolicyWindow.num_bytes = r->l2_window_bytes;
-        av.accessPolicyWindow.hitRatio = r->l2_hit_ratio;
-        av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        CU(cudaStreamSetAttribute(stream, cudaStreamAttributeAccessPolicyWindow, &av));
-    }
     CU(launch_raster(r->ds, r->view, r->d_frames[slot], r->d_work[slot], r->stride, r->slot_n[slot], d_index, d_rgba, stream));
-    if (r->l2_window_bytes) {
-        cudaStreamAttrValue av{};
-        av.accessPolicyWindow.num_bytes = 0;
-        CU(cudaStreamSetAttribute(stream, cudaStreamAttributeAccessPolicyWindow, &av));
-    }
     if (r->profiling) {
         CU(cudaEventRecord(ev[1], stream));
         for (auto e : ev) r->prof_events.push_back(e);
@@ -662,10 +648,8 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
         // (frame, 32-column strip) of a full batch -- frames defer a handful of entries per strip -- and never more than the
         // worst case (every strip at its cap).  1000 x 1080p: 63 MB instead of the 1 GB a fixed per-strip list takes.
         const size_t strips = (size_t)(view->width + 31) / 32;
-        int cap = d.nmids + d.nsprites;
-        cap = cap < 8 ? 8 : (cap > kMaskedCapMax ? kMaskedCapMax : cap);
-        d.masked_cap = cap;
-        const size_t per_strip = ((size_t)cap + kMaskedChunk - 1) / kMaskedChunk;
+        d.masked_cap = strip_masked_cap(d.nmids, d.nsprites);
+        const size_t per_strip = ((size_t)d.masked_cap + kMaskedChunk - 1) / kMaskedChunk;
         size_t chunks = strips * (size_t)max_batch * (per_strip < 2 ? per_strip : 2);
         if (chunks < 4096) chunks = 4096;
         const size_t worst = strips * (size_t)max_batch * per_strip;
@@ -693,17 +677,6 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
         CUR(launch_prelight_textures(d.colormap, d.texels, d.tex, (int)h[H_NTEX], r->d_lit, tstride, nullptr));
         CUR(launch_prelight(d.colormap, d.flats, r->d_lit_flats, fstride, fstride, nullptr));
         CUR(cudaDeviceSynchronize());
-        if (getenv("B2D_L2PERSIST")) {      // texel planes only (one window per launch; the flats are a separate mapping)
-            cudaDeviceProp prop;
-            CUR(cudaGetDeviceProperties(&prop, device));
-            const size_t want = 33 * (size_t)tstride;
-            const size_t carve = std::min<size_t>(want, (size_t)prop.persistingL2CacheMaxSize);
-            if (carve && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve) == cudaSuccess) {
-                r->l2_window_bytes = std::min<size_t>(want, (size_t)prop.accessPolicyMaxWindowSize);
-                r->l2_hit_ratio = (float)std::min(1.0, (double)carve / (double)r->l2_window_bytes);
-            }
-            cudaGetLastError();
-        }
         d.lit_texels = r->d_lit; d.lit_flats = r->d_lit_flats;           // low 32 address bits of lit_flats are zero
         d.lit_texel_stride = (uint32_t)tstride; d.lit_flat_stride = (uint32_t)fstride;
     }
@@ -717,10 +690,6 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
     d.nflats = (int32_t)h[H_NFLATS]; d.sky_tex = (int32_t)h[H_SKY_TEX];
     d.root = h[H_ROOT];
     d.invF = (uint32_t)(4294967296ULL / (uint64_t)view->F);
-    {
-        const char *tune = getenv("B2D_TUNE");
-        d.tune = tune ? (uint32_t)strtoul(tune, nullptr, 0) : 0u;
-    }
     if (d.nsegs + d.nsprites > 65535) { free_renderer(r); return fail(B2D_ERR_INVALID_ARG, "level has more than 65535 segs + sprites"); }
     if (walk_smem_per_warp(d) > 227 * 1024) { free_renderer(r); return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory"); }
     if (scene_is_timed(s->blob.data())) {
@@ -902,9 +871,9 @@ int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tic
     CU(cudaMemcpy(&status, r->d_status, sizeof status, cudaMemcpyDeviceToHost));
     if (status) {
         CU(cudaMemset(r->d_status, 0, sizeof(int32_t)));
-        return fail(B2D_ERR_INVALID_ARG, status & 1 ? "BSP traversal stack overflow (tree deeper than 128 pending nodes): frames incomplete"
-                                            : (status & 4 ? "BSP traversal did not terminate (cyclic node graph): frames incomplete"
-                                              : (status & 8 ? "more masked middle textures / sprites deferred in one 32-column strip than the renderer holds (min(level total, 128)): frames incomplete"
+        return fail(B2D_ERR_INVALID_ARG, status & kStatusStackOverflow ? "BSP traversal stack overflow (tree deeper than 128 pending nodes): frames incomplete"
+                                            : (status & kStatusNoTermination ? "BSP traversal did not terminate (cyclic node graph): frames incomplete"
+                                              : (status & kStatusMaskedFull ? "more masked middle textures / sprites deferred in one 32-column strip than the renderer holds (min(level total, 128)): frames incomplete"
                                                             : "worklist overflow: frames incomplete")));
     }
     return B2D_OK;

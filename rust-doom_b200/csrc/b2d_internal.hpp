@@ -68,8 +68,6 @@ struct b2d_renderer {
     int timed_next = 0;
     size_t timed_bytes = 0;
     uint8_t *d_walk_static = nullptr;                     // node / subsector tables as the walk kernel's shared memory holds them
-    size_t l2_window_bytes = 0;                           // B2D_L2PERSIST: persisting L2 access window over the pre-lit texel planes
-    float l2_hit_ratio = 0.f;
     std::vector<int32_t> floor_off, ceil_off;             // state of the moving sectors (one offset per sector; empty = at rest)
     std::vector<uint8_t> cur_tables, scratch_tables;      // host copies: tables of the last upload / of a candidate time
     cudaEvent_t masked_done = nullptr;                    // last raster that used the masked-entry arena

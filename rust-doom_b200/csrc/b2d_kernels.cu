@@ -15,49 +15,12 @@
 // kernels are integer/LSU/latency bound and are tuned against the HBM write roofline (DESIGN.md).
 #include "b2d_kernels.cuh"
 
-#include <cstdlib>
-
 namespace b2d {
 
 namespace {
 
 constexpr unsigned kFull = 0xFFFFFFFFu;
 
-// texel / table loads of the raster: read-only path; B2D_LOAD_EL (A/B build variant) asks L1 to keep them
-#if defined(B2D_LOAD_L2EL)
-// A/B: ask L2 to keep the pre-lit planes (a 2 GB/ms write stream passes through the same L2)
-__device__ __forceinline__ uint64_t l2_keep_policy() {
-    uint64_t pol;
-    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
-#endif
-__device__ __forceinline__ uint32_t tex_ld(const uint8_t *p) {
-#if defined(B2D_LOAD_L2EL)
-    uint32_t v;
-    asm("ld.global.nc.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(l2_keep_policy()));
-    return v;
-#elif defined(B2D_LOAD_EL)
-    uint32_t v;
-    asm("ld.global.nc.L1::evict_last.u8 %0, [%1];" : "=r"(v) : "l"(p));
-    return v;
-#else
-    return __ldg(p);
-#endif
-}
-__device__ __forceinline__ uint32_t tex_ld(const uint32_t *p) {
-#if defined(B2D_LOAD_L2EL)
-    uint32_t v;
-    asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(l2_keep_policy()));
-    return v;
-#elif defined(B2D_LOAD_EL)
-    uint32_t v;
-    asm("ld.global.nc.L1::evict_last.u32 %0, [%1];" : "=r"(v) : "l"(p));
-    return v;
-#else
-    return __ldg(p);
-#endif
-}
 constexpr int kMaskWords = 128;      // up to 4096 columns
 constexpr int kStackDepth = 128;
 
@@ -131,7 +94,6 @@ __host__ __device__ inline WalkSmem walk_layout(int nverts, int nsegs, int nnode
 }
 
 // 1-D bulk copy global -> shared memory through the TMA unit (cp.async.bulk, SASS UBLKCP), completion on an mbarrier.
-// B2D_WALK_NO_BULK (A/B build variant) stages the same bytes with a thread loop instead.
 __device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t arrivals) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(arrivals));
@@ -183,21 +145,17 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
 
     // One frame per CTA when the grid has a CTA per frame; a smaller (persistent) grid loops: that is the form for running
     // under another batch's raster -- a CTA per SM keeps the walk's footprint at 1/8 of the register file while it takes
-    // a few frame latencies, all hidden behind the raster (launch_walk, B2D_TUNE bit 2).
+    // a few frame latencies, all hidden behind the raster (launch_walk).
     // The traversal tables (node partition lines + children, subsector records) do not depend on the frame: one bulk copy
     // per CTA brings them into shared memory while the threads are busy with steps 1-3 of the first frame.
     const uint32_t static_bytes = 32u * (uint32_t)sc.nnodes + 16u * (uint32_t)sc.nss;
     bool static_pending = false;
-#if !defined(B2D_WALK_NO_BULK)
     if (static_bytes) {
         if (tid == 0) mbar_init(&s_bar, 1);
         __syncthreads();
         if (tid == 0) bulk_copy_g2s(node_s, sc.walk_static, static_bytes, &s_bar);
         static_pending = true;
     }
-#else
-    for (uint32_t i = tid; i < static_bytes / 16u; i += nthr) node_s[i] = reinterpret_cast<const int4 *>(sc.walk_static)[i];
-#endif
     for (int frame = blockIdx.x; frame < n; frame += gridDim.x) {
     FrameConst fc;
     frame_setup(poses[frame], fc);
@@ -218,11 +176,9 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
         int32_t flags = S.flags;
         if (!(flags & kSegInvalid)) {
             SegFrame sf;
-            const bool closes = !(flags & kSegTwoSided) || S.otop <= S.obot;   // every column it covers closes
-            if (seg_frame_setup(vw, tx[S.v1], tz[S.v1], tx[S.v2], tz[S.v2], sf, closes)) {
-                bool solid = closes && (sf.flags & kSegFrameNoSkip);
-                packed = pack_range(sf.xlo, sf.xhi, kVisBit | (solid ? kSolidBit : 0u));
-            }
+            const bool closes = seg_closes(flags & kSegTwoSided, S.otop, S.obot);
+            if (seg_frame_setup(vw, tx[S.v1], tz[S.v1], tx[S.v2], tz[S.v2], sf, closes))
+                packed = pack_range(sf.xlo, sf.xhi, kVisBit | (seg_solid(closes, sf) ? kSolidBit : 0u));
         }
         segr[i] = packed;
     }
@@ -258,7 +214,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
     int sp = warp == 0 ? 1 : 0, count = 0, status = 0;
     int budget = 2 * (sc.nnodes + sc.nss) + 64;      // a corrupt BSP with a cycle must not hang the GPU
     while (sp > 0) {
-        if (--budget < 0) { status |= 4; break; }
+        if (--budget < 0) { status |= kStatusNoTermination; break; }
         uint32_t child = stack[--sp];
         __syncwarp();
         if (child & kLeaf) {
@@ -332,7 +288,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
             bool far_vis = (rf & kVisBit) && range_open(mask, lane, range_lo(rf), range_hi(rf), passes);
             bool near_vis = (rn & kVisBit) && range_open(mask, lane, range_lo(rn), range_hi(rn), passes);
             int need = (far_vis ? 1 : 0) + (near_vis ? 1 : 0);
-            if (sp + need > kStackDepth) { status = 1; break; }
+            if (sp + need > kStackDepth) { status = kStatusStackOverflow; break; }
             if (lane == 0) {
                 int p = sp;
                 if (far_vis) stack[p++] = far_c;
@@ -344,7 +300,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
     }
     __syncwarp();
     if (warp == 0 && lane == 0) {
-        if (count > stride) { count = stride; status |= 2; }
+        if (count > stride) { count = stride; status |= kStatusWorklistFull; }
         s_count = count; s_status = status;
     }
     __syncthreads();
@@ -354,13 +310,12 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
     for (int k = tid; k < count; k += nthr) {
         int si = list[k];
         SegFrame sf;
-        if (si >= sc.nsegs) {                         // sprite entry: seg = -1 - sprite index, (cx, cz) in Nc/Nx
+        if (si >= sc.nsegs) {
             const int pi = si - sc.nsegs;
             const SpriteRec &P = sc.sprites[pi];
             SpriteFrame sp;
             sprite_setup(fc, vw, P.x, P.y, (int32_t)sc.tex[P.tex].w, sp);
-            sf.Nc = sp.cx; sf.Nx = sp.cz; sf.Dc = 0; sf.Dx = 0; sf.Dmax = 0; sf.Rm = 0; sf.sh = 0; sf.e = 0;
-            sf.seg = -1 - pi; sf.xlo = (int16_t)sp.lo; sf.xhi = (int16_t)sp.hi; sf.flags = 0; sf.pad = 0;
+            sprite_entry(pi, sp, sf);
             work[(size_t)frame * stride + k] = sf;
             continue;
         }
@@ -406,13 +361,7 @@ struct RasterCtx {
 template <bool kRgba>
 __device__ __forceinline__ void put_px(const RasterCtx &c, uint8_t *p8, uint32_t *p32, bool on, uint32_t v) {
     if (on) {
-#if defined(B2D_STORE_CS)
-        __stcs(p8, (uint8_t)v);       // A/B: streaming store, keeps frame bytes from displacing texels
-#elif defined(B2D_STORE_WT)
-        __stwt(p8, (uint8_t)v);
-#else
         *p8 = (uint8_t)v;
-#endif
         if (kRgba) *p32 = lds_u32(c.pal_s + 4u * v);
     }
 }
@@ -424,13 +373,8 @@ __host__ __device__ __forceinline__ bool tex_interleaved(const TexRec &T) { retu
 // form serialises load -> lookup -> store and leaves the LSU idle while each warp waits).  `full` (warp-uniform)
 // says every lane owns all rows of the batch, so the stores need no predicate.
 constexpr int kBatch = 8;
-#if defined(B2D_FLAT_BATCH)
-constexpr int kFlatBatch = B2D_FLAT_BATCH;     // A/B: gathers in flight per warp in the flat loop
-#else
-constexpr int kFlatBatch = 8;
-#endif
 
-template <bool kRgba, int kW, int kBatch = ::b2d::kBatch>
+template <bool kRgba, int kW>
 __device__ __forceinline__ void store_batch(const RasterCtx &c, uint8_t *p8, uint32_t *p32, const uint32_t (&v)[kBatch],
                                             int y, int ya, int yb, bool full) {
     const int Wc = kW ? kW : c.W;
@@ -477,7 +421,7 @@ __device__ __forceinline__ void draw_sky_warp(const RasterCtx &c, int ya, int yb
 #pragma unroll 2
     for (int y = y0; y < y1; y++, p8 += Wc, p32 += Wc) {
         const uint32_t r = sc.skyrow[y];                                   // warp-uniform table entry
-        put_px<kRgba>(c, p8, p32, y >= ya && y < yb, tex_ld(px + (inter ? (r >> 2) * w4 + (r & 3u) : r * T.w)));
+        put_px<kRgba>(c, p8, p32, y >= ya && y < yb, __ldg(px + (inter ? (r >> 2) * w4 + (r & 3u) : r * T.w)));
     }
 }
 
@@ -516,21 +460,21 @@ __device__ __forceinline__ void draw_plane_warp(const RasterCtx &c, const FrameC
         __syncwarp();
         const int rows = min(32, y1 - yc);
         int j = 0;
-        for (; j + kFlatBatch <= rows; j += kFlatBatch, p8 += (size_t)kFlatBatch * Wc, p32 += (size_t)kFlatBatch * Wc) {
-            uint32_t v[kFlatBatch];
+        for (; j + kBatch <= rows; j += kBatch, p8 += (size_t)kBatch * Wc, p32 += (size_t)kBatch * Wc) {
+            uint32_t v[kBatch];
 #pragma unroll
-            for (int k = 0; k < kFlatBatch; k++) {
+            for (int k = 0; k < kBatch; k++) {
                 const uint2 rz = c.rowz[j + k];                               // shared-memory broadcast: one 64-bit word per row
-                v[k] = tex_ld(reinterpret_cast<const uint8_t *>(px_hi | flat_offset(rz.y, bu + rz.x * ax, bv + rz.x * ay)));   // always in bounds
+                v[k] = __ldg(reinterpret_cast<const uint8_t *>(px_hi | flat_offset(rz.y, bu + rz.x * ax, bv + rz.x * ay)));   // always in bounds
             }
             const int y = yc + j;
-            store_batch<kRgba, kW, kFlatBatch>(c, p8, p32, v, y, ya, yb, y >= full_lo && y + kFlatBatch <= full_hi);
+            store_batch<kRgba, kW>(c, p8, p32, v, y, ya, yb, y >= full_lo && y + kBatch <= full_hi);
         }
         for (; j < rows; j++, p8 += Wc, p32 += Wc) {
             const uint2 rz = c.rowz[j];
             const int y = yc + j;
             put_px<kRgba>(c, p8, p32, y >= ya && y < yb,
-                          tex_ld(reinterpret_cast<const uint8_t *>(px_hi | flat_offset(rz.y, bu + rz.x * ax, bv + rz.x * ay))));
+                          __ldg(reinterpret_cast<const uint8_t *>(px_hi | flat_offset(rz.y, bu + rz.x * ax, bv + rz.x * ay))));
         }
         __syncwarp();
     }
@@ -549,8 +493,8 @@ __device__ __forceinline__ void wall_fast_loop(const RasterCtx &c, const uint8_t
 #pragma unroll 1
     for (int y = y0; y < y1; y += R, p8 += (size_t)R * Wc, p32 += (size_t)R * Wc) {
         const uint32_t q1 = q + 1u == nq ? 0u : q + 1u;
-        const uint32_t w0 = tex_ld(reinterpret_cast<const uint32_t *>(plq + (size_t)q * w4));
-        const uint32_t w1 = tex_ld(reinterpret_cast<const uint32_t *>(plq + (size_t)q1 * w4));
+        const uint32_t w0 = __ldg(reinterpret_cast<const uint32_t *>(plq + (size_t)q * w4));
+        const uint32_t w1 = __ldg(reinterpret_cast<const uint32_t *>(plq + (size_t)q1 * w4));
         if (y >= full_lo && y + R <= full_hi) {
 #pragma unroll
             for (int k = 0; k < R; k++) {
@@ -593,10 +537,10 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
     uint32_t *p32 = kRgba ? c.rgba + (size_t)y0 * Wc : nullptr;
     // Texel loads are unconditional (t is a bounded linear function of y for every lane, so the row index
     // is always inside the texture); only the store is predicated.  That keeps the loops branch-free.
-    if (tex_interleaved(T) && T.h >= 8u && !(sc.tune & 1u)) {
+    if (tex_interleaved(T) && T.h >= 8u) {
         // magnified columns: the whole piece runs on the incremental path when every lane qualifies (inactive lanes step 0)
         const uint32_t ts = act ? tstep : 0u;
-        const bool f16 = !(sc.tune & 2u) && __all_sync(kFull, ts <= kWallFast16);
+        const bool f16 = __all_sync(kFull, ts <= kWallFast16);
         if (f16 || __all_sync(kFull, ts <= kWallFast8)) {
             const uint32_t tt = act ? t : 0u;
             const uint32_t r0 = wall_row((int32_t)tt, T.h, T.hmagic, T.hbias);
@@ -620,8 +564,8 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
             uint32_t v[kBatch];
             if (__all_sync(kFull, b7 < 8u)) {
                 const uint32_t q0 = r0 >> 2, q1 = next_quad(q0, T.h);
-                const uint32_t w0 = tex_ld(reinterpret_cast<const uint32_t *>(pl + (q0 * w4 + colb)));
-                const uint32_t w1 = tex_ld(reinterpret_cast<const uint32_t *>(pl + (q1 * w4 + colb)));
+                const uint32_t w0 = __ldg(reinterpret_cast<const uint32_t *>(pl + (q0 * w4 + colb)));
+                const uint32_t w1 = __ldg(reinterpret_cast<const uint32_t *>(pl + (q1 * w4 + colb)));
 #pragma unroll
                 for (int k = 0; k < kBatch; k++) {
                     v[k] = pick_byte(w0, w1, (acc + (uint32_t)k * tstep) >> 16);
@@ -635,10 +579,10 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
                 const uint32_t acc4 = wall_acc(t4, r4);
                 if (__all_sync(kFull, ((acc + 3u * tstep) >> 16) < 8u && ((acc4 + 3u * tstep) >> 16) < 8u)) {
                     const uint32_t q0 = r0 >> 2, q4 = r4 >> 2;
-                    const uint32_t a0 = tex_ld(reinterpret_cast<const uint32_t *>(pl + (q0 * w4 + colb)));
-                    const uint32_t a1 = tex_ld(reinterpret_cast<const uint32_t *>(pl + (next_quad(q0, T.h) * w4 + colb)));
-                    const uint32_t b0 = tex_ld(reinterpret_cast<const uint32_t *>(pl + (q4 * w4 + colb)));
-                    const uint32_t b1 = tex_ld(reinterpret_cast<const uint32_t *>(pl + (next_quad(q4, T.h) * w4 + colb)));
+                    const uint32_t a0 = __ldg(reinterpret_cast<const uint32_t *>(pl + (q0 * w4 + colb)));
+                    const uint32_t a1 = __ldg(reinterpret_cast<const uint32_t *>(pl + (next_quad(q0, T.h) * w4 + colb)));
+                    const uint32_t b0 = __ldg(reinterpret_cast<const uint32_t *>(pl + (q4 * w4 + colb)));
+                    const uint32_t b1 = __ldg(reinterpret_cast<const uint32_t *>(pl + (next_quad(q4, T.h) * w4 + colb)));
 #pragma unroll
                     for (int k = 0; k < 4; k++) {
                         v[k] = pick_byte(a0, a1, (acc + (uint32_t)k * tstep) >> 16);
@@ -649,7 +593,7 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
 #pragma unroll
                     for (int k = 0; k < kBatch; k++) {
                         const uint32_t rk = wall_row((int32_t)(t + (uint32_t)k * tstep), T.h, T.hmagic, T.hbias);
-                        v[k] = tex_ld(pl + ((rk >> 2) * w4 + colb + (rk & 3u)));
+                        v[k] = __ldg(pl + ((rk >> 2) * w4 + colb + (rk & 3u)));
                     }
                 }
             }
@@ -661,7 +605,7 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
         const uint8_t *px = pl + col;
 #pragma unroll 1
         for (int y = y0; y < y1; y++, p8 += Wc, p32 += Wc, t += tstep)
-            put_px<kRgba>(c, p8, p32, y >= ya && y < yb, tex_ld(px + wall_row((int32_t)t, T.h, T.hmagic, T.hbias) * T.w));
+            put_px<kRgba>(c, p8, p32, y >= ya && y < yb, __ldg(px + wall_row((int32_t)t, T.h, T.hmagic, T.hbias) * T.w));
     }
 }
 
@@ -671,7 +615,7 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
 __device__ __forceinline__ uint32_t *masked_entry(const DeviceScene &sc, const uint32_t *chunks, int e) {
     return sc.masked_list + ((size_t)chunks[e / kMaskedChunk] * kMaskedChunk + (size_t)(e % kMaskedChunk)) * 33u;
 }
-// next entry of this warp, or nullptr when the strip's cap or the arena is exhausted (status bit 8: frames incomplete)
+// next entry of this warp, or nullptr when the strip's cap or the arena is exhausted (frames incomplete)
 __device__ __forceinline__ uint32_t *masked_push(const DeviceScene &sc, uint32_t *chunks, int &mcount, int lane) {
     bool ok = mcount < sc.masked_cap;
     if (ok && mcount % kMaskedChunk == 0) {
@@ -683,7 +627,7 @@ __device__ __forceinline__ uint32_t *masked_push(const DeviceScene &sc, uint32_t
         __syncwarp();
     }
     if (!ok) {
-        if (lane == 0) atomicOr(sc.status_flag, 8);
+        if (lane == 0) atomicOr(sc.status_flag, kStatusMaskedFull);
         return nullptr;
     }
     return masked_entry(sc, chunks, mcount++);
@@ -711,23 +655,19 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
         int ya = (int)(packed & 0xFFFFu), yb = (int)(packed >> 16);
         const SegFrame sf = wl[k];
         int32_t tex, tA, hA, ucol = 0, iscale = 1, row = 0;
-        if (sf.seg < 0) {
+        if (is_sprite_entry(sf)) {
             // decoration sprite (billboard at constant depth): everything but the column is warp-uniform
-            const SpriteRec P = sc.sprites[-1 - sf.seg];
+            SpriteFrame sp;
+            const SpriteRec P = sc.sprites[entry_sprite(sf, sp)];
             if (P.tex < 0 || P.tex >= sc.ntex) continue;
             const int32_t sw = (int32_t)sc.tex[P.tex].w, sh = (int32_t)sc.tex[P.tex].h;
-            SpriteFrame sp;
-            sp.cx = sf.Nc; sp.cz = sf.Nx;
-            int64_t scale = ((int64_t)vw.FY2 << 25) / sp.cz;
-            const int64_t cap = (int64_t)vw.FY2 << 17;
-            if (scale > cap) scale = cap;
-            iscale = (int32_t)clampv<int64_t>(((int64_t)1 << 38) / scale, 1, 1 << 23);
-            int64_t z8 = ((int64_t)iscale * vw.FY2) >> 18;
-            row = light_row_sprite(P.light, z8 > 65535 ? 65535 : (int32_t)z8);
+            const int64_t scale = sprite_scale(vw, sp.cz);      // >= 1: the walk's sprite_setup accepted the sprite
+            int32_t z8;
+            scale_depth(vw, scale, iscale, z8);
+            row = light_row_sprite(P.light, z8);
             tex = P.tex; tA = 0; hA = P.low + sh;
             if (ya < yb) {
-                ya = max(ya, yrow(P.low + sh, (int32_t)scale, pose_z, c.H));
-                yb = min(yb, yrow(P.low, (int32_t)scale, pose_z, c.H));
+                clip_rows(P.low + sh, P.low, (int32_t)scale, pose_z, c.H, ya, yb);
                 ucol = sprite_column(sp, vw, c.x, sw);
             }
         } else {
@@ -737,9 +677,8 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
             tex = M.tex; tA = M.t_high; hA = M.high;
             ColumnEval ce = {0u, 1, 1, 0};
             if (ya < yb && column_eval(sf, vw, c.x, ce)) {
-                ya = max(ya, yrow(M.high, ce.scale, pose_z, c.H));
-                yb = min(yb, yrow(M.low, ce.scale, pose_z, c.H));
-                ucol = S.uoff + (int32_t)(((uint64_t)ce.s24 * (uint32_t)S.len_q12) >> 36);
+                clip_rows(M.high, M.low, ce.scale, pose_z, c.H, ya, yb);
+                ucol = wall_column(S.uoff, S.len_q12, ce.s24);
                 iscale = ce.iscale;
                 row = light_row(S.light, ce.z8);
             } else {
@@ -776,12 +715,12 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
                 uint32_t v[kBatch], o[kBatch];
                 if (__all_sync(kFull, ((acc + 7u * tstep) >> 16) < 8u)) {
                     const uint32_t o0 = (r0 >> 2) * w4 + colb, o1 = next_quad(r0 >> 2, T.h) * w4 + colb;
-                    const uint32_t w0 = tex_ld(reinterpret_cast<const uint32_t *>(pl + o0));
-                    const uint32_t w1 = tex_ld(reinterpret_cast<const uint32_t *>(pl + o1));
+                    const uint32_t w0 = __ldg(reinterpret_cast<const uint32_t *>(pl + o0));
+                    const uint32_t w1 = __ldg(reinterpret_cast<const uint32_t *>(pl + o1));
                     uint32_t m0 = 0x01010101u, m1 = 0x01010101u;
                     if (has_mask) {
-                        m0 = tex_ld(reinterpret_cast<const uint32_t *>(pm + o0));
-                        m1 = tex_ld(reinterpret_cast<const uint32_t *>(pm + o1));
+                        m0 = __ldg(reinterpret_cast<const uint32_t *>(pm + o0));
+                        m1 = __ldg(reinterpret_cast<const uint32_t *>(pm + o1));
                     }
 #pragma unroll
                     for (int k = 0; k < kBatch; k++) {
@@ -794,8 +733,8 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
                     for (int k = 0; k < kBatch; k++) {
                         const uint32_t rk = wall_row((int32_t)(t + (uint32_t)k * tstep), T.h, T.hmagic, T.hbias);
                         const uint32_t off = (rk >> 2) * w4 + colb + (rk & 3u);
-                        v[k] = tex_ld(pl + off);
-                        o[k] = has_mask ? (uint32_t)tex_ld(pm + off) : 1u;
+                        v[k] = __ldg(pl + off);
+                        o[k] = has_mask ? (uint32_t)__ldg(pm + off) : 1u;
                     }
                 }
 #pragma unroll
@@ -806,21 +745,21 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
 #pragma unroll 1
             for (int y = y0; y < y1; y++, p8 += Wc, p32 += Wc, t += tstep) {
                 const uint32_t off = wall_row((int32_t)t, T.h, T.hmagic, T.hbias) * T.w + col;
-                const bool on = (uint32_t)(y - ya) < len && (!has_mask || tex_ld(pm + off) != 0);
-                put_px<kRgba>(c, p8, p32, on, tex_ld(pl + off));
+                const bool on = (uint32_t)(y - ya) < len && (!has_mask || __ldg(pm + off) != 0);
+                put_px<kRgba>(c, p8, p32, on, __ldg(pl + off));
             }
         }
     }
 }
 
-template <bool kRgba, int kMinBlocks, int kW, int kWarps, bool kMasked>
-__global__ void __launch_bounds__(kWarps * 32, kMinBlocks)
+template <bool kRgba, int kW, bool kMasked>
+__global__ void __launch_bounds__(32, 24)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb) {
     __shared__ uint32_t s_pal[kRgba ? 256 : 1];
-    __shared__ uint2 s_rowz[kWarps][32];
-    __shared__ uint32_t s_chunks[kMasked ? kWarps : 1][kMasked ? kMaskedCapMax / kMaskedChunk : 1];
+    __shared__ uint2 s_rowz[32];
+    __shared__ uint32_t s_chunks[kMasked ? kMaskedCapMax / kMaskedChunk : 1];
     if (kRgba) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
         for (int i = threadIdx.x; i < 256; i += blockDim.x) s_pal[i] = sc.palette[i];
         __syncthreads();
@@ -838,7 +777,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     RasterCtx c;
     c.sc = &sc;
     c.pal_s = (uint32_t)__cvta_generic_to_shared(s_pal);
-    c.rowz = s_rowz[threadIdx.x >> 5];
+    c.rowz = s_rowz;
     c.dir = plane_dir(fc, vw, inside ? x : 0, sc.invF);
     c.fb = index_fb + (size_t)frame * W * H + (inside ? x : 0);
     c.rgba = kRgba ? rgba_fb + (size_t)frame * W * H + (inside ? x : 0) : nullptr;
@@ -847,7 +786,8 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     if (sc.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), sc.tex[sc.sky_tex].w);
 
     int ct = 0, cb = inside ? H : 0;              // open window [ct, cb) of this lane's column
-    uint32_t *chunks = s_chunks[kMasked ? (threadIdx.x >> 5) : 0];
+    uint32_t *chunks = s_chunks;
+    asm("" : "+l"(chunks));        // a run-time value: propagated into masked_pass as a constant, it makes that pass spill more
     const bool defer = kMasked && sc.masked_list != nullptr;
     int mcount = 0;
     const SegFrame *wl = work + (size_t)frame * stride;
@@ -869,7 +809,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             const SegFrame sf = wl[k0 + j];                              // warp-uniform 64 B
             bool in = inside && ct < cb && x >= sf.xlo && x <= sf.xhi;
             if (!__any_sync(kFull, in)) continue;
-            if (sf.seg < 0) {
+            if (is_sprite_entry(sf)) {
                 // decoration sprite: remember the windows open right now; it is drawn in the masked pass
                 if (defer) {
                     uint32_t *ml = masked_push(sc, chunks, mcount, lane);
@@ -888,26 +828,16 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             const SectorRec SF = sc.sectors[S.front];
             const int32_t fcl = SF.ceil, ffl = SF.floor;
             const bool two = S.flags & kSegTwoSided;
-            const bool ceil_vis = ((int64_t)fcl << 16) > fc.pose.z || SF.ceil_flat == kFlatSky;
-            const bool floor_vis = ((int64_t)ffl << 16) < fc.pose.z || SF.floor_flat == kFlatSky;
+            const bool ceil_vis = plane_visible(true, fcl, SF.ceil_flat == kFlatSky, fc.pose.z);
+            const bool floor_vis = plane_visible(false, ffl, SF.floor_flat == kFlatSky, fc.pose.z);
 
-            // per-lane rows: y1 wall top, y2 end of upper, y3 start of lower, y4 start of floor
-            int y1 = ct, y2 = ct, y3 = ct, y4 = ct, yend = ct, row = 0;
+            WallRows wr = {ct, ct, ct, ct};          // per lane
+            int yend = ct, row = 0;
             int32_t ucol = 0;
             if (ok) {
                 row = light_row(S.light, ce.z8);
-                ucol = S.uoff + (int32_t)(((uint64_t)ce.s24 * (uint32_t)S.len_q12) >> 36);
-                int yfc = yrow(fcl, ce.scale, fc.pose.z, H), yff = yrow(ffl, ce.scale, fc.pose.z, H);
-                y1 = clampv(yfc, ct, cb);
-                if (!two) {
-                    y2 = clampv(yff, y1, cb);       // one-sided: [y1,y2) is the middle texture
-                    y3 = y2; y4 = y2;
-                } else {
-                    int yot = yrow(S.otop, ce.scale, fc.pose.z, H), yob = yrow(S.obot, ce.scale, fc.pose.z, H);
-                    y2 = clampv(yot, y1, cb);
-                    y3 = clampv(yob, y2, cb);
-                    y4 = clampv(yff, y3, cb);
-                }
+                ucol = wall_column(S.uoff, S.len_q12, ce.s24);
+                wr = wall_rows(fcl, ffl, two, S.otop, S.obot, ce.scale, fc.pose.z, H, ct, cb);
                 yend = cb;
             }
             // The two flat spans (ceiling [ct, y1), floor [y4, cb)) and the two wall pieces go through ONE inlined
@@ -916,30 +846,27 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
 #pragma unroll 1
             for (int pz = 0; pz < 2; pz++) {
                 const bool top = pz == 0;
-                draw_plane_warp<kRgba, kW>(c, fc, vw, ok ? (top ? ct : y4) : 0, ok ? (top ? y1 : yend) : 0,
+                draw_plane_warp<kRgba, kW>(c, fc, vw, ok ? (top ? ct : wr.y4) : 0, ok ? (top ? wr.y1 : yend) : 0,
                                                     top ? fcl : ffl, top ? SF.ceil_flat : SF.floor_flat, SF.light,
                                                     top ? ceil_vis : floor_vis);
             }
 #pragma unroll 1
             for (int pw = 0; pw < 2; pw++) {
-                const bool upper = pw == 0;            // A: upper (two-sided) or the one-sided middle; B: lower
-                if (upper ? (two && !(S.otop < fcl)) : !(two && S.obot > ffl)) continue;
-                draw_wall_warp<kRgba, kW>(c, fc, ok ? (upper ? y1 : y3) : 0, ok ? (upper ? y2 : y4) : 0,
+                const bool upper = pw == 0;            // piece A, then piece B
+                if (!wall_piece(upper, two, fcl, ffl, S.otop, S.obot)) continue;
+                draw_wall_warp<kRgba, kW>(c, fc, ok ? (upper ? wr.y1 : wr.y3) : 0, ok ? (upper ? wr.y2 : wr.y4) : 0,
                                                    upper ? S.texA : S.texB, upper ? S.tA : S.tB, upper ? S.hA : S.hB,
                                                    ucol, ce.iscale, row);
             }
-            if (ok) {
-                if (!two || y2 >= y3) { ct = H; cb = 0; }
-                else { ct = y2; cb = y3; }
-            }
+            if (ok) wall_window(two, wr, H, ct, cb);
             if (defer && two && S.mid >= 0) {
                 // defer the masked middle texture: remember the window that is open behind this seg
-                const bool keep = ok && y2 < y3;
+                const bool keep = ok && wr.y2 < wr.y3;
                 if (__any_sync(kFull, keep)) {
                     uint32_t *ml = masked_push(sc, chunks, mcount, lane);
                     if (ml) {
                         if (lane == 0) ml[0] = (uint32_t)(k0 + j);
-                        ml[1 + lane] = keep ? ((uint32_t)y2 | ((uint32_t)y3 << 16)) : 0u;
+                        ml[1 + lane] = keep ? ((uint32_t)wr.y2 | ((uint32_t)wr.y3 << 16)) : 0u;
                     }
                 }
             }
@@ -1010,9 +937,8 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
     // background (b2d_walk_device: the walk of the NEXT batch, meant to run under another batch's raster): a persistent grid
     // of one CTA per SM.  It takes n/SMs frame latencies instead of one, but holds 1/8 of the register file instead of
     // 7/8, so the raster keeps 22 of its 24 warps per SM while the walk hides behind it.
-    // B2D_TUNE bit 2 (4) turns it off for A/B.
     const int sms = device_sms();
-    const int blocks = (background && !(sc.tune & 4u) && n > sms) ? sms : n, warps = 4;
+    const int blocks = (background && n > sms) ? sms : n, warps = 4;
     b2d_walk_kernel<<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride);
     return cudaGetLastError();
 }
@@ -1027,35 +953,16 @@ cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameCons
     // 14 % more frames/s on an H100 SXM (bench.py c2).  Strips differ a lot in cost; with several warps per CTA the finished warps' slots
     // stay empty until the slowest warp of the CTA is done.
     // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
-#if defined(B2D_RASTER_WARPS)         // A/B: more resident warps per SM at fewer registers per thread
-    constexpr int kWarps = B2D_RASTER_WARPS, kMinBlocks = B2D_RASTER_MINBLOCKS;
-#else
-    constexpr int kWarps = 1, kMinBlocks = 24;
-#endif
-    const long long total_warps = (long long)n * strips;
-    const int nblocks = (int)((total_warps + kWarps - 1) / kWarps);
-    static const bool generic_w = getenv("B2D_RASTER_GENERIC_W") != nullptr;   // A/B knob
-    const bool w1920 = vw.W == 1920 && !generic_w;
-    // B2D_CARVEOUT=<percent of the SM's L1/shared array given to shared memory> (A/B): the raster uses ~300 B of it per warp
-    static const int carve = getenv("B2D_CARVEOUT") ? atoi(getenv("B2D_CARVEOUT")) : -1;
+    const int nblocks = (int)((long long)n * strips);     // one warp per (frame, strip)
+    const bool masked = (sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list;
 #define B2D_RASTER_GO(RGBA, KW) do { \
-    if ((sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list) { \
-        static const bool once = carve >= 0 && cudaFuncSetAttribute(b2d_raster_kernel<RGBA, kMinBlocks, KW, kWarps, true>, \
-                                                                     cudaFuncAttributePreferredSharedMemoryCarveout, carve) == cudaSuccess; \
-        (void)once; \
-        b2d_raster_kernel<RGBA, kMinBlocks, KW, kWarps, true><<<nblocks, kWarps * 32, 0, stream>>>( \
-            sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
-    } else { \
-        static const bool once = carve >= 0 && cudaFuncSetAttribute(b2d_raster_kernel<RGBA, kMinBlocks, KW, kWarps, false>, \
-                                                                     cudaFuncAttributePreferredSharedMemoryCarveout, carve) == cudaSuccess; \
-        (void)once; \
-        b2d_raster_kernel<RGBA, kMinBlocks, KW, kWarps, false><<<nblocks, kWarps * 32, 0, stream>>>( \
-            sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); } } while (0)
-    if (d_rgba) { if (w1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
-    else {
-        const bool w3840 = vw.W == 3840 && !generic_w;      // BASELINE.json's 4K configuration (index frames only)
-        if (w1920) B2D_RASTER_GO(false, 1920); else if (w3840) B2D_RASTER_GO(false, 3840); else B2D_RASTER_GO(false, 0);
-    }
+    if (masked) b2d_raster_kernel<RGBA, KW, true><<<nblocks, 32, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
+    else b2d_raster_kernel<RGBA, KW, false><<<nblocks, 32, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
+    } while (0)
+    if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
+    else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
+    else if (vw.W == 3840) B2D_RASTER_GO(false, 3840);      // BASELINE.json's 4K configuration (index frames only)
+    else B2D_RASTER_GO(false, 0);
 #undef B2D_RASTER_GO
     return cudaGetLastError();
 }

@@ -35,19 +35,14 @@ struct DeviceScene {
     int32_t nverts, nnodes, nss, nsegs, nsectors, ntex, nflats, sky_tex, nmids, nsprites;
     uint32_t root;
     uint32_t invF;               // floor(2^32 / F)
-    int32_t *status_flag;        // device int: OR of per-frame walk status bits (0 = all frames complete)
+    int32_t *status_flag;        // device int: OR of the kStatus* bits of every frame (0 = all frames complete)
     uint32_t *masked_list;       // arena of deferred masked entries (33 words each: worklist index + 32 packed windows),
                                  // handed out in chunks of kMaskedChunk entries; nullptr = level without masked content
     uint32_t *masked_counter;    // chunks handed out by the current raster launch (reset before every launch)
-    uint32_t masked_chunks;      // arena capacity in chunks (exhausted -> status bit 8)
-    int32_t masked_cap;          // entries one 32-column strip can defer per frame (more -> status bit 8)
-    uint32_t tune;               // A/B switches (env B2D_TUNE, default 0): 1 no incremental wall path,
-                                 // 2 no 16-row batches, 4 no persistent grid for background walks
+    uint32_t masked_chunks;      // arena capacity in chunks (exhausted -> kStatusMaskedFull)
+    int32_t masked_cap;          // strip_masked_cap(): entries one 32-column strip can defer per frame
 };
 
-// masked middle textures + sprites one 32-column strip can defer per frame: min(masked mids + sprites of the level,
-// kMaskedCapMax), at least 8 (more deferred in one strip -> status bit 8, frames incomplete)
-constexpr int kMaskedCapMax = 128;
 constexpr int kMaskedChunk = 4;      // entries per arena chunk (528 bytes)
 
 // Bytes of dynamic shared memory the BSP-walk kernel needs per frame (= per CTA) for this scene.

@@ -32,10 +32,17 @@ struct FrameConst {
     int32_t cosq, sinq;        // Q30
     int32_t px8, py8;          // camera position, Q8
     int32_t count;             // worklist length
-    int32_t status;            // 0 ok, 1 = traversal stack overflow
+    int32_t status;            // 0 ok, else kStatus* bits
     int32_t pad[6];
 };
 static_assert(sizeof(FrameConst) == 64, "FrameConst");
+
+// Completeness status of a frame (FrameConst::status), OR-ed over every launch into the renderer's status flag
+// (b2d_renderer_status).  Any bit set: the frame is incomplete.
+constexpr int32_t kStatusStackOverflow = 1;   // BSP traversal stack overflow
+constexpr int32_t kStatusWorklistFull = 2;    // more worklist entries than the per-frame stride
+constexpr int32_t kStatusNoTermination = 4;   // BSP traversal budget exhausted (cyclic node graph)
+constexpr int32_t kStatusMaskedFull = 8;      // deferred masked entries: strip cap or arena exhausted
 
 // One worklist entry: a front-facing seg that may be visible, with its per-frame projection
 // coefficients.  N(x) = Nc + Nx*x and D(x) = Dc + Dx*x are the numerator / denominator of the
@@ -149,6 +156,14 @@ struct ColumnEval {
 B2D_HD bool seg_frame_setup(const View &vw, int32_t ax_, int32_t az_, int32_t bx_, int32_t bz_, SegFrame &sf,
                             bool want_noskip = true);
 
+// map units per pixel (Q20, clamped to [1, 2^23]) and view depth in 1/8 map units (<= 65535) of a column drawn at
+// `scale` pixels per map unit (Q18, >= 1)
+B2D_HD void scale_depth(const View &vw, int64_t scale, int32_t &iscale, int32_t &z8) {
+    iscale = (int32_t)clampv<int64_t>(((int64_t)1 << 38) / scale, 1, 1 << 23);
+    const int64_t z = ((int64_t)iscale * vw.FY2) >> 18;
+    z8 = z > 65535 ? 65535 : (int32_t)z;
+}
+
 // Column predicate + per-column projection values.  Exact: does not rely on xlo/xhi.
 B2D_HD bool column_eval(const SegFrame &sf, const View &vw, int x, ColumnEval &out) {
     int64_t N = sf.Nc + sf.Nx * x, D = sf.Dc + sf.Dx * x;
@@ -170,10 +185,7 @@ B2D_HD bool column_eval(const SegFrame &sf, const View &vw, int x, ColumnEval &o
     if (scale > cap) scale = cap;
     if (scale < 1) return false;
     out.scale = (int32_t)scale;
-    int64_t isc = ((int64_t)1 << 38) / scale;
-    out.iscale = (int32_t)clampv<int64_t>(isc, 1, 1 << 23);
-    int64_t z8 = ((int64_t)out.iscale * vw.FY2) >> 18;
-    out.z8 = z8 > 65535 ? 65535 : (int32_t)z8;
+    scale_depth(vw, scale, out.iscale, out.z8);
     return true;
 }
 
@@ -223,6 +235,11 @@ B2D_HD bool seg_frame_setup(const View &vw, int32_t ax_, int32_t az_, int32_t bx
     return true;
 }
 
+// A seg closes every column it covers when it is one-sided or its back sector is shut.  It is solid for the walk (marks
+// its columns in the solid-column mask) when it closes and passes column_eval on every column of [xlo, xhi].
+B2D_HD bool seg_closes(bool two, int32_t otop, int32_t obot) { return !two || otop <= obot; }
+B2D_HD bool seg_solid(bool closes, const SegFrame &sf) { return closes && (sf.flags & kSegFrameNoSkip); }
+
 // colormap row from light byte b and depth z8: clamp(floor(64(255-b)/255 - 2880/(z+90)), 0, 31)
 B2D_HD int light_row(int b, int32_t z8) {
     uint32_t Z = (uint32_t)z8 + 720u;
@@ -238,6 +255,51 @@ B2D_HD int yrow(int32_t h, int32_t scale, int32_t pose_z, int32_t H) {
     int64_t Y = ((int64_t)H << 25) - hrel8 * scale;
     int64_t r = (Y + ((int64_t)1 << 25) - 1) >> 26;
     return (int)clampv<int64_t>(r, 0, H);
+}
+
+// ---- one wall column inside the open window [ct, cb) of its screen column (DESIGN.md C6, C7) ----
+// A ceiling is drawn only above the eye and a floor only below it; a sky plane either way.
+B2D_HD bool plane_visible(bool ceiling, int32_t h, bool sky, int32_t pose_z) {
+    const int64_t h16 = (int64_t)h << 16;
+    return (ceiling ? h16 > pose_z : h16 < pose_z) || sky;
+}
+// y1 wall top, y2 end of the upper piece (one-sided: of the middle), y3 start of the lower piece, y4 start of the floor:
+// ceiling [ct, y1), upper [y1, y2), opening [y2, y3), lower [y3, y4), floor [y4, cb)
+struct WallRows { int y1, y2, y3, y4; };
+B2D_HD WallRows wall_rows(int32_t ceil, int32_t floor, bool two, int32_t otop, int32_t obot, int32_t scale, int32_t pose_z,
+                          int32_t H, int ct, int cb) {
+    WallRows r;
+    const int yfc = yrow(ceil, scale, pose_z, H), yff = yrow(floor, scale, pose_z, H);
+    r.y1 = clampv(yfc, ct, cb);
+    if (!two) {
+        r.y2 = clampv(yff, r.y1, cb);
+        r.y3 = r.y2; r.y4 = r.y2;
+    } else {
+        r.y2 = clampv(yrow(otop, scale, pose_z, H), r.y1, cb);
+        r.y3 = clampv(yrow(obot, scale, pose_z, H), r.y2, cb);
+        r.y4 = clampv(yff, r.y3, cb);
+    }
+    return r;
+}
+// Piece A is the upper piece of a two-sided seg (only below a higher front ceiling) or the middle of a one-sided one;
+// piece B is the lower piece of a two-sided seg (only above a lower front floor).
+B2D_HD bool wall_piece(bool upper, bool two, int32_t ceil, int32_t floor, int32_t otop, int32_t obot) {
+    return upper ? (!two || otop < ceil) : (two && obot > floor);
+}
+// the window the column leaves open behind the seg: the opening of a two-sided seg, else none
+B2D_HD void wall_window(bool two, const WallRows &r, int32_t H, int &ct, int &cb) {
+    if (!two || r.y2 >= r.y3) { ct = H; cb = 0; }
+    else { ct = r.y2; cb = r.y3; }
+}
+// texture column at seg parameter s24 (Q24) of a seg with offset uoff and length len_q12 (Q12), before the floor-mod
+B2D_HD int32_t wall_column(int32_t uoff, int32_t len_q12, uint32_t s24) {
+    return uoff + (int32_t)(((uint64_t)s24 * (uint32_t)len_q12) >> 36);
+}
+// clip a deferred window [ya, yb) to the rows of a masked piece (masked middle or sprite) between heights low and high
+B2D_HD void clip_rows(int32_t high, int32_t low, int32_t scale, int32_t pose_z, int32_t H, int &ya, int &yb) {
+    const int a = yrow(high, scale, pose_z, H), b = yrow(low, scale, pose_z, H);
+    if (a > ya) ya = a;
+    if (b < yb) yb = b;
 }
 
 B2D_HD uint32_t yslope_entry(int y, const View &vw) {
@@ -412,6 +474,12 @@ struct SpriteFrame {
     int32_t scale, iscale, z8;
 };
 
+// pixels per map unit (Q18, capped as in column_eval) of a sprite at view depth cz (Q8, >= 256); < 1: no size on screen
+B2D_HD int64_t sprite_scale(const View &vw, int64_t cz) {
+    const int64_t scale = ((int64_t)vw.FY2 << 25) / cz, cap = (int64_t)vw.FY2 << 17;
+    return scale > cap ? cap : scale;
+}
+
 // Per-frame projection of a sprite of width w (map units) centred at world (x, y).  false = not on screen.
 B2D_HD bool sprite_setup(const FrameConst &f, const View &vw, int32_t x, int32_t y, int32_t w, SpriteFrame &sp) {
     int32_t tx, tz;
@@ -425,16 +493,31 @@ B2D_HD bool sprite_setup(const FrameConst &f, const View &vw, int32_t x, int32_t
     constrain(lo, hi, R - 1 - sp.cz * (1 - W), -2 * sp.cz, 0);       // cz*c2 <= R-1
     if (lo > hi) return false;
     sp.lo = (int32_t)lo; sp.hi = (int32_t)hi;
-    int64_t scale = ((int64_t)vw.FY2 << 25) / sp.cz;
-    const int64_t cap = (int64_t)vw.FY2 << 17;
-    if (scale > cap) scale = cap;
+    const int64_t scale = sprite_scale(vw, sp.cz);
     if (scale < 1) return false;
     sp.scale = (int32_t)scale;
-    sp.iscale = (int32_t)clampv<int64_t>(((int64_t)1 << 38) / scale, 1, 1 << 23);
-    int64_t z8 = ((int64_t)sp.iscale * vw.FY2) >> 18;
-    sp.z8 = z8 > 65535 ? 65535 : (int32_t)z8;
+    scale_depth(vw, scale, sp.iscale, sp.z8);
     return true;
 }
+
+// A sprite travels through the worklist as a SegFrame: seg = -1 - sprite index, view-space centre (cx, cz) in (Nc, Nx),
+// column interval in (xlo, xhi), every other field zero.
+B2D_HD void sprite_entry(int sprite, const SpriteFrame &sp, SegFrame &sf) {
+    sf.Nc = sp.cx; sf.Nx = sp.cz; sf.Dc = 0; sf.Dx = 0; sf.Dmax = 0; sf.Rm = 0; sf.sh = 0; sf.e = 0;
+    sf.seg = -1 - sprite; sf.xlo = (int16_t)sp.lo; sf.xhi = (int16_t)sp.hi; sf.flags = 0; sf.pad = 0;
+}
+B2D_HD bool is_sprite_entry(const SegFrame &sf) { return sf.seg < 0; }
+// sprite index of a sprite entry; sp.cx, sp.cz := its view-space centre
+B2D_HD int entry_sprite(const SegFrame &sf, SpriteFrame &sp) {
+    sp.cx = sf.Nc; sp.cz = sf.Nx;
+    return -1 - sf.seg;
+}
+
+// Masked middles and sprites met by the raster's front-to-back pass are deferred to a back-to-front pass, at most
+// strip_masked_cap() entries per 32-column strip and frame: the level's total, at least 8, at most kMaskedCapMax
+// (more -> kStatusMaskedFull).
+constexpr int kMaskedCapMax = 128;
+B2D_HD int strip_masked_cap(int nmids, int nsprites) { return clampv(nmids + nsprites, 8, kMaskedCapMax); }
 
 // texture column of screen column x (0..w-1)
 B2D_HD int32_t sprite_column(const SpriteFrame &sp, const View &vw, int x, int32_t w) {

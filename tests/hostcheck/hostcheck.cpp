@@ -1,6 +1,6 @@
-// TEST-ONLY: runs the product's pixel-contract arithmetic (rust-doom_b200/csrc/b2d_math.cuh) and the
-// exact algorithms of the CUDA kernels on the CPU, one lane at a time, so that the maths can be
-// checked against the oracle without a GPU.  This file is compiled into tests/hostcheck/
+// TEST-ONLY: runs the product's pixel-contract arithmetic and per-column rules (rust-doom_b200/csrc/b2d_math.cuh,
+// the same functions the CUDA kernels call) in the kernels' algorithms on the CPU, one lane at a time, so that
+// they can be checked against the oracle without a GPU.  This file is compiled into tests/hostcheck/
 // libb2d_hostcheck.so by tests/conftest.py; it is NOT part of libb2d.so and no product code calls it.
 #include <cstdint>
 #include <algorithm>
@@ -93,11 +93,11 @@ void walk(const HostScene &sc, const View &vw, const Pose &pose, FrameConst &fc,
         const SegRec &S = sc.segs[i];
         if (S.flags & kSegInvalid) continue;
         SegFrame sf;
-        const bool closes = !(S.flags & kSegTwoSided) || S.otop <= S.obot;
+        const bool closes = seg_closes(S.flags & kSegTwoSided, S.otop, S.obot);
         if (seg_frame_setup(vw, tx[(size_t)S.v1], tz[(size_t)S.v1], tx[(size_t)S.v2], tz[(size_t)S.v2], sf, closes)) {
             Range &r = segr[(size_t)i];
             r.vis = true; r.lo = sf.xlo; r.hi = sf.xhi;
-            r.solid = closes && (sf.flags & kSegFrameNoSkip);
+            r.solid = seg_solid(closes, sf);
         }
     }
     for (int i = 0; i < 2 * sc.nnodes; i++) {
@@ -130,7 +130,7 @@ void walk(const HostScene &sc, const View &vw, const Pose &pose, FrameConst &fc,
     int status = 0;
     int budget = 2 * (sc.nnodes + sc.nss) + 64;
     while (!stack.empty()) {
-        if (--budget < 0) { status |= 4; break; }
+        if (--budget < 0) { status |= kStatusNoTermination; break; }
         uint32_t child = stack.back();
         stack.pop_back();
         if (child & kLeaf) {
@@ -168,7 +168,7 @@ void walk(const HostScene &sc, const View &vw, const Pose &pose, FrameConst &fc,
             const Range &rn = boxr[2 * (size_t)child + (size_t)side], &rf = boxr[2 * (size_t)child + (size_t)(side ^ 1)];
             bool far_vis = rf.vis && range_open(rf.lo, rf.hi);
             bool near_vis = rn.vis && range_open(rn.lo, rn.hi);
-            if (stack.size() + (far_vis ? 1 : 0) + (near_vis ? 1 : 0) > 128) { status = 1; break; }
+            if (stack.size() + (far_vis ? 1 : 0) + (near_vis ? 1 : 0) > 128) { status = kStatusStackOverflow; break; }
             if (far_vis) stack.push_back(N.child[side ^ 1]);
             if (near_vis) stack.push_back(N.child[side]);
         }
@@ -181,8 +181,7 @@ void walk(const HostScene &sc, const View &vw, const Pose &pose, FrameConst &fc,
             const SpriteRec &P = sc.sprites[pi];
             SpriteFrame sp;
             sprite_setup(fc, vw, P.x, P.y, (int32_t)sc.tex[P.tex].w, sp);
-            std::memset(&sf, 0, sizeof sf);
-            sf.Nc = sp.cx; sf.Nx = sp.cz; sf.seg = -1 - pi; sf.xlo = (int16_t)sp.lo; sf.xhi = (int16_t)sp.hi;
+            sprite_entry(pi, sp, sf);
             out.push_back(sf);
             continue;
         }
@@ -313,8 +312,7 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
             if (sc.sky_tex >= 0 && x < W) lanes[l].skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), sc.tex[sc.sky_tex].w);
         }
         struct Deferred { size_t k; std::vector<uint32_t> win; };
-        int masked_cap = sc.nmids + sc.nsprites;          // as b2d_renderer_create sizes the deferred lists
-        masked_cap = masked_cap < 8 ? 8 : (masked_cap > 128 ? 128 : masked_cap);
+        const int masked_cap = strip_masked_cap(sc.nmids, sc.nsprites);
         std::vector<Deferred> deferred;
         for (size_t k = 0; k < wl.size(); k++) {
             const SegFrame &sf = wl[k];
@@ -322,7 +320,7 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
             bool any_open = false;
             for (int l = 0; l < SW; l++) any_open |= lanes[l].ct < lanes[l].cb;
             if (!any_open) break;
-            if (sf.seg < 0) {        // decoration sprite: defer with the windows open right now
+            if (is_sprite_entry(sf)) {        // decoration sprite: defer with the windows open right now
                 Deferred d{k, std::vector<uint32_t>((size_t)SW, 0u)};
                 bool any = false;
                 for (int l = 0; l < SW; l++) {
@@ -340,8 +338,9 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
             const SectorRec &SF = sc.sectors[S.front];
             const int32_t fcl = SF.ceil, ffl = SF.floor;
             const bool two = S.flags & kSegTwoSided;
-            const bool ceil_vis = ((int64_t)fcl << 16) > fc.pose.z || SF.ceil_flat == kFlatSky;
-            const bool floor_vis = ((int64_t)ffl << 16) < fc.pose.z || SF.floor_flat == kFlatSky;
+            const bool ceil_vis = plane_visible(true, fcl, SF.ceil_flat == kFlatSky, fc.pose.z);
+            const bool floor_vis = plane_visible(false, ffl, SF.floor_flat == kFlatSky, fc.pose.z);
+            const bool has_a = wall_piece(true, two, fcl, ffl, S.otop, S.obot), has_b = wall_piece(false, two, fcl, ffl, S.otop, S.obot);
             Deferred dfr{k, std::vector<uint32_t>((size_t)SW, 0u)};
             bool any_deferred = false;
             // lock-step extents of the five draws (ceiling, A, B, floor) over the strip, for statistics
@@ -354,33 +353,23 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
                 ColumnEval ce;
                 if (!column_eval(sf, vw, x, ce)) continue;
                 if (st) st->evals++;
-                int ct = ln.ct, cb = ln.cb;
-                int row = light_row(S.light, ce.z8);
-                int32_t ucol = S.uoff + (int32_t)(((uint64_t)ce.s24 * (uint32_t)S.len_q12) >> 36);
-                int yfc = yrow(fcl, ce.scale, fc.pose.z, H), yff = yrow(ffl, ce.scale, fc.pose.z, H);
-                int y1 = clampv(yfc, ct, cb), y2, y3, y4;
-                if (!two) { y2 = clampv(yff, y1, cb); y3 = y2; y4 = y2; }
-                else {
-                    int yot = yrow(S.otop, ce.scale, fc.pose.z, H), yob = yrow(S.obot, ce.scale, fc.pose.z, H);
-                    y2 = clampv(yot, y1, cb); y3 = clampv(yob, y2, cb); y4 = clampv(yff, y3, cb);
-                }
+                const int ct = ln.ct, cb = ln.cb;
+                const int row = light_row(S.light, ce.z8);
+                const int32_t ucol = wall_column(S.uoff, S.len_q12, ce.s24);
+                const WallRows r = wall_rows(fcl, ffl, two, S.otop, S.obot, ce.scale, fc.pose.z, H, ct, cb);
                 if (st) {
                     auto acc = [&](int d, int a, int b) { if (a < b) { if (a < lo[d]) lo[d] = a; if (b > hi[d]) hi[d] = b; st->pixels += b - a; } };
-                    acc(0, ct, y1);
-                    if (!two || S.otop < fcl) acc(1, y1, y2);
-                    if (two && S.obot > ffl) acc(2, y3, y4);
-                    acc(3, y4, cb);
+                    acc(0, ct, r.y1);
+                    if (has_a) acc(1, r.y1, r.y2);
+                    if (has_b) acc(2, r.y3, r.y4);
+                    acc(3, r.y4, cb);
                 }
-                draw_plane(x, ln, ct, y1, fcl, SF.ceil_flat, SF.light, ceil_vis);
-                if (!two) draw_wall(x, y1, y2, S.texA, S.tA, S.hA, ucol, ce.iscale, row);
-                else {
-                    if (S.otop < fcl) draw_wall(x, y1, y2, S.texA, S.tA, S.hA, ucol, ce.iscale, row);
-                    if (S.obot > ffl) draw_wall(x, y3, y4, S.texB, S.tB, S.hB, ucol, ce.iscale, row);
-                }
-                draw_plane(x, ln, y4, cb, ffl, SF.floor_flat, SF.light, floor_vis);
-                if (!two || y2 >= y3) { ln.ct = H; ln.cb = 0; }
-                else { ln.ct = y2; ln.cb = y3; }
-                if (two && S.mid >= 0 && y2 < y3) { dfr.win[(size_t)l] = (uint32_t)y2 | ((uint32_t)y3 << 16); any_deferred = true; }
+                draw_plane(x, ln, ct, r.y1, fcl, SF.ceil_flat, SF.light, ceil_vis);
+                if (has_a) draw_wall(x, r.y1, r.y2, S.texA, S.tA, S.hA, ucol, ce.iscale, row);
+                if (has_b) draw_wall(x, r.y3, r.y4, S.texB, S.tB, S.hB, ucol, ce.iscale, row);
+                draw_plane(x, ln, r.y4, cb, ffl, SF.floor_flat, SF.light, floor_vis);
+                wall_window(two, r, H, ln.ct, ln.cb);
+                if (two && S.mid >= 0 && r.y2 < r.y3) { dfr.win[(size_t)l] = (uint32_t)r.y2 | ((uint32_t)r.y3 << 16); any_deferred = true; }
             }
             if (any_deferred && deferred.size() < (size_t)masked_cap) deferred.push_back(dfr);
             if (st) for (int d = 0; d < 4; d++) if (hi[d] > lo[d]) st->iters += hi[d] - lo[d];
@@ -395,21 +384,17 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
                 int ya = (int)(packed & 0xFFFFu), yb = (int)(packed >> 16), x = x0 + l;
                 if (!(ya < yb)) continue;
                 int32_t tex, tA, hA, ucol, iscale, row;
-                if (sf.seg < 0) {
-                    const SpriteRec &P = sc.sprites[-1 - sf.seg];
+                if (is_sprite_entry(sf)) {
+                    SpriteFrame sp;
+                    const SpriteRec &P = sc.sprites[entry_sprite(sf, sp)];
                     if (P.tex < 0 || P.tex >= sc.ntex) continue;
                     const int32_t sw = (int32_t)sc.tex[P.tex].w, sh = (int32_t)sc.tex[P.tex].h;
-                    SpriteFrame sp;
-                    sp.cx = sf.Nc; sp.cz = sf.Nx;
-                    int64_t scale = ((int64_t)vw.FY2 << 25) / sp.cz;
-                    const int64_t cap = (int64_t)vw.FY2 << 17;
-                    if (scale > cap) scale = cap;
-                    iscale = (int32_t)clampv<int64_t>(((int64_t)1 << 38) / scale, 1, 1 << 23);
-                    int64_t z8 = ((int64_t)iscale * vw.FY2) >> 18;
-                    row = light_row_sprite(P.light, z8 > 65535 ? 65535 : (int32_t)z8);
+                    const int64_t scale = sprite_scale(vw, sp.cz);
+                    int32_t z8;
+                    scale_depth(vw, scale, iscale, z8);
+                    row = light_row_sprite(P.light, z8);
                     tex = P.tex; tA = 0; hA = P.low + sh;
-                    ya = std::max(ya, yrow(P.low + sh, (int32_t)scale, fc.pose.z, H));
-                    yb = std::min(yb, yrow(P.low, (int32_t)scale, fc.pose.z, H));
+                    clip_rows(P.low + sh, P.low, (int32_t)scale, fc.pose.z, H, ya, yb);
                     ucol = sprite_column(sp, vw, x, sw);
                 } else {
                     const SegRec &S = sc.segs[sf.seg];
@@ -418,9 +403,8 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
                     ColumnEval ce;
                     if (!column_eval(sf, vw, x, ce)) continue;
                     tex = M.tex; tA = M.t_high; hA = M.high;
-                    ya = std::max(ya, yrow(M.high, ce.scale, fc.pose.z, H));
-                    yb = std::min(yb, yrow(M.low, ce.scale, fc.pose.z, H));
-                    ucol = S.uoff + (int32_t)(((uint64_t)ce.s24 * (uint32_t)S.len_q12) >> 36);
+                    clip_rows(M.high, M.low, ce.scale, fc.pose.z, H, ya, yb);
+                    ucol = wall_column(S.uoff, S.len_q12, ce.s24);
                     iscale = ce.iscale;
                     row = light_row(S.light, ce.z8);
                 }
