@@ -753,7 +753,7 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
 }
 
 template <bool kRgba, int kW, bool kMasked>
-__global__ void __launch_bounds__(32, 24)
+__global__ void __launch_bounds__(32, 16)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb) {
@@ -936,7 +936,7 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
     }
     // background (b2d_walk_device: the walk of the NEXT batch, meant to run under another batch's raster): a persistent grid
     // of one CTA per SM.  It takes n/SMs frame latencies instead of one, but holds 1/8 of the register file instead of
-    // 7/8, so the raster keeps 22 of its 24 warps per SM while the walk hides behind it.
+    // 7/8, so the raster keeps 18 of its 21 warps per SM while the walk hides behind it.
     const int sms = device_sms();
     const int blocks = (background && n > sms) ? sms : n, warps = 4;
     b2d_walk_kernel<<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride);
@@ -948,10 +948,13 @@ cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameCons
                           uint32_t *d_rgba, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
-    // Launch shape: ONE warp per CTA and 80 registers/thread, i.e. 24 CTAs = 24 warps resident per SM.  On sm_90a the
-    // kernel spills at a 64-register cap (32 warps/SM); the 80-register cap keeps most of it in registers and measured
-    // 14 % more frames/s on an H100 SXM (bench.py c2).  Strips differ a lot in cost; with several warps per CTA the finished warps' slots
-    // stay empty until the slowest warp of the CTA is done.
+    // Launch shape: ONE warp per CTA.  __launch_bounds__(32, 16) leaves the register allocation unconstrained (the cap is
+    // 128): the 1080p and 4K index-only kernels take 95 registers, i.e. 21 CTAs = 21 warps resident per SM, their masked
+    // variants 106 (18 warps).
+    // On the H100 more resident warps make the raster slower, not faster: capped at 80 registers (25 warps) it takes 5 %
+    // longer per bench.py c2 step, and a build that fits 64 registers without spilling (32 warps) 17 % longer (DESIGN.md
+    // §6).  Strips differ a lot in cost; with several warps per CTA the finished warps' slots stay empty until the
+    // slowest warp of the CTA is done.
     // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
     const int nblocks = (int)((long long)n * strips);     // one warp per (frame, strip)
     const bool masked = (sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list;
