@@ -361,8 +361,17 @@ struct RasterCtx {
 template <bool kRgba>
 __device__ __forceinline__ void put_px(const RasterCtx &c, uint8_t *p8, uint32_t *p32, bool on, uint32_t v) {
     if (on) {
-        *p8 = (uint8_t)v;
-        if (kRgba) *p32 = lds_u32(c.pal_s + 4u * v);
+        // Index-only kernels store with st.global.cs (streaming: evict-first in L1 and L2).  The raster writes every
+        // index byte once and never reads it back, while every warp re-reads the pre-lit texel and flat planes; the frames
+        // in flight are larger than the L2, and default stores push those planes out.  With RGBA output, whose lines
+        // are four times as many, evict-first index lines leave L2 before they are complete and the kernel is slower,
+        // so those kernels keep default stores (DESIGN.md §6).
+        if (kRgba) {
+            *p8 = (uint8_t)v;
+            *p32 = lds_u32(c.pal_s + 4u * v);
+        } else {
+            __stcs(p8, (uint8_t)v);
+        }
     }
 }
 
@@ -936,7 +945,7 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
     }
     // background (b2d_walk_device: the walk of the NEXT batch, meant to run under another batch's raster): a persistent grid
     // of one CTA per SM.  It takes n/SMs frame latencies instead of one, but holds 1/8 of the register file instead of
-    // 7/8, so the raster keeps 18 of its 21 warps per SM while the walk hides behind it.
+    // 7/8, so the raster keeps 16 of its 19 warps per SM while the walk hides behind it.
     const int sms = device_sms();
     const int blocks = (background && n > sms) ? sms : n, warps = 4;
     b2d_walk_kernel<<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride);
@@ -949,7 +958,7 @@ cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameCons
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
     // Launch shape: ONE warp per CTA.  __launch_bounds__(32, 16) leaves the register allocation unconstrained (the cap is
-    // 128): the 1080p and 4K index-only kernels take 95 registers, i.e. 21 CTAs = 21 warps resident per SM, their masked
+    // 128): the 1080p and 4K index-only kernels take 100 registers, i.e. 19 CTAs = 19 warps resident per SM, their masked
     // variants 106 (18 warps).
     // On the H100 more resident warps make the raster slower, not faster: capped at 80 registers (25 warps) it takes 5 %
     // longer per bench.py c2 step, and a build that fits 64 registers without spilling (32 warps) 17 % longer (DESIGN.md
