@@ -541,7 +541,8 @@ def compile_scene(archive: W.Archive, tex: W.TextureDirectory, level_index: int,
         if j - k > 255:
             raise W.WadError("more than 255 decoration things in one subsector")
         cnt = j - k
-        ssectors[ssid, 3] = k | (cnt << 24)
+        word = k | (cnt << 24)                            # a count of 128..255 sets the sign bit of the int32 record
+        ssectors[ssid, 3] = word - (1 << 32) if word >= 1 << 31 else word
         k = j
 
     # --- nodes -----------------------------------------------------------------------------------

@@ -644,16 +644,23 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
     d.nsprites = (int32_t)h[H_NSPRITES];
     d.masked_list = nullptr; d.masked_counter = nullptr; d.masked_chunks = 0; d.masked_cap = 0;
     if (d.nmids > 0 || d.nsprites > 0) {
-        // arena of deferred masked entries: chunks of kMaskedChunk entries handed out on demand.  Sized for two chunks per
-        // (frame, 32-column strip) of a full batch -- frames defer a handful of entries per strip -- and never more than the
-        // worst case (every strip at its cap).  1000 x 1080p: 63 MB instead of the 1 GB a fixed per-strip list takes.
+        // arena of deferred masked entries: chunks of kMaskedChunk entries handed out on demand.  Sized for the worst case
+        // -- every (frame, 32-column strip) of a full batch at its cap -- whenever that takes at most kMaskedArenaBudget, so
+        // that no valid batch can run out of it: a crowded subsector puts dozens of sprites into every strip of a 1080p
+        // frame.  Past the budget (1080p batches of more than ~1000 frames, 4K of more than ~500, with a cap of 128) two
+        // chunks per strip on average, at least 4096: frames usually defer a handful of entries per strip, and a batch
+        // that needs more reports kStatusMaskedFull instead of drawing wrong pixels.
+        constexpr size_t kMaskedArenaBudget = (size_t)1 << 30;
         const size_t strips = (size_t)(view->width + 31) / 32;
         d.masked_cap = strip_masked_cap(d.nmids, d.nsprites);
         const size_t per_strip = ((size_t)d.masked_cap + kMaskedChunk - 1) / kMaskedChunk;
-        size_t chunks = strips * (size_t)max_batch * (per_strip < 2 ? per_strip : 2);
-        if (chunks < 4096) chunks = 4096;
         const size_t worst = strips * (size_t)max_batch * per_strip;
-        if (chunks > worst) chunks = worst;
+        size_t chunks = worst;
+        if (sizeof(uint32_t) * 33 * kMaskedChunk * worst > kMaskedArenaBudget) {
+            chunks = strips * (size_t)max_batch * (per_strip < 2 ? per_strip : 2);
+            if (chunks < 4096) chunks = 4096;
+            if (chunks > worst) chunks = worst;
+        }
         if (const char *env = getenv("B2D_MASKED_CHUNKS")) chunks = (size_t)strtoull(env, nullptr, 0);   // tests: force exhaustion
         if (chunks < 1) chunks = 1;
         d.masked_chunks = (uint32_t)chunks;

@@ -112,6 +112,11 @@ def test_gpu_rgba_and_palette_kernel(b2d, product_scene):
     idx, rgba = r.render(poses, rgba=True)
     ofb, orgba = render.render(product_scene.blob, render.make_view(640, 400), poses, rgba=True)
     assert np.array_equal(idx, ofb) and np.array_equal(rgba, orgba)
+    # 1080p RGBA on a level without masked content: the unmasked variant of the kernel compiled for W = 1920 with RGBA
+    idx2, rgba2 = b2d.Renderer(product_scene, b2d.make_view(1920, 1080), max_batch=4).render(poses[:3], rgba=True)
+    oi2, orgba2 = render.render(product_scene.blob, render.make_view(1920, 1080), poses[:3], rgba=True, threads=8)
+    _assert_same(oi2, idx2, "1080p RGBA (index)")
+    assert np.array_equal(rgba2, orgba2)
     # stand-alone palette kernel, incl. a pixel count that is not a multiple of 16
     for npx in (640 * 400 * 6, 1003):
         di = torch.from_numpy(ofb.reshape(-1)[:npx].copy()).cuda()
@@ -280,6 +285,9 @@ def test_gpu_masked_middle_textures(b2d):
         ofb, orgba = render.render(sc.blob, render.make_view(w, h), p, rgba=True, threads=8)
         _assert_same(ofb, idx, "masked %dx%d" % (w, h))
         assert np.array_equal(rgba, orgba)
+    # 4K index frames only: the masked variant of the kernel compiled for W = 3840 (RGBA at 4K takes the generic one)
+    gfb = b2d.Renderer(sc, b2d.make_view(3840, 2160), max_batch=2).render(poses[:2])
+    _assert_same(render.render(sc.blob, render.make_view(3840, 2160), poses[:2], threads=8), gfb, "masked 4K")
 
 
 def test_gpu_full_benchmark_workload_matches_oracle(b2d, product_scene):
@@ -315,6 +323,8 @@ def test_gpu_decoration_sprites(b2d, hostcheck):
         ofb, orgba = render.render(sc.blob, render.make_view(w, h), p, rgba=True, threads=8)
         _assert_same(ofb, idx, "sprites %dx%d" % (w, h))
         assert np.array_equal(rgba, orgba)
+    gfb = b2d.Renderer(sc, b2d.make_view(3840, 2160), max_batch=2).render(poses[:2])     # masked W = 3840 kernel, index only
+    _assert_same(render.render(sc.blob, render.make_view(3840, 2160), poses[:2], threads=8), gfb, "sprites 4K")
     view = b2d.make_view(320, 200)
     r = b2d.Renderer(sc, view, max_batch=48)
     dp = torch.from_numpy(poses.view(np.int32).reshape(-1, 4).copy()).cuda()
