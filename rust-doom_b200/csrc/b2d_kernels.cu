@@ -761,14 +761,17 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
     }
 }
 
+// Warps per raster CTA: the four 32-column strips of one 128-column line group (for widths that are a multiple of 128).
+constexpr int kRasterWarps = 4;
+
 template <bool kRgba, int kW, bool kMasked>
-__global__ void __launch_bounds__(32, 16)
+__global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb) {
     __shared__ uint32_t s_pal[kRgba ? 256 : 1];
-    __shared__ uint2 s_rowz[32];
-    __shared__ uint32_t s_chunks[kMasked ? kMaskedCapMax / kMaskedChunk : 1];
+    __shared__ uint2 s_rowz[kRasterWarps][32];
+    __shared__ uint32_t s_chunks[kRasterWarps][kMasked ? kMaskedCapMax / kMaskedChunk : 1];
     if (kRgba) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
         for (int i = threadIdx.x; i < 256; i += blockDim.x) s_pal[i] = sc.palette[i];
         __syncthreads();
@@ -786,7 +789,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     RasterCtx c;
     c.sc = &sc;
     c.pal_s = (uint32_t)__cvta_generic_to_shared(s_pal);
-    c.rowz = s_rowz;
+    c.rowz = s_rowz[threadIdx.x >> 5];
     c.dir = plane_dir(fc, vw, inside ? x : 0, sc.invF);
     c.fb = index_fb + (size_t)frame * W * H + (inside ? x : 0);
     c.rgba = kRgba ? rgba_fb + (size_t)frame * W * H + (inside ? x : 0) : nullptr;
@@ -795,7 +798,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     if (sc.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), sc.tex[sc.sky_tex].w);
 
     int ct = 0, cb = inside ? H : 0;              // open window [ct, cb) of this lane's column
-    uint32_t *chunks = s_chunks;
+    uint32_t *chunks = s_chunks[threadIdx.x >> 5];
     asm("" : "+l"(chunks));        // a run-time value: propagated into masked_pass as a constant, it makes that pass spill more
     const bool defer = kMasked && sc.masked_list != nullptr;
     int mcount = 0;
@@ -957,19 +960,19 @@ cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameCons
                           uint32_t *d_rgba, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
-    // Launch shape: ONE warp per CTA.  __launch_bounds__(32, 16) leaves the register allocation unconstrained (the cap is
-    // 128): the 1080p and 4K index-only kernels take 100 registers, i.e. 19 CTAs = 19 warps resident per SM, their masked
-    // variants 106 (18 warps).
-    // On the H100 more resident warps make the raster slower, not faster: capped at 80 registers (25 warps) it takes 5 %
-    // longer per bench.py c2 step, and a build that fits 64 registers without spilling (32 warps) 17 % longer (DESIGN.md
-    // §6).  Strips differ a lot in cost; with several warps per CTA the finished warps' slots stay empty until the
-    // slowest warp of the CTA is done.
+    // Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 4 warps per CTA, so a CTA holds the four strips of
+    // a 128-column line group (at 1920 and 3840 columns; a CTA may straddle two frames at other widths).  The four warps
+    // that write the sectors of the same 128-byte frame lines then start together on one SM and finish those lines
+    // close together in time, so fewer partly written lines sit in L2.  That is worth 6 % of the bench.py c2 step over
+    // one-warp CTAs; the slots of a CTA's finished warps idle until its slowest strip is done, and that costs less.
+    // The registers are left to the compiler (cap 128): 86 for the 1080p and 4K index-only kernels, i.e. 5 CTAs = 20
+    // warps per SM (DESIGN.md §6).
     // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
-    const int nblocks = (int)((long long)n * strips);     // one warp per (frame, strip)
+    const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
     const bool masked = (sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list;
 #define B2D_RASTER_GO(RGBA, KW) do { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true><<<nblocks, 32, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
-    else b2d_raster_kernel<RGBA, KW, false><<<nblocks, 32, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
+    if (masked) b2d_raster_kernel<RGBA, KW, true><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
+    else b2d_raster_kernel<RGBA, KW, false><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
     } while (0)
     if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
     else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
