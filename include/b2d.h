@@ -203,12 +203,39 @@ int b2d_renderer_status(b2d_renderer *r, int32_t *bits_out);
  * (R in the low byte).  n may exceed max_batch; it is processed in batches. */
 int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_fb, uint32_t *rgba_fb);
 
-/* Per-pose level time (SURVEY 8-f2: poses (x, y, z, yaw, t)): pose i is rendered at level time tics[i] (HOST array).  A batch
- * shares its scene tables, so consecutive poses are launched together as long as their tables are byte-identical
- * (equal tics, or tics that change nothing: inside one 8-tic animation frame of a level without light effects or
- * scrolling walls) and the tables are re-uploaded in stream order where they change; a timeline sorted by time costs
- * one launch per table change, an unsorted one a launch per pose.  Leaves the renderer at the last pose's time.
- * tics == NULL in b2d_render_timed is b2d_render. */
+/* Per-frame state: every pose carries its own level time and state of the moving sectors (a demo replay, a recorded
+ * session where a door opens while the camera moves, a fly-through with the clock running).  Frame i is byte-identical to
+ * what b2d_render_device gives after b2d_renderer_set_time(states[i].tics) and b2d_renderer_set_sector_moves(
+ * moves + states[i].first_move, states[i].n_moves).  `states` and `moves` are HOST arrays; the renderer's own per-batch
+ * time and moves are neither read nor changed.  A batch costs one walk, one raster and one launch that expands the
+ * batch's distinct states on the device into an arena of up to max_batch table sets per worklist slot (allocated by the
+ * first such call; frames with equal states share a set wherever they are in the batch; DESIGN.md §3); the host uploads a
+ * compact state per distinct state (a few hundred bytes) instead of the tables.  A scene without time-dependent content
+ * or dynamic sectors renders every batch as b2d_render_device does (two launches).  Moves of undeclared sectors or outside
+ * their range, move ranges past n_moves and a NULL `states` are B2D_ERR_INVALID_ARG, detected before anything is enqueued.
+ *
+ * b2d_render_states: host poses and frames like b2d_render; b2d_render_device_states: like b2d_render_device, n may exceed
+ * max_batch (split into batches).  b2d_walk_device_states: like b2d_walk_device (1..max_batch poses); the ticket is
+ * rastered by b2d_raster_device, and its table sets live in the ticket's worklist slot until then.  The device-resident
+ * calls do not synchronise the device, but before a batch's compact states are written into the worklist slot's pinned
+ * staging, the host waits for the copy that read that staging two batches earlier (normally finished long before); the
+ * first call of a renderer also waits for its one-time upload of the rest-state sections. */
+typedef struct b2d_frame_state {
+    uint32_t tics;                    /* level time */
+    uint32_t first_move, n_moves;     /* moves[first_move .. first_move + n_moves) of the call's list; n_moves = 0: all at rest */
+} b2d_frame_state;
+int b2d_render_states(b2d_renderer *r, const b2d_pose *poses, const b2d_frame_state *states, size_t n,
+                      const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb);
+int b2d_render_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
+                             const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb, uint32_t *d_rgba_fb,
+                             void *cuda_stream);
+int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
+                           const b2d_sector_move *moves, size_t n_moves, void *cuda_stream, int64_t *ticket_out);
+
+/* Per-pose level time (SURVEY 8-f2: poses (x, y, z, yaw, t)): pose i is rendered at level time tics[i] (HOST array) with
+ * the renderer's current sector moves -- b2d_render_states / b2d_render_device_states with those states, so a batch costs
+ * the same three launches whatever the timeline (two on a level without time-dependent content).  Leaves the renderer at
+ * the last pose's time (one stream-ordered table upload at the end).  tics == NULL in b2d_render_timed is b2d_render. */
 int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tics, size_t n, uint8_t *index_fb, uint32_t *rgba_fb);
 int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *tics, size_t n, uint8_t *d_index_fb,
                             uint32_t *d_rgba_fb, void *cuda_stream);
@@ -295,6 +322,10 @@ int b2d_device_download(int device, void *host_dst, const void *d_src, size_t by
 /* Introspection for tests/profiling: copies the BSP-walk worklist of the LAST b2d_render_device
  * batch to the host.  counts_out[n], and for frame i seg ids seg_ids_out[i*stride .. +counts[i]). */
 int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *seg_ids_out, size_t stride);
+
+/* Introspection for tests: the table-set slot of frames 0..n-1 of the LAST walked batch, which must have been walked with
+ * per-frame states (frames with equal compact states share a slot). */
+int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out);
 
 /* Per-kernel device timing for the roofline report: while enabled, every batch records CUDA events
  * around the walk and raster launches on the launching stream.  b2d_profile_read synchronises the

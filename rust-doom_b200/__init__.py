@@ -128,6 +128,23 @@ def _moves_array(moves):
     return arr, len(m)
 
 
+def _frame_states(tics, moves_per_pose, n: int):
+    """(b2d_frame_state array, concatenated move list, its length) for n poses: pose i at level time tics[i] with the
+    sector moves moves_per_pose[i] (a list of (sector, floor_offset, ceil_offset); None = every pose at rest)."""
+    t = np.ascontiguousarray(tics, dtype=np.uint64).astype(np.uint32) if not np.isscalar(tics) else np.full(n, int(tics) & 0xFFFFFFFF, np.uint32)
+    assert len(t) == n, "one tic per pose"
+    per = [()] * n if moves_per_pose is None else list(moves_per_pose)
+    assert len(per) == n, "one move list per pose"
+    states = (_lib.FrameState * max(n, 1))()
+    flat = []
+    for i in range(n):
+        m = list(per[i])
+        states[i] = _lib.FrameState(int(t[i]), len(flat), len(m))
+        flat += m
+    arr, nm = _moves_array(flat)
+    return states, arr, nm
+
+
 class Scene:
     def __init__(self, archive: Optional[Archive], level_index: int = 0, _handle=None, dynamic=()):
         """`dynamic`: (sector, floor_min, floor_max, ceil_min, ceil_max) per sector that may move (b2d_scene_create_dynamic)"""
@@ -352,6 +369,33 @@ class Renderer:
         assert len(t) == n
         _check(_lib.load().b2d_render_device_timed(self._h, poses_ptr, t.ctypes.data, n, index_ptr, rgba_ptr or None, stream or None))
 
+    def render_states(self, poses: np.ndarray, tics, moves_per_pose=None, rgba: bool = False):
+        """b2d_render_states: pose i at level time tics[i] with the sector moves moves_per_pose[i] (list of (sector,
+        floor_offset, ceil_offset); None = at rest) -- a per-frame state, without touching the renderer's own time and moves."""
+        poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
+        n = len(poses)
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        out_index = np.empty((n, self.height, self.width), dtype=np.uint8)
+        out_rgba = np.empty((n, self.height, self.width), dtype=np.uint32) if rgba else None
+        _check(_lib.load().b2d_render_states(self._h, poses.ctypes.data, states, n, arr, nm, out_index.ctypes.data,
+                                             out_rgba.ctypes.data if rgba else None))
+        return (out_index, out_rgba) if rgba else out_index
+
+    def render_device_states(self, poses_ptr: int, tics, n: int, index_ptr: int, rgba_ptr: int = 0, moves_per_pose=None,
+                             stream: int = 0):
+        """b2d_render_device_states: device poses / frames, per-frame states as in render_states; n may exceed max_batch."""
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        _check(_lib.load().b2d_render_device_states(self._h, poses_ptr, states, n, arr, nm, index_ptr, rgba_ptr or None,
+                                                    stream or None))
+
+    def walk_device_states(self, poses_ptr: int, tics, n: int, moves_per_pose=None, stream: int = 0) -> int:
+        """b2d_walk_device_states: the walk of a batch (1..max_batch) with per-frame states; returns the ticket for
+        raster_device."""
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        t = ctypes.c_int64(-1)
+        _check(_lib.load().b2d_walk_device_states(self._h, poses_ptr, states, n, arr, nm, stream or None, ctypes.byref(t)))
+        return int(t.value)
+
     def render_ptr(self, poses_ptr: int, n: int, index_ptr: int, rgba_ptr: int = 0):
         """b2d_render on raw host pointers (e.g. pinned torch tensors)."""
         _check(_lib.load().b2d_render(self._h, poses_ptr, n, index_ptr, rgba_ptr or None))
@@ -377,6 +421,12 @@ class Renderer:
         ids = np.full((n, self.worklist_stride), -1, dtype=np.int32)
         _check(_lib.load().b2d_debug_worklist(self._h, n, counts.ctypes.data, ids.ctypes.data, ids.shape[1]))
         return counts, ids
+
+    def state_slots(self, n: int) -> np.ndarray:
+        """b2d_debug_state_slots: table-set slot of each of the first n frames of the last batch walked with per-frame states."""
+        out = np.zeros(n, dtype=np.uint32)
+        _check(_lib.load().b2d_debug_state_slots(self._h, n, out.ctypes.data))
+        return out
 
     def profile(self, enable: bool):
         _check(_lib.load().b2d_profile_enable(self._h, 1 if enable else 0))

@@ -35,6 +35,11 @@ class SectorMove(ctypes.Structure):
     _fields_ = [("sector", ctypes.c_int32), ("floor_offset", ctypes.c_int32), ("ceil_offset", ctypes.c_int32)]
 
 
+class FrameState(ctypes.Structure):
+    """b2d_frame_state: level time + moves[first_move .. first_move + n_moves) of the call's move list"""
+    _fields_ = [("tics", ctypes.c_uint32), ("first_move", ctypes.c_uint32), ("n_moves", ctypes.c_uint32)]
+
+
 EXPORTS = [
     "b2d_last_error", "b2d_archive_open", "b2d_archive_open_memory", "b2d_archive_open_files", "b2d_archive_open_memory_files", "b2d_archive_num_levels",
     "b2d_archive_level_name", "b2d_archive_close", "b2d_wad_name", "b2d_scene_create", "b2d_scene_create_from_lumps", "b2d_scene_create_dynamic",
@@ -42,8 +47,9 @@ EXPORTS = [
     "b2d_scene_blob", "b2d_scene_sector_at", "b2d_scene_destroy", "b2d_view_init", "b2d_renderer_create",
     "b2d_renderer_destroy", "b2d_renderer_set_time", "b2d_renderer_set_time_async", "b2d_renderer_status", "b2d_render", "b2d_render_device",
     "b2d_render_timed", "b2d_render_device_timed", "b2d_walk_device",
+    "b2d_render_states", "b2d_render_device_states", "b2d_walk_device_states",
     "b2d_raster_device", "b2d_palette_lut_device",
-    "b2d_debug_worklist", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
+    "b2d_debug_worklist", "b2d_debug_state_slots", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
     "b2d_comm_unique_id", "b2d_comm_create", "b2d_comm_destroy", "b2d_comm_info", "b2d_render_sharded",
     "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_download",
 ]
@@ -141,8 +147,13 @@ def load() -> ctypes.CDLL:
     L.b2d_render_device.argtypes = [vp, vp, cs, vp, vp, vp]
     L.b2d_render_timed.argtypes = [vp, vp, vp, cs, vp, vp]
     L.b2d_render_device_timed.argtypes = [vp, vp, vp, cs, vp, vp, vp]
+    L.b2d_render_states.argtypes = [vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, vp, vp]
+    L.b2d_render_device_states.argtypes = [vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, vp, vp, vp]
+    L.b2d_walk_device_states.argtypes = [vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, vp,
+                                         ctypes.POINTER(ctypes.c_int64)]
     L.b2d_palette_lut_device.argtypes = [vp, vp, vp, cs, vp]
     L.b2d_debug_worklist.argtypes = [vp, cs, vp, vp, cs]
+    L.b2d_debug_state_slots.argtypes = [vp, cs, vp]
     L.b2d_profile_enable.argtypes = [vp, ci]
     L.b2d_profile_read.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
                                    ctypes.POINTER(ctypes.c_int64)]

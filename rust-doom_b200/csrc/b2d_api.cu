@@ -7,6 +7,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "b2d_internal.hpp"
@@ -168,6 +169,13 @@ void free_renderer(b2d_renderer *r) {
         if (r->h_timed[i]) cudaFreeHost(r->h_timed[i]);
         if (r->timed_copied[i]) cudaEventDestroy(r->timed_copied[i]);
     }
+    for (int i = 0; i < 2; i++) {
+        if (r->d_arena[i]) cudaFree(r->d_arena[i]);
+        if (r->d_states[i]) cudaFree(r->d_states[i]);
+        if (r->h_states[i]) cudaFreeHost(r->h_states[i]);
+        if (r->states_copied[i]) cudaEventDestroy(r->states_copied[i]);
+    }
+    if (r->d_pristine) cudaFree(r->d_pristine);
     if (r->d_lit) cudaFree(r->d_lit);
     if (r->d_walk_static) cudaFree(r->d_walk_static);
     free_aligned_4g(r);
@@ -175,12 +183,91 @@ void free_renderer(b2d_renderer *r) {
     delete r;
 }
 
+size_t state_table_bytes(const uint8_t *blob);
+
+// Per-frame states: the rest-state sections the state rule reads, uploaded once next to the blob (whose own sections
+// set_time / set_sector_moves overwrite), and the two worklist slots' arenas and staging.
+int ensure_states(b2d_renderer *r) {
+    if (r->d_pristine) return B2D_OK;
+    const uint8_t *blob = r->h_blob.data();
+    const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
+    const StateLayout &L = r->layout;
+    auto a256 = [](size_t v) { return (v + 255) & ~(size_t)255; };
+    struct Sec { const void *src; size_t bytes; size_t off; };
+    Sec secs[10] = {{blob + h[H_OFF_TEX], h[H_NTEX] * sizeof(TexRec), 0}, {blob + h[H_OFF_SECTORS], h[H_NSECTORS] * sizeof(SectorRec), 0},
+                    {blob + h[H_OFF_SEGS], h[H_NSEGS] * sizeof(SegRec), 0}, {blob + h[H_OFF_SPRITES], h[H_NSPRITES] * sizeof(SpriteRec), 0},
+                    {blob + h[H_OFF_MIDS], h[H_NMIDS] * sizeof(MidRec), 0}, {blob + h[H_OFF_ANIM], h[H_NANIM] * sizeof(int32_t), 0},
+                    {blob + h[H_OFF_FLAT_ANIM], h[H_NFLATS] * sizeof(FlatAnimRec), 0}, {blob + h[H_OFF_SEGDYN], h[H_NSEGS] * sizeof(SegDynRec), 0},
+                    {L.sector_slots.data(), L.sector_slots.size() * 4, 0}, {L.mid_seg.data(), L.mid_seg.size() * 4, 0}};
+    size_t total = 0;
+    for (Sec &q : secs) { q.off = total; total = a256(total + q.bytes); }
+    std::vector<uint8_t> img(total + 256, 0);
+    for (const Sec &q : secs) if (q.bytes) std::memcpy(img.data() + q.off, q.src, q.bytes);
+    const size_t words = L.words, mb = (size_t)r->max_batch;
+    StateTables &t = r->state_tables;
+    t.slot_bytes = (uint32_t)a256(state_table_bytes(blob));        // one table set: [tex | sectors | segs | sprites | mids]
+    for (int i = 0; i < 2; i++) {
+        if (!r->d_arena[i]) CU(cudaMalloc(&r->d_arena[i], mb * t.slot_bytes));
+        if (!r->d_states[i]) CU(cudaMalloc(&r->d_states[i], 4 * mb * (words + 1)));
+        if (!r->h_states[i]) CU(cudaMallocHost(&r->h_states[i], 4 * mb * (words + 1)));
+        if (!r->states_copied[i]) CU(cudaEventCreateWithFlags(&r->states_copied[i], cudaEventDisableTiming));
+    }
+    uint8_t *d = nullptr;
+    CU(cudaMalloc(&d, img.size()));
+    // A copy from pageable memory may return before its DMA has landed, and the expansion that first reads these sections
+    // runs on the caller's stream, which need not be ordered after the legacy default stream: wait for the copy here (once
+    // per renderer, like the uploads at creation).
+    cudaError_t e = cudaMemcpy(d, img.data(), img.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { cudaFree(d); return cuda_fail(e, "cudaMemcpy (rest-state sections)"); }
+    r->d_pristine = d;
+    StateSrc s = state_src(blob, L);
+    s.tex = reinterpret_cast<const TexRec *>(d + secs[0].off); s.sectors = reinterpret_cast<const SectorRec *>(d + secs[1].off);
+    s.segs = reinterpret_cast<const SegRec *>(d + secs[2].off); s.sprites = reinterpret_cast<const SpriteRec *>(d + secs[3].off);
+    s.mids = reinterpret_cast<const MidRec *>(d + secs[4].off); s.anim = reinterpret_cast<const int32_t *>(d + secs[5].off);
+    s.flat_anim = reinterpret_cast<const FlatAnimRec *>(d + secs[6].off); s.segdyn = reinterpret_cast<const SegDynRec *>(d + secs[7].off);
+    s.sector_slots = reinterpret_cast<const uint32_t *>(d + secs[8].off); s.mid_seg = reinterpret_cast<const int32_t *>(d + secs[9].off);
+    r->src = s;
+    t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
+    t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
+    t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
+    t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
+    return B2D_OK;
+}
+
+// the arena view of worklist slot `slot` (after ensure_states)
+StateTables slot_tables(const b2d_renderer *r, int slot) {
+    StateTables t = r->state_tables;
+    t.base = r->d_arena[slot];
+    t.frame_slot = r->d_states[slot] + (size_t)r->max_batch * r->layout.words;
+    return t;
+}
+
 // BSP walk of a batch into the next worklist slot, on `stream`.  The slot's previous raster (if any, on whatever
 // stream) is awaited through an event, so a caller may run walks and rasters on two streams and have the walk of
-// batch k+1 overlap the raster of batch k.
-int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background = false) {
+// batch k+1 overlap the raster of batch k.  `frame_states` (nullable): one compact state per frame; the batch's distinct
+// states are expanded into the slot's arena on `stream` first (frames with equal states share one table set).
+int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background = false,
+                   const uint32_t *frame_states = nullptr) {
     const int slot = (int)(r->next_ticket & 1);
     if (!r->slot_rastered[slot]) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
+    int nstates = 0;
+    if (frame_states) {
+        int rc = ensure_states(r);
+        if (rc != B2D_OK) return rc;
+        // distinct states -> slots 0, 1, ... in order of first appearance, anywhere in the batch
+        const size_t words = r->layout.words;
+        CU(cudaEventSynchronize(r->states_copied[slot]));      // the copy issued two batches ago has read the staging
+        uint32_t *hs = r->h_states[slot], *hslot = hs + (size_t)r->max_batch * words;
+        std::unordered_map<std::string, uint32_t> seen;
+        seen.reserve((size_t)n);
+        for (int f = 0; f < n; f++) {
+            const uint32_t *w = frame_states + (size_t)f * words;
+            auto it = seen.emplace(std::string(reinterpret_cast<const char *>(w), 4 * words), (uint32_t)nstates);
+            if (it.second) std::memcpy(hs + (size_t)nstates++ * words, w, 4 * words);
+            hslot[f] = it.first->second;
+        }
+    }
     if (!r->d_frames[slot]) {
         CU(cudaMalloc(&r->d_frames[slot], sizeof(FrameConst) * (size_t)r->max_batch));
         CU(cudaMalloc(&r->d_work[slot], sizeof(SegFrame) * (size_t)r->max_batch * (size_t)r->stride));
@@ -192,12 +279,24 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
         CU(cudaStreamWaitEvent(stream, r->raster_done[slot], 0));      // the raster that last read this slot
     }
     if (r->tables_pending) CU(cudaStreamWaitEvent(stream, r->tables_ready, 0));   // a table upload on another stream
+    const StateTables stt = frame_states ? slot_tables(r, slot) : StateTables{};
+    if (frame_states) {
+        const size_t words = r->layout.words;
+        uint32_t *hs = r->h_states[slot];
+        CU(cudaMemcpyAsync(r->d_states[slot], hs, 4 * words * (size_t)nstates, cudaMemcpyHostToDevice, stream));
+        CU(cudaMemcpyAsync(const_cast<uint32_t *>(stt.frame_slot), hs + (size_t)r->max_batch * words, 4 * (size_t)n,
+                           cudaMemcpyHostToDevice, stream));
+        CU(cudaEventRecord(r->states_copied[slot], stream));
+        CU(launch_state_tables(r->src, r->d_states[slot], (uint32_t)words, nstates, r->d_arena[slot], stt, stream));
+        r->launches += 1;
+    }
     cudaEvent_t ev[2] = {nullptr, nullptr};
     if (r->profiling) {
         for (auto &e : ev) CU(cudaEventCreate(&e));
         CU(cudaEventRecord(ev[0], stream));
     }
-    CU(launch_walk(r->ds, r->view, d_poses, n, r->d_frames[slot], r->d_work[slot], r->stride, stream, background));
+    CU(launch_walk(r->ds, r->view, d_poses, n, r->d_frames[slot], r->d_work[slot], r->stride, stream, background,
+                   frame_states ? &stt : nullptr));
     if (r->profiling) {
         CU(cudaEventRecord(ev[1], stream));
         for (auto e : ev) r->prof_events.push_back(e);
@@ -205,6 +304,7 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
     }
     CU(cudaEventRecord(r->walk_done[slot], stream));
     r->slot_n[slot] = n;
+    r->slot_states[slot] = frame_states != nullptr;
     r->slot_ticket[slot] = r->next_ticket;
     r->slot_rastered[slot] = false;
     r->last_slot = slot;
@@ -231,7 +331,9 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
         for (auto &e : ev) CU(cudaEventCreate(&e));
         CU(cudaEventRecord(ev[0], stream));
     }
-    CU(launch_raster(r->ds, r->view, r->d_frames[slot], r->d_work[slot], r->stride, r->slot_n[slot], d_index, d_rgba, stream));
+    const StateTables stt = r->slot_states[slot] ? slot_tables(r, slot) : StateTables{};
+    CU(launch_raster(r->ds, r->view, r->d_frames[slot], r->d_work[slot], r->stride, r->slot_n[slot], d_index, d_rgba, stream,
+                     r->slot_states[slot] ? &stt : nullptr));
     if (r->profiling) {
         CU(cudaEventRecord(ev[1], stream));
         for (auto e : ev) r->prof_events.push_back(e);
@@ -255,19 +357,21 @@ size_t state_table_bytes(const uint8_t *blob) {
            h[H_NSPRITES] * sizeof(SpriteRec) + h[H_NMIDS] * sizeof(MidRec);
 }
 
-void state_tables(const uint8_t *blob, uint32_t tics, const int32_t *floor_off, const int32_t *ceil_off, uint8_t *out) {
+void state_tables(const uint8_t *blob, uint32_t tics, const int32_t *floor_off, const int32_t *ceil_off, uint8_t *out,
+                  const StateLayout *layout = nullptr) {
     const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
     TexRec *tex = reinterpret_cast<TexRec *>(out);
     SectorRec *sectors = reinterpret_cast<SectorRec *>(tex + h[H_NTEX]);
     SegRec *segs = reinterpret_cast<SegRec *>(sectors + h[H_NSECTORS]);
     SpriteRec *sprites = reinterpret_cast<SpriteRec *>(segs + h[H_NSEGS]);
     MidRec *mids = reinterpret_cast<MidRec *>(sprites + h[H_NSPRITES]);
-    scene_at_time(blob, tics, tex, sectors, segs, sprites, mids, floor_off, ceil_off);
+    scene_at_time(blob, tics, tex, sectors, segs, sprites, mids, floor_off, ceil_off, layout);
 }
 
 void tables_at(const b2d_renderer *r, uint32_t tics, uint8_t *out) {
     const bool moved = !r->floor_off.empty();
-    state_tables(r->h_blob.data(), tics, moved ? r->floor_off.data() : nullptr, moved ? r->ceil_off.data() : nullptr, out);
+    state_tables(r->h_blob.data(), tics, moved ? r->floor_off.data() : nullptr, moved ? r->ceil_off.data() : nullptr, out,
+                 &r->layout);
 }
 
 int upload_tables(b2d_renderer *r, const uint8_t *tables, cudaStream_t stream) {
@@ -303,32 +407,50 @@ int upload_timed_tables(b2d_renderer *r, uint32_t tics, cudaStream_t stream) {
     return upload_tables(r, r->scratch_tables.data(), stream);
 }
 
-// Per-pose time: poses [i, n) with their tics; makes the tables of tics[i] current on `stream` (uploading only if they
-// differ from what is there) and returns in *end the end of the run of poses that can share this launch: consecutive
-// poses whose tables are byte-identical (equal tics, or different tics that change nothing -- e.g. inside one 8-tic
-// animation frame of a level without light effects or scrolling walls).
-int timed_run(b2d_renderer *r, const uint32_t *tics, size_t i, size_t n, size_t limit, cudaStream_t stream, size_t *end) {
-    if (r->h_blob.empty() || !tics) { *end = n < i + limit ? n : i + limit; return B2D_OK; }
-    r->scratch_tables.resize(r->timed_bytes);
-    tables_at(r, tics[i], r->scratch_tables.data());
-    if (r->cur_tables.size() != r->timed_bytes || std::memcmp(r->cur_tables.data(), r->scratch_tables.data(), r->timed_bytes) != 0) {
-        int rc = upload_tables(r, r->scratch_tables.data(), stream);
-        if (rc != B2D_OK) return rc;
+// The compact state of every frame of a b2d_render_states-style call into `out` (r->layout.words words per frame), checking
+// everything first: nothing is enqueued for a call with an invalid frame.  `out` stays empty for a scene without
+// time-dependent content or dynamic sectors: its frames all render with the per-batch tables.
+int build_states(const b2d_renderer *r, const b2d_frame_state *states, size_t n, const b2d_sector_move *moves, size_t n_moves,
+                 std::vector<uint32_t> &out) {
+    out.clear();
+    if (!states || (n_moves && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    for (size_t i = 0; i < n; i++)
+        if (states[i].first_move > n_moves || states[i].n_moves > n_moves - states[i].first_move)
+            return fail(B2D_ERR_INVALID_ARG, "a frame's move range runs past the end of the move list");
+    if (r->h_blob.empty()) {
+        for (size_t i = 0; i < n; i++)
+            if (states[i].n_moves) return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
+        return B2D_OK;
     }
-    r->tics = tics[i];
-    size_t j = i + 1;
-    uint32_t same = tics[i];
-    while (j < n && j < i + limit) {
-        if (tics[j] != same) {
-            tables_at(r, tics[j], r->scratch_tables.data());
-            if (std::memcmp(r->cur_tables.data(), r->scratch_tables.data(), r->timed_bytes) != 0) break;
-            same = tics[j];
-            r->tics = same;
+    const size_t words = r->layout.words;
+    out.resize(n * words);
+    std::vector<int32_t> fo, co;
+    for (size_t i = 0; i < n; i++) {
+        bool moved = false;
+        if (states[i].n_moves) {
+            if (const char *why = expand_moves(r->h_blob.data(), reinterpret_cast<const SectorMove *>(moves) + states[i].first_move,
+                                               states[i].n_moves, fo, co)) {
+                out.clear();
+                return fail(B2D_ERR_INVALID_ARG, why);
+            }
+            for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
         }
-        j++;
+        compact_state(r->h_blob.data(), r->layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
+                      out.data() + i * words);
     }
-    *end = j;
     return B2D_OK;
+}
+
+// b2d_render_timed: tics[i] with the renderer's current moves
+void timed_states(const b2d_renderer *r, const uint32_t *tics, size_t n, std::vector<uint32_t> &out) {
+    out.clear();
+    if (r->h_blob.empty()) return;
+    const size_t words = r->layout.words;
+    const bool moved = !r->floor_off.empty();
+    out.resize(n * words);
+    for (size_t i = 0; i < n; i++)
+        compact_state(r->h_blob.data(), r->layout, tics[i], moved ? r->floor_off.data() : nullptr, moved ? r->ceil_off.data() : nullptr,
+                      out.data() + i * words);
 }
 
 }  // namespace
@@ -342,9 +464,9 @@ int b2d::raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32
 
 // walk -> raster on the caller's stream
 int b2d::enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba,
-                        cudaStream_t stream) {
+                        cudaStream_t stream, const uint32_t *frame_states) {
     int64_t ticket = -1;
-    int rc = walk_into_slot(r, d_poses, n, stream, &ticket);
+    int rc = walk_into_slot(r, d_poses, n, stream, &ticket, false, frame_states);
     if (rc != B2D_OK) return rc;
     return raster_from_slot(r, ticket, d_index, d_rgba, stream);
 }
@@ -702,6 +824,12 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
     if (scene_is_timed(s->blob.data())) {
         r->h_blob = s->blob;
         r->timed_bytes = state_table_bytes(r->h_blob.data());
+        try {
+            r->layout = state_layout(r->h_blob.data());
+        } catch (const std::exception &ex) {
+            free_renderer(r);
+            return fail(B2D_ERR_INVALID_ARG, ex.what());
+        }
         for (int i = 0; i < 2; i++) {
             CUR(cudaMallocHost(&r->h_timed[i], r->timed_bytes ? r->timed_bytes : 1));
             CUR(cudaEventCreateWithFlags(&r->timed_copied[i], cudaEventDisableTiming));
@@ -794,23 +922,54 @@ int b2d_render_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, uint8_
                           static_cast<cudaStream_t>(cuda_stream));
 }
 
+// frames_states (nullable, r->layout.words words per frame): walk + raster of n device poses in batches of max_batch
+static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, size_t n, const uint32_t *frame_states, uint8_t *d_index_fb,
+                           uint32_t *d_rgba_fb, cudaStream_t st) {
+    const size_t npix = (size_t)r->view.W * r->view.H;
+    for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
+        const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
+        int rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, (int)cnt, d_index_fb + i * npix,
+                                d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st, frame_states ? frame_states + i * r->layout.words : nullptr);
+        if (rc != B2D_OK) return rc;
+    }
+    return B2D_OK;
+}
+
 int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *tics, size_t n, uint8_t *d_index_fb,
                             uint32_t *d_rgba_fb, void *cuda_stream) {
     if (!r || !d_poses || !d_index_fb || !tics) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    const size_t npix = (size_t)r->view.W * r->view.H;
-    size_t i = 0;
-    while (i < n) {
-        size_t j = i;
-        int rc = timed_run(r, tics, i, n, (size_t)r->max_batch, st, &j);
-        if (rc != B2D_OK) return rc;
-        rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, (int)(j - i), d_index_fb + i * npix,
-                            d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st);
-        if (rc != B2D_OK) return rc;
-        i = j;
-    }
-    return B2D_OK;
+    std::vector<uint32_t> fs;
+    int rc = guarded([&] { timed_states(r, tics, n, fs); return B2D_OK; });
+    if (rc != B2D_OK) return rc;
+    rc = enqueue_batches(r, d_poses, n, fs.empty() ? nullptr : fs.data(), d_index_fb, d_rgba_fb, st);
+    if (rc != B2D_OK) return rc;
+    return b2d_renderer_set_time_async(r, tics[n - 1], cuda_stream);       // the renderer is left at the last pose's time
+}
+
+int b2d_render_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
+                             const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb, uint32_t *d_rgba_fb,
+                             void *cuda_stream) {
+    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    std::vector<uint32_t> fs;
+    int rc = guarded([&] { return build_states(r, states, n, moves, n_moves, fs); });
+    if (rc != B2D_OK || n == 0) return rc;
+    CU(cudaSetDevice(r->device));
+    return enqueue_batches(r, d_poses, n, fs.empty() ? nullptr : fs.data(), d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
+                           const b2d_sector_move *moves, size_t n_moves, void *cuda_stream, int64_t *ticket_out) {
+    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
+    std::vector<uint32_t> fs;
+    int rc = guarded([&] { return build_states(r, states, n, moves, n_moves, fs); });
+    if (rc != B2D_OK) return rc;
+    CU(cudaSetDevice(r->device));
+    return walk_into_slot(r, reinterpret_cast<const Pose *>(d_poses), (int)n, static_cast<cudaStream_t>(cuda_stream), ticket_out, true,
+                          fs.empty() ? nullptr : fs.data());
 }
 
 int b2d_walk_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, void *cuda_stream, int64_t *ticket_out) {
@@ -826,12 +985,9 @@ int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint
     return raster_from_slot(r, ticket, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
-int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
-    return b2d_render_timed(r, poses, nullptr, n, index_fb, rgba_fb);
-}
-
-int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tics, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
-    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+// Host poses in, host frames out; frame_states as in enqueue_frames (for all n frames)
+static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const uint32_t *frame_states, uint8_t *index_fb,
+                       uint32_t *rgba_fb) {
     if (n == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
@@ -852,16 +1008,14 @@ int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tic
     size_t done = 0;
     int b = 0;
     while (done < n) {
-        size_t run_end = done;                                      // per-pose time: a batch ends where the tables change
-        int trc = timed_run(r, tics, done, n, (size_t)r->max_batch, r->render_stream, &run_end);
-        if (trc != B2D_OK) return trc;
-        const int cnt = (int)(run_end - done);
+        const int cnt = (int)(n - done < (size_t)r->max_batch ? n - done : (size_t)r->max_batch);
         const int buf = b & 1;
         if (b >= 2) CU(cudaEventSynchronize(r->copied[buf]));       // buffer + pose slot free again
         Pose *hp = r->h_poses + (size_t)buf * r->max_batch;
         std::memcpy(hp, poses + done, sizeof(Pose) * (size_t)cnt);
         CU(cudaMemcpyAsync(r->d_poses, hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, r->render_stream));
-        int rc = enqueue_frames(r, r->d_poses, cnt, r->d_index[buf], rgba_fb ? r->d_rgba[buf] : nullptr, r->render_stream);
+        int rc = enqueue_frames(r, r->d_poses, cnt, r->d_index[buf], rgba_fb ? r->d_rgba[buf] : nullptr, r->render_stream,
+                                frame_states ? frame_states + done * r->layout.words : nullptr);
         if (rc != B2D_OK) return rc;
         CU(cudaEventRecord(r->rendered[buf], r->render_stream));
         CU(cudaStreamWaitEvent(r->copy_stream[buf], r->rendered[buf], 0));
@@ -884,6 +1038,32 @@ int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tic
                                                             : "worklist overflow: frames incomplete")));
     }
     return B2D_OK;
+}
+
+int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    return render_host(r, poses, n, nullptr, index_fb, rgba_fb);
+}
+
+int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tics, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
+    if (!tics) return b2d_render(r, poses, n, index_fb, rgba_fb);
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return B2D_OK;
+    std::vector<uint32_t> fs;
+    int rc = guarded([&] { timed_states(r, tics, n, fs); return B2D_OK; });
+    if (rc != B2D_OK) return rc;
+    rc = render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
+    const int trc = b2d_renderer_set_time(r, tics[n - 1]);                // the renderer is left at the last pose's time
+    return rc != B2D_OK ? rc : trc;
+}
+
+int b2d_render_states(b2d_renderer *r, const b2d_pose *poses, const b2d_frame_state *states, size_t n,
+                      const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    std::vector<uint32_t> fs;
+    int rc = guarded([&] { return build_states(r, states, n, moves, n_moves, fs); });
+    if (rc != B2D_OK) return rc;
+    return render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
 }
 
 int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_rgba, size_t n_pixels, void *cuda_stream) {
@@ -935,6 +1115,17 @@ int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *
         if (c) CU(cudaMemcpy(work.data(), r->d_work[slot] + i * (size_t)r->stride, sizeof(SegFrame) * c, cudaMemcpyDeviceToHost));
         for (size_t k = 0; k < c && k < stride; k++) seg_ids_out[i * stride + k] = work[k].seg;
     }
+    return B2D_OK;
+}
+
+int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
+    if (!r || !slots_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    const int slot = r->last_slot;
+    if (!r->slot_states[slot] || n > (size_t)r->slot_n[slot])
+        return fail(B2D_ERR_INVALID_ARG, "the last walked batch has no per-frame states or fewer than n frames");
+    CU(cudaSetDevice(r->device));
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpy(slots_out, slot_tables(r, slot).frame_slot, 4 * n, cudaMemcpyDeviceToHost));
     return B2D_OK;
 }
 

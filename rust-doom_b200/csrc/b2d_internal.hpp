@@ -70,6 +70,18 @@ struct b2d_renderer {
     uint8_t *d_walk_static = nullptr;                     // node / subsector tables as the walk kernel's shared memory holds them
     std::vector<int32_t> floor_off, ceil_off;             // state of the moving sectors (one offset per sector; empty = at rest)
     std::vector<uint8_t> cur_tables, scratch_tables;      // host copies: tables of the last upload / of a candidate time
+    // per-frame states (b2d_render_states & co., DESIGN.md §3 "State arena"): the device copy of the rest-state sections
+    // the state rule reads, and per worklist slot an arena of up to max_batch expanded table sets, the batch's distinct
+    // compact states + per-frame slot indices on the device and their pinned staging.  Allocated by the first such call.
+    StateLayout layout;                                   // scenes with time-dependent content or dynamic sectors
+    uint8_t *d_pristine = nullptr;
+    StateSrc src{};                                       // device pointers into d_pristine
+    StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
+    uint8_t *d_arena[2] = {nullptr, nullptr};
+    uint32_t *d_states[2] = {nullptr, nullptr};           // max_batch compact states, then max_batch slot indices
+    uint32_t *h_states[2] = {nullptr, nullptr};           // pinned, same layout
+    cudaEvent_t states_copied[2] = {nullptr, nullptr};    // h_states[i] has been read by its copy
+    bool slot_states[2] = {false, false};                 // the batch in worklist slot i was walked with per-frame states
     cudaEvent_t masked_done = nullptr;                    // last raster that used the masked-entry arena
     uint32_t *d_masked_counter = nullptr;
     int64_t launches = 0;
@@ -83,8 +95,10 @@ struct b2d_renderer {
 namespace b2d {
 int fail(int code, const std::string &msg);            // sets the thread-local message, returns code
 int cuda_fail(cudaError_t e, const char *what);
-// BSP walk + raster of n device poses into d_index / d_rgba (nullable) on `stream`; not synchronised
-int enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);
+// BSP walk + raster of n device poses into d_index / d_rgba (nullable) on `stream`; not synchronised.  `frame_states`
+// (nullable): n compact states (r->layout.words words each), frame i rendered at its own state.
+int enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
+                   const uint32_t *frame_states = nullptr);
 // the two halves (b2d_walk_device / b2d_raster_device): a background walk into a worklist slot, the raster of a ticket
 int walk_frames(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background);
 int raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);

@@ -117,9 +117,16 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity) {     
 // ------------------------------------------------------------------------------------------------
 // Kernel 1: BSP walk -> worklist
 // ------------------------------------------------------------------------------------------------
+// Per-frame states: the frame's table of kind T in its arena slot (tb = slot base), else the scene's one table.
+template <bool kStates, typename T>
+__device__ __forceinline__ const T *state_table(const T *plain, const uint8_t *tb, uint32_t off) {
+    return kStates ? reinterpret_cast<const T *>(tb + off) : plain;
+}
+
+template <bool kStates>
 __global__ void __launch_bounds__(128, 7)     // 7 CTAs/SM (72 registers): 924 frames resident on an H100's 132 SMs
 b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const Pose *__restrict__ poses, int n,
-                FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride) {
+                FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride, const __grid_constant__ StateTables st) {
     // One CTA per frame.  The per-frame setup (steps 1-3) and the worklist records (step 5) are data-parallel and
     // use all 128 threads; the traversal itself (step 4) is sequential and runs in warp 0 with the lanes working
     // on the segs of a subsector / the words of the column mask.  The kernel is latency-bound (one frame = one
@@ -159,6 +166,12 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
     for (int frame = blockIdx.x; frame < n; frame += gridDim.x) {
     FrameConst fc;
     frame_setup(poses[frame], fc);
+    uint32_t slot = 0;                  // per-frame states: this frame's slot of the arena
+    const uint8_t *tb = nullptr;
+    if (kStates) {
+        slot = st.frame_slot[frame];
+        tb = st.base + (size_t)slot * st.slot_bytes;
+    }
 
     // 1. all vertices into view space (lane-parallel)
     for (int i = tid; i < sc.nverts; i += nthr) {
@@ -171,7 +184,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
 
     // 2. per-seg exact column interval + static/solid flags (lane-parallel, 64-bit setup)
     for (int i = tid; i < sc.nsegs; i += nthr) {
-        const SegRec &S = sc.segs[i];
+        const SegRec &S = state_table<kStates>(sc.segs, tb, st.off_segs)[i];
         uint32_t packed = 0;
         int32_t flags = S.flags;
         if (!(flags & kSegInvalid)) {
@@ -195,11 +208,11 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
         static_pending = false;
     }
     for (int i = tid; i < sc.nsprites; i += nthr) {          // decoration sprites: exact column interval
-        const SpriteRec &P = sc.sprites[i];
+        const SpriteRec &P = state_table<kStates>(sc.sprites, tb, st.off_sprites)[i];
         SpriteFrame sp;
         uint32_t packed = 0;
         sp.cz = 0;
-        if (P.tex >= 0 && P.tex < sc.ntex && sprite_setup(fc, vw, P.x, P.y, (int32_t)sc.tex[P.tex].w, sp))
+        if (P.tex >= 0 && P.tex < sc.ntex && sprite_setup(fc, vw, P.x, P.y, (int32_t)state_table<kStates>(sc.tex, tb, 0u)[P.tex].w, sp))
             packed = pack_range(sp.lo, sp.hi, kVisBit);
         sprr[i] = packed;
         sprz[i] = (int32_t)sp.cz;
@@ -312,14 +325,14 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
         SegFrame sf;
         if (si >= sc.nsegs) {
             const int pi = si - sc.nsegs;
-            const SpriteRec &P = sc.sprites[pi];
+            const SpriteRec &P = state_table<kStates>(sc.sprites, tb, st.off_sprites)[pi];
             SpriteFrame sp;
-            sprite_setup(fc, vw, P.x, P.y, (int32_t)sc.tex[P.tex].w, sp);
+            sprite_setup(fc, vw, P.x, P.y, (int32_t)state_table<kStates>(sc.tex, tb, 0u)[P.tex].w, sp);
             sprite_entry(pi, sp, sf);
             work[(size_t)frame * stride + k] = sf;
             continue;
         }
-        const SegRec &S = sc.segs[si];
+        const SegRec &S = state_table<kStates>(sc.segs, tb, st.off_segs)[si];
         seg_frame_setup(vw, tx[S.v1], tz[S.v1], tx[S.v2], tz[S.v2], sf, false);
         sf.seg = si;
         work[(size_t)frame * stride + k] = sf;
@@ -330,6 +343,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
         fc.status = status;
 #pragma unroll
         for (int i = 0; i < 6; i++) fc.pad[i] = 0;
+        if (kStates) fc.pad[0] = (int32_t)slot;      // the raster reads the frame's tables from the same slot
         frames[frame] = fc;
     }
     __syncthreads();                              // the next frame of this CTA reuses the shared-memory tables
@@ -646,8 +660,9 @@ __device__ __forceinline__ uint32_t *masked_push(const DeviceScene &sc, uint32_t
 // holds the worklist index and, per lane, the clip window [ya, yb) that was open behind the seg when the
 // front-to-back walk reached it (the per-column silhouette of everything nearer).  Texels whose opacity plane
 // is 0 leave the pixel as the solid pass drew it (static.frag:21-22).  Kept out of line so that the
-// register allocation of the solid pass is not affected.
-template <bool kRgba, int kW>
+// register allocation of the solid pass is not affected.  kStates only gives each raster variant its own copy (one caller
+// each, so that what the compiler propagates into it from its caller stays as it is).
+template <bool kRgba, int kW, bool kStates>
 __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, int32_t pose_z, uint8_t *fb,
                                          uint32_t *rgba, uint32_t pal_s, int x, int lane,
                                          const SegFrame *wl, const uint32_t *chunks, int count) {
@@ -764,11 +779,11 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
 // Warps per raster CTA: the four 32-column strips of one 128-column line group (for widths that are a multiple of 128).
 constexpr int kRasterWarps = 4;
 
-template <bool kRgba, int kW, bool kMasked>
+template <bool kRgba, int kW, bool kMasked, bool kStates>
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
-                  uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb) {
+                  uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st) {
     __shared__ uint32_t s_pal[kRgba ? 256 : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
     __shared__ uint32_t s_chunks[kRasterWarps][kMasked ? kMaskedCapMax / kMaskedChunk : 1];
@@ -786,8 +801,30 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     const bool inside = x < W;
 
     const FrameConst fc = frames[frame];
+    const DeviceScene *scp = &sc;
+    if constexpr (kStates) {
+        // per-frame states: this warp's copy of the scene description, its five state-dependent tables pointed into the
+        // frame's arena slot (the walk passed the slot on in FrameConst::pad[0]); every table read below goes through it
+        __shared__ DeviceScene s_sc[kRasterWarps];
+        DeviceScene *d = &s_sc[threadIdx.x >> 5];
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(&sc);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(d);
+        for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
+        __syncwarp();
+        if (lane == 0) {
+            const uint8_t *tb = st.base + (size_t)(uint32_t)fc.pad[0] * st.slot_bytes;
+            d->tex = reinterpret_cast<const TexRec *>(tb);
+            d->sectors = reinterpret_cast<const SectorRec *>(tb + st.off_sectors);
+            d->segs = reinterpret_cast<const SegRec *>(tb + st.off_segs);
+            d->sprites = reinterpret_cast<const SpriteRec *>(tb + st.off_sprites);
+            d->mids = reinterpret_cast<const MidRec *>(tb + st.off_mids);
+        }
+        __syncwarp();
+        scp = d;
+    }
+    const DeviceScene &ts = *scp;      // = sc without per-frame states
     RasterCtx c;
-    c.sc = &sc;
+    c.sc = &ts;
     c.pal_s = (uint32_t)__cvta_generic_to_shared(s_pal);
     c.rowz = s_rowz[threadIdx.x >> 5];
     c.dir = plane_dir(fc, vw, inside ? x : 0, sc.invF);
@@ -795,7 +832,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     c.rgba = kRgba ? rgba_fb + (size_t)frame * W * H + (inside ? x : 0) : nullptr;
     c.W = W; c.H = H; c.x = x; c.lane = lane;
     c.skycol = 0;
-    if (sc.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), sc.tex[sc.sky_tex].w);
+    if (sc.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), ts.tex[sc.sky_tex].w);
 
     int ct = 0, cb = inside ? H : 0;              // open window [ct, cb) of this lane's column
     uint32_t *chunks = s_chunks[threadIdx.x >> 5];
@@ -836,8 +873,8 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             bool ok = in && column_eval(sf, vw, x, ce);
             if (!__any_sync(kFull, ok)) continue;
 
-            const SegRec S = sc.segs[sf.seg];
-            const SectorRec SF = sc.sectors[S.front];
+            const SegRec S = ts.segs[sf.seg];
+            const SectorRec SF = ts.sectors[S.front];
             const int32_t fcl = SF.ceil, ffl = SF.floor;
             const bool two = S.flags & kSegTwoSided;
             const bool ceil_vis = plane_visible(true, fcl, SF.ceil_flat == kFlatSky, fc.pose.z);
@@ -888,7 +925,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     fill_void_warp<kRgba, kW>(c, inside ? ct : 0, inside ? cb : 0);
     if (kMasked && mcount > 0) {
         __syncwarp();
-        masked_pass<kRgba, kW>(sc, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
+        masked_pass<kRgba, kW, kStates>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
     }
 }
 
@@ -938,12 +975,14 @@ static int device_sms() {
 }
 
 cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
-                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background) {
+                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background,
+                        const StateTables *states) {
     if (n <= 0) return cudaSuccess;
     const size_t smem = walk_smem_per_warp(sc);          // one frame per CTA
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
     if (smem > 48 * 1024) {   // per device and cheap: set it on every launch that needs the opt-in
-        cudaError_t e = cudaFuncSetAttribute(b2d_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = states ? cudaFuncSetAttribute(b2d_walk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                               : cudaFuncSetAttribute(b2d_walk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
     // background (b2d_walk_device: the walk of the NEXT batch, meant to run under another batch's raster): a persistent grid
@@ -951,13 +990,15 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
     // 7/8, so the raster keeps 16 of its 19 warps per SM while the walk hides behind it.
     const int sms = device_sms();
     const int blocks = (background && n > sms) ? sms : n, warps = 4;
-    b2d_walk_kernel<<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride);
+    const StateTables none{};
+    if (states) b2d_walk_kernel<true><<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride, *states);
+    else b2d_walk_kernel<false><<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride, none);
     return cudaGetLastError();
 }
 
 cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameConst *d_frames,
                           const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb,
-                          uint32_t *d_rgba, cudaStream_t stream) {
+                          uint32_t *d_rgba, cudaStream_t stream, const StateTables *states) {
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
     // Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 4 warps per CTA, so a CTA holds the four strips of
@@ -970,15 +1011,19 @@ cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameCons
     // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
     const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
     const bool masked = (sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list;
-#define B2D_RASTER_GO(RGBA, KW) do { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
-    else b2d_raster_kernel<RGBA, KW, false><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba); \
+    // Per-frame states (`states`) take the kStates variant of each shape; the frames are the same pixel for pixel.
+    const StateTables none{};
+#define B2D_RASTER_GO2(RGBA, KW, KS) do { \
+    if (masked) b2d_raster_kernel<RGBA, KW, true, KS><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, KS ? *states : none); \
+    else b2d_raster_kernel<RGBA, KW, false, KS><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, KS ? *states : none); \
     } while (0)
+#define B2D_RASTER_GO(RGBA, KW) do { if (states) B2D_RASTER_GO2(RGBA, KW, true); else B2D_RASTER_GO2(RGBA, KW, false); } while (0)
     if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
     else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
     else if (vw.W == 3840) B2D_RASTER_GO(false, 3840);      // BASELINE.json's 4K configuration (index frames only)
     else B2D_RASTER_GO(false, 0);
 #undef B2D_RASTER_GO
+#undef B2D_RASTER_GO2
     return cudaGetLastError();
 }
 
@@ -1034,6 +1079,43 @@ cudaError_t launch_prelight(const uint8_t *d_colormap, const uint8_t *d_src, uin
     int blocks = (int)((n + 255) / 256);
     if (blocks > device_sms() * 8) blocks = device_sms() * 8;
     b2d_prelight_kernel<<<blocks, 256, 0, stream>>>(d_colormap, d_src, d_dst, n, stride);
+    return cudaGetLastError();
+}
+
+namespace {
+// Per-frame states: one thread per output record of every state of the batch -- the state rule of b2d_scene.hpp, the same
+// functions scene_at_time runs on the host.
+__global__ void __launch_bounds__(256)
+b2d_state_tables_kernel(const __grid_constant__ StateSrc src, const uint32_t *__restrict__ states, uint32_t words, int nstates,
+                        uint8_t *__restrict__ arena, const __grid_constant__ StateTables L) {
+    const uint32_t per = src.ntex + src.nsectors + src.nsegs + src.nsprites + src.nmids;
+    const size_t total = (size_t)per * (size_t)nstates;
+    for (size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t k = (uint32_t)(g / per);
+        uint32_t i = (uint32_t)(g - (size_t)k * per);
+        const StateIn st = state_in(states + (size_t)k * words, src.ndyn);
+        uint8_t *out = arena + (size_t)k * L.slot_bytes;
+        if (i < src.ntex) { reinterpret_cast<TexRec *>(out)[i] = tex_at(src, st, i); continue; }
+        i -= src.ntex;
+        if (i < src.nsectors) { reinterpret_cast<SectorRec *>(out + L.off_sectors)[i] = sector_at(src, st, i); continue; }
+        i -= src.nsectors;
+        if (i < src.nsegs) { reinterpret_cast<SegRec *>(out + L.off_segs)[i] = seg_at(src, st, i); continue; }
+        i -= src.nsegs;
+        if (i < src.nsprites) { reinterpret_cast<SpriteRec *>(out + L.off_sprites)[i] = sprite_at(src, st, i); continue; }
+        i -= src.nsprites;
+        reinterpret_cast<MidRec *>(out + L.off_mids)[i] = mid_at(src, st, i);
+    }
+}
+}  // namespace
+
+cudaError_t launch_state_tables(const StateSrc &src, const uint32_t *d_states, uint32_t words, int nstates, uint8_t *d_arena,
+                                const StateTables &layout, cudaStream_t stream) {
+    const size_t total = (size_t)(src.ntex + src.nsectors + src.nsegs + src.nsprites + src.nmids) * (size_t)nstates;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    const size_t cap = (size_t)device_sms() * 16;
+    if (blocks > cap) blocks = cap;
+    b2d_state_tables_kernel<<<(int)blocks, 256, 0, stream>>>(src, d_states, words, nstates, d_arena, layout);
     return cudaGetLastError();
 }
 

@@ -45,19 +45,36 @@ struct DeviceScene {
 
 constexpr int kMaskedChunk = 4;      // entries per arena chunk (528 bytes)
 
+// Per-frame states (b2d_render_states): the walk and raster variants that take it read the five state-dependent tables of
+// each frame from its slot of a state arena instead of DeviceScene::{tex, sectors, segs, sprites, mids}.  Slot s holds
+// [tex | sectors | segs | sprites | mids] at base + s * slot_bytes (the layout of b2d_scene_tables_at).
+struct StateTables {
+    const uint8_t *base;
+    const uint32_t *frame_slot;      // slot of each frame of the batch: read by the walk, passed on in FrameConst::pad[0]
+    uint32_t slot_bytes, off_sectors, off_segs, off_sprites, off_mids, pad;
+};
+
 // Bytes of dynamic shared memory the BSP-walk kernel needs per frame (= per CTA) for this scene.
 size_t walk_smem_per_warp(const DeviceScene &sc);
 
 // Kernel 1: front-to-back BSP walk, one CTA per frame.  Writes frames[i] and up to `stride`
 // worklist entries per frame at work[i*stride ...].
+// `states` (nullable): per-frame tables.
 cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
-                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background = false);
+                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background = false,
+                        const StateTables *states = nullptr);
 
 // Kernel 2: wall-column / flat-span / sky rasteriser, one warp per (frame, 32-column strip).
 // Writes every pixel of d_index_fb exactly once; if d_rgba != nullptr also the palette-mapped RGBA8.
+// `states` (nullable): per-frame tables, the arena the walk of these frames read.
 cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameConst *d_frames,
                           const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb,
-                          uint32_t *d_rgba, cudaStream_t stream);
+                          uint32_t *d_rgba, cudaStream_t stream, const StateTables *states = nullptr);
+
+// Expands `nstates` compact states (StateLayout::words words each, b2d_scene.hpp) from `src` (device pointers to the
+// rest-state sections) into slots 0 .. nstates-1 of `arena`: one thread per output record.
+cudaError_t launch_state_tables(const StateSrc &src, const uint32_t *d_states, uint32_t words, int nstates, uint8_t *d_arena,
+                                const StateTables &layout, cudaStream_t stream);
 
 // Pre-light kernels (once per renderer).  Flats: dst[r * stride + i] = colormap[r][src[i]] for r < 32, i < n.
 cudaError_t launch_prelight(const uint8_t *d_colormap, const uint8_t *d_src, uint8_t *d_dst, size_t n, size_t stride,
