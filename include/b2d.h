@@ -150,8 +150,8 @@ int b2d_scene_create_dynamic(const b2d_archive *a, int level_index, const b2d_dy
 int b2d_scene_create_from_lumps_dynamic(const b2d_level_lumps *level, const b2d_textures *tex,
                                         const b2d_dynamic_sector *dynamic, size_t n_dynamic, b2d_scene **out);
 /* The state-dependent tables of a scene at level time `tics` with the given sectors moved, laid out
- * [textures | sectors | segs | sprites | mids] as in the blob (host only, no device needed: what the renderer uploads
- * before a batch).  out = NULL: only *size_out is set.  A move of an undeclared sector or outside its range (or with the
+ * [textures | sectors | segs | sprites | mids] as in the blob (host only, no device needed: the tables a batch at that
+ * state reads, which the renderer expands on the device).  out = NULL: only *size_out is set.  A move of an undeclared sector or outside its range (or with the
  * floor above the ceiling) is B2D_ERR_INVALID_ARG. */
 int b2d_scene_tables_at(const b2d_scene *s, uint32_t tics, const b2d_sector_move *moves, size_t n_moves, void *out,
                         size_t capacity, size_t *size_out);
@@ -179,15 +179,16 @@ void b2d_renderer_destroy(b2d_renderer *r);
  * scrolling lines (special 0x30, wad/src/visitor.rs:922) shift their texture column by one texel per tic; sector
  * light effects (wad/src/light.rs:27-80) are re-evaluated.  A no-op for levels without time-dependent content.
  *
- * _async: the time-dependent scene tables (a few KB ... ~200 KB) are rebuilt on the host and copied in stream order
- * on `cuda_stream`; everything this renderer enqueued before -- on any stream -- is awaited by that stream first and
- * later launches on other streams wait for the upload, so the host never blocks on the device (this is the call for
- * a per-frame System::update loop).  b2d_renderer_set_time additionally waits until the upload has completed. */
+ * The call records the renderer's state on the host and enqueues nothing; the host never blocks on the device (this is
+ * the call for a per-frame System::update loop).  A batch is rendered at the state in force when it is walked
+ * (b2d_render*, b2d_walk_device): a ticket walked before the call is rastered at the old state.  The first batch of each
+ * of the renderer's two worklist slots after a change costs one more launch, which expands the state's tables (a few
+ * KB ... ~200 KB) on the device from a compact state of a few words.  _async is the same call; `cuda_stream` is ignored
+ * (kept for compatibility). */
 int b2d_renderer_set_time_async(b2d_renderer *r, uint32_t tics, void *cuda_stream);
 int b2d_renderer_set_time(b2d_renderer *r, uint32_t tics);
-/* The state of the moving sectors for the batches enqueued after this call (sectors not listed are at rest; n = 0 puts
- * everything back).  Stream-ordered like b2d_renderer_set_time_async: the re-derived tables are uploaded behind every
- * batch already enqueued, the host does not wait.  The plain variant returns when the tables are in place. */
+/* The state of the moving sectors for the batches walked after this call (sectors not listed are at rest; n = 0 puts
+ * everything back), recorded like b2d_renderer_set_time's; _async is the same call. */
 int b2d_renderer_set_sector_moves_async(b2d_renderer *r, const b2d_sector_move *moves, size_t n, void *cuda_stream);
 int b2d_renderer_set_sector_moves(b2d_renderer *r, const b2d_sector_move *moves, size_t n);
 
@@ -218,8 +219,7 @@ int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_
  * max_batch (split into batches).  b2d_walk_device_states: like b2d_walk_device (1..max_batch poses); the ticket is
  * rastered by b2d_raster_device, and its table sets live in the ticket's worklist slot until then.  The device-resident
  * calls do not synchronise the device, but before a batch's compact states are written into the worklist slot's pinned
- * staging, the host waits for the copy that read that staging two batches earlier (normally finished long before); the
- * first call of a renderer also waits for its one-time upload of the rest-state sections. */
+ * staging, the host waits for the copy that read that staging two batches earlier (normally finished long before). */
 typedef struct b2d_frame_state {
     uint32_t tics;                    /* level time */
     uint32_t first_move, n_moves;     /* moves[first_move .. first_move + n_moves) of the call's list; n_moves = 0: all at rest */
@@ -235,7 +235,7 @@ int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_f
 /* Per-pose level time (SURVEY 8-f2: poses (x, y, z, yaw, t)): pose i is rendered at level time tics[i] (HOST array) with
  * the renderer's current sector moves -- b2d_render_states / b2d_render_device_states with those states, so a batch costs
  * the same three launches whatever the timeline (two on a level without time-dependent content).  Leaves the renderer at
- * the last pose's time (one stream-ordered table upload at the end).  tics == NULL in b2d_render_timed is b2d_render. */
+ * the last pose's time, as b2d_renderer_set_time does.  tics == NULL in b2d_render_timed is b2d_render. */
 int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tics, size_t n, uint8_t *index_fb, uint32_t *rgba_fb);
 int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *tics, size_t n, uint8_t *d_index_fb,
                             uint32_t *d_rgba_fb, void *cuda_stream);

@@ -315,17 +315,18 @@ class Renderer:
         self.worklist_stride = max(1, scene.info.n_segs + scene.info.n_sprites)
 
     def set_time(self, tics: int):
-        """Level time in 1/35 s for the batches rendered afterwards (animated flats / walls, scrolling walls)."""
+        """Level time in 1/35 s for the batches walked afterwards (animated flats / walls, scrolling walls, light
+        effects).  Host only: nothing is enqueued; a ticket walked before the call keeps its time."""
         _check(_lib.load().b2d_renderer_set_time(self._h, int(tics) & 0xFFFFFFFF))
 
     def set_time_async(self, tics: int, stream: int = 0):
-        """Same, without blocking the host: the table upload is ordered on `stream` (a cudaStream_t as int)."""
+        """b2d_renderer_set_time_async: the same call (`stream` is ignored)."""
         _check(_lib.load().b2d_renderer_set_time_async(self._h, int(tics) & 0xFFFFFFFF, ctypes.c_void_p(stream)))
 
     def set_sector_moves(self, moves=(), stream: Optional[int] = None):
-        """State of the moving sectors for the batches rendered afterwards: (sector, floor_offset, ceil_offset) in map
-        units relative to the level lumps; sectors not listed are at rest.  With `stream` (a cudaStream_t as int) the
-        host does not wait for the table upload (b2d_renderer_set_sector_moves_async)."""
+        """State of the moving sectors for the batches walked afterwards: (sector, floor_offset, ceil_offset) in map
+        units relative to the level lumps; sectors not listed are at rest.  Host only, like set_time; with `stream` it
+        calls b2d_renderer_set_sector_moves_async, the same call."""
         arr, n = _moves_array(moves)
         if stream is None:
             _check(_lib.load().b2d_renderer_set_sector_moves(self._h, arr, n))

@@ -1,7 +1,9 @@
 // C-ABI of libb2d.so (declared in include/b2d.h).  Thin, exception-free boundary over the C++ host
 // side (WAD loader, scene compiler) and the CUDA kernels.  There is deliberately no CPU rendering
 // path here: every render entry point launches the sm_90a kernels or fails with B2D_ERR_CUDA.
+#include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -164,18 +166,14 @@ void free_renderer(b2d_renderer *r) {
     if (r->d_masked) cudaFree(r->d_masked);
     if (r->d_masked_counter) cudaFree(r->d_masked_counter);
     if (r->masked_done) cudaEventDestroy(r->masked_done);
-    if (r->tables_ready) cudaEventDestroy(r->tables_ready);
-    for (int i = 0; i < 2; i++) {
-        if (r->h_timed[i]) cudaFreeHost(r->h_timed[i]);
-        if (r->timed_copied[i]) cudaEventDestroy(r->timed_copied[i]);
-    }
     for (int i = 0; i < 2; i++) {
         if (r->d_arena[i]) cudaFree(r->d_arena[i]);
         if (r->d_states[i]) cudaFree(r->d_states[i]);
         if (r->h_states[i]) cudaFreeHost(r->h_states[i]);
         if (r->states_copied[i]) cudaEventDestroy(r->states_copied[i]);
     }
-    if (r->d_pristine) cudaFree(r->d_pristine);
+    if (r->d_slot_tables) cudaFree(r->d_slot_tables);
+    if (r->d_slot_maps) cudaFree(r->d_slot_maps);
     if (r->d_lit) cudaFree(r->d_lit);
     if (r->d_walk_static) cudaFree(r->d_walk_static);
     free_aligned_4g(r);
@@ -183,55 +181,10 @@ void free_renderer(b2d_renderer *r) {
     delete r;
 }
 
-size_t state_table_bytes(const uint8_t *blob);
-
-// Per-frame states: the rest-state sections the state rule reads, uploaded once next to the blob (whose own sections
-// set_time / set_sector_moves overwrite), and the two worklist slots' arenas and staging.
+// Per-frame states: the two worklist slots' arenas of max_batch table sets, allocated by the first such call.
 int ensure_states(b2d_renderer *r) {
-    if (r->d_pristine) return B2D_OK;
-    const uint8_t *blob = r->h_blob.data();
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
-    const StateLayout &L = r->layout;
-    auto a256 = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    struct Sec { const void *src; size_t bytes; size_t off; };
-    Sec secs[10] = {{blob + h[H_OFF_TEX], h[H_NTEX] * sizeof(TexRec), 0}, {blob + h[H_OFF_SECTORS], h[H_NSECTORS] * sizeof(SectorRec), 0},
-                    {blob + h[H_OFF_SEGS], h[H_NSEGS] * sizeof(SegRec), 0}, {blob + h[H_OFF_SPRITES], h[H_NSPRITES] * sizeof(SpriteRec), 0},
-                    {blob + h[H_OFF_MIDS], h[H_NMIDS] * sizeof(MidRec), 0}, {blob + h[H_OFF_ANIM], h[H_NANIM] * sizeof(int32_t), 0},
-                    {blob + h[H_OFF_FLAT_ANIM], h[H_NFLATS] * sizeof(FlatAnimRec), 0}, {blob + h[H_OFF_SEGDYN], h[H_NSEGS] * sizeof(SegDynRec), 0},
-                    {L.sector_slots.data(), L.sector_slots.size() * 4, 0}, {L.mid_seg.data(), L.mid_seg.size() * 4, 0}};
-    size_t total = 0;
-    for (Sec &q : secs) { q.off = total; total = a256(total + q.bytes); }
-    std::vector<uint8_t> img(total + 256, 0);
-    for (const Sec &q : secs) if (q.bytes) std::memcpy(img.data() + q.off, q.src, q.bytes);
-    const size_t words = L.words, mb = (size_t)r->max_batch;
-    StateTables &t = r->state_tables;
-    t.slot_bytes = (uint32_t)a256(state_table_bytes(blob));        // one table set: [tex | sectors | segs | sprites | mids]
-    for (int i = 0; i < 2; i++) {
-        if (!r->d_arena[i]) CU(cudaMalloc(&r->d_arena[i], mb * t.slot_bytes));
-        if (!r->d_states[i]) CU(cudaMalloc(&r->d_states[i], 4 * mb * (words + 1)));
-        if (!r->h_states[i]) CU(cudaMallocHost(&r->h_states[i], 4 * mb * (words + 1)));
-        if (!r->states_copied[i]) CU(cudaEventCreateWithFlags(&r->states_copied[i], cudaEventDisableTiming));
-    }
-    uint8_t *d = nullptr;
-    CU(cudaMalloc(&d, img.size()));
-    // A copy from pageable memory may return before its DMA has landed, and the expansion that first reads these sections
-    // runs on the caller's stream, which need not be ordered after the legacy default stream: wait for the copy here (once
-    // per renderer, like the uploads at creation).
-    cudaError_t e = cudaMemcpy(d, img.data(), img.size(), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { cudaFree(d); return cuda_fail(e, "cudaMemcpy (rest-state sections)"); }
-    r->d_pristine = d;
-    StateSrc s = state_src(blob, L);
-    s.tex = reinterpret_cast<const TexRec *>(d + secs[0].off); s.sectors = reinterpret_cast<const SectorRec *>(d + secs[1].off);
-    s.segs = reinterpret_cast<const SegRec *>(d + secs[2].off); s.sprites = reinterpret_cast<const SpriteRec *>(d + secs[3].off);
-    s.mids = reinterpret_cast<const MidRec *>(d + secs[4].off); s.anim = reinterpret_cast<const int32_t *>(d + secs[5].off);
-    s.flat_anim = reinterpret_cast<const FlatAnimRec *>(d + secs[6].off); s.segdyn = reinterpret_cast<const SegDynRec *>(d + secs[7].off);
-    s.sector_slots = reinterpret_cast<const uint32_t *>(d + secs[8].off); s.mid_seg = reinterpret_cast<const int32_t *>(d + secs[9].off);
-    r->src = s;
-    t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
-    t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
-    t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
-    t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
+    for (int i = 0; i < 2; i++)
+        if (!r->d_arena[i]) CU(cudaMalloc(&r->d_arena[i], (size_t)r->max_batch * r->state_tables.slot_bytes));
     return B2D_OK;
 }
 
@@ -243,29 +196,54 @@ StateTables slot_tables(const b2d_renderer *r, int slot) {
     return t;
 }
 
+// the scene as the plain kernels of worklist slot `slot` read it: on a timed scene, the five state-dependent tables are
+// the slot's own table set
+DeviceScene slot_scene(const b2d_renderer *r, int slot) {
+    DeviceScene d = r->ds;
+    if (!r->d_slot_tables) return d;
+    const StateTables &t = r->state_tables;
+    const uint8_t *set = r->d_slot_tables + (size_t)slot * t.slot_bytes;
+    d.tex = reinterpret_cast<const TexRec *>(set);
+    d.sectors = reinterpret_cast<const SectorRec *>(set + t.off_sectors);
+    d.segs = reinterpret_cast<const SegRec *>(set + t.off_segs);
+    d.sprites = reinterpret_cast<const SpriteRec *>(set + t.off_sprites);
+    d.mids = reinterpret_cast<const MidRec *>(set + t.off_mids);
+    return d;
+}
+
 // BSP walk of a batch into the next worklist slot, on `stream`.  The slot's previous raster (if any, on whatever
 // stream) is awaited through an event, so a caller may run walks and rasters on two streams and have the walk of
 // batch k+1 overlap the raster of batch k.  `frame_states` (nullable): one compact state per frame; the batch's distinct
-// states are expanded into the slot's arena on `stream` first (frames with equal states share one table set).
+// states are expanded into the slot's arena on `stream` first (frames with equal states share one table set).  A plain
+// batch on a timed scene reads the slot's own table set, which is re-expanded on `stream` when the renderer's state
+// differs from the one the set holds: the walk and the raster of a ticket read one state whatever is set in between.
 int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background = false,
                    const uint32_t *frame_states = nullptr) {
     const int slot = (int)(r->next_ticket & 1);
     if (!r->slot_rastered[slot]) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
-    int nstates = 0;
     if (frame_states) {
         int rc = ensure_states(r);
         if (rc != B2D_OK) return rc;
-        // distinct states -> slots 0, 1, ... in order of first appearance, anywhere in the batch
-        const size_t words = r->layout.words;
+    }
+    const bool restate = !frame_states && r->d_slot_tables && r->slot_state[slot] != r->state;
+    const size_t words = r->layout.words;
+    int nstates = 0;
+    if (frame_states || restate) {
         CU(cudaEventSynchronize(r->states_copied[slot]));      // the copy issued two batches ago has read the staging
         uint32_t *hs = r->h_states[slot], *hslot = hs + (size_t)r->max_batch * words;
-        std::unordered_map<std::string, uint32_t> seen;
-        seen.reserve((size_t)n);
-        for (int f = 0; f < n; f++) {
-            const uint32_t *w = frame_states + (size_t)f * words;
-            auto it = seen.emplace(std::string(reinterpret_cast<const char *>(w), 4 * words), (uint32_t)nstates);
-            if (it.second) std::memcpy(hs + (size_t)nstates++ * words, w, 4 * words);
-            hslot[f] = it.first->second;
+        if (restate) {
+            std::memcpy(hs, r->state.data(), 4 * words);
+            nstates = 1;
+        } else {
+            // distinct states -> slots 0, 1, ... in order of first appearance, anywhere in the batch
+            std::unordered_map<std::string, uint32_t> seen;
+            seen.reserve((size_t)n);
+            for (int f = 0; f < n; f++) {
+                const uint32_t *w = frame_states + (size_t)f * words;
+                auto it = seen.emplace(std::string(reinterpret_cast<const char *>(w), 4 * words), (uint32_t)nstates);
+                if (it.second) std::memcpy(hs + (size_t)nstates++ * words, w, 4 * words);
+                hslot[f] = it.first->second;
+            }
         }
     }
     if (!r->d_frames[slot]) {
@@ -278,24 +256,25 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
     } else {
         CU(cudaStreamWaitEvent(stream, r->raster_done[slot], 0));      // the raster that last read this slot
     }
-    if (r->tables_pending) CU(cudaStreamWaitEvent(stream, r->tables_ready, 0));   // a table upload on another stream
     const StateTables stt = frame_states ? slot_tables(r, slot) : StateTables{};
-    if (frame_states) {
-        const size_t words = r->layout.words;
+    if (nstates) {
         uint32_t *hs = r->h_states[slot];
         CU(cudaMemcpyAsync(r->d_states[slot], hs, 4 * words * (size_t)nstates, cudaMemcpyHostToDevice, stream));
-        CU(cudaMemcpyAsync(const_cast<uint32_t *>(stt.frame_slot), hs + (size_t)r->max_batch * words, 4 * (size_t)n,
-                           cudaMemcpyHostToDevice, stream));
+        if (frame_states)
+            CU(cudaMemcpyAsync(const_cast<uint32_t *>(stt.frame_slot), hs + (size_t)r->max_batch * words, 4 * (size_t)n,
+                               cudaMemcpyHostToDevice, stream));
         CU(cudaEventRecord(r->states_copied[slot], stream));
-        CU(launch_state_tables(r->src, r->d_states[slot], (uint32_t)words, nstates, r->d_arena[slot], stt, stream));
+        uint8_t *sets = frame_states ? r->d_arena[slot] : r->d_slot_tables + (size_t)slot * r->state_tables.slot_bytes;
+        CU(launch_state_tables(r->src, r->d_states[slot], (uint32_t)words, nstates, sets, r->state_tables, stream));
         r->launches += 1;
+        if (restate) r->slot_state[slot] = r->state;
     }
     cudaEvent_t ev[2] = {nullptr, nullptr};
     if (r->profiling) {
         for (auto &e : ev) CU(cudaEventCreate(&e));
         CU(cudaEventRecord(ev[0], stream));
     }
-    CU(launch_walk(r->ds, r->view, d_poses, n, r->d_frames[slot], r->d_work[slot], r->stride, stream, background,
+    CU(launch_walk(slot_scene(r, slot), r->view, d_poses, n, r->d_frames[slot], r->d_work[slot], r->stride, stream, background,
                    frame_states ? &stt : nullptr));
     if (r->profiling) {
         CU(cudaEventRecord(ev[1], stream));
@@ -308,7 +287,6 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
     r->slot_ticket[slot] = r->next_ticket;
     r->slot_rastered[slot] = false;
     r->last_slot = slot;
-    r->last_n = n;
     r->launches += 1;
     *ticket_out = r->next_ticket++;
     return B2D_OK;
@@ -319,7 +297,6 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
     if (ticket < 0 || r->slot_ticket[slot] != ticket || r->slot_rastered[slot])
         return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
     CU(cudaStreamWaitEvent(stream, r->walk_done[slot], 0));
-    if (r->tables_pending) CU(cudaStreamWaitEvent(stream, r->tables_ready, 0));
     if (r->ds.masked_list) {
         // one arena of deferred masked entries per renderer: rasters that use it run one after the other (each fills the
         // machine on its own, so nothing is lost), whatever streams they were enqueued on
@@ -332,7 +309,7 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
         CU(cudaEventRecord(ev[0], stream));
     }
     const StateTables stt = r->slot_states[slot] ? slot_tables(r, slot) : StateTables{};
-    CU(launch_raster(r->ds, r->view, r->d_frames[slot], r->d_work[slot], r->stride, r->slot_n[slot], d_index, d_rgba, stream,
+    CU(launch_raster(slot_scene(r, slot), r->view, r->d_frames[slot], r->d_work[slot], r->stride, r->slot_n[slot], d_index, d_rgba, stream,
                      r->slot_states[slot] ? &stt : nullptr));
     if (r->profiling) {
         CU(cudaEventRecord(ev[1], stream));
@@ -346,10 +323,6 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
     return B2D_OK;
 }
 
-// Rebuild the time-dependent tables for `tics` on the host (scene_at_time) and copy them over their sections of the
-// device blob in stream order.  Everything this renderer has enqueued so far -- on any stream -- is awaited by `stream`
-// first (the walk/raster events of both worklist slots), and later launches on other streams wait for the upload, so the
-// host never blocks on the device: no cudaDeviceSynchronize in the System::update loop this stands in for.
 // the state-dependent tables (level time `tics`, sector offsets), laid out [tex | sectors | segs | sprites | mids]
 size_t state_table_bytes(const uint8_t *blob) {
     const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
@@ -357,54 +330,21 @@ size_t state_table_bytes(const uint8_t *blob) {
            h[H_NSPRITES] * sizeof(SpriteRec) + h[H_NMIDS] * sizeof(MidRec);
 }
 
-void state_tables(const uint8_t *blob, uint32_t tics, const int32_t *floor_off, const int32_t *ceil_off, uint8_t *out,
-                  const StateLayout *layout = nullptr) {
+void state_tables(const uint8_t *blob, uint32_t tics, const int32_t *floor_off, const int32_t *ceil_off, uint8_t *out) {
     const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
     TexRec *tex = reinterpret_cast<TexRec *>(out);
     SectorRec *sectors = reinterpret_cast<SectorRec *>(tex + h[H_NTEX]);
     SegRec *segs = reinterpret_cast<SegRec *>(sectors + h[H_NSECTORS]);
     SpriteRec *sprites = reinterpret_cast<SpriteRec *>(segs + h[H_NSEGS]);
     MidRec *mids = reinterpret_cast<MidRec *>(sprites + h[H_NSPRITES]);
-    scene_at_time(blob, tics, tex, sectors, segs, sprites, mids, floor_off, ceil_off, layout);
+    scene_at_time(blob, tics, tex, sectors, segs, sprites, mids, floor_off, ceil_off);
 }
 
-void tables_at(const b2d_renderer *r, uint32_t tics, uint8_t *out) {
-    const bool moved = !r->floor_off.empty();
-    state_tables(r->h_blob.data(), tics, moved ? r->floor_off.data() : nullptr, moved ? r->ceil_off.data() : nullptr, out,
-                 &r->layout);
-}
-
-int upload_tables(b2d_renderer *r, const uint8_t *tables, cudaStream_t stream) {
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(r->h_blob.data());
-    const int buf = r->timed_next;
-    r->timed_next ^= 1;
-    CU(cudaEventSynchronize(r->timed_copied[buf]));          // the copy issued two uploads ago has read this buffer
-    uint8_t *p = r->h_timed[buf];
-    std::memcpy(p, tables, r->timed_bytes);
-    const uint8_t *tex = p, *sectors = tex + h[H_NTEX] * sizeof(TexRec), *segs = sectors + h[H_NSECTORS] * sizeof(SectorRec),
-                  *sprites = segs + h[H_NSEGS] * sizeof(SegRec), *mids = sprites + h[H_NSPRITES] * sizeof(SpriteRec);
-    for (int i = 0; i < 2; i++) {
-        if (r->walk_done[i]) CU(cudaStreamWaitEvent(stream, r->walk_done[i], 0));
-        if (r->raster_done[i]) CU(cudaStreamWaitEvent(stream, r->raster_done[i], 0));
-    }
-    CU(cudaMemcpyAsync(r->d_blob + h[H_OFF_TEX], tex, h[H_NTEX] * sizeof(TexRec), cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(r->d_blob + h[H_OFF_SECTORS], sectors, h[H_NSECTORS] * sizeof(SectorRec), cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(r->d_blob + h[H_OFF_SEGS], segs, h[H_NSEGS] * sizeof(SegRec), cudaMemcpyHostToDevice, stream));
-    if (h[H_NSPRITES])
-        CU(cudaMemcpyAsync(r->d_blob + h[H_OFF_SPRITES], sprites, h[H_NSPRITES] * sizeof(SpriteRec), cudaMemcpyHostToDevice, stream));
-    if (h[H_NMIDS] && h[H_NDYN])        // masked middle textures only move with their sector
-        CU(cudaMemcpyAsync(r->d_blob + h[H_OFF_MIDS], mids, h[H_NMIDS] * sizeof(MidRec), cudaMemcpyHostToDevice, stream));
-    CU(cudaEventRecord(r->timed_copied[buf], stream));
-    CU(cudaEventRecord(r->tables_ready, stream));
-    r->tables_pending = true;
-    r->cur_tables.assign(tables, tables + r->timed_bytes);
-    return B2D_OK;
-}
-
-int upload_timed_tables(b2d_renderer *r, uint32_t tics, cudaStream_t stream) {
-    r->scratch_tables.resize(r->timed_bytes);
-    tables_at(r, tics, r->scratch_tables.data());
-    return upload_tables(r, r->scratch_tables.data(), stream);
+// The compact state of level time `tics` with the renderer's current sector moves into out[layout.words] (out is not
+// r->state): the moved flag and the offsets, words 1 .. 2 + 2 * ndyn, do not depend on the time.
+void state_at(const b2d_renderer *r, uint32_t tics, uint32_t *out) {
+    compact_state(r->h_blob.data(), r->layout, tics, nullptr, nullptr, out);
+    std::copy(r->state.begin() + 1, r->state.begin() + 2 + 2 * (ptrdiff_t)r->layout.dyn_sectors.size(), out + 1);
 }
 
 // The compact state of every frame of a b2d_render_states-style call into `out` (r->layout.words words per frame), checking
@@ -446,11 +386,8 @@ void timed_states(const b2d_renderer *r, const uint32_t *tics, size_t n, std::ve
     out.clear();
     if (r->h_blob.empty()) return;
     const size_t words = r->layout.words;
-    const bool moved = !r->floor_off.empty();
     out.resize(n * words);
-    for (size_t i = 0; i < n; i++)
-        compact_state(r->h_blob.data(), r->layout, tics[i], moved ? r->floor_off.data() : nullptr, moved ? r->ceil_off.data() : nullptr,
-                      out.data() + i * words);
+    for (size_t i = 0; i < n; i++) state_at(r, tics[i], out.data() + i * words);
 }
 
 }  // namespace
@@ -823,24 +760,48 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
     if (walk_smem_per_warp(d) > 227 * 1024) { free_renderer(r); return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory"); }
     if (scene_is_timed(s->blob.data())) {
         r->h_blob = s->blob;
-        r->timed_bytes = state_table_bytes(r->h_blob.data());
         try {
             r->layout = state_layout(r->h_blob.data());
         } catch (const std::exception &ex) {
             free_renderer(r);
             return fail(B2D_ERR_INVALID_ARG, ex.what());
         }
+        const uint8_t *blob = r->h_blob.data();
+        const StateLayout &L = r->layout;
+        const size_t words = L.words, mb = (size_t)max_batch;
+        // the state rule reads the blob's rest-state sections and the two slot maps
+        CUR(cudaMalloc(&r->d_slot_maps, 4 * (L.sector_slots.size() + L.mid_seg.size()) + 4));
+        CUR(cudaMemcpy(r->d_slot_maps, L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
+        CUR(cudaMemcpy(r->d_slot_maps + L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
+        StateSrc &src = r->src = state_src(blob, L);
+        auto on_device = [&](auto p) { return reinterpret_cast<decltype(p)>(r->d_blob + (reinterpret_cast<const uint8_t *>(p) - blob)); };
+        src.tex = on_device(src.tex); src.sectors = on_device(src.sectors); src.segs = on_device(src.segs);
+        src.sprites = on_device(src.sprites); src.mids = on_device(src.mids); src.anim = on_device(src.anim);
+        src.flat_anim = on_device(src.flat_anim); src.segdyn = on_device(src.segdyn);
+        src.sector_slots = r->d_slot_maps;
+        src.mid_seg = reinterpret_cast<const int32_t *>(r->d_slot_maps + L.sector_slots.size());
+        StateTables &t = r->state_tables;              // one table set: [tex | sectors | segs | sprites | mids], 256 B aligned
+        t.slot_bytes = (uint32_t)((state_table_bytes(blob) + 255) & ~(size_t)255);
+        t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
+        t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
+        t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
+        t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
+        CUR(cudaMalloc(&r->d_slot_tables, 2 * (size_t)t.slot_bytes));
         for (int i = 0; i < 2; i++) {
-            CUR(cudaMallocHost(&r->h_timed[i], r->timed_bytes ? r->timed_bytes : 1));
-            CUR(cudaEventCreateWithFlags(&r->timed_copied[i], cudaEventDisableTiming));
+            CUR(cudaMalloc(&r->d_states[i], 4 * mb * (words + 1)));
+            CUR(cudaMallocHost(&r->h_states[i], 4 * mb * (words + 1)));
+            CUR(cudaEventCreateWithFlags(&r->states_copied[i], cudaEventDisableTiming));
         }
-        CUR(cudaEventCreateWithFlags(&r->tables_ready, cudaEventDisableTiming));
         // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306).  The
-        // pre-lit planes above were built from the blob's own (per-image) records; from here on the records are re-pointed.
-        int rc = upload_timed_tables(r, 0, nullptr);
-        if (rc != B2D_OK) { free_renderer(r); return rc; }
-        CUR(cudaStreamSynchronize(nullptr));
-        r->tables_pending = false;
+        // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0.
+        r->state.assign(words, 0);
+        compact_state(blob, L, 0, nullptr, nullptr, r->state.data());
+        CUR(cudaMemcpy(r->d_states[0], r->state.data(), 4 * words, cudaMemcpyHostToDevice));
+        for (int i = 0; i < 2; i++) {
+            CUR(launch_state_tables(r->src, r->d_states[0], (uint32_t)words, 1, r->d_slot_tables + i * (size_t)t.slot_bytes, t, nullptr));
+            r->slot_state[i] = r->state;
+        }
+        CUR(cudaDeviceSynchronize());
     }
     CUR(cudaMalloc(&r->d_poses, sizeof(Pose) * (size_t)max_batch));
     CUR(cudaMalloc(&r->d_frames[0], sizeof(FrameConst) * (size_t)max_batch));
@@ -852,53 +813,43 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
 
 void b2d_renderer_destroy(b2d_renderer *r) { free_renderer(r); }
 
-int b2d_renderer_set_time_async(b2d_renderer *r, uint32_t tics, void *cuda_stream) {
+// The renderer's own state is host data: the setters enqueue nothing (the stream is kept for ABI compatibility), and the
+// next plain batch of each worklist slot expands it into the slot's table set.
+int b2d_renderer_set_time(b2d_renderer *r, uint32_t tics) {
     if (!r) return fail(B2D_ERR_INVALID_ARG, "null renderer");
-    if (r->h_blob.empty() || tics == r->tics) { r->tics = tics; return B2D_OK; }
-    CU(cudaSetDevice(r->device));
-    int rc = upload_timed_tables(r, tics, static_cast<cudaStream_t>(cuda_stream));
-    if (rc == B2D_OK) r->tics = tics;
-    return rc;
+    if (r->h_blob.empty()) { r->tics = tics; return B2D_OK; }
+    return guarded([&] {
+        std::vector<uint32_t> s(r->layout.words);
+        state_at(r, tics, s.data());
+        r->state.swap(s);
+        r->tics = tics;
+        return B2D_OK;
+    });
 }
 
-int b2d_renderer_set_sector_moves_async(b2d_renderer *r, const b2d_sector_move *moves, size_t n, void *cuda_stream) {
+int b2d_renderer_set_time_async(b2d_renderer *r, uint32_t tics, void *) { return b2d_renderer_set_time(r, tics); }
+
+int b2d_renderer_set_sector_moves(b2d_renderer *r, const b2d_sector_move *moves, size_t n) {
     if (!r || (n && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (r->h_blob.empty()) {
         if (n == 0) return B2D_OK;
         return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
     }
     static_assert(sizeof(b2d_sector_move) == sizeof(SectorMove), "ABI record");
-    std::vector<int32_t> fo, co;
-    if (const char *why = expand_moves(r->h_blob.data(), reinterpret_cast<const SectorMove *>(moves), n, fo, co))
-        return fail(B2D_ERR_INVALID_ARG, why);
-    bool any = false;
-    for (size_t i = 0; i < fo.size(); i++) any |= fo[i] != 0 || co[i] != 0;
-    if (!any) { fo.clear(); co.clear(); }
-    if (fo == r->floor_off && co == r->ceil_off) return B2D_OK;
-    r->floor_off.swap(fo);
-    r->ceil_off.swap(co);
-    CU(cudaSetDevice(r->device));
-    return upload_timed_tables(r, r->tics, static_cast<cudaStream_t>(cuda_stream));
+    return guarded([&] {
+        std::vector<int32_t> fo, co;
+        if (const char *why = expand_moves(r->h_blob.data(), reinterpret_cast<const SectorMove *>(moves), n, fo, co))
+            return fail(B2D_ERR_INVALID_ARG, why);
+        bool moved = false;
+        for (size_t i = 0; i < fo.size() && !moved; i++) moved = fo[i] != 0 || co[i] != 0;      // all zero: at rest
+        compact_state(r->h_blob.data(), r->layout, r->tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
+                      r->state.data());
+        return B2D_OK;
+    });
 }
 
-int b2d_renderer_set_sector_moves(b2d_renderer *r, const b2d_sector_move *moves, size_t n) {
-    int rc = b2d_renderer_set_sector_moves_async(r, moves, n, nullptr);
-    if (rc != B2D_OK) return rc;
-    if (r->tables_pending) {
-        CU(cudaEventSynchronize(r->tables_ready));
-        r->tables_pending = false;
-    }
-    return B2D_OK;
-}
-
-int b2d_renderer_set_time(b2d_renderer *r, uint32_t tics) {
-    int rc = b2d_renderer_set_time_async(r, tics, nullptr);
-    if (rc != B2D_OK) return rc;
-    if (r->tables_pending) {
-        CU(cudaEventSynchronize(r->tables_ready));
-        r->tables_pending = false;
-    }
-    return B2D_OK;
+int b2d_renderer_set_sector_moves_async(b2d_renderer *r, const b2d_sector_move *moves, size_t n, void *) {
+    return b2d_renderer_set_sector_moves(r, moves, n);
 }
 
 int b2d_renderer_status(b2d_renderer *r, int32_t *bits_out) {
@@ -946,7 +897,7 @@ int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint
     if (rc != B2D_OK) return rc;
     rc = enqueue_batches(r, d_poses, n, fs.empty() ? nullptr : fs.data(), d_index_fb, d_rgba_fb, st);
     if (rc != B2D_OK) return rc;
-    return b2d_renderer_set_time_async(r, tics[n - 1], cuda_stream);       // the renderer is left at the last pose's time
+    return b2d_renderer_set_time(r, tics[n - 1]);                          // the renderer is left at the last pose's time
 }
 
 int b2d_render_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,

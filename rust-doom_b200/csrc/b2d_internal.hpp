@@ -57,26 +57,23 @@ struct b2d_renderer {
     Pose *h_poses = nullptr;        // pinned
     cudaStream_t render_stream = nullptr, copy_stream[2] = {nullptr, nullptr};   // one copy stream per staging buffer
     cudaEvent_t rendered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
-    std::vector<uint8_t> h_blob;    // host copy of the scene, kept only when it has time-dependent content
-    uint32_t tics = 0;
-    // time-dependent tables (texture records, sectors, segs, sprites): rebuilt on the host into one of two pinned
-    // staging buffers and copied over their sections of the device blob in stream order (b2d_renderer_set_time_async)
-    uint8_t *h_timed[2] = {nullptr, nullptr};
-    cudaEvent_t timed_copied[2] = {nullptr, nullptr};     // staging buffer i has been read by its copy
-    cudaEvent_t tables_ready = nullptr;                   // last table upload; launches on other streams wait for it
-    bool tables_pending = false;
-    int timed_next = 0;
-    size_t timed_bytes = 0;
     uint8_t *d_walk_static = nullptr;                     // node / subsector tables as the walk kernel's shared memory holds them
-    std::vector<int32_t> floor_off, ceil_off;             // state of the moving sectors (one offset per sector; empty = at rest)
-    std::vector<uint8_t> cur_tables, scratch_tables;      // host copies: tables of the last upload / of a candidate time
-    // per-frame states (b2d_render_states & co., DESIGN.md §3 "State arena"): the device copy of the rest-state sections
-    // the state rule reads, and per worklist slot an arena of up to max_batch expanded table sets, the batch's distinct
-    // compact states + per-frame slot indices on the device and their pinned staging.  Allocated by the first such call.
-    StateLayout layout;                                   // scenes with time-dependent content or dynamic sectors
-    uint8_t *d_pristine = nullptr;
-    StateSrc src{};                                       // device pointers into d_pristine
+    // Scenes with time-dependent content or dynamic sectors (DESIGN.md §3 "State arena"); the rest stays empty.  The
+    // device blob is never written after creation: the state rule reads its rest-state sections, and every batch reads
+    // its five state-dependent tables from a table set expanded on the device from a compact state.
+    std::vector<uint8_t> h_blob;                          // host copy of the scene
+    StateLayout layout;
+    uint32_t tics = 0;
+    std::vector<uint32_t> state;                          // the renderer's own compact state (set_time, set_sector_moves)
+    uint32_t *d_slot_maps = nullptr;                      // StateLayout::sector_slots, then ::mid_seg
+    StateSrc src{};                                       // device pointers into d_blob and d_slot_maps
     StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
+    // per worklist slot: the table set its plain batches read and the compact state it was expanded from
+    uint8_t *d_slot_tables = nullptr;                     // two table sets
+    std::vector<uint32_t> slot_state[2];
+    // per-frame states (b2d_render_states & co.): per worklist slot an arena of up to max_batch expanded table sets
+    // (allocated by the first such call), and the compact states + per-frame slot indices on the device and their
+    // pinned staging, shared with the expansion of the slot's own table set
     uint8_t *d_arena[2] = {nullptr, nullptr};
     uint32_t *d_states[2] = {nullptr, nullptr};           // max_batch compact states, then max_batch slot indices
     uint32_t *h_states[2] = {nullptr, nullptr};           // pinned, same layout
@@ -85,7 +82,6 @@ struct b2d_renderer {
     cudaEvent_t masked_done = nullptr;                    // last raster that used the masked-entry arena
     uint32_t *d_masked_counter = nullptr;
     int64_t launches = 0;
-    int last_n = 0;
     bool profiling = false;
     std::vector<cudaEvent_t> prof_events;   // pairs: before / after one kernel launch
     std::vector<int> prof_kinds;            // per pair: 0 = walk, 1 = raster

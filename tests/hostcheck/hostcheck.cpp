@@ -433,9 +433,9 @@ static int render_impl(const uint8_t *blob, const View *vw, const Pose *poses, i
                        int n_moves = 0) {
     HostScene sc = bind(blob);
     LitPlanes lit;
-    build_lit(sc, lit);                // from the blob's own table: set_time only re-points records
-    // the product's time handling: the three time-dependent tables are rebuilt by scene_at_time (b2d_scene.hpp)
-    // exactly as b2d_renderer_set_time does before it uploads them
+    build_lit(sc, lit);                // from the blob's own table: a state only re-points records
+    // the product's state rule: the state-dependent tables are rebuilt by scene_at_time (b2d_scene.hpp), the host loop
+    // over the per-record functions the renderer's expansion kernel runs on the device
     std::vector<TexRec> tex_t((size_t)sc.ntex);
     std::vector<SectorRec> sectors_t((size_t)sc.hdr[H_NSECTORS]);
     std::vector<SegRec> segs_t((size_t)sc.nsegs);

@@ -10,10 +10,10 @@ Arms, alternated in one process, `--rounds` times each:
   B   walk_device_states / raster_device, pipelined the same way: every frame at its own tic
   B1  B with every frame of a batch at the batch's first tic, so that all frames share one table set (separates the cost of
       the per-frame addressing from the cost of 1000 table sets' L2 footprint)
-  C   set_time_async + render_device per pose: what a per-pose timeline cost before per-frame states (one batch per round)
+  C   set_time_async + render_device per pose: a per-pose timeline without per-frame states (one batch per round)
 Per arm: ms per 1000 frames and frames/s (CUDA events around the arm's batches), host ms per batch in the calls that
-build and enqueue states or tables, H2D bytes per batch (B: the batch's distinct compact states, counted from the
-table-set index of every frame, plus one set index per frame).  Before timing, sampled frames of batch 0 are checked: B equal to
+build and enqueue states, H2D bytes per batch (A: the renderer's one compact state; B: the batch's distinct compact
+states, counted from the table-set index of every frame, plus one set index per frame; C: one compact state per pose).  Before timing, sampled frames of batch 0 are checked: B equal to
 C and to the oracle at each frame's tic, A equal to the oracle at the batch's tic.  The card, its power limit and SM clock
 are printed with the numbers.
 """
@@ -149,7 +149,7 @@ def run_level(name, cfg, rounds, batches):
     torch.cuda.synchronize()
     nb = {"A": rounds * batches, "B": rounds * batches, "B1": rounds * batches, "C": rounds}
     sb = state_bytes(sc.blob)
-    h2d = {"A": table_bytes, "B": round(float(np.mean(distinct)) * sb) + 4 * N, "B1": sb + 4 * N, "C": N * table_bytes}
+    h2d = {"A": sb, "B": round(float(np.mean(distinct)) * sb) + 4 * N, "B1": sb + 4 * N, "C": N * sb}
     res = {}
     for arm in host:
         med = float(np.median(times[arm]))
