@@ -51,15 +51,15 @@ const Vmm &vmm() {
 }
 constexpr size_t k4G = (size_t)1 << 32;
 
-// device memory of `bytes` bytes at an address that is a multiple of 4 GiB
-bool alloc_aligned_4g(b2d_renderer *r, size_t bytes) {
+// device memory of `bytes` bytes at an address that is a multiple of 4 GiB (empty if there is none)
+Aligned4G alloc_aligned_4g(int device, size_t bytes) {
     const Vmm &v = vmm();
     if (v.ok && !getenv("B2D_NO_VMM")) {
         CUmemAllocationProp prop;
         std::memset(&prop, 0, sizeof prop);
         prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
         prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-        prop.location.id = r->device;
+        prop.location.id = device;
         size_t gran = 0;
         if (v.GetGranularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) == CUDA_SUCCESS && gran) {
             const size_t size = (bytes + gran - 1) / gran * gran;
@@ -72,12 +72,8 @@ bool alloc_aligned_4g(b2d_renderer *r, size_t bytes) {
                     acc.location = prop.location;
                     acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
                     if (v.Map(ptr, size, 0, h, 0) == CUDA_SUCCESS) {
-                        if (v.SetAccess(ptr, size, &acc, 1) == CUDA_SUCCESS) {
-                            r->d_lit_flats = reinterpret_cast<uint8_t *>(ptr);
-                            r->lit_flats_bytes = size;
-                            r->lit_flats_handle = (unsigned long long)h;
-                            return true;
-                        }
+                        if (v.SetAccess(ptr, size, &acc, 1) == CUDA_SUCCESS)
+                            return Aligned4G(reinterpret_cast<uint8_t *>(ptr), Aligned4GFree{size, (unsigned long long)h, nullptr});
                         v.Unmap(ptr, size);
                     }
                     v.Release(h);
@@ -88,24 +84,21 @@ bool alloc_aligned_4g(b2d_renderer *r, size_t bytes) {
     }
     // fall-back: a plain allocation 4 GiB larger than needed always contains an aligned address
     void *raw = nullptr;
-    if (cudaMalloc(&raw, bytes + k4G) != cudaSuccess) { cudaGetLastError(); return false; }
-    r->d_lit_flats_raw = static_cast<uint8_t *>(raw);
-    r->d_lit_flats = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(raw) + k4G - 1) & ~(uintptr_t)(k4G - 1));
-    r->lit_flats_bytes = 0;
-    return true;
+    if (cudaMalloc(&raw, bytes + k4G) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    return Aligned4G(reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(raw) + k4G - 1) & ~(uintptr_t)(k4G - 1)),
+                     Aligned4GFree{0, 0, raw});
+}
 }
 
-void free_aligned_4g(b2d_renderer *r) {
-    if (r->lit_flats_bytes) {
+void b2d::Aligned4GFree::operator()(uint8_t *p) const {
+    if (mapped) {
         const Vmm &v = vmm();
-        v.Unmap(reinterpret_cast<CUdeviceptr>(r->d_lit_flats), r->lit_flats_bytes);
-        v.Release((CUmemGenericAllocationHandle)r->lit_flats_handle);
-        v.AddressFree(reinterpret_cast<CUdeviceptr>(r->d_lit_flats), r->lit_flats_bytes);
-    } else if (r->d_lit_flats_raw) {
-        cudaFree(r->d_lit_flats_raw);
+        v.Unmap(reinterpret_cast<CUdeviceptr>(p), mapped);
+        v.Release((CUmemGenericAllocationHandle)handle);
+        v.AddressFree(reinterpret_cast<CUdeviceptr>(p), mapped);
+    } else {
+        cudaFree(raw);
     }
-    r->d_lit_flats = nullptr; r->d_lit_flats_raw = nullptr; r->lit_flats_bytes = 0;
-}
 }
 
 namespace b2d {
@@ -140,59 +133,34 @@ int guarded(Fn fn) {
     }
 }
 
-void free_renderer(b2d_renderer *r) {
-    if (!r) return;
-    cudaSetDevice(r->device);
-    for (int i = 0; i < 2; i++) {
-        if (r->d_index[i]) cudaFree(r->d_index[i]);
-        if (r->d_rgba[i]) cudaFree(r->d_rgba[i]);
-        if (r->rendered[i]) cudaEventDestroy(r->rendered[i]);
-        if (r->copied[i]) cudaEventDestroy(r->copied[i]);
-    }
-    for (cudaEvent_t e : r->prof_events) cudaEventDestroy(e);
-    if (r->h_poses) cudaFreeHost(r->h_poses);
-    if (r->render_stream) cudaStreamDestroy(r->render_stream);
-    for (int i = 0; i < 2; i++) if (r->copy_stream[i]) cudaStreamDestroy(r->copy_stream[i]);
-    for (int i = 0; i < 2; i++) {
-        if (r->d_work[i]) cudaFree(r->d_work[i]);
-        if (r->d_frames[i]) cudaFree(r->d_frames[i]);
-        if (r->walk_done[i]) cudaEventDestroy(r->walk_done[i]);
-        if (r->raster_done[i]) cudaEventDestroy(r->raster_done[i]);
-    }
-    if (r->d_poses) cudaFree(r->d_poses);
-    if (r->d_yslope) cudaFree(r->d_yslope);
-    if (r->d_skyrow) cudaFree(r->d_skyrow);
-    if (r->d_status) cudaFree(r->d_status);
-    if (r->d_masked) cudaFree(r->d_masked);
-    if (r->d_masked_counter) cudaFree(r->d_masked_counter);
-    if (r->masked_done) cudaEventDestroy(r->masked_done);
-    for (int i = 0; i < 2; i++) {
-        if (r->d_arena[i]) cudaFree(r->d_arena[i]);
-        if (r->d_states[i]) cudaFree(r->d_states[i]);
-        if (r->h_states[i]) cudaFreeHost(r->h_states[i]);
-        if (r->states_copied[i]) cudaEventDestroy(r->states_copied[i]);
-    }
-    if (r->d_slot_tables) cudaFree(r->d_slot_tables);
-    if (r->d_slot_maps) cudaFree(r->d_slot_maps);
-    if (r->d_lit) cudaFree(r->d_lit);
-    if (r->d_walk_static) cudaFree(r->d_walk_static);
-    free_aligned_4g(r);
-    if (r->d_blob) cudaFree(r->d_blob);
-    delete r;
+// A worklist slot's frames, worklist and events, created together: a failed call leaves the slot without any of them.
+int ensure_slot(const b2d_renderer *r, WorkSlot &s) {
+    if (s.frames) return B2D_OK;
+    DeviceBuf<FrameConst> frames; DeviceBuf<SegFrame> work;
+    Event walk_done, raster_done;
+    CU(allocate(frames, sizeof(FrameConst) * (size_t)r->max_batch));
+    CU(allocate(work, sizeof(SegFrame) * (size_t)r->max_batch * (size_t)r->stride));
+    CU(event_create(walk_done));
+    CU(event_create(raster_done));
+    s.frames = std::move(frames); s.work = std::move(work);
+    s.walk_done = std::move(walk_done); s.raster_done = std::move(raster_done);
+    return B2D_OK;
 }
 
-// Per-frame states: the two worklist slots' arenas of max_batch table sets, allocated by the first such call.
+// Per-frame states: the two worklist slots' arenas of max_batch table sets, allocated together by the first such call.
 int ensure_states(b2d_renderer *r) {
-    for (int i = 0; i < 2; i++)
-        if (!r->d_arena[i]) CU(cudaMalloc(&r->d_arena[i], (size_t)r->max_batch * r->state_tables.slot_bytes));
+    if (r->slot[0].arena) return B2D_OK;
+    DeviceBuf<uint8_t> arena[2];
+    for (auto &a : arena) CU(allocate(a, (size_t)r->max_batch * r->state_tables.slot_bytes));
+    for (int i = 0; i < 2; i++) r->slot[i].arena = std::move(arena[i]);
     return B2D_OK;
 }
 
 // the arena view of worklist slot `slot` (after ensure_states)
 StateTables slot_tables(const b2d_renderer *r, int slot) {
     StateTables t = r->state_tables;
-    t.base = r->d_arena[slot];
-    t.frame_slot = r->d_states[slot] + (size_t)r->max_batch * r->layout.words;
+    t.base = r->slot[slot].arena.get();
+    t.frame_slot = r->slot[slot].states.get() + (size_t)r->max_batch * r->layout.words;
     return t;
 }
 
@@ -200,9 +168,9 @@ StateTables slot_tables(const b2d_renderer *r, int slot) {
 // the slot's own table set
 DeviceScene slot_scene(const b2d_renderer *r, int slot) {
     DeviceScene d = r->ds;
-    if (!r->d_slot_tables) return d;
+    const uint8_t *set = r->slot[slot].tables.get();
+    if (!set) return d;
     const StateTables &t = r->state_tables;
-    const uint8_t *set = r->d_slot_tables + (size_t)slot * t.slot_bytes;
     d.tex = reinterpret_cast<const TexRec *>(set);
     d.sectors = reinterpret_cast<const SectorRec *>(set + t.off_sectors);
     d.segs = reinterpret_cast<const SegRec *>(set + t.off_segs);
@@ -220,17 +188,17 @@ DeviceScene slot_scene(const b2d_renderer *r, int slot) {
 int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background = false,
                    const uint32_t *frame_states = nullptr) {
     const int slot = (int)(r->next_ticket & 1);
-    if (!r->slot_rastered[slot]) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
-    if (frame_states) {
-        int rc = ensure_states(r);
-        if (rc != B2D_OK) return rc;
-    }
-    const bool restate = !frame_states && r->d_slot_tables && r->slot_state[slot] != r->state;
+    WorkSlot &s = r->slot[slot];
+    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
+    int rc = frame_states ? ensure_states(r) : B2D_OK;
+    if (rc == B2D_OK) rc = ensure_slot(r, s);
+    if (rc != B2D_OK) return rc;
+    const bool restate = !frame_states && s.tables && s.state != r->state;
     const size_t words = r->layout.words;
     int nstates = 0;
     if (frame_states || restate) {
-        CU(cudaEventSynchronize(r->states_copied[slot]));      // the copy issued two batches ago has read the staging
-        uint32_t *hs = r->h_states[slot], *hslot = hs + (size_t)r->max_batch * words;
+        CU(cudaEventSynchronize(s.states_copied.get()));     // the copy issued two batches ago has read the staging
+        uint32_t *hs = s.h_states.get(), *hslot = hs + (size_t)r->max_batch * words;
         if (restate) {
             std::memcpy(hs, r->state.data(), 4 * words);
             nstates = 1;
@@ -246,46 +214,37 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
             }
         }
     }
-    if (!r->d_frames[slot]) {
-        CU(cudaMalloc(&r->d_frames[slot], sizeof(FrameConst) * (size_t)r->max_batch));
-        CU(cudaMalloc(&r->d_work[slot], sizeof(SegFrame) * (size_t)r->max_batch * (size_t)r->stride));
-    }
-    if (!r->walk_done[slot]) {
-        CU(cudaEventCreateWithFlags(&r->walk_done[slot], cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&r->raster_done[slot], cudaEventDisableTiming));
-    } else {
-        CU(cudaStreamWaitEvent(stream, r->raster_done[slot], 0));      // the raster that last read this slot
-    }
+    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
     const StateTables stt = frame_states ? slot_tables(r, slot) : StateTables{};
     if (nstates) {
-        uint32_t *hs = r->h_states[slot];
-        CU(cudaMemcpyAsync(r->d_states[slot], hs, 4 * words * (size_t)nstates, cudaMemcpyHostToDevice, stream));
+        uint32_t *hs = s.h_states.get();
+        CU(cudaMemcpyAsync(s.states.get(), hs, 4 * words * (size_t)nstates, cudaMemcpyHostToDevice, stream));
         if (frame_states)
             CU(cudaMemcpyAsync(const_cast<uint32_t *>(stt.frame_slot), hs + (size_t)r->max_batch * words, 4 * (size_t)n,
                                cudaMemcpyHostToDevice, stream));
-        CU(cudaEventRecord(r->states_copied[slot], stream));
-        uint8_t *sets = frame_states ? r->d_arena[slot] : r->d_slot_tables + (size_t)slot * r->state_tables.slot_bytes;
-        CU(launch_state_tables(r->src, r->d_states[slot], (uint32_t)words, nstates, sets, r->state_tables, stream));
+        CU(cudaEventRecord(s.states_copied.get(), stream));
+        uint8_t *sets = (frame_states ? s.arena : s.tables).get();
+        CU(launch_state_tables(r->src, s.states.get(), (uint32_t)words, nstates, sets, r->state_tables, stream));
         r->launches += 1;
-        if (restate) r->slot_state[slot] = r->state;
+        if (restate) s.state = r->state;
     }
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    Event ev[2];
     if (r->profiling) {
-        for (auto &e : ev) CU(cudaEventCreate(&e));
-        CU(cudaEventRecord(ev[0], stream));
+        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
+        CU(cudaEventRecord(ev[0].get(), stream));
     }
-    CU(launch_walk(slot_scene(r, slot), r->view, d_poses, n, r->d_frames[slot], r->d_work[slot], r->stride, stream, background,
+    CU(launch_walk(slot_scene(r, slot), r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background,
                    frame_states ? &stt : nullptr));
     if (r->profiling) {
-        CU(cudaEventRecord(ev[1], stream));
-        for (auto e : ev) r->prof_events.push_back(e);
+        CU(cudaEventRecord(ev[1].get(), stream));
+        for (auto &e : ev) r->prof_events.push_back(std::move(e));
         r->prof_kinds.push_back(0);
     }
-    CU(cudaEventRecord(r->walk_done[slot], stream));
-    r->slot_n[slot] = n;
-    r->slot_states[slot] = frame_states != nullptr;
-    r->slot_ticket[slot] = r->next_ticket;
-    r->slot_rastered[slot] = false;
+    CU(cudaEventRecord(s.walk_done.get(), stream));
+    s.n = n;
+    s.per_frame = frame_states != nullptr;
+    s.ticket = r->next_ticket;
+    s.rastered = false;
     r->last_slot = slot;
     r->launches += 1;
     *ticket_out = r->next_ticket++;
@@ -294,31 +253,31 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
 
 int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
     const int slot = (int)(ticket & 1);
-    if (ticket < 0 || r->slot_ticket[slot] != ticket || r->slot_rastered[slot])
-        return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
-    CU(cudaStreamWaitEvent(stream, r->walk_done[slot], 0));
+    WorkSlot &s = r->slot[slot];
+    if (ticket < 0 || s.ticket != ticket || s.rastered) return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
+    CU(cudaStreamWaitEvent(stream, s.walk_done.get(), 0));
     if (r->ds.masked_list) {
         // one arena of deferred masked entries per renderer: rasters that use it run one after the other (each fills the
         // machine on its own, so nothing is lost), whatever streams they were enqueued on
-        CU(cudaStreamWaitEvent(stream, r->masked_done, 0));
-        CU(cudaMemsetAsync(r->d_masked_counter, 0, sizeof(uint32_t), stream));
+        CU(cudaStreamWaitEvent(stream, r->masked_done.get(), 0));
+        CU(cudaMemsetAsync(r->d_masked_counter.get(), 0, sizeof(uint32_t), stream));
     }
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    Event ev[2];
     if (r->profiling) {
-        for (auto &e : ev) CU(cudaEventCreate(&e));
-        CU(cudaEventRecord(ev[0], stream));
+        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
+        CU(cudaEventRecord(ev[0].get(), stream));
     }
-    const StateTables stt = r->slot_states[slot] ? slot_tables(r, slot) : StateTables{};
-    CU(launch_raster(slot_scene(r, slot), r->view, r->d_frames[slot], r->d_work[slot], r->stride, r->slot_n[slot], d_index, d_rgba, stream,
-                     r->slot_states[slot] ? &stt : nullptr));
+    const StateTables stt = s.per_frame ? slot_tables(r, slot) : StateTables{};
+    CU(launch_raster(slot_scene(r, slot), r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba, stream,
+                     s.per_frame ? &stt : nullptr));
     if (r->profiling) {
-        CU(cudaEventRecord(ev[1], stream));
-        for (auto e : ev) r->prof_events.push_back(e);
+        CU(cudaEventRecord(ev[1].get(), stream));
+        for (auto &e : ev) r->prof_events.push_back(std::move(e));
         r->prof_kinds.push_back(1);
     }
-    CU(cudaEventRecord(r->raster_done[slot], stream));
-    if (r->ds.masked_list) CU(cudaEventRecord(r->masked_done, stream));
-    r->slot_rastered[slot] = true;
+    CU(cudaEventRecord(s.raster_done.get(), stream));
+    if (r->ds.masked_list) CU(cudaEventRecord(r->masked_done.get(), stream));
+    s.rastered = true;
     r->launches += 1;
     return B2D_OK;
 }
@@ -651,21 +610,20 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
                                       (e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0"));
     if (device < 0 || device >= count) return fail(B2D_ERR_INVALID_ARG, "device index out of range");
     CU(cudaSetDevice(device));
-    b2d_renderer *r = new (std::nothrow) b2d_renderer();
+    std::unique_ptr<b2d_renderer> r(new (std::nothrow) b2d_renderer());
     if (!r) return fail(B2D_ERR_NO_MEMORY, "out of host memory");
     r->device = device;
     r->view = View{view->width, view->height, view->F, view->FY2};
     r->max_batch = max_batch;
     const uint32_t *h = reinterpret_cast<const uint32_t *>(s->blob.data());
     r->stride = (int)(h[H_NSEGS] + h[H_NSPRITES]) > 0 ? (int)(h[H_NSEGS] + h[H_NSPRITES]) : 1;   // worklist entries per frame
-    auto bail = [&](cudaError_t err, const char *what) { free_renderer(r); return cuda_fail(err, what); };
-#define CUR(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return bail(e_, #call); } while (0)
-    CUR(cudaMalloc(&r->d_blob, s->blob.size()));
-    CUR(cudaMemcpy(r->d_blob, s->blob.data(), s->blob.size(), cudaMemcpyHostToDevice));
+    CU(allocate(r->d_blob, s->blob.size()));
+    CU(cudaMemcpy(r->d_blob.get(), s->blob.data(), s->blob.size(), cudaMemcpyHostToDevice));
+    const uint8_t *db = r->d_blob.get();
     std::vector<uint32_t> ys((size_t)view->height);
     for (int y = 0; y < view->height; y++) ys[(size_t)y] = yslope_entry(y, r->view);
-    CUR(cudaMalloc(&r->d_yslope, ys.size() * 4));
-    CUR(cudaMemcpy(r->d_yslope, ys.data(), ys.size() * 4, cudaMemcpyHostToDevice));
+    CU(allocate(r->d_yslope, ys.size() * 4));
+    CU(cudaMemcpy(r->d_yslope.get(), ys.data(), ys.size() * 4, cudaMemcpyHostToDevice));
     {   // sky texture row per screen row (sky.frag:12-26 at pitch 0)
         std::vector<uint16_t> sr((size_t)view->height, 0);
         int32_t sky = (int32_t)h[H_SKY_TEX];
@@ -673,13 +631,13 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
             const TexRec *tr = reinterpret_cast<const TexRec *>(s->blob.data() + h[H_OFF_TEX]) + sky;
             for (int y = 0; y < view->height; y++) sr[(size_t)y] = (uint16_t)sky_row(y, view->height, (int32_t)tr->h);
         }
-        CUR(cudaMalloc(&r->d_skyrow, sr.size() * 2));
-        CUR(cudaMemcpy(r->d_skyrow, sr.data(), sr.size() * 2, cudaMemcpyHostToDevice));
+        CU(allocate(r->d_skyrow, sr.size() * 2));
+        CU(cudaMemcpy(r->d_skyrow.get(), sr.data(), sr.size() * 2, cudaMemcpyHostToDevice));
     }
     DeviceScene &d = r->ds;
-    d.verts = reinterpret_cast<const int32_t *>(r->d_blob + h[H_OFF_VERTS]);
-    d.nodes = reinterpret_cast<const NodeRec *>(r->d_blob + h[H_OFF_NODES]);
-    d.ssectors = reinterpret_cast<const SSectorRec *>(r->d_blob + h[H_OFF_SSECTORS]);
+    d.verts = reinterpret_cast<const int32_t *>(db + h[H_OFF_VERTS]);
+    d.nodes = reinterpret_cast<const NodeRec *>(db + h[H_OFF_NODES]);
+    d.ssectors = reinterpret_cast<const SSectorRec *>(db + h[H_OFF_SSECTORS]);
     {   // the walk kernel's traversal tables in the layout of its shared memory (one cp.async.bulk per CTA)
         const NodeRec *nodes = reinterpret_cast<const NodeRec *>(s->blob.data() + h[H_OFF_NODES]);
         std::vector<int32_t> img(8 * (size_t)h[H_NNODES] + 4 * (size_t)h[H_NSSECTORS]);
@@ -690,16 +648,16 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
         }
         if (h[H_NSSECTORS])
             std::memcpy(&img[8 * (size_t)h[H_NNODES]], s->blob.data() + h[H_OFF_SSECTORS], sizeof(SSectorRec) * h[H_NSSECTORS]);
-        CUR(cudaMalloc(&r->d_walk_static, img.size() * 4 + 16));
-        if (!img.empty()) CUR(cudaMemcpy(r->d_walk_static, img.data(), img.size() * 4, cudaMemcpyHostToDevice));
-        d.walk_static = r->d_walk_static;
+        CU(allocate(r->d_walk_static, img.size() * 4 + 16));
+        if (!img.empty()) CU(cudaMemcpy(r->d_walk_static.get(), img.data(), img.size() * 4, cudaMemcpyHostToDevice));
+        d.walk_static = r->d_walk_static.get();
     }
-    d.segs = reinterpret_cast<const SegRec *>(r->d_blob + h[H_OFF_SEGS]);
-    d.sectors = reinterpret_cast<const SectorRec *>(r->d_blob + h[H_OFF_SECTORS]);
-    d.tex = reinterpret_cast<const TexRec *>(r->d_blob + h[H_OFF_TEX]);
-    d.mids = reinterpret_cast<const MidRec *>(r->d_blob + h[H_OFF_MIDS]);
+    d.segs = reinterpret_cast<const SegRec *>(db + h[H_OFF_SEGS]);
+    d.sectors = reinterpret_cast<const SectorRec *>(db + h[H_OFF_SECTORS]);
+    d.tex = reinterpret_cast<const TexRec *>(db + h[H_OFF_TEX]);
+    d.mids = reinterpret_cast<const MidRec *>(db + h[H_OFF_MIDS]);
     d.nmids = (int32_t)h[H_NMIDS];
-    d.sprites = reinterpret_cast<const SpriteRec *>(r->d_blob + h[H_OFF_SPRITES]);
+    d.sprites = reinterpret_cast<const SpriteRec *>(db + h[H_OFF_SPRITES]);
     d.nsprites = (int32_t)h[H_NSPRITES];
     d.masked_list = nullptr; d.masked_counter = nullptr; d.masked_chunks = 0; d.masked_cap = 0;
     if (d.nmids > 0 || d.nsprites > 0) {
@@ -723,95 +681,93 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
         if (const char *env = getenv("B2D_MASKED_CHUNKS")) chunks = (size_t)strtoull(env, nullptr, 0);   // tests: force exhaustion
         if (chunks < 1) chunks = 1;
         d.masked_chunks = (uint32_t)chunks;
-        CUR(cudaMalloc(&r->d_masked, sizeof(uint32_t) * 33 * kMaskedChunk * chunks));
-        CUR(cudaMalloc(&r->d_masked_counter, sizeof(uint32_t)));
-        CUR(cudaMemset(r->d_masked_counter, 0, sizeof(uint32_t)));
-        CUR(cudaEventCreateWithFlags(&r->masked_done, cudaEventDisableTiming));
-        CUR(cudaEventRecord(r->masked_done, nullptr));
-        d.masked_list = r->d_masked;
-        d.masked_counter = r->d_masked_counter;
+        CU(allocate(r->d_masked, sizeof(uint32_t) * 33 * kMaskedChunk * chunks));
+        CU(allocate(r->d_masked_counter, sizeof(uint32_t)));
+        CU(cudaMemset(r->d_masked_counter.get(), 0, sizeof(uint32_t)));
+        CU(event_create(r->masked_done));
+        CU(cudaEventRecord(r->masked_done.get(), nullptr));
+        d.masked_list = r->d_masked.get();
+        d.masked_counter = r->d_masked_counter.get();
     }
-    d.texels = r->d_blob + h[H_OFF_TEXELS];
-    d.flats = r->d_blob + h[H_OFF_FLATS];
-    d.colormap = r->d_blob + h[H_OFF_COLORMAP];
-    d.palette = reinterpret_cast<const uint32_t *>(r->d_blob + h[H_OFF_PALETTE]);
+    d.texels = db + h[H_OFF_TEXELS];
+    d.flats = db + h[H_OFF_FLATS];
+    d.colormap = db + h[H_OFF_COLORMAP];
+    d.palette = reinterpret_cast<const uint32_t *>(db + h[H_OFF_PALETTE]);
     {   // pre-lit texel and flat planes: 32 x (texel bytes + flat bytes)
         const size_t tstride = (h[H_TEXEL_BYTES] + 255u) & ~(size_t)255, fstride = (size_t)h[H_NFLATS] * 4096u;
-        if (tstride * 33 > 0xFFFFFFFFull || fstride * 32 > 0xFFFFFFFFull) { free_renderer(r); return fail(B2D_ERR_INVALID_ARG, "level textures too large"); }
-        CUR(cudaMalloc(&r->d_lit, 33 * tstride + 256));                    // plane 32 of the texels: opacity
-        if (!alloc_aligned_4g(r, 32 * fstride + 256)) { free_renderer(r); return fail(B2D_ERR_NO_MEMORY, "no 4 GiB aligned device memory for the pre-lit flats"); }
-        CUR(launch_prelight_textures(d.colormap, d.texels, d.tex, (int)h[H_NTEX], r->d_lit, tstride, nullptr));
-        CUR(launch_prelight(d.colormap, d.flats, r->d_lit_flats, fstride, fstride, nullptr));
-        CUR(cudaDeviceSynchronize());
-        d.lit_texels = r->d_lit; d.lit_flats = r->d_lit_flats;           // low 32 address bits of lit_flats are zero
+        if (tstride * 33 > 0xFFFFFFFFull || fstride * 32 > 0xFFFFFFFFull) return fail(B2D_ERR_INVALID_ARG, "level textures too large");
+        CU(allocate(r->d_lit, 33 * tstride + 256));                    // plane 32 of the texels: opacity
+        r->d_lit_flats = alloc_aligned_4g(device, 32 * fstride + 256);
+        if (!r->d_lit_flats) return fail(B2D_ERR_NO_MEMORY, "no 4 GiB aligned device memory for the pre-lit flats");
+        CU(launch_prelight_textures(d.colormap, d.texels, d.tex, (int)h[H_NTEX], r->d_lit.get(), tstride, nullptr));
+        CU(launch_prelight(d.colormap, d.flats, r->d_lit_flats.get(), fstride, fstride, nullptr));
+        CU(cudaDeviceSynchronize());
+        d.lit_texels = r->d_lit.get(); d.lit_flats = r->d_lit_flats.get();     // low 32 address bits of lit_flats are zero
         d.lit_texel_stride = (uint32_t)tstride; d.lit_flat_stride = (uint32_t)fstride;
     }
-    d.yslope = r->d_yslope;
-    d.skyrow = r->d_skyrow;
-    CUR(cudaMalloc(&r->d_status, sizeof(int32_t)));
-    CUR(cudaMemset(r->d_status, 0, sizeof(int32_t)));
-    d.status_flag = r->d_status;
+    d.yslope = r->d_yslope.get();
+    d.skyrow = r->d_skyrow.get();
+    CU(allocate(r->d_status, sizeof(int32_t)));
+    CU(cudaMemset(r->d_status.get(), 0, sizeof(int32_t)));
+    d.status_flag = r->d_status.get();
     d.nverts = (int32_t)h[H_NVERTS]; d.nnodes = (int32_t)h[H_NNODES]; d.nss = (int32_t)h[H_NSSECTORS];
     d.nsegs = (int32_t)h[H_NSEGS]; d.nsectors = (int32_t)h[H_NSECTORS]; d.ntex = (int32_t)h[H_NTEX];
     d.nflats = (int32_t)h[H_NFLATS]; d.sky_tex = (int32_t)h[H_SKY_TEX];
     d.root = h[H_ROOT];
     d.invF = (uint32_t)(4294967296ULL / (uint64_t)view->F);
-    if (d.nsegs + d.nsprites > 65535) { free_renderer(r); return fail(B2D_ERR_INVALID_ARG, "level has more than 65535 segs + sprites"); }
-    if (walk_smem_per_warp(d) > 227 * 1024) { free_renderer(r); return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory"); }
+    if (d.nsegs + d.nsprites > 65535) return fail(B2D_ERR_INVALID_ARG, "level has more than 65535 segs + sprites");
+    if (walk_smem_per_warp(d) > 227 * 1024) return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory");
     if (scene_is_timed(s->blob.data())) {
         r->h_blob = s->blob;
         try {
             r->layout = state_layout(r->h_blob.data());
         } catch (const std::exception &ex) {
-            free_renderer(r);
             return fail(B2D_ERR_INVALID_ARG, ex.what());
         }
         const uint8_t *blob = r->h_blob.data();
         const StateLayout &L = r->layout;
         const size_t words = L.words, mb = (size_t)max_batch;
         // the state rule reads the blob's rest-state sections and the two slot maps
-        CUR(cudaMalloc(&r->d_slot_maps, 4 * (L.sector_slots.size() + L.mid_seg.size()) + 4));
-        CUR(cudaMemcpy(r->d_slot_maps, L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
-        CUR(cudaMemcpy(r->d_slot_maps + L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
+        CU(allocate(r->d_slot_maps, 4 * (L.sector_slots.size() + L.mid_seg.size()) + 4));
+        CU(cudaMemcpy(r->d_slot_maps.get(), L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(r->d_slot_maps.get() + L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
         StateSrc &src = r->src = state_src(blob, L);
-        auto on_device = [&](auto p) { return reinterpret_cast<decltype(p)>(r->d_blob + (reinterpret_cast<const uint8_t *>(p) - blob)); };
+        auto on_device = [&](auto p) { return reinterpret_cast<decltype(p)>(db + (reinterpret_cast<const uint8_t *>(p) - blob)); };
         src.tex = on_device(src.tex); src.sectors = on_device(src.sectors); src.segs = on_device(src.segs);
         src.sprites = on_device(src.sprites); src.mids = on_device(src.mids); src.anim = on_device(src.anim);
         src.flat_anim = on_device(src.flat_anim); src.segdyn = on_device(src.segdyn);
-        src.sector_slots = r->d_slot_maps;
-        src.mid_seg = reinterpret_cast<const int32_t *>(r->d_slot_maps + L.sector_slots.size());
+        src.sector_slots = r->d_slot_maps.get();
+        src.mid_seg = reinterpret_cast<const int32_t *>(r->d_slot_maps.get() + L.sector_slots.size());
         StateTables &t = r->state_tables;              // one table set: [tex | sectors | segs | sprites | mids], 256 B aligned
         t.slot_bytes = (uint32_t)((state_table_bytes(blob) + 255) & ~(size_t)255);
         t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
         t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
         t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
         t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
-        CUR(cudaMalloc(&r->d_slot_tables, 2 * (size_t)t.slot_bytes));
-        for (int i = 0; i < 2; i++) {
-            CUR(cudaMalloc(&r->d_states[i], 4 * mb * (words + 1)));
-            CUR(cudaMallocHost(&r->h_states[i], 4 * mb * (words + 1)));
-            CUR(cudaEventCreateWithFlags(&r->states_copied[i], cudaEventDisableTiming));
+        for (WorkSlot &sl : r->slot) {
+            CU(allocate(sl.tables, t.slot_bytes));
+            CU(allocate(sl.states, 4 * mb * (words + 1)));
+            CU(allocate(sl.h_states, 4 * mb * (words + 1)));
+            CU(event_create(sl.states_copied));
         }
         // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306).  The
         // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0.
         r->state.assign(words, 0);
         compact_state(blob, L, 0, nullptr, nullptr, r->state.data());
-        CUR(cudaMemcpy(r->d_states[0], r->state.data(), 4 * words, cudaMemcpyHostToDevice));
-        for (int i = 0; i < 2; i++) {
-            CUR(launch_state_tables(r->src, r->d_states[0], (uint32_t)words, 1, r->d_slot_tables + i * (size_t)t.slot_bytes, t, nullptr));
-            r->slot_state[i] = r->state;
+        CU(cudaMemcpy(r->slot[0].states.get(), r->state.data(), 4 * words, cudaMemcpyHostToDevice));
+        for (WorkSlot &sl : r->slot) {
+            CU(launch_state_tables(r->src, r->slot[0].states.get(), (uint32_t)words, 1, sl.tables.get(), t, nullptr));
+            sl.state = r->state;
         }
-        CUR(cudaDeviceSynchronize());
+        CU(cudaDeviceSynchronize());
     }
-    CUR(cudaMalloc(&r->d_poses, sizeof(Pose) * (size_t)max_batch));
-    CUR(cudaMalloc(&r->d_frames[0], sizeof(FrameConst) * (size_t)max_batch));
-    CUR(cudaMalloc(&r->d_work[0], sizeof(SegFrame) * (size_t)max_batch * (size_t)r->stride));
-#undef CUR
-    *out = r;
-    return B2D_OK;
+    CU(allocate(r->d_poses, sizeof(Pose) * (size_t)max_batch));
+    int rc = ensure_slot(r.get(), r->slot[0]);
+    if (rc == B2D_OK) *out = r.release();
+    return rc;
 }
 
-void b2d_renderer_destroy(b2d_renderer *r) { free_renderer(r); }
+void b2d_renderer_destroy(b2d_renderer *r) { delete r; }
 
 // The renderer's own state is host data: the setters enqueue nothing (the stream is kept for ABI compatibility), and the
 // next plain batch of each worklist slot expands it into the slot's table set.
@@ -857,8 +813,8 @@ int b2d_renderer_status(b2d_renderer *r, int32_t *bits_out) {
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
     int32_t status = 0;
-    CU(cudaMemcpy(&status, r->d_status, sizeof status, cudaMemcpyDeviceToHost));
-    if (status) CU(cudaMemset(r->d_status, 0, sizeof(int32_t)));
+    CU(cudaMemcpy(&status, r->d_status.get(), sizeof status, cudaMemcpyDeviceToHost));
+    if (status) CU(cudaMemset(r->d_status.get(), 0, sizeof(int32_t)));
     *bits_out = status;
     return B2D_OK;
 }
@@ -942,18 +898,25 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const u
     if (n == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
-    if (!r->render_stream) {
-        CU(cudaStreamCreateWithFlags(&r->render_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; i++) CU(cudaStreamCreateWithFlags(&r->copy_stream[i], cudaStreamNonBlocking));
+    if (!r->host) {       // created whole, or not at all
+        std::unique_ptr<HostStaging> staging(new (std::nothrow) HostStaging());
+        if (!staging) return fail(B2D_ERR_NO_MEMORY, "out of host memory");
+        CU(stream_create(staging->render_stream));
         for (int i = 0; i < 2; i++) {
-            CU(cudaEventCreateWithFlags(&r->rendered[i], cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&r->copied[i], cudaEventDisableTiming));
-            CU(cudaMalloc(&r->d_index[i], npix * (size_t)r->max_batch));
+            CU(stream_create(staging->copy_stream[i]));
+            CU(event_create(staging->rendered[i]));
+            CU(event_create(staging->copied[i]));
+            CU(allocate(staging->index[i], npix * (size_t)r->max_batch));
         }
-        CU(cudaMallocHost(&r->h_poses, sizeof(Pose) * (size_t)r->max_batch * 2));
+        CU(allocate(staging->poses, sizeof(Pose) * (size_t)r->max_batch * 2));
+        r->host = std::move(staging);
     }
-    if (rgba_fb && !r->d_rgba[0])
-        for (int i = 0; i < 2; i++) CU(cudaMalloc(&r->d_rgba[i], npix * 4 * (size_t)r->max_batch));
+    HostStaging &hs = *r->host;
+    if (rgba_fb && !hs.rgba[0]) {
+        std::array<DeviceBuf<uint32_t>, 2> rgba;
+        for (auto &buf : rgba) CU(allocate(buf, npix * 4 * (size_t)r->max_batch));
+        hs.rgba = std::move(rgba);
+    }
     // Double-buffered pipeline: batch b renders into buffer b&1 on render_stream while the copy
     // stream drains buffer (b-1)&1 to the caller's host memory.
     size_t done = 0;
@@ -961,28 +924,29 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const u
     while (done < n) {
         const int cnt = (int)(n - done < (size_t)r->max_batch ? n - done : (size_t)r->max_batch);
         const int buf = b & 1;
-        if (b >= 2) CU(cudaEventSynchronize(r->copied[buf]));       // buffer + pose slot free again
-        Pose *hp = r->h_poses + (size_t)buf * r->max_batch;
+        if (b >= 2) CU(cudaEventSynchronize(hs.copied[buf].get()));       // buffer + pose slot free again
+        Pose *hp = hs.poses.get() + (size_t)buf * r->max_batch;
         std::memcpy(hp, poses + done, sizeof(Pose) * (size_t)cnt);
-        CU(cudaMemcpyAsync(r->d_poses, hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, r->render_stream));
-        int rc = enqueue_frames(r, r->d_poses, cnt, r->d_index[buf], rgba_fb ? r->d_rgba[buf] : nullptr, r->render_stream,
+        cudaStream_t rs = hs.render_stream.get(), cs = hs.copy_stream[buf].get();
+        CU(cudaMemcpyAsync(r->d_poses.get(), hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, rs));
+        int rc = enqueue_frames(r, r->d_poses.get(), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs,
                                 frame_states ? frame_states + done * r->layout.words : nullptr);
         if (rc != B2D_OK) return rc;
-        CU(cudaEventRecord(r->rendered[buf], r->render_stream));
-        CU(cudaStreamWaitEvent(r->copy_stream[buf], r->rendered[buf], 0));
-        CU(cudaMemcpyAsync(index_fb + done * npix, r->d_index[buf], npix * (size_t)cnt, cudaMemcpyDeviceToHost, r->copy_stream[buf]));
+        CU(cudaEventRecord(hs.rendered[buf].get(), rs));
+        CU(cudaStreamWaitEvent(cs, hs.rendered[buf].get(), 0));
+        CU(cudaMemcpyAsync(index_fb + done * npix, hs.index[buf].get(), npix * (size_t)cnt, cudaMemcpyDeviceToHost, cs));
         if (rgba_fb)
-            CU(cudaMemcpyAsync(rgba_fb + done * npix, r->d_rgba[buf], npix * 4 * (size_t)cnt, cudaMemcpyDeviceToHost, r->copy_stream[buf]));
-        CU(cudaEventRecord(r->copied[buf], r->copy_stream[buf]));
+            CU(cudaMemcpyAsync(rgba_fb + done * npix, hs.rgba[buf].get(), npix * 4 * (size_t)cnt, cudaMemcpyDeviceToHost, cs));
+        CU(cudaEventRecord(hs.copied[buf].get(), cs));
         done += (size_t)cnt;
         b++;
     }
-    for (int i = 0; i < 2; i++) CU(cudaStreamSynchronize(r->copy_stream[i]));
-    CU(cudaStreamSynchronize(r->render_stream));
+    for (auto &st : hs.copy_stream) CU(cudaStreamSynchronize(st.get()));
+    CU(cudaStreamSynchronize(hs.render_stream.get()));
     int32_t status = 0;
-    CU(cudaMemcpy(&status, r->d_status, sizeof status, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&status, r->d_status.get(), sizeof status, cudaMemcpyDeviceToHost));
     if (status) {
-        CU(cudaMemset(r->d_status, 0, sizeof(int32_t)));
+        CU(cudaMemset(r->d_status.get(), 0, sizeof(int32_t)));
         return fail(B2D_ERR_INVALID_ARG, status & kStatusStackOverflow ? "BSP traversal stack overflow (tree deeper than 128 pending nodes): frames incomplete"
                                             : (status & kStatusNoTermination ? "BSP traversal did not terminate (cyclic node graph): frames incomplete"
                                               : (status & kStatusMaskedFull ? "more masked middle textures / sprites deferred in one 32-column strip than the renderer holds (min(level total, 128)): frames incomplete"
@@ -1051,11 +1015,11 @@ int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *
     if (!r || !counts_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n exceeds max_batch");
     const int slot = r->last_slot;
-    if (!r->d_frames[slot] || n > (size_t)r->slot_n[slot]) return fail(B2D_ERR_INVALID_ARG, "n exceeds the frames of the last walked batch");
+    if (!r->slot[slot].frames || n > (size_t)r->slot[slot].n) return fail(B2D_ERR_INVALID_ARG, "n exceeds the frames of the last walked batch");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
     std::vector<FrameConst> frames(n);
-    CU(cudaMemcpy(frames.data(), r->d_frames[slot], sizeof(FrameConst) * n, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(frames.data(), r->slot[slot].frames.get(), sizeof(FrameConst) * n, cudaMemcpyDeviceToHost));
     std::vector<SegFrame> work;
     for (size_t i = 0; i < n; i++) {
         counts_out[i] = frames[i].status ? -frames[i].status : frames[i].count;
@@ -1063,7 +1027,7 @@ int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *
         size_t c = frames[i].count > 0 ? (size_t)frames[i].count : 0;
         if (c > (size_t)r->stride) c = (size_t)r->stride;
         work.resize(c);
-        if (c) CU(cudaMemcpy(work.data(), r->d_work[slot] + i * (size_t)r->stride, sizeof(SegFrame) * c, cudaMemcpyDeviceToHost));
+        if (c) CU(cudaMemcpy(work.data(), r->slot[slot].work.get() + i * (size_t)r->stride, sizeof(SegFrame) * c, cudaMemcpyDeviceToHost));
         for (size_t k = 0; k < c && k < stride; k++) seg_ids_out[i * stride + k] = work[k].seg;
     }
     return B2D_OK;
@@ -1072,7 +1036,7 @@ int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *
 int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
     if (!r || !slots_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     const int slot = r->last_slot;
-    if (!r->slot_states[slot] || n > (size_t)r->slot_n[slot])
+    if (!r->slot[slot].per_frame || n > (size_t)r->slot[slot].n)
         return fail(B2D_ERR_INVALID_ARG, "the last walked batch has no per-frame states or fewer than n frames");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
@@ -1095,14 +1059,13 @@ int b2d_profile_read(b2d_renderer *r, double *walk_ms, double *raster_ms, int64_
     int64_t nb = 0;
     for (size_t i = 0; i + 1 < r->prof_events.size(); i += 2) {
         float a = 0.f;
-        CU(cudaEventElapsedTime(&a, r->prof_events[i], r->prof_events[i + 1]));
+        CU(cudaEventElapsedTime(&a, r->prof_events[i].get(), r->prof_events[i + 1].get()));
         if (r->prof_kinds[i / 2] == 0) w += a; else { ra += a; nb++; }
     }
     if (walk_ms) *walk_ms = w;
     if (raster_ms) *raster_ms = ra;
     if (batches) *batches = nb;
     r->prof_kinds.clear();
-    for (cudaEvent_t e : r->prof_events) cudaEventDestroy(e);
     r->prof_events.clear();
     return B2D_OK;
 }

@@ -147,16 +147,16 @@ struct b2d_comm {
     void *reg[2] = {nullptr, nullptr};
     ncclWindow_t win[2] = {nullptr, nullptr};
     const char *registration = "none";
-    cudaStream_t render_stream = nullptr, gather_stream = nullptr, consume_stream = nullptr, walk_stream = nullptr;
+    Stream render_stream, gather_stream, consume_stream, walk_stream;
     // copy-engine transport (B2D_GATHER=ce): every rank pushes its slice into the peers' buffers with cudaMemcpyAsync over
     // CUDA-IPC mappings -- no SM is used for the exchange; two tiny NCCL all-reduces per chunk order it across ranks
     bool ce = false;
     std::vector<uint8_t *> peer[2];                 // [buffer][rank]: that rank's buffer as mapped here (own rank: buf[b])
-    std::vector<cudaStream_t> push_stream;          // one per peer
-    std::vector<cudaEvent_t> push_done;
-    cudaEvent_t push_go = nullptr;
-    int32_t *d_token = nullptr;
-    Pose *d_poses = nullptr, *h_poses = nullptr;
+    std::vector<Stream> push_stream;                // one per peer
+    std::vector<Event> push_done;
+    Event push_go;
+    DeviceBuf<int32_t> d_token;
+    DeviceBuf<Pose> d_poses; PinnedBuf<Pose> h_poses;
     size_t poses_cap = 0;
 };
 
@@ -223,14 +223,13 @@ int ensure_buffers(b2d_comm *c, size_t bytes) {
             B2D_CU(cudaIpcGetMemHandle(&h, c->buf[i]));
             std::memcpy(&mine[(size_t)i * hb], &h, hb);
         }
-        uint8_t *d_h = nullptr;
-        B2D_CU(cudaMalloc(&d_h, all.size()));
-        B2D_CU(cudaMemcpy(d_h + (size_t)c->rank * 2 * hb, mine.data(), 2 * hb, cudaMemcpyHostToDevice));
-        int nrc = n.AllGather(d_h + (size_t)c->rank * 2 * hb, d_h, 2 * hb, kNcclUint8, c->comm, c->gather_stream);
-        if (nrc != 0) { cudaFree(d_h); return nccl_fail(nrc, "ncclAllGather (ipc handles)"); }
-        B2D_CU(cudaStreamSynchronize(c->gather_stream));
-        B2D_CU(cudaMemcpy(all.data(), d_h, all.size(), cudaMemcpyDeviceToHost));
-        cudaFree(d_h);
+        DeviceBuf<uint8_t> d_h;
+        B2D_CU(allocate(d_h, all.size()));
+        B2D_CU(cudaMemcpy(d_h.get() + (size_t)c->rank * 2 * hb, mine.data(), 2 * hb, cudaMemcpyHostToDevice));
+        int nrc = n.AllGather(d_h.get() + (size_t)c->rank * 2 * hb, d_h.get(), 2 * hb, kNcclUint8, c->comm, c->gather_stream.get());
+        if (nrc != 0) return nccl_fail(nrc, "ncclAllGather (ipc handles)");
+        B2D_CU(cudaStreamSynchronize(c->gather_stream.get()));
+        B2D_CU(cudaMemcpy(all.data(), d_h.get(), all.size(), cudaMemcpyDeviceToHost));
         int32_t mapped = 1;
         for (int i = 0; i < 2; i++) {
             c->peer[i].assign((size_t)c->world, nullptr);
@@ -244,14 +243,14 @@ int ensure_buffers(b2d_comm *c, size_t bytes) {
             }
         }
         // every rank must have mapped every peer, or nobody uses the mappings (minimum over ranks = sum of the failures == 0)
-        int32_t failures = mapped ? 0 : 1, *d_flag = nullptr;
-        B2D_CU(cudaMalloc(&d_flag, sizeof(int32_t)));
-        B2D_CU(cudaMemcpy(d_flag, &failures, sizeof failures, cudaMemcpyHostToDevice));
-        nrc = n.AllReduce(d_flag, d_flag, 1, kNcclInt32, kNcclSum, c->comm, c->gather_stream);
-        if (nrc != 0) { cudaFree(d_flag); return nccl_fail(nrc, "ncclAllReduce (ipc agreement)"); }
-        B2D_CU(cudaStreamSynchronize(c->gather_stream));
-        B2D_CU(cudaMemcpy(&failures, d_flag, sizeof failures, cudaMemcpyDeviceToHost));
-        cudaFree(d_flag);
+        int32_t failures = mapped ? 0 : 1;
+        DeviceBuf<int32_t> d_flag;
+        B2D_CU(allocate(d_flag, sizeof(int32_t)));
+        B2D_CU(cudaMemcpy(d_flag.get(), &failures, sizeof failures, cudaMemcpyHostToDevice));
+        nrc = n.AllReduce(d_flag.get(), d_flag.get(), 1, kNcclInt32, kNcclSum, c->comm, c->gather_stream.get());
+        if (nrc != 0) return nccl_fail(nrc, "ncclAllReduce (ipc agreement)");
+        B2D_CU(cudaStreamSynchronize(c->gather_stream.get()));
+        B2D_CU(cudaMemcpy(&failures, d_flag.get(), sizeof failures, cudaMemcpyDeviceToHost));
         if (failures) {
             for (int i = 0; i < 2; i++) {
                 for (size_t q = 0; q < c->peer[i].size(); q++)
@@ -263,17 +262,20 @@ int ensure_buffers(b2d_comm *c, size_t bytes) {
             c->buf_bytes = bytes;
             return B2D_OK;
         }
-        if (c->push_stream.empty()) {
-            c->push_stream.resize((size_t)c->world, nullptr);
-            c->push_done.resize((size_t)c->world, nullptr);
+        if (c->push_stream.empty()) {       // created whole, or not at all
+            std::vector<Stream> push_stream((size_t)c->world);
+            std::vector<Event> push_done((size_t)c->world);
+            Event push_go; DeviceBuf<int32_t> d_token;
             for (int q = 0; q < c->world; q++) {
                 if (q == c->rank) continue;
-                B2D_CU(cudaStreamCreateWithFlags(&c->push_stream[(size_t)q], cudaStreamNonBlocking));
-                B2D_CU(cudaEventCreateWithFlags(&c->push_done[(size_t)q], cudaEventDisableTiming));
+                B2D_CU(stream_create(push_stream[(size_t)q]));
+                B2D_CU(event_create(push_done[(size_t)q]));
             }
-            B2D_CU(cudaEventCreateWithFlags(&c->push_go, cudaEventDisableTiming));
-            B2D_CU(cudaMalloc(&c->d_token, sizeof(int32_t)));
-            B2D_CU(cudaMemset(c->d_token, 0, sizeof(int32_t)));
+            B2D_CU(event_create(push_go));
+            B2D_CU(allocate(d_token, sizeof(int32_t)));
+            B2D_CU(cudaMemset(d_token.get(), 0, sizeof(int32_t)));
+            c->push_stream = std::move(push_stream); c->push_done = std::move(push_done);
+            c->push_go = std::move(push_go); c->d_token = std::move(d_token);
         }
         c->registration = "copy engines: cudaMemcpyAsync over CUDA-IPC peer mappings";
     }
@@ -285,19 +287,19 @@ int ensure_buffers(b2d_comm *c, size_t bytes) {
 int ce_gather(b2d_comm *c, int b, size_t slice_off, size_t bytes) {
     Nccl &n = nccl();
     // 1. every rank's buffer b is free again (each rank enqueues this after the event that says so locally)
-    B2D_NC(n.AllReduce(c->d_token, c->d_token, 1, kNcclInt32, kNcclSum, c->comm, c->gather_stream));
-    B2D_CU(cudaEventRecord(c->push_go, c->gather_stream));
+    B2D_NC(n.AllReduce(c->d_token.get(), c->d_token.get(), 1, kNcclInt32, kNcclSum, c->comm, c->gather_stream.get()));
+    B2D_CU(cudaEventRecord(c->push_go.get(), c->gather_stream.get()));
     // 2. push my slice into every peer's buffer, one stream (one copy engine queue) per peer
     for (int k = 1; k < c->world; k++) {
         const int q = (c->rank + k) % c->world;                        // stagger the targets across ranks
-        cudaStream_t ps = c->push_stream[(size_t)q];
-        B2D_CU(cudaStreamWaitEvent(ps, c->push_go, 0));
+        cudaStream_t ps = c->push_stream[(size_t)q].get();
+        B2D_CU(cudaStreamWaitEvent(ps, c->push_go.get(), 0));
         B2D_CU(cudaMemcpyAsync(c->peer[b][(size_t)q] + slice_off, c->buf[b] + slice_off, bytes, cudaMemcpyDeviceToDevice, ps));
-        B2D_CU(cudaEventRecord(c->push_done[(size_t)q], ps));
-        B2D_CU(cudaStreamWaitEvent(c->gather_stream, c->push_done[(size_t)q], 0));
+        B2D_CU(cudaEventRecord(c->push_done[(size_t)q].get(), ps));
+        B2D_CU(cudaStreamWaitEvent(c->gather_stream.get(), c->push_done[(size_t)q].get(), 0));
     }
     // 3. everybody's pushes have landed
-    B2D_NC(n.AllReduce(c->d_token, c->d_token, 1, kNcclInt32, kNcclSum, c->comm, c->gather_stream));
+    B2D_NC(n.AllReduce(c->d_token.get(), c->d_token.get(), 1, kNcclInt32, kNcclSum, c->comm, c->gather_stream.get()));
     return B2D_OK;
 }
 
@@ -328,10 +330,10 @@ int b2d_comm_create(const uint8_t id[B2D_COMM_ID_BYTES], int rank, int world, in
     std::memcpy(&uid, id, sizeof uid);
     int rc = n.CommInitRank(&c->comm, world, uid, rank);
     if (rc != 0) { delete c; return nccl_fail(rc, "ncclCommInitRank"); }
-    cudaError_t e = cudaStreamCreateWithFlags(&c->render_stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->gather_stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->consume_stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->walk_stream, cudaStreamNonBlocking);
+    cudaError_t e = stream_create(c->render_stream);
+    if (e == cudaSuccess) e = stream_create(c->gather_stream);
+    if (e == cudaSuccess) e = stream_create(c->consume_stream);
+    if (e == cudaSuccess) e = stream_create(c->walk_stream);
     if (e != cudaSuccess) { b2d_comm_destroy(c); return b2d::cuda_fail(e, "cudaStreamCreate"); }
     *out = c;
     return B2D_OK;
@@ -342,18 +344,8 @@ void b2d_comm_destroy(b2d_comm *c) {
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
     release_buffers(c);
-    if (c->d_poses) cudaFree(c->d_poses);
-    if (c->h_poses) cudaFreeHost(c->h_poses);
-    if (c->render_stream) cudaStreamDestroy(c->render_stream);
-    if (c->gather_stream) cudaStreamDestroy(c->gather_stream);
-    if (c->consume_stream) cudaStreamDestroy(c->consume_stream);
-    if (c->walk_stream) cudaStreamDestroy(c->walk_stream);
-    for (cudaStream_t ps : c->push_stream) if (ps) cudaStreamDestroy(ps);
-    for (cudaEvent_t e : c->push_done) if (e) cudaEventDestroy(e);
-    if (c->push_go) cudaEventDestroy(c->push_go);
-    if (c->d_token) cudaFree(c->d_token);
     if (c->comm) nccl().CommDestroy(c->comm);
-    delete c;
+    delete c;                               // the streams, events and pose buffers, on this device
 }
 
 int b2d_comm_info(const b2d_comm *c, int *rank_out, int *world_out, int *nccl_version_out) {
@@ -399,97 +391,97 @@ int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size
     if (rc != B2D_OK) return rc;
     // this rank's block of poses, padded by repeating the last pose of the list, on the device in one copy
     if (c->poses_cap < per) {
-        if (c->d_poses) cudaFree(c->d_poses);
-        if (c->h_poses) cudaFreeHost(c->h_poses);
-        c->d_poses = nullptr; c->h_poses = nullptr; c->poses_cap = 0;
-        B2D_CU(cudaMalloc(&c->d_poses, per * sizeof(Pose)));
-        B2D_CU(cudaMallocHost(&c->h_poses, per * sizeof(Pose)));
+        c->poses_cap = 0; c->d_poses.reset(); c->h_poses.reset();
+        B2D_CU(allocate(c->d_poses, per * sizeof(Pose)));
+        B2D_CU(allocate(c->h_poses, per * sizeof(Pose)));
         c->poses_cap = per;
     }
     for (size_t i = 0; i < per; i++) {
         size_t g = rank * per + i;
         if (g >= n_total) g = n_total - 1;
-        std::memcpy(&c->h_poses[i], &poses[g], sizeof(Pose));
+        std::memcpy(&c->h_poses.get()[i], &poses[g], sizeof(Pose));
     }
-    B2D_CU(cudaMemcpyAsync(c->d_poses, c->h_poses, per * sizeof(Pose), cudaMemcpyHostToDevice, c->render_stream));
-    cudaEvent_t poses_up;
-    B2D_CU(cudaEventCreateWithFlags(&poses_up, cudaEventDisableTiming));
-    B2D_CU(cudaEventRecord(poses_up, c->render_stream));
-    B2D_CU(cudaStreamWaitEvent(c->walk_stream, poses_up, 0));
+    cudaStream_t render_stream = c->render_stream.get(), gather_stream = c->gather_stream.get(),
+                 consume_stream = c->consume_stream.get(), walk_stream = c->walk_stream.get();
+    B2D_CU(cudaMemcpyAsync(c->d_poses.get(), c->h_poses.get(), per * sizeof(Pose), cudaMemcpyHostToDevice, render_stream));
+    Event poses_up;
+    B2D_CU(event_create(poses_up));
+    B2D_CU(cudaEventRecord(poses_up.get(), render_stream));
+    B2D_CU(cudaStreamWaitEvent(walk_stream, poses_up.get(), 0));
     // the BSP walk of chunk k+1 runs as a background grid on its own stream under the raster of chunk k
     auto chunk_count = [&](size_t k) { const size_t f = k * chunk; return (per - f) < chunk ? (per - f) : chunk; };
     int64_t ticket = -1;
     if (do_render) {
-        int wrc = b2d::walk_frames(r, c->d_poses, (int)chunk_count(0), c->walk_stream, &ticket, true);
-        if (wrc != B2D_OK) { cudaEventDestroy(poses_up); return wrc; }
+        int wrc = b2d::walk_frames(r, c->d_poses.get(), (int)chunk_count(0), walk_stream, &ticket, true);
+        if (wrc != B2D_OK) return wrc;
     }
 
     // events: per buffer "rendered", "gathered", "consumed"; timing pairs per chunk
-    cudaEvent_t rendered[2], gathered[2], consumed[2], t_begin, t_end;
+    Event rendered[2], gathered[2], consumed[2], t_begin, t_end;
     for (int i = 0; i < 2; i++) {
-        B2D_CU(cudaEventCreateWithFlags(&rendered[i], cudaEventDisableTiming));
-        B2D_CU(cudaEventCreateWithFlags(&gathered[i], cudaEventDisableTiming));
-        B2D_CU(cudaEventCreateWithFlags(&consumed[i], cudaEventDisableTiming));
+        B2D_CU(event_create(rendered[i]));
+        B2D_CU(event_create(gathered[i]));
+        B2D_CU(event_create(consumed[i]));
     }
-    B2D_CU(cudaEventCreate(&t_begin));
-    B2D_CU(cudaEventCreate(&t_end));
-    std::vector<cudaEvent_t> rt(2 * nchunks), gt(2 * nchunks);
-    for (auto &e : rt) B2D_CU(cudaEventCreate(&e));
-    for (auto &e : gt) B2D_CU(cudaEventCreate(&e));
+    B2D_CU(event_create(t_begin, cudaEventDefault));
+    B2D_CU(event_create(t_end, cudaEventDefault));
+    std::vector<Event> rt(2 * nchunks), gt(2 * nchunks);
+    for (auto &e : rt) B2D_CU(event_create(e, cudaEventDefault));
+    for (auto &e : gt) B2D_CU(event_create(e, cudaEventDefault));
 
-    B2D_CU(cudaEventRecord(t_begin, c->render_stream));
+    B2D_CU(cudaEventRecord(t_begin.get(), render_stream));
     int result = B2D_OK;
     for (size_t k = 0; k < nchunks && result == B2D_OK; k++) {
         const int b = (int)(k & 1);
         const size_t first = k * chunk;
         const size_t cnt = (per - first) < chunk ? (per - first) : chunk;
         uint8_t *slice = c->buf[b] + rank * cnt * npix;                  // in-place all-gather: rank-major slices of cnt frames
-        if (k >= 2) B2D_CU(cudaStreamWaitEvent(c->render_stream, consumed[b], 0));     // chunk k-2 has left this buffer
-        B2D_CU(cudaEventRecord(rt[2 * k], c->render_stream));
+        if (k >= 2) B2D_CU(cudaStreamWaitEvent(render_stream, consumed[b].get(), 0));     // chunk k-2 has left this buffer
+        B2D_CU(cudaEventRecord(rt[2 * k].get(), render_stream));
         if (do_render) {
-            result = b2d::raster_frames(r, ticket, slice, nullptr, c->render_stream);
+            result = b2d::raster_frames(r, ticket, slice, nullptr, render_stream);
             if (result != B2D_OK) break;
             if (k + 1 < nchunks) {
-                result = b2d::walk_frames(r, c->d_poses + (k + 1) * chunk, (int)chunk_count(k + 1), c->walk_stream, &ticket, true);
+                result = b2d::walk_frames(r, c->d_poses.get() + (k + 1) * chunk, (int)chunk_count(k + 1), walk_stream, &ticket, true);
                 if (result != B2D_OK) break;
             }
         }
-        B2D_CU(cudaEventRecord(rt[2 * k + 1], c->render_stream));
-        B2D_CU(cudaEventRecord(rendered[b], c->render_stream));
+        B2D_CU(cudaEventRecord(rt[2 * k + 1].get(), render_stream));
+        B2D_CU(cudaEventRecord(rendered[b].get(), render_stream));
         if (do_gather) {
-            B2D_CU(cudaStreamWaitEvent(c->gather_stream, rendered[b], 0));
-            B2D_CU(cudaEventRecord(gt[2 * k], c->gather_stream));
+            B2D_CU(cudaStreamWaitEvent(gather_stream, rendered[b].get(), 0));
+            B2D_CU(cudaEventRecord(gt[2 * k].get(), gather_stream));
             if (c->ce) {
                 result = ce_gather(c, b, rank * cnt * npix, cnt * npix);
                 if (result != B2D_OK) break;
             } else {
-                int nrc = n.AllGather(slice, c->buf[b], cnt * npix, kNcclUint8, c->comm, c->gather_stream);
+                int nrc = n.AllGather(slice, c->buf[b], cnt * npix, kNcclUint8, c->comm, gather_stream);
                 if (nrc != 0) { result = nccl_fail(nrc, "ncclAllGather"); break; }
             }
-            B2D_CU(cudaEventRecord(gt[2 * k + 1], c->gather_stream));
-            B2D_CU(cudaEventRecord(gathered[b], c->gather_stream));
+            B2D_CU(cudaEventRecord(gt[2 * k + 1].get(), gather_stream));
+            B2D_CU(cudaEventRecord(gathered[b].get(), gather_stream));
         }
         // consumer of the chunk (gathered: world x cnt frames, rank-major; render only: this rank's cnt frames)
-        B2D_CU(cudaStreamWaitEvent(c->consume_stream, do_gather ? gathered[b] : rendered[b], 0));
-        if (fn) fn(user, (int)k, first, cnt, do_gather ? c->buf[b] : slice, do_gather ? c->world : 1, c->consume_stream);
-        B2D_CU(cudaEventRecord(consumed[b], c->consume_stream));
+        B2D_CU(cudaStreamWaitEvent(consume_stream, (do_gather ? gathered[b] : rendered[b]).get(), 0));
+        if (fn) fn(user, (int)k, first, cnt, do_gather ? c->buf[b] : slice, do_gather ? c->world : 1, consume_stream);
+        B2D_CU(cudaEventRecord(consumed[b].get(), consume_stream));
     }
     // the end of the job on this rank: everything on the three streams
-    B2D_CU(cudaStreamWaitEvent(c->consume_stream, rendered[(nchunks - 1) & 1], 0));
-    B2D_CU(cudaEventRecord(t_end, c->consume_stream));
-    cudaError_t se = cudaStreamSynchronize(c->consume_stream);
-    if (se == cudaSuccess) se = cudaStreamSynchronize(c->gather_stream);
-    if (se == cudaSuccess) se = cudaStreamSynchronize(c->render_stream);
+    B2D_CU(cudaStreamWaitEvent(consume_stream, rendered[(nchunks - 1) & 1].get(), 0));
+    B2D_CU(cudaEventRecord(t_end.get(), consume_stream));
+    cudaError_t se = cudaStreamSynchronize(consume_stream);
+    if (se == cudaSuccess) se = cudaStreamSynchronize(gather_stream);
+    if (se == cudaSuccess) se = cudaStreamSynchronize(render_stream);
     if (se != cudaSuccess && result == B2D_OK) result = b2d::cuda_fail(se, "cudaStreamSynchronize");
     if (result == B2D_OK && stats_out) {
         b2d_sharded_stats st;
         std::memset(&st, 0, sizeof st);
         float ms = 0.f;
-        cudaEventElapsedTime(&ms, t_begin, t_end);
+        cudaEventElapsedTime(&ms, t_begin.get(), t_end.get());
         st.total_ms = ms;
         for (size_t k = 0; k < nchunks; k++) {
-            cudaEventElapsedTime(&ms, rt[2 * k], rt[2 * k + 1]); st.render_ms += ms;
-            if (do_gather) { cudaEventElapsedTime(&ms, gt[2 * k], gt[2 * k + 1]); st.gather_ms += ms; }
+            cudaEventElapsedTime(&ms, rt[2 * k].get(), rt[2 * k + 1].get()); st.render_ms += ms;
+            if (do_gather) { cudaEventElapsedTime(&ms, gt[2 * k].get(), gt[2 * k + 1].get()); st.gather_ms += ms; }
         }
         st.frames_local = (int64_t)per;
         st.frames_gathered = do_gather ? (int64_t)(per * world) : 0;
@@ -499,11 +491,6 @@ int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size
         std::strncpy(st.registration, c->registration, sizeof st.registration - 1);
         *stats_out = st;
     }
-    cudaEventDestroy(poses_up);
-    for (int i = 0; i < 2; i++) { cudaEventDestroy(rendered[i]); cudaEventDestroy(gathered[i]); cudaEventDestroy(consumed[i]); }
-    cudaEventDestroy(t_begin); cudaEventDestroy(t_end);
-    for (auto e : rt) cudaEventDestroy(e);
-    for (auto e : gt) cudaEventDestroy(e);
     return result;
 }
 
