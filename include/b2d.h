@@ -327,6 +327,14 @@ int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *
  * per-frame states (frames with equal compact states share a slot). */
 int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out);
 
+/* Introspection for tests: the expanded table set `set` of the LAST walked batch, in b2d_scene_tables_at's layout
+ * [textures | sectors | segs | sprites | mids] and size (without the device copy's padding).  A batch walked with
+ * per-frame states has one set per distinct state (`set` below their number, as b2d_debug_state_slots numbers them); a
+ * plain batch has one, the set its worklist slot read (`set` = 0).  With out = NULL only *size_out is written.
+ * Synchronises the device.  B2D_ERR_INVALID_ARG for a scene without time-dependent content or dynamic sectors, a set
+ * out of range, or a renderer that has walked no batch. */
+int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capacity, size_t *size_out);
+
 /* Per-kernel device timing for the roofline report: while enabled, every batch records CUDA events
  * around the walk and raster launches on the launching stream.  b2d_profile_read synchronises the
  * device, returns the summed milliseconds and batch count since the last read, and resets them. */

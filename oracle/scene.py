@@ -791,6 +791,48 @@ def apply_moves(blob: bytes, moves) -> bytes:
     return bytes(out)
 
 
+def tables_at(blob: bytes, tics: int, moves=()) -> bytes:
+    """The state-dependent tables at level time `tics` with `moves` applied, laid out [textures | sectors | segs | sprites |
+    mids] as the product's b2d_scene_tables_at returns them.  Restated from DESIGN.md C14-C16 on top of apply_moves:
+    an animated texture or flat shows group frame (tics >> 3) mod n, whichever frame name the map uses (the texture record
+    is that frame's record); a scrolling seg adds tics & 0xFFFFFF to its column offset; a sector with a light effect, its
+    segs and its sprites carry its light byte at `tics`."""
+    tics = int(tics) & 0xFFFFFFFF
+    b = apply_moves(blob, moves)
+    h = header(b)
+    anim = np.frombuffer(b, dtype="<i4", count=h[H_NANIM], offset=h[H_OFF_ANIM])
+
+    def frame_now(first: int, nk: int, own: int) -> int:
+        n = nk & 0xFFFF
+        return own if n < 2 else int(anim[first + (tics >> 3) % n])
+
+    tex0 = section(b, "textures")
+    tex = np.array([tex0[frame_now(int(t[6]), int(t[7]), i)] for i, t in enumerate(tex0)], dtype="<u4").reshape(-1, 8)
+    flatanim = np.frombuffer(b, dtype="<i4", count=2 * h[H_NFLATS], offset=h[H_OFF_FLAT_ANIM]).reshape(-1, 2)
+    sectors = section(b, "sectors").astype(np.int64)
+    for row in sectors:
+        for c in (2, 3):
+            if row[c] >= 0:
+                row[c] = frame_now(int(flatanim[row[c], 0]), int(flatanim[row[c], 1]), int(row[c]))
+    segs = section(b, "segs").astype(np.int64)
+    sprites = section(b, "sprites").astype(np.int64)
+    lights = sector_lights_at(b, tics)
+    effect = lights >= 0
+    sectors[effect, 4] = lights[effect]
+    for S in segs:
+        if S[3] & SEG_INVALID:
+            continue
+        if S[3] & SEG_SCROLL:
+            S[4] = (S[4] + (tics & 0xFFFFFF) + (1 << 31)) % (1 << 32) - (1 << 31)
+        if effect[S[2]]:
+            S[12] = lights[S[2]]
+    for P in sprites:
+        if effect[P[5]]:
+            P[4] = lights[P[5]]
+    return b"".join([tex.tobytes(), sectors.astype("<i4").tobytes(), segs.astype("<i4").tobytes(),
+                     sprites.astype("<i4").tobytes(), section(b, "mids").astype("<i4").tobytes()])
+
+
 def header(blob: bytes) -> List[int]:
     return list(struct.unpack_from("<%dI" % HEADER_WORDS, blob, 0))
 

@@ -429,6 +429,15 @@ class Renderer:
         _check(_lib.load().b2d_debug_state_slots(self._h, n, out.ctypes.data))
         return out
 
+    def state_tables(self, set: int = 0) -> bytes:
+        """b2d_debug_state_tables: table set `set` of the last walked batch, laid out as Scene.tables_at returns it (a plain
+        batch has the one set 0)."""
+        size = ctypes.c_size_t()
+        _check(_lib.load().b2d_debug_state_tables(self._h, set, None, 0, ctypes.byref(size)))
+        buf = ctypes.create_string_buffer(max(size.value, 1))
+        _check(_lib.load().b2d_debug_state_tables(self._h, set, buf, size.value, ctypes.byref(size)))
+        return buf.raw[:size.value]
+
     def profile(self, enable: bool):
         _check(_lib.load().b2d_profile_enable(self._h, 1 if enable else 0))
 

@@ -49,7 +49,7 @@ EXPORTS = [
     "b2d_render_timed", "b2d_render_device_timed", "b2d_walk_device",
     "b2d_render_states", "b2d_render_device_states", "b2d_walk_device_states",
     "b2d_raster_device", "b2d_palette_lut_device",
-    "b2d_debug_worklist", "b2d_debug_state_slots", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
+    "b2d_debug_worklist", "b2d_debug_state_slots", "b2d_debug_state_tables", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
     "b2d_comm_unique_id", "b2d_comm_create", "b2d_comm_destroy", "b2d_comm_info", "b2d_render_sharded",
     "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_download",
 ]
@@ -154,6 +154,7 @@ def load() -> ctypes.CDLL:
     L.b2d_palette_lut_device.argtypes = [vp, vp, vp, cs, vp]
     L.b2d_debug_worklist.argtypes = [vp, cs, vp, vp, cs]
     L.b2d_debug_state_slots.argtypes = [vp, cs, vp]
+    L.b2d_debug_state_tables.argtypes = [vp, cs, vp, cs, ctypes.POINTER(cs)]
     L.b2d_profile_enable.argtypes = [vp, ci]
     L.b2d_profile_read.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
                                    ctypes.POINTER(ctypes.c_int64)]

@@ -243,6 +243,7 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
     CU(cudaEventRecord(s.walk_done.get(), stream));
     s.n = n;
     s.per_frame = frame_states != nullptr;
+    s.sets = frame_states ? nstates : 0;
     s.ticket = r->next_ticket;
     s.rastered = false;
     r->last_slot = slot;
@@ -1041,6 +1042,23 @@ int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
     CU(cudaMemcpy(slots_out, slot_tables(r, slot).frame_slot, 4 * n, cudaMemcpyDeviceToHost));
+    return B2D_OK;
+}
+
+int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capacity, size_t *size_out) {
+    if (!r) return fail(B2D_ERR_INVALID_ARG, "null renderer");
+    if (r->h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
+    const WorkSlot &s = r->slot[r->last_slot];
+    if (s.ticket < 0) return fail(B2D_ERR_INVALID_ARG, "no batch has been walked");
+    if (set >= (s.per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
+    const size_t need = state_table_bytes(r->h_blob.data());
+    if (size_out) *size_out = need;
+    if (!out) return B2D_OK;
+    if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");
+    CU(cudaSetDevice(r->device));
+    CU(cudaDeviceSynchronize());
+    const uint8_t *src = s.per_frame ? s.arena.get() + set * (size_t)r->state_tables.slot_bytes : s.tables.get();
+    CU(cudaMemcpy(out, src, need, cudaMemcpyDeviceToHost));
     return B2D_OK;
 }
 

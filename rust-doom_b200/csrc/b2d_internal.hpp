@@ -86,6 +86,7 @@ struct WorkSlot {
     int64_t ticket = -1;
     bool rastered = true;
     bool per_frame = false;                               // the batch was walked with per-frame states
+    int sets = 0;                                         // ... into this many table sets of the arena (distinct states)
     // timed scenes: the table set the slot's plain batches read and the compact state it was expanded from
     DeviceBuf<uint8_t> tables;
     std::vector<uint32_t> state;

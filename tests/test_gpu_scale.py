@@ -60,24 +60,71 @@ def _level(b2d, name):
 
 
 # ---- A. persistent walk grid and the pipelined jobs path ----------------------------------------------------------------
+def _states_level(b2d, name):
+    """_level with per-frame state inputs: the level's scene, oracle blob and dynamic sectors (tests/refcheck/moves.py's
+    declaration on the "32x32" level, which then takes the kStates walk through the shared-memory opt-in) and a pool of
+    move lists (at rest only where nothing is declared)."""
+    from oracle import scene as S, wad as W
+    from rust_doom_b200 import synthwad
+    from tests.refcheck import moves as MV
+    data = synthwad.build_iwad(1, ("E1M1",)) if name == "default" else sweep_level(int(name.split("x")[0]))[0]
+    a = W.Archive(data)
+    level = W.Level(a, 0)
+    dyn = MV.declare(level, 11, 12) if name != "default" else []
+    pool = [[]] + [MV.state(level, dyn, 300 + k, hole_free=False) for k in range(3)] if dyn else [[]]
+    sc = b2d.Scene(b2d.Archive.from_bytes(data), 0, dynamic=dyn)
+    blob = S.compile_scene(a, W.TextureDirectory(a), 0, dynamic=dyn)
+    assert sc.blob == blob
+    return sc, blob, pool
+
+
+@pytest.mark.parametrize("states", [False, True])
 @pytest.mark.parametrize("level", ["default", "32x32"])
-def test_gpu_persistent_walk_grid_matches_oracle(b2d, hostcheck, level):
+def test_gpu_persistent_walk_grid_matches_oracle(b2d, hostcheck, level, states):
     """n = SMs + 1 and 2 SMs + 5 frames: the background grid has one CTA per SM, so CTAs walk two or three frames each and
     every frame after a CTA's first reuses the bulk-copied tables.  Frames vs the oracle, worklists vs hostcheck, and the
-    same bytes from the per-frame grid (b2d_render_device)."""
+    same bytes from the per-frame grid (b2d_render_device).  With `states` the batch goes through walk_device_states with
+    a tic of its own for every frame (and a move list from a pool where the level declares dynamic sectors), so that each
+    CTA's later frames must read their own table-set index; worklists and frames are checked at each frame's own state."""
     import torch
-    sc, blob = _level(b2d, level)
+    from tests.test_gpu_states import _oracle
+    if states:
+        sc, blob, pool = _states_level(b2d, level)
+    else:
+        sc, blob = _level(b2d, level)
     view, oview = b2d.make_view(320, 200), render.make_view(320, 200)
     sms = _sms()
     for n in (sms + 1, 2 * sms + 5):
         poses = sample_poses(b2d, sc, n, 600 + n)
         r = b2d.Renderer(sc, view, max_batch=n)
-        dp, out = _background_walk(r, poses, 320, 200)
-        assert r.status() == 0
-        _assert_worklists(r, hostcheck, blob, view, poses, "%s n=%d" % (level, n))
-        _assert_same(render.render(blob, oview, poses, threads=8), out.cpu().numpy(), "%s background walk n=%d" % (level, n))
-        per_frame = torch.full_like(out, 0x5A)
-        r.render_device(dp.data_ptr(), n, per_frame.data_ptr())
+        if not states:
+            dp, out = _background_walk(r, poses, 320, 200)
+            assert r.status() == 0
+            _assert_worklists(r, hostcheck, blob, view, poses, "%s n=%d" % (level, n))
+            _assert_same(render.render(blob, oview, poses, threads=8), out.cpu().numpy(), "%s background walk n=%d" % (level, n))
+            per_frame = torch.full_like(out, 0x5A)
+            r.render_device(dp.data_ptr(), n, per_frame.data_ptr())
+        else:
+            tics = (np.arange(n, dtype=np.uint64) * 37 + 1000).astype(np.uint32)
+            moves = [pool[i % len(pool)] for i in range(n)]
+            dp = _dev_poses(poses)
+            out = torch.full((n, 200, 320), 0xA5, dtype=torch.uint8, device="cuda")
+            st = torch.cuda.Stream()
+            torch.cuda.synchronize()
+            ticket = r.walk_device_states(dp.data_ptr(), tics, n, moves, st.cuda_stream)
+            r.raster_device(ticket, out.data_ptr(), 0, st.cuda_stream)
+            st.synchronize()
+            assert r.status() == 0
+            slots = r.state_slots(n)
+            assert any(slots[f] != slots[f % sms] for f in range(sms, n)), "no CTA walks frames of different table sets"
+            counts, ids = r.worklist(n)
+            for i in range(n):
+                _, hc, hids = hostcheck(blob, view, poses[i:i + 1], int(tics[i]), moves[i])
+                assert counts[i] == hc[0] and ids[i, :counts[i]].tolist() == hids[0, :hc[0]].tolist(), \
+                    "%s n=%d: worklist of frame %d" % (level, n, i)
+            _assert_same(_oracle(blob, 320, 200, poses, tics, moves), out.cpu().numpy(), "%s background walk with states n=%d" % (level, n))
+            per_frame = torch.full_like(out, 0x5A)
+            r.render_device_states(dp.data_ptr(), tics, n, per_frame.data_ptr(), moves_per_pose=moves)
         torch.cuda.synchronize()
         assert r.status() == 0
         assert torch.equal(out, per_frame), "%s n=%d: persistent and per-frame walk grids disagree" % (level, n)

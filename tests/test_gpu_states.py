@@ -2,12 +2,14 @@
 with the oracle's frame at that pose's state: its own scene with the pose's moves applied (oracle/scene.py apply_moves),
 rendered at the pose's tics."""
 import ctypes
+import os
 
 import numpy as np
 import pytest
 
 from oracle import render
 from tests.conftest import sample_poses
+from tests.test_scene import EDGE_TICS, STATE_KINDS, assert_kind, declare_doors, state_level, state_moves
 
 pytestmark = pytest.mark.gpu
 
@@ -18,17 +20,10 @@ def _level(b2d, seed=1, doors=True, **cfg):
     (closed doors)."""
     from oracle import scene as S, wad as W
     from rust_doom_b200 import synthwad
-    from tests.refcheck import moves as MV
     data = synthwad.build_iwad(seed, ("E1M1",), cfg=synthwad.SynthConfig(anim=True, **cfg))
     a = W.Archive(data)
     level = W.Level(a, 0)
-    dyn = MV.declare(level, 5, 16) if doors else []
-    doors_ = []
-    for k, (s, fmin, fmax, cmin, cmax) in enumerate(dyn):
-        f0, c0 = int(level.sectors[s]["floor"]), int(level.sectors[s]["ceil"])
-        if cmin != cmax and len(doors_) < 4:
-            dyn[k] = (s, fmin, fmax, min(cmin, f0), cmax)
-            doors_.append((s, f0, c0))
+    dyn, doors_ = declare_doors(level) if doors else ([], [])
     oblob = S.compile_scene(a, W.TextureDirectory(a), 0, dynamic=dyn)
     sc = b2d.Scene(b2d.Archive.from_bytes(data), 0, dynamic=dyn)
     assert sc.blob == oblob
@@ -50,10 +45,24 @@ def _states(level, dyn, doors, n, seed):
 
 
 def _oracle(oblob, w, h, poses, tics, moves):
+    """The oracle's frame of every pose at its own (tics, moves): apply_moves once per distinct move list, the frames on a
+    thread pool (the oracle's ctypes calls release the GIL)."""
+    from concurrent.futures import ThreadPoolExecutor
     from oracle import scene as S
     view = render.make_view(w, h)
-    return np.stack([render.render(S.apply_moves(oblob, moves[i]) if moves[i] else oblob, view, poses[i:i + 1], threads=8,
-                                   tics=int(tics[i]))[0] for i in range(len(poses))])
+    blobs = {}
+    for m in moves:
+        key = tuple(map(tuple, m))
+        if key not in blobs:
+            blobs[key] = S.apply_moves(oblob, m) if m else oblob
+    out = np.empty((len(poses), h, w), np.uint8)
+
+    def one(i):
+        render.render(blobs[tuple(map(tuple, moves[i]))], view, poses[i:i + 1], tics=int(tics[i]), out=out[i:i + 1])
+
+    with ThreadPoolExecutor(os.cpu_count() or 4) as ex:
+        list(ex.map(one, range(len(poses))))
+    return out
 
 
 def _assert_same(want, got, what):
@@ -205,3 +214,72 @@ def test_states_invalid_inputs_enqueue_nothing(b2d):
     plain = b2d.Scene(b2d.Archive.from_bytes(synthwad.build_iwad(1, ("E1M1",), cfg=synthwad.SynthConfig(light_fx=False))), 0)
     with pytest.raises(b2d.B2dError):
         b2d.Renderer(plain, b2d.make_view(320, 200), max_batch=4).render_states(poses[:1], [0], [[(0, 1, 0)]])
+
+
+def check_state_sets(r, oblob, tics, moves, n):
+    """The table sets of the last batch r walked with per-frame states, read back: each equals oracle/scene.py tables_at of
+    the frames that read it, so frames that share a set have equal oracle tables.  -> (set index per frame, oracle tables
+    per frame)."""
+    from oracle import scene as S
+    from rust_doom_b200 import B2dError
+    slots = r.state_slots(n)
+    nsets = int(slots.max()) + 1
+    assert set(slots.tolist()) == set(range(nsets)), "set indices are not 0 .. n_sets-1"
+    cache = {}
+    want = []
+    for i in range(n):
+        key = (int(tics[i]), tuple(map(tuple, moves[i])))
+        if key not in cache:
+            cache[key] = S.tables_at(oblob, key[0], moves[i])
+        want.append(cache[key])
+    got = [r.state_tables(k) for k in range(nsets)]
+    for i in range(n):
+        if got[slots[i]] != want[i]:
+            g, w = np.frombuffer(got[slots[i]], np.int32), np.frombuffer(want[i], np.int32)
+            pytest.fail("frame %d (tics %d): table set %d differs from the oracle's tables at words %s" % (
+                i, int(tics[i]), slots[i], np.nonzero(g != w)[0][:8]))
+    with pytest.raises(B2dError):
+        r.state_tables(nsets)
+    return slots, want
+
+
+@pytest.mark.parametrize("kind", STATE_KINDS)
+def test_states_level_kinds_at_edge_tics(b2d, kind):
+    """One batch per level kind (tests/test_scene.py state_level: light effects only, animation only, scrolling only,
+    dynamic sectors only, everything) through render_device_states, every edge tic with every move list of the kind (at
+    rest, all offsets zero, doors shut, random): frames equal the oracle, every expanded table set equals the oracle's
+    tables_at, and the number of sets is what the compact state makes of the kind -- one per distinct tables where the
+    state keeps exactly what the tables depend on, one per (tics >> 3, moves) where the level only animates (its frames
+    repeat every n steps, the state does not know n), and a move list of zeros is the rest state."""
+    import torch
+    from oracle import scene as S, wad as W
+    data, dyn, doors, level = state_level(kind)
+    a = W.Archive(data)
+    oblob = S.compile_scene(a, W.TextureDirectory(a), 0, dynamic=dyn)
+    sc = b2d.Scene(b2d.Archive.from_bytes(data), 0, dynamic=dyn)
+    assert sc.blob == oblob
+    assert_kind(oblob, kind)
+    lists = state_moves(level, dyn, doors, 40)
+    pairs = [(t, m) for t in EDGE_TICS for m in range(len(lists))]
+    n = len(pairs)
+    tics = np.array([t for t, _ in pairs], np.uint64).astype(np.uint32)
+    moves = [lists[m] for _, m in pairs]
+    poses = sample_poses(b2d, sc, n, 76)
+    r = b2d.Renderer(sc, b2d.make_view(320, 200), max_batch=n)
+    with pytest.raises(b2d.B2dError):
+        r.state_tables(0)                                           # nothing walked yet
+    dp = torch.from_numpy(poses.view(np.int32).reshape(-1, 4).copy()).cuda()
+    out = torch.empty((n, 200, 320), dtype=torch.uint8, device="cuda")
+    r.render_device_states(dp.data_ptr(), tics, n, out.data_ptr(), moves_per_pose=moves)
+    torch.cuda.synchronize()
+    assert r.status() == 0
+    _assert_same(_oracle(oblob, 320, 200, poses, tics, moves), out.cpu().numpy(), kind)
+    slots, want = check_state_sets(r, oblob, tics, moves, n)
+    nsets = int(slots.max()) + 1
+    if kind == "anim":
+        assert nsets == len({(int(t) >> 3, m) for t, m in pairs})
+    elif kind != "all":
+        assert nsets == len(set(want)), "same set if and only if same tables"
+    if kind == "moves":
+        for k in range(len(EDGE_TICS)):                             # [] and the all-zero list: one set, at every tic
+            assert slots[len(lists) * k] == slots[len(lists) * k + 1] == slots[0]

@@ -307,14 +307,6 @@ def _moving_case(seed, cfg):
     return data, a, tex, dyn, mv
 
 
-def _state_tables(blob):
-    """[textures | sectors | segs | sprites | mids] of a blob, as b2d_scene_tables_at lays them out"""
-    h = S.header(blob)
-    spans = [(h[S.H_OFF_TEX], h[S.H_NTEX] * 32), (h[S.H_OFF_SECTORS], h[S.H_NSECTORS] * 32), (h[S.H_OFF_SEGS], h[S.H_NSEGS] * 64),
-             (h[S.H_OFF_SPRITES], h[S.H_NSPRITES] * 32), (h[S.H_OFF_MIDS], h[S.H_NMIDS] * 32)]
-    return b"".join(blob[o:o + n] for o, n in spans)
-
-
 @pytest.mark.parametrize("seed", [1, 9])
 def test_dynamic_sectors_compile_and_move_like_the_oracle(b2d, seed):
     """Moving sectors (DESIGN.md C16): the product's scene compiler given the dynamic-sector list, and its re-derivation
@@ -329,16 +321,16 @@ def test_dynamic_sectors_compile_and_move_like_the_oracle(b2d, seed):
     assert S.header(ob)[S.H_NTEX] >= S.header(static)[S.H_NTEX]
     assert (S.section(ob, "sectors") == S.section(static, "sectors")).all()
     moved = S.apply_moves(ob, mv)
-    assert sc.tables_at(0, mv) == _state_tables(moved)
-    assert sc.tables_at(0, ()) == _state_tables(ob)
+    assert sc.tables_at(0, mv) == S.tables_at(ob, 0, mv)
+    assert sc.tables_at(0, ()) == S.tables_at(ob, 0)
     assert moved != ob and S.apply_moves(ob, ()) == ob
     from tests.refcheck import moves as MV
     level = W.Level(a, 0)
     for k in range(25):                                  # more states of the same declaration, any height inside the ranges
         st = MV.state(level, dyn, 1000 * seed + k, hole_free=False)
         assert sc.tables_at(k, st) == sc.tables_at(k, list(reversed(st)))            # order of the list does not matter
-        got = np.frombuffer(sc.tables_at(0, st), np.int32)
-        want = np.frombuffer(_state_tables(S.apply_moves(ob, st)), np.int32)
+        got = np.frombuffer(sc.tables_at(k, st), np.int32)
+        want = np.frombuffer(S.tables_at(ob, k, st), np.int32)
         assert (got == want).all(), "state %d" % k
     # rest heights + offsets, openings follow
     s0, s1 = S.section(ob, "sectors"), S.section(moved, "sectors")
@@ -394,10 +386,114 @@ def test_time_and_moves_compose(b2d):
     h = S.header(ob)
     for tics in (0, 9, 1000):
         t0, t1 = sc.tables_at(tics, ()), sc.tables_at(tics, mv)
-        # texture records do not depend on heights; sectors / segs / sprites / mids differ exactly where apply_moves says
+        # texture records do not depend on heights
         ntex = h[S.H_NTEX] * 32
         assert t0[:ntex] == t1[:ntex]
-        rest, moved = _state_tables(ob), _state_tables(S.apply_moves(ob, mv))
-        a0, a1 = np.frombuffer(t0, np.int32), np.frombuffer(t1, np.int32)
-        r0, r1 = np.frombuffer(rest, np.int32), np.frombuffer(moved, np.int32)
-        assert ((a1 - a0) == (r1 - r0)).all()
+        assert t0 == S.tables_at(ob, tics) and t1 == S.tables_at(ob, tics, mv)
+
+
+# ---- the state rule over level kinds and edge tics ----------------------------------------------------------------------
+# Five generated levels whose tables depend on different parts of a state, so that each reduction of the compact state
+# (DESIGN.md §3: the tic kept as tics & ~7 when a level only animates, tics & 0xFFFFFF when it only scrolls, 0 when it does
+# neither) is taken by one of them.
+STATE_KINDS = ("lights", "anim", "scroll", "moves", "all")
+EDGE_TICS = (0, 7, 8, 15, (1 << 24) - 1, 1 << 24, (1 << 24) + 7, (1 << 32) - 8, (1 << 32) - 1)
+
+
+def declare_doors(level, seed=5, n_sectors=16):
+    """tests/refcheck/moves.py's declaration, with the ceilings of the first few non-sky sectors allowed down to their floor;
+    -> (dynamic, doors = [(sector, floor, ceiling)])"""
+    from tests.refcheck import moves as MV
+    dyn = MV.declare(level, seed, n_sectors)
+    doors = []
+    for k, (s, fmin, fmax, cmin, cmax) in enumerate(dyn):
+        f0, c0 = int(level.sectors[s]["floor"]), int(level.sectors[s]["ceil"])
+        if cmin != cmax and len(doors) < 4:
+            dyn[k] = (s, fmin, fmax, min(cmin, f0), cmax)
+            doors.append((s, f0, c0))
+    return dyn, doors
+
+
+def _patch_level(data: bytes, lump: str, record: int, fields, fn) -> bytes:
+    """`data` with fn(8-byte name) -> 8-byte name applied to the name fields at byte offsets `fields` of every `record`-byte
+    record of the first level's lump `lump` (one of Scene.LUMP_ORDER)"""
+    from rust_doom_b200 import Scene
+    a = W.Archive(data)
+    _, pos, size = a.lumps[a.levels[0] + 1 + Scene.LUMP_ORDER.index(lump)]
+    out = bytearray(data)
+    for r in range(pos, pos + size, record):
+        for f in fields:
+            out[r + f:r + f + 8] = fn(bytes(out[r + f:r + f + 8]))
+    return bytes(out)
+
+
+def _static_names(groups, replacement: bytes):
+    frames = {W.wad_name(n.encode()) for g in groups for n in g}
+    return lambda name: replacement if W.wad_name(name) in frames else name
+
+
+def state_level(kind: str):
+    """-> (wad bytes, dynamic sectors, doors, level) of one level kind:
+    lights  the c2 level (bench.py): light effects only
+    anim    animated textures and flats only (the scrolling special 0x30 cleared in LINEDEFS)
+    scroll  scrolling walls only (animated names in SIDEDEFS and SECTORS replaced by static ones)
+    moves   dynamic sectors only (doors)
+    all     animation, scrolling, light effects, doors, masked middles and sprites"""
+    import struct
+    from oracle.anim_table import FLATS, WALLS
+    from rust_doom_b200 import synthwad
+    cfg = {"lights": {}, "anim": dict(anim=True, light_fx=False), "scroll": dict(anim=True, light_fx=False),
+           "moves": dict(light_fx=False), "all": dict(anim=True, mid_pct=20, thing_pct=30)}[kind]
+    data = synthwad.build_iwad(1, ("E1M1",), cfg=synthwad.SynthConfig(**cfg))
+    if kind == "anim":                          # special (u16 at byte 6 of a linedef) 0x30 -> 0
+        data = _patch_level(data, "linedefs", 14, [6], lambda b: struct.pack("<H", 0) + b[2:] if b[:2] == b"\x30\0" else b)
+    if kind == "scroll":
+        data = _patch_level(data, "sidedefs", 30, [4, 12, 20], _static_names(WALLS, W.wad_name(b"BRICK1")))
+        data = _patch_level(data, "sectors", 26, [4, 12], _static_names(FLATS, W.wad_name(b"FLOOR1")))
+    level = W.Level(W.Archive(data), 0)
+    dyn, doors = declare_doors(level) if kind in ("moves", "all") else ([], [])
+    return data, dyn, doors, level
+
+
+def state_moves(level, dyn, doors, seed):
+    """move lists for a level kind: at rest, all offsets zero (at rest too), doors shut, one random state"""
+    from tests.refcheck import moves as MV
+    if not dyn:
+        return [[]]
+    return [[], [(dyn[0][0], 0, 0), (dyn[-1][0], 0, 0)], [(s, 0, f0 - c0) for (s, f0, c0) in doors],
+            MV.state(level, dyn, seed, hole_free=False)]
+
+
+def assert_kind(blob: bytes, kind: str):
+    """what the blob holds is what the kind says"""
+    h = S.header(blob)
+    n = h[S.H_NSECTORS]
+    lights = set(np.frombuffer(blob, "<u4", 8 * n, h[S.H_OFF_LIGHTS]).reshape(n, 8)[:, 0].tolist()) - {S.LIGHT_NONE}
+    scrolls = bool((S.section(blob, "segs")[:, 3] & S.SEG_SCROLL).any())
+    want = {"lights": (False, False, True, False), "anim": (True, False, False, False), "scroll": (False, True, False, False),
+            "moves": (False, False, False, True), "all": (True, True, True, True)}[kind]
+    assert (h[S.H_NANIM] > 0, scrolls, bool(lights), h[S.H_NDYN] > 0) == want, kind
+    assert lights <= {S.LIGHT_GLOW, S.LIGHT_RANDOM, S.LIGHT_ALTERNATE}
+    if kind == "all":
+        assert lights == {S.LIGHT_GLOW, S.LIGHT_RANDOM, S.LIGHT_ALTERNATE}
+
+
+@pytest.mark.parametrize("kind", STATE_KINDS)
+def test_tables_at_equals_oracle_restatement(b2d, kind):
+    """b2d_scene_tables_at (the product's state rule, scene_at_time) equals oracle/scene.py tables_at byte for byte on every
+    level kind, at the edge tics of the animation step, the 24-bit scroll wrap and the 32-bit tic range, and at random tics,
+    with no moves, an all-zero move list, shut doors and random states."""
+    data, dyn, doors, level = state_level(kind)
+    a = W.Archive(data)
+    ob = S.compile_scene(a, W.TextureDirectory(a), 0, dynamic=dyn)
+    sc = b2d.Scene(b2d.Archive.from_bytes(data), 0, dynamic=dyn)
+    assert sc.blob == ob
+    assert_kind(ob, kind)
+    rng = np.random.default_rng(STATE_KINDS.index(kind))
+    tics = list(EDGE_TICS) + rng.integers(0, 1 << 32, 6, dtype=np.uint64).tolist()
+    for i, t in enumerate(tics):
+        for mv in state_moves(level, dyn, doors, 100 + i):
+            got, want = sc.tables_at(t, mv), S.tables_at(ob, t, mv)
+            if got != want:
+                g, w = np.frombuffer(got, np.int32), np.frombuffer(want, np.int32)
+                pytest.fail("%s: tics %d, moves %s: tables differ at word %s" % (kind, t, mv, np.nonzero(g != w)[0][:8]))
