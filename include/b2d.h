@@ -264,6 +264,43 @@ int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_
 int b2d_walk_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, void *cuda_stream, int64_t *ticket_out);
 int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint32_t *d_rgba_fb, void *cuda_stream);
 
+/* ---- level sets: frames of several levels in one batch --------------------------------------
+ * The reference switches levels at run time (game/src/wad_system.rs:37-45, game/src/level.rs:188-197); many agents or
+ * cameras may each be on their own map.  A renderer over a set of levels keeps every level resident (its scene, pre-lit
+ * planes and walk tables; DESIGN.md §3) and renders each frame of a batch from its own level, in the same two launches per
+ * batch as one level: switching levels is a per-frame index, not a new renderer.
+ *
+ * b2d_renderer_create_levels: a renderer over n_levels scenes (1 <= n_levels <= B2D_MAX_LEVELS) with one view, device and
+ * max_batch.  Level k is scenes[k]; the scenes are copied (they may be destroyed afterwards).  Every other entry point acts
+ * on level 0, so b2d_renderer_create(s, ...) behaves as a set of one.  b2d_renderer_set_time applies to every level;
+ * b2d_renderer_set_sector_moves is b2d_renderer_set_level_sector_moves(r, 0, ...).
+ *
+ * b2d_render_levels: host poses and frames as b2d_render; frame i is rendered from level levels[i] (HOST array), at the
+ * renderer's level time and that level's sector moves, byte-identical to a b2d_renderer_create renderer of that level in
+ * the same state.  b2d_render_device_levels: like b2d_render_device, n may exceed max_batch (split into batches).
+ * b2d_walk_device_levels: like b2d_walk_device (1..max_batch poses); the ticket is rastered by b2d_raster_device.  A batch
+ * costs one walk and one raster whatever the number of levels it mixes, plus, after a change of the time or of a level's
+ * moves, one launch per changed level the batch uses (the first batch of each worklist slot).  The device-resident calls
+ * do not synchronise the device, but before a batch's levels are written into the worklist slot's pinned staging, the host
+ * waits for the copy that read that staging two batches earlier.  A level index >= n_levels, a NULL `levels` or `scenes`
+ * entry and n_levels out of range are B2D_ERR_INVALID_ARG, detected before anything is enqueued.  The per-frame-level
+ * walk keeps the resident level's description in shared memory next to the walk tables: b2d_renderer_create_levels refuses
+ * (B2D_ERR_INVALID_ARG) a level whose walk tables leave no room for it, a level b2d_renderer_create still accepts by a few
+ * hundred bytes; the level calls on such a renderer are B2D_ERR_INVALID_ARG.
+ *
+ * Not covered: per-frame states together with per-frame levels (b2d_render_states & co. act on level 0), levels in
+ * b2d_render_sharded, and the CLI. */
+#define B2D_MAX_LEVELS 64
+int b2d_renderer_create_levels(const b2d_scene *const *scenes, size_t n_levels, const b2d_view *view, int device,
+                               int max_batch, b2d_renderer **out);
+int b2d_render_levels(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, size_t n, uint8_t *index_fb,
+                      uint32_t *rgba_fb);
+int b2d_render_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n,
+                             uint8_t *d_index_fb, uint32_t *d_rgba_fb, void *cuda_stream);
+int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, void *cuda_stream,
+                           int64_t *ticket_out);
+int b2d_renderer_set_level_sector_moves(b2d_renderer *r, int level, const b2d_sector_move *moves, size_t n);
+
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
  * per-frame `frame.finish()` of engine/src/renderer.rs:160-167.  One process per GPU.  NCCL (libnccl.so.2) is bound

@@ -300,19 +300,42 @@ def make_view(width: int, height: int, fov_deg: float = DEFAULT_FOV_DEG) -> "_li
     return v
 
 
+MAX_LEVELS = 64                 # B2D_MAX_LEVELS
+
+
+def _levels_array(levels, n: int) -> np.ndarray:
+    """the uint32 level array of n poses (the library refuses an index out of range)"""
+    lv = np.asarray(levels, dtype=np.int64).reshape(-1)
+    assert lv.shape == (n,), "one level per pose"
+    return np.ascontiguousarray(lv & 0xFFFFFFFF, dtype=np.uint32)
+
+
 class Renderer:
     """Bound to one CUDA device; owns the scene copy in HBM and the per-batch work buffers."""
 
-    def __init__(self, scene: Scene, view, device: int = 0, max_batch: int = 64):
+    def __init__(self, scene: Scene, view, device: int = 0, max_batch: int = 64, _scenes=None):
         h = ctypes.c_void_p()
-        _check(_lib.load().b2d_renderer_create(scene._h, ctypes.byref(view), device, max_batch, ctypes.byref(h)))
+        scenes = [scene] if _scenes is None else list(_scenes)
+        if _scenes is None:
+            _check(_lib.load().b2d_renderer_create(scene._h, ctypes.byref(view), device, max_batch, ctypes.byref(h)))
+        else:
+            arr = (ctypes.c_void_p * max(len(scenes), 1))(*[s._h for s in scenes])
+            _check(_lib.load().b2d_renderer_create_levels(arr, len(scenes), ctypes.byref(view), device, max_batch, ctypes.byref(h)))
         self._h = h
         self.view = view
         self.width, self.height = view.width, view.height
         self.max_batch = max_batch
         self.device = device
-        self.n_segs = scene.info.n_segs
-        self.worklist_stride = max(1, scene.info.n_segs + scene.info.n_sprites)
+        self.n_levels = len(scenes)
+        self.n_segs = scenes[0].info.n_segs
+        # worklist entries per frame: the library's stride, the largest of the levels
+        self.worklist_stride = max(1, max(s.info.n_segs + s.info.n_sprites for s in scenes))
+
+    @classmethod
+    def from_levels(cls, scenes, view, device: int = 0, max_batch: int = 64) -> "Renderer":
+        """b2d_renderer_create_levels: one renderer over a set of levels (1 .. MAX_LEVELS scenes, copied); every call
+        without a level argument acts on level 0 (scenes[0])."""
+        return cls(None, view, device, max_batch, _scenes=scenes)
 
     def set_time(self, tics: int):
         """Level time in 1/35 s for the batches walked afterwards (animated flats / walls, scrolling walls, light
@@ -332,6 +355,12 @@ class Renderer:
             _check(_lib.load().b2d_renderer_set_sector_moves(self._h, arr, n))
         else:
             _check(_lib.load().b2d_renderer_set_sector_moves_async(self._h, arr, n, ctypes.c_void_p(stream)))
+
+    def set_level_sector_moves(self, level: int, moves=()):
+        """b2d_renderer_set_level_sector_moves: the moving sectors of level `level` for the batches walked afterwards, as
+        set_sector_moves does for level 0."""
+        arr, n = _moves_array(moves)
+        _check(_lib.load().b2d_renderer_set_level_sector_moves(self._h, int(level), arr, n))
 
     def status(self) -> int:
         """Sticky completeness bits of everything rendered since the last call (0 = every frame complete); synchronises
@@ -395,6 +424,31 @@ class Renderer:
         states, arr, nm = _frame_states(tics, moves_per_pose, n)
         t = ctypes.c_int64(-1)
         _check(_lib.load().b2d_walk_device_states(self._h, poses_ptr, states, n, arr, nm, stream or None, ctypes.byref(t)))
+        return int(t.value)
+
+    def render_levels(self, poses: np.ndarray, levels, rgba: bool = False):
+        """b2d_render_levels: pose i rendered from level levels[i], at the renderer's time and that level's sector moves."""
+        poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
+        n = len(poses)
+        lv = _levels_array(levels, n)
+        out_index = np.empty((n, self.height, self.width), dtype=np.uint8)
+        out_rgba = np.empty((n, self.height, self.width), dtype=np.uint32) if rgba else None
+        _check(_lib.load().b2d_render_levels(self._h, poses.ctypes.data, lv.ctypes.data, n, out_index.ctypes.data,
+                                             out_rgba.ctypes.data if rgba else None))
+        return (out_index, out_rgba) if rgba else out_index
+
+    def render_device_levels(self, poses_ptr: int, levels, n: int, index_ptr: int, rgba_ptr: int = 0, stream: int = 0):
+        """b2d_render_device_levels: device poses / frames, per-frame levels as in render_levels; n may exceed max_batch."""
+        lv = _levels_array(levels, n)
+        _check(_lib.load().b2d_render_device_levels(self._h, poses_ptr, lv.ctypes.data, n, index_ptr, rgba_ptr or None,
+                                                    stream or None))
+
+    def walk_device_levels(self, poses_ptr: int, levels, n: int, stream: int = 0) -> int:
+        """b2d_walk_device_levels: the walk of a batch (1..max_batch) with per-frame levels; returns the ticket for
+        raster_device."""
+        lv = _levels_array(levels, n)
+        t = ctypes.c_int64(-1)
+        _check(_lib.load().b2d_walk_device_levels(self._h, poses_ptr, lv.ctypes.data, n, stream or None, ctypes.byref(t)))
         return int(t.value)
 
     def render_ptr(self, poses_ptr: int, n: int, index_ptr: int, rgba_ptr: int = 0):

@@ -48,6 +48,8 @@ EXPORTS = [
     "b2d_renderer_destroy", "b2d_renderer_set_time", "b2d_renderer_set_time_async", "b2d_renderer_status", "b2d_render", "b2d_render_device",
     "b2d_render_timed", "b2d_render_device_timed", "b2d_walk_device",
     "b2d_render_states", "b2d_render_device_states", "b2d_walk_device_states",
+    "b2d_renderer_create_levels", "b2d_render_levels", "b2d_render_device_levels", "b2d_walk_device_levels",
+    "b2d_renderer_set_level_sector_moves",
     "b2d_raster_device", "b2d_palette_lut_device",
     "b2d_debug_worklist", "b2d_debug_state_slots", "b2d_debug_state_tables", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
     "b2d_comm_unique_id", "b2d_comm_create", "b2d_comm_destroy", "b2d_comm_info", "b2d_render_sharded",
@@ -151,6 +153,11 @@ def load() -> ctypes.CDLL:
     L.b2d_render_device_states.argtypes = [vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, vp, vp, vp]
     L.b2d_walk_device_states.argtypes = [vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, vp,
                                          ctypes.POINTER(ctypes.c_int64)]
+    L.b2d_renderer_create_levels.argtypes = [ctypes.POINTER(vp), cs, ctypes.POINTER(View), ci, ci, ctypes.POINTER(vp)]
+    L.b2d_render_levels.argtypes = [vp, vp, vp, cs, vp, vp]
+    L.b2d_render_device_levels.argtypes = [vp, vp, vp, cs, vp, vp, vp]
+    L.b2d_walk_device_levels.argtypes = [vp, vp, vp, cs, vp, ctypes.POINTER(ctypes.c_int64)]
+    L.b2d_renderer_set_level_sector_moves.argtypes = [vp, ci, ctypes.POINTER(SectorMove), cs]
     L.b2d_palette_lut_device.argtypes = [vp, vp, vp, cs, vp]
     L.b2d_debug_worklist.argtypes = [vp, cs, vp, vp, cs]
     L.b2d_debug_state_slots.argtypes = [vp, cs, vp]

@@ -151,26 +151,46 @@ int ensure_slot(const b2d_renderer *r, WorkSlot &s) {
 int ensure_states(b2d_renderer *r) {
     if (r->slot[0].arena) return B2D_OK;
     DeviceBuf<uint8_t> arena[2];
-    for (auto &a : arena) CU(allocate(a, (size_t)r->max_batch * r->state_tables.slot_bytes));
+    for (auto &a : arena) CU(allocate(a, (size_t)r->max_batch * r->lv[0].state_tables.slot_bytes));
     for (int i = 0; i < 2; i++) r->slot[i].arena = std::move(arena[i]);
+    return B2D_OK;
+}
+
+// Per-frame levels: both worklist slots' scene arrays, level staging and events, allocated together by the first such call.
+int ensure_levels(b2d_renderer *r) {
+    if (r->slot[0].levels) return B2D_OK;
+    const size_t bytes = r->levels_frames_off + 4 * (size_t)r->max_batch;
+    DeviceBuf<uint8_t> d[2];
+    PinnedBuf<uint8_t> h[2];
+    Event ev[2];
+    for (int i = 0; i < 2; i++) {
+        CU(allocate(d[i], bytes));
+        CU(allocate(h[i], bytes));
+        CU(event_create(ev[i]));
+    }
+    for (int i = 0; i < 2; i++) {
+        r->slot[i].levels = std::move(d[i]);
+        r->slot[i].h_levels = std::move(h[i]);
+        r->slot[i].levels_copied = std::move(ev[i]);
+    }
     return B2D_OK;
 }
 
 // the arena view of worklist slot `slot` (after ensure_states)
 StateTables slot_tables(const b2d_renderer *r, int slot) {
-    StateTables t = r->state_tables;
+    StateTables t = r->lv[0].state_tables;
     t.base = r->slot[slot].arena.get();
-    t.frame_slot = r->slot[slot].states.get() + (size_t)r->max_batch * r->layout.words;
+    t.frame_slot = r->slot[slot].states.get() + (size_t)r->max_batch * r->lv[0].layout.words;
     return t;
 }
 
-// the scene as the plain kernels of worklist slot `slot` read it: on a timed scene, the five state-dependent tables are
-// the slot's own table set
-DeviceScene slot_scene(const b2d_renderer *r, int slot) {
-    DeviceScene d = r->ds;
-    const uint8_t *set = r->slot[slot].tables.get();
+// a level's scene as the kernels of worklist slot `slot` read it: on a timed scene, the five state-dependent tables are the
+// level's table set of that slot
+DeviceScene slot_scene(const LevelRes &lv, int slot) {
+    DeviceScene d = lv.ds;
+    const uint8_t *set = lv.slot[slot].tables.get();
     if (!set) return d;
-    const StateTables &t = r->state_tables;
+    const StateTables &t = lv.state_tables;
     d.tex = reinterpret_cast<const TexRec *>(set);
     d.sectors = reinterpret_cast<const SectorRec *>(set + t.off_sectors);
     d.segs = reinterpret_cast<const SegRec *>(set + t.off_segs);
@@ -193,14 +213,15 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
     int rc = frame_states ? ensure_states(r) : B2D_OK;
     if (rc == B2D_OK) rc = ensure_slot(r, s);
     if (rc != B2D_OK) return rc;
-    const bool restate = !frame_states && s.tables && s.state != r->state;
-    const size_t words = r->layout.words;
+    LevelRes &lv = r->lv[0];
+    const bool restate = !frame_states && lv.slot[slot].tables && lv.slot[slot].state != lv.state;
+    const size_t words = lv.layout.words;
     int nstates = 0;
     if (frame_states || restate) {
         CU(cudaEventSynchronize(s.states_copied.get()));     // the copy issued two batches ago has read the staging
         uint32_t *hs = s.h_states.get(), *hslot = hs + (size_t)r->max_batch * words;
         if (restate) {
-            std::memcpy(hs, r->state.data(), 4 * words);
+            std::memcpy(hs, lv.state.data(), 4 * words);
             nstates = 1;
         } else {
             // distinct states -> slots 0, 1, ... in order of first appearance, anywhere in the batch
@@ -223,17 +244,17 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
             CU(cudaMemcpyAsync(const_cast<uint32_t *>(stt.frame_slot), hs + (size_t)r->max_batch * words, 4 * (size_t)n,
                                cudaMemcpyHostToDevice, stream));
         CU(cudaEventRecord(s.states_copied.get(), stream));
-        uint8_t *sets = (frame_states ? s.arena : s.tables).get();
-        CU(launch_state_tables(r->src, s.states.get(), (uint32_t)words, nstates, sets, r->state_tables, stream));
+        uint8_t *sets = (frame_states ? s.arena : lv.slot[slot].tables).get();
+        CU(launch_state_tables(lv.src, s.states.get(), (uint32_t)words, nstates, sets, lv.state_tables, stream));
         r->launches += 1;
-        if (restate) s.state = r->state;
+        if (restate) lv.slot[slot].state = lv.state;
     }
     Event ev[2];
     if (r->profiling) {
         for (auto &e : ev) CU(event_create(e, cudaEventDefault));
         CU(cudaEventRecord(ev[0].get(), stream));
     }
-    CU(launch_walk(slot_scene(r, slot), r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background,
+    CU(launch_walk(slot_scene(lv, slot), r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background,
                    frame_states ? &stt : nullptr));
     if (r->profiling) {
         CU(cudaEventRecord(ev[1].get(), stream));
@@ -243,7 +264,75 @@ int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t str
     CU(cudaEventRecord(s.walk_done.get(), stream));
     s.n = n;
     s.per_frame = frame_states != nullptr;
+    s.per_level = false;
     s.sets = frame_states ? nstates : 0;
+    s.ticket = r->next_ticket;
+    s.rastered = false;
+    r->last_slot = slot;
+    r->launches += 1;
+    *ticket_out = r->next_ticket++;
+    return B2D_OK;
+}
+
+// BSP walk of a batch with per-frame levels (levels[i] < r->lv.size(), checked by the caller) into the next worklist slot,
+// as walk_into_slot.  The frame levels, the DeviceScene of every level as the slot reads it and the compact states of the
+// timed levels the batch uses whose table set of the slot is stale go to the device in one copy; each stale set is then
+// re-expanded (one launch per such level) before the walk.
+int walk_levels_into_slot(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, int n, cudaStream_t stream,
+                          int64_t *ticket_out, bool background) {
+    const int slot = (int)(r->next_ticket & 1);
+    WorkSlot &s = r->slot[slot];
+    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
+    int rc = ensure_levels(r);
+    if (rc == B2D_OK) rc = ensure_slot(r, s);
+    if (rc != B2D_OK) return rc;
+    CU(cudaEventSynchronize(s.levels_copied.get()));     // the copy issued two batches ago has read the staging
+    uint8_t *h = s.h_levels.get();
+    DeviceScene *scenes = reinterpret_cast<DeviceScene *>(h);
+    uint32_t *frame_level = reinterpret_cast<uint32_t *>(h + r->levels_frames_off);
+    const size_t nlev = r->lv.size();
+    std::vector<char> used(nlev, 0);
+    for (int f = 0; f < n; f++) {
+        frame_level[f] = levels[f];
+        used[levels[f]] = 1;
+    }
+    std::vector<size_t> stale;
+    for (size_t k = 0; k < nlev; k++) {
+        LevelRes &lv = r->lv[k];
+        scenes[k] = slot_scene(lv, slot);
+        if (used[k] && lv.slot[slot].tables && lv.slot[slot].state != lv.state) {
+            std::memcpy(h + lv.stage_off, lv.state.data(), 4 * lv.layout.words);
+            stale.push_back(k);
+        }
+    }
+    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
+    CU(cudaMemcpyAsync(s.levels.get(), h, r->levels_frames_off + 4 * (size_t)n, cudaMemcpyHostToDevice, stream));
+    CU(cudaEventRecord(s.levels_copied.get(), stream));
+    for (size_t k : stale) {
+        LevelRes &lv = r->lv[k];
+        CU(launch_state_tables(lv.src, reinterpret_cast<const uint32_t *>(s.levels.get() + lv.stage_off), (uint32_t)lv.layout.words,
+                               1, lv.slot[slot].tables.get(), lv.state_tables, stream));
+        r->launches += 1;
+        lv.slot[slot].state = lv.state;
+    }
+    Event ev[2];
+    if (r->profiling) {
+        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
+        CU(cudaEventRecord(ev[0].get(), stream));
+    }
+    const LevelTables lt{reinterpret_cast<const DeviceScene *>(s.levels.get()),
+                         reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off)};
+    CU(launch_walk_levels(lt, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background));
+    if (r->profiling) {
+        CU(cudaEventRecord(ev[1].get(), stream));
+        for (auto &e : ev) r->prof_events.push_back(std::move(e));
+        r->prof_kinds.push_back(0);
+    }
+    CU(cudaEventRecord(s.walk_done.get(), stream));
+    s.n = n;
+    s.per_frame = false;
+    s.per_level = true;
+    s.sets = 0;
     s.ticket = r->next_ticket;
     s.rastered = false;
     r->last_slot = slot;
@@ -257,7 +346,7 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
     WorkSlot &s = r->slot[slot];
     if (ticket < 0 || s.ticket != ticket || s.rastered) return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
     CU(cudaStreamWaitEvent(stream, s.walk_done.get(), 0));
-    if (r->ds.masked_list) {
+    if (r->d_masked) {
         // one arena of deferred masked entries per renderer: rasters that use it run one after the other (each fills the
         // machine on its own, so nothing is lost), whatever streams they were enqueued on
         CU(cudaStreamWaitEvent(stream, r->masked_done.get(), 0));
@@ -268,16 +357,23 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
         for (auto &e : ev) CU(event_create(e, cudaEventDefault));
         CU(cudaEventRecord(ev[0].get(), stream));
     }
-    const StateTables stt = s.per_frame ? slot_tables(r, slot) : StateTables{};
-    CU(launch_raster(slot_scene(r, slot), r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba, stream,
-                     s.per_frame ? &stt : nullptr));
+    if (s.per_level) {
+        const LevelTables lt{reinterpret_cast<const DeviceScene *>(s.levels.get()),
+                             reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off)};
+        CU(launch_raster_levels(lt, r->d_masked != nullptr, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index,
+                                d_rgba, stream));
+    } else {
+        const StateTables stt = s.per_frame ? slot_tables(r, slot) : StateTables{};
+        CU(launch_raster(slot_scene(r->lv[0], slot), r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba,
+                         stream, s.per_frame ? &stt : nullptr));
+    }
     if (r->profiling) {
         CU(cudaEventRecord(ev[1].get(), stream));
         for (auto &e : ev) r->prof_events.push_back(std::move(e));
         r->prof_kinds.push_back(1);
     }
     CU(cudaEventRecord(s.raster_done.get(), stream));
-    if (r->ds.masked_list) CU(cudaEventRecord(r->masked_done.get(), stream));
+    if (r->d_masked) CU(cudaEventRecord(r->masked_done.get(), stream));
     s.rastered = true;
     r->launches += 1;
     return B2D_OK;
@@ -300,14 +396,14 @@ void state_tables(const uint8_t *blob, uint32_t tics, const int32_t *floor_off, 
     scene_at_time(blob, tics, tex, sectors, segs, sprites, mids, floor_off, ceil_off);
 }
 
-// The compact state of level time `tics` with the renderer's current sector moves into out[layout.words] (out is not
-// r->state): the moved flag and the offsets, words 1 .. 2 + 2 * ndyn, do not depend on the time.
-void state_at(const b2d_renderer *r, uint32_t tics, uint32_t *out) {
-    compact_state(r->h_blob.data(), r->layout, tics, nullptr, nullptr, out);
-    std::copy(r->state.begin() + 1, r->state.begin() + 2 + 2 * (ptrdiff_t)r->layout.dyn_sectors.size(), out + 1);
+// The compact state of level time `tics` with the level's current sector moves into out[layout.words] (out is not
+// lv.state): the moved flag and the offsets, words 1 .. 2 + 2 * ndyn, do not depend on the time.
+void state_at(const LevelRes &lv, uint32_t tics, uint32_t *out) {
+    compact_state(lv.h_blob.data(), lv.layout, tics, nullptr, nullptr, out);
+    std::copy(lv.state.begin() + 1, lv.state.begin() + 2 + 2 * (ptrdiff_t)lv.layout.dyn_sectors.size(), out + 1);
 }
 
-// The compact state of every frame of a b2d_render_states-style call into `out` (r->layout.words words per frame), checking
+// The compact state of every frame of a b2d_render_states-style call into `out` (level 0's layout.words words per frame), checking
 // everything first: nothing is enqueued for a call with an invalid frame.  `out` stays empty for a scene without
 // time-dependent content or dynamic sectors: its frames all render with the per-batch tables.
 int build_states(const b2d_renderer *r, const b2d_frame_state *states, size_t n, const b2d_sector_move *moves, size_t n_moves,
@@ -317,25 +413,26 @@ int build_states(const b2d_renderer *r, const b2d_frame_state *states, size_t n,
     for (size_t i = 0; i < n; i++)
         if (states[i].first_move > n_moves || states[i].n_moves > n_moves - states[i].first_move)
             return fail(B2D_ERR_INVALID_ARG, "a frame's move range runs past the end of the move list");
-    if (r->h_blob.empty()) {
+    const LevelRes &lv = r->lv[0];
+    if (lv.h_blob.empty()) {
         for (size_t i = 0; i < n; i++)
             if (states[i].n_moves) return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
         return B2D_OK;
     }
-    const size_t words = r->layout.words;
+    const size_t words = lv.layout.words;
     out.resize(n * words);
     std::vector<int32_t> fo, co;
     for (size_t i = 0; i < n; i++) {
         bool moved = false;
         if (states[i].n_moves) {
-            if (const char *why = expand_moves(r->h_blob.data(), reinterpret_cast<const SectorMove *>(moves) + states[i].first_move,
+            if (const char *why = expand_moves(lv.h_blob.data(), reinterpret_cast<const SectorMove *>(moves) + states[i].first_move,
                                                states[i].n_moves, fo, co)) {
                 out.clear();
                 return fail(B2D_ERR_INVALID_ARG, why);
             }
             for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
         }
-        compact_state(r->h_blob.data(), r->layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
+        compact_state(lv.h_blob.data(), lv.layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
                       out.data() + i * words);
     }
     return B2D_OK;
@@ -344,10 +441,11 @@ int build_states(const b2d_renderer *r, const b2d_frame_state *states, size_t n,
 // b2d_render_timed: tics[i] with the renderer's current moves
 void timed_states(const b2d_renderer *r, const uint32_t *tics, size_t n, std::vector<uint32_t> &out) {
     out.clear();
-    if (r->h_blob.empty()) return;
-    const size_t words = r->layout.words;
+    const LevelRes &lv = r->lv[0];
+    if (lv.h_blob.empty()) return;
+    const size_t words = lv.layout.words;
     out.resize(n * words);
-    for (size_t i = 0; i < n; i++) state_at(r, tics[i], out.data() + i * words);
+    for (size_t i = 0; i < n; i++) state_at(lv, tics[i], out.data() + i * words);
 }
 
 }  // namespace
@@ -600,8 +698,131 @@ int b2d_view_init(b2d_view *v, int width, int height, double fov_y_degrees) {
 }
 
 // ---- renderer --------------------------------------------------------------------------------
-int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, int max_batch, b2d_renderer **out) {
-    if (!s || !view || !out || max_batch < 1) return fail(B2D_ERR_INVALID_ARG, "bad renderer arguments");
+namespace {
+// Level `lv` of renderer `r` (device, view and max_batch set) from scene `s`: the scene, its pre-lit planes and walk tables
+// on the device and, for a timed scene, its table set of each worklist slot at tic 0.  The DeviceScene's per-renderer fields
+// (yslope, status word, masked-entry arena) are the caller's.
+int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
+    const View &view = r->view;
+    const uint32_t *h = reinterpret_cast<const uint32_t *>(s->blob.data());
+    CU(allocate(lv.d_blob, s->blob.size()));
+    CU(cudaMemcpy(lv.d_blob.get(), s->blob.data(), s->blob.size(), cudaMemcpyHostToDevice));
+    const uint8_t *db = lv.d_blob.get();
+    {   // sky texture row per screen row (sky.frag:12-26 at pitch 0)
+        std::vector<uint16_t> sr((size_t)view.H, 0);
+        int32_t sky = (int32_t)h[H_SKY_TEX];
+        if (sky >= 0) {
+            const TexRec *tr = reinterpret_cast<const TexRec *>(s->blob.data() + h[H_OFF_TEX]) + sky;
+            for (int y = 0; y < view.H; y++) sr[(size_t)y] = (uint16_t)sky_row(y, view.H, (int32_t)tr->h);
+        }
+        CU(allocate(lv.d_skyrow, sr.size() * 2));
+        CU(cudaMemcpy(lv.d_skyrow.get(), sr.data(), sr.size() * 2, cudaMemcpyHostToDevice));
+    }
+    DeviceScene &d = lv.ds;
+    d.verts = reinterpret_cast<const int32_t *>(db + h[H_OFF_VERTS]);
+    d.nodes = reinterpret_cast<const NodeRec *>(db + h[H_OFF_NODES]);
+    d.ssectors = reinterpret_cast<const SSectorRec *>(db + h[H_OFF_SSECTORS]);
+    {   // the walk kernel's traversal tables in the layout of its shared memory (one cp.async.bulk per CTA)
+        const NodeRec *nodes = reinterpret_cast<const NodeRec *>(s->blob.data() + h[H_OFF_NODES]);
+        std::vector<int32_t> img(8 * (size_t)h[H_NNODES] + 4 * (size_t)h[H_NSSECTORS]);
+        for (uint32_t i = 0; i < h[H_NNODES]; i++) {
+            int32_t *o = &img[8 * (size_t)i];
+            o[0] = nodes[i].x; o[1] = nodes[i].y; o[2] = nodes[i].dx; o[3] = nodes[i].dy;
+            o[4] = (int32_t)nodes[i].child[0]; o[5] = (int32_t)nodes[i].child[1]; o[6] = 0; o[7] = 0;
+        }
+        if (h[H_NSSECTORS])
+            std::memcpy(&img[8 * (size_t)h[H_NNODES]], s->blob.data() + h[H_OFF_SSECTORS], sizeof(SSectorRec) * h[H_NSSECTORS]);
+        CU(allocate(lv.d_walk_static, img.size() * 4 + 16));
+        if (!img.empty()) CU(cudaMemcpy(lv.d_walk_static.get(), img.data(), img.size() * 4, cudaMemcpyHostToDevice));
+        d.walk_static = lv.d_walk_static.get();
+    }
+    d.segs = reinterpret_cast<const SegRec *>(db + h[H_OFF_SEGS]);
+    d.sectors = reinterpret_cast<const SectorRec *>(db + h[H_OFF_SECTORS]);
+    d.tex = reinterpret_cast<const TexRec *>(db + h[H_OFF_TEX]);
+    d.mids = reinterpret_cast<const MidRec *>(db + h[H_OFF_MIDS]);
+    d.nmids = (int32_t)h[H_NMIDS];
+    d.sprites = reinterpret_cast<const SpriteRec *>(db + h[H_OFF_SPRITES]);
+    d.nsprites = (int32_t)h[H_NSPRITES];
+    d.masked_list = nullptr; d.masked_counter = nullptr; d.masked_chunks = 0; d.masked_cap = 0;
+    if (d.nmids > 0 || d.nsprites > 0) d.masked_cap = strip_masked_cap(d.nmids, d.nsprites);
+    d.texels = db + h[H_OFF_TEXELS];
+    d.flats = db + h[H_OFF_FLATS];
+    d.colormap = db + h[H_OFF_COLORMAP];
+    d.palette = reinterpret_cast<const uint32_t *>(db + h[H_OFF_PALETTE]);
+    {   // pre-lit texel and flat planes: 32 x (texel bytes + flat bytes)
+        const size_t tstride = (h[H_TEXEL_BYTES] + 255u) & ~(size_t)255, fstride = (size_t)h[H_NFLATS] * 4096u;
+        if (tstride * 33 > 0xFFFFFFFFull || fstride * 32 > 0xFFFFFFFFull) return fail(B2D_ERR_INVALID_ARG, "level textures too large");
+        CU(allocate(lv.d_lit, 33 * tstride + 256));                    // plane 32 of the texels: opacity
+        lv.d_lit_flats = alloc_aligned_4g(r->device, 32 * fstride + 256);
+        if (!lv.d_lit_flats) return fail(B2D_ERR_NO_MEMORY, "no 4 GiB aligned device memory for the pre-lit flats");
+        CU(launch_prelight_textures(d.colormap, d.texels, d.tex, (int)h[H_NTEX], lv.d_lit.get(), tstride, nullptr));
+        CU(launch_prelight(d.colormap, d.flats, lv.d_lit_flats.get(), fstride, fstride, nullptr));
+        CU(cudaDeviceSynchronize());
+        d.lit_texels = lv.d_lit.get(); d.lit_flats = lv.d_lit_flats.get();     // low 32 address bits of lit_flats are zero
+        d.lit_texel_stride = (uint32_t)tstride; d.lit_flat_stride = (uint32_t)fstride;
+    }
+    d.skyrow = lv.d_skyrow.get();
+    d.nverts = (int32_t)h[H_NVERTS]; d.nnodes = (int32_t)h[H_NNODES]; d.nss = (int32_t)h[H_NSSECTORS];
+    d.nsegs = (int32_t)h[H_NSEGS]; d.nsectors = (int32_t)h[H_NSECTORS]; d.ntex = (int32_t)h[H_NTEX];
+    d.nflats = (int32_t)h[H_NFLATS]; d.sky_tex = (int32_t)h[H_SKY_TEX];
+    d.root = h[H_ROOT];
+    d.invF = (uint32_t)(4294967296ULL / (uint64_t)view.F);
+    if (d.nsegs + d.nsprites > 65535) return fail(B2D_ERR_INVALID_ARG, "level has more than 65535 segs + sprites");
+    if (walk_smem_per_warp(d) > 227 * 1024) return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory");
+    if (scene_is_timed(s->blob.data())) {
+        lv.h_blob = s->blob;
+        try {
+            lv.layout = state_layout(lv.h_blob.data());
+        } catch (const std::exception &ex) {
+            return fail(B2D_ERR_INVALID_ARG, ex.what());
+        }
+        const uint8_t *blob = lv.h_blob.data();
+        const StateLayout &L = lv.layout;
+        const size_t words = L.words;
+        // the state rule reads the blob's rest-state sections and the two slot maps
+        CU(allocate(lv.d_slot_maps, 4 * (L.sector_slots.size() + L.mid_seg.size()) + 4));
+        CU(cudaMemcpy(lv.d_slot_maps.get(), L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(lv.d_slot_maps.get() + L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
+        StateSrc &src = lv.src = state_src(blob, L);
+        auto on_device = [&](auto p) { return reinterpret_cast<decltype(p)>(db + (reinterpret_cast<const uint8_t *>(p) - blob)); };
+        src.tex = on_device(src.tex); src.sectors = on_device(src.sectors); src.segs = on_device(src.segs);
+        src.sprites = on_device(src.sprites); src.mids = on_device(src.mids); src.anim = on_device(src.anim);
+        src.flat_anim = on_device(src.flat_anim); src.segdyn = on_device(src.segdyn);
+        src.sector_slots = lv.d_slot_maps.get();
+        src.mid_seg = reinterpret_cast<const int32_t *>(lv.d_slot_maps.get() + L.sector_slots.size());
+        StateTables &t = lv.state_tables;              // one table set: [tex | sectors | segs | sprites | mids], 256 B aligned
+        t.slot_bytes = (uint32_t)((state_table_bytes(blob) + 255) & ~(size_t)255);
+        t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
+        t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
+        t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
+        t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
+        for (auto &sl : lv.slot) CU(allocate(sl.tables, t.slot_bytes));
+        // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306).  The
+        // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0.
+        lv.state.assign(words, 0);
+        compact_state(blob, L, 0, nullptr, nullptr, lv.state.data());
+        DeviceBuf<uint32_t> d_state;
+        CU(allocate(d_state, 4 * words));
+        CU(cudaMemcpy(d_state.get(), lv.state.data(), 4 * words, cudaMemcpyHostToDevice));
+        for (auto &sl : lv.slot) {
+            CU(launch_state_tables(lv.src, d_state.get(), (uint32_t)words, 1, sl.tables.get(), t, nullptr));
+            sl.state = lv.state;
+        }
+        CU(cudaDeviceSynchronize());
+    }
+    return B2D_OK;
+}
+}  // namespace
+
+// b2d_renderer_create_levels / b2d_renderer_create: the latter (level_walk = false) keeps accepting a level whose walk fits
+// the plain walk kernel but not the per-frame-level one (whose static shared memory comes on top); its level calls then
+// refuse before enqueuing anything.
+static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, const b2d_view *view, int device, int max_batch,
+                           b2d_renderer **out, bool level_walk) {
+    if (!scenes || !view || !out || max_batch < 1) return fail(B2D_ERR_INVALID_ARG, "bad renderer arguments");
+    if (n_levels < 1 || n_levels > B2D_MAX_LEVELS) return fail(B2D_ERR_INVALID_ARG, "n_levels out of range (1 .. B2D_MAX_LEVELS)");
+    for (size_t k = 0; k < n_levels; k++)
+        if (!scenes[k]) return fail(B2D_ERR_INVALID_ARG, "null scene");
     if (view->width < 1 || view->width > 4096 || view->height < 2 || view->height > 2160 || view->F < 2 || view->FY2 < 2)
         return fail(B2D_ERR_INVALID_ARG, "view out of range");
     int count = 0;
@@ -616,62 +837,39 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
     r->device = device;
     r->view = View{view->width, view->height, view->F, view->FY2};
     r->max_batch = max_batch;
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(s->blob.data());
-    r->stride = (int)(h[H_NSEGS] + h[H_NSPRITES]) > 0 ? (int)(h[H_NSEGS] + h[H_NSPRITES]) : 1;   // worklist entries per frame
-    CU(allocate(r->d_blob, s->blob.size()));
-    CU(cudaMemcpy(r->d_blob.get(), s->blob.data(), s->blob.size(), cudaMemcpyHostToDevice));
-    const uint8_t *db = r->d_blob.get();
+    int rc = guarded([&] { r->lv.resize(n_levels); return B2D_OK; });
+    if (rc != B2D_OK) return rc;
+    for (size_t k = 0; k < n_levels; k++) {
+        rc = guarded([&] { return create_level(r.get(), r->lv[k], scenes[k]); });
+        if (rc != B2D_OK) return rc;
+    }
+    // what the levels share: the worklist stride, the walk's shared memory, the masked-entry arena, yslope and the status word
+    r->stride = 1;
+    int32_t masked_cap = 0;
+    for (const LevelRes &lv : r->lv) {
+        r->stride = std::max(r->stride, lv.ds.nsegs + lv.ds.nsprites);            // worklist entries per frame
+        r->walk_smem = std::max(r->walk_smem, walk_smem_per_warp(lv.ds));
+        masked_cap = std::max(masked_cap, lv.ds.masked_cap);
+    }
+    if (level_walk && r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
+        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
     std::vector<uint32_t> ys((size_t)view->height);
     for (int y = 0; y < view->height; y++) ys[(size_t)y] = yslope_entry(y, r->view);
     CU(allocate(r->d_yslope, ys.size() * 4));
     CU(cudaMemcpy(r->d_yslope.get(), ys.data(), ys.size() * 4, cudaMemcpyHostToDevice));
-    {   // sky texture row per screen row (sky.frag:12-26 at pitch 0)
-        std::vector<uint16_t> sr((size_t)view->height, 0);
-        int32_t sky = (int32_t)h[H_SKY_TEX];
-        if (sky >= 0) {
-            const TexRec *tr = reinterpret_cast<const TexRec *>(s->blob.data() + h[H_OFF_TEX]) + sky;
-            for (int y = 0; y < view->height; y++) sr[(size_t)y] = (uint16_t)sky_row(y, view->height, (int32_t)tr->h);
-        }
-        CU(allocate(r->d_skyrow, sr.size() * 2));
-        CU(cudaMemcpy(r->d_skyrow.get(), sr.data(), sr.size() * 2, cudaMemcpyHostToDevice));
-    }
-    DeviceScene &d = r->ds;
-    d.verts = reinterpret_cast<const int32_t *>(db + h[H_OFF_VERTS]);
-    d.nodes = reinterpret_cast<const NodeRec *>(db + h[H_OFF_NODES]);
-    d.ssectors = reinterpret_cast<const SSectorRec *>(db + h[H_OFF_SSECTORS]);
-    {   // the walk kernel's traversal tables in the layout of its shared memory (one cp.async.bulk per CTA)
-        const NodeRec *nodes = reinterpret_cast<const NodeRec *>(s->blob.data() + h[H_OFF_NODES]);
-        std::vector<int32_t> img(8 * (size_t)h[H_NNODES] + 4 * (size_t)h[H_NSSECTORS]);
-        for (uint32_t i = 0; i < h[H_NNODES]; i++) {
-            int32_t *o = &img[8 * (size_t)i];
-            o[0] = nodes[i].x; o[1] = nodes[i].y; o[2] = nodes[i].dx; o[3] = nodes[i].dy;
-            o[4] = (int32_t)nodes[i].child[0]; o[5] = (int32_t)nodes[i].child[1]; o[6] = 0; o[7] = 0;
-        }
-        if (h[H_NSSECTORS])
-            std::memcpy(&img[8 * (size_t)h[H_NNODES]], s->blob.data() + h[H_OFF_SSECTORS], sizeof(SSectorRec) * h[H_NSSECTORS]);
-        CU(allocate(r->d_walk_static, img.size() * 4 + 16));
-        if (!img.empty()) CU(cudaMemcpy(r->d_walk_static.get(), img.data(), img.size() * 4, cudaMemcpyHostToDevice));
-        d.walk_static = r->d_walk_static.get();
-    }
-    d.segs = reinterpret_cast<const SegRec *>(db + h[H_OFF_SEGS]);
-    d.sectors = reinterpret_cast<const SectorRec *>(db + h[H_OFF_SECTORS]);
-    d.tex = reinterpret_cast<const TexRec *>(db + h[H_OFF_TEX]);
-    d.mids = reinterpret_cast<const MidRec *>(db + h[H_OFF_MIDS]);
-    d.nmids = (int32_t)h[H_NMIDS];
-    d.sprites = reinterpret_cast<const SpriteRec *>(db + h[H_OFF_SPRITES]);
-    d.nsprites = (int32_t)h[H_NSPRITES];
-    d.masked_list = nullptr; d.masked_counter = nullptr; d.masked_chunks = 0; d.masked_cap = 0;
-    if (d.nmids > 0 || d.nsprites > 0) {
+    CU(allocate(r->d_status, sizeof(int32_t)));
+    CU(cudaMemset(r->d_status.get(), 0, sizeof(int32_t)));
+    uint32_t masked_chunks = 0;
+    if (masked_cap > 0) {
         // arena of deferred masked entries: chunks of kMaskedChunk entries handed out on demand.  Sized for the worst case
-        // -- every (frame, 32-column strip) of a full batch at its cap -- whenever that takes at most kMaskedArenaBudget, so
-        // that no valid batch can run out of it: a crowded subsector puts dozens of sprites into every strip of a 1080p
-        // frame.  Past the budget (1080p batches of more than ~1000 frames, 4K of more than ~500, with a cap of 128) two
-        // chunks per strip on average, at least 4096: frames usually defer a handful of entries per strip, and a batch
-        // that needs more reports kStatusMaskedFull instead of drawing wrong pixels.
+        // -- every (frame, 32-column strip) of a full batch at its cap (the largest of the levels) -- whenever that takes
+        // at most kMaskedArenaBudget, so that no valid batch can run out of it: a crowded subsector puts dozens of sprites
+        // into every strip of a 1080p frame.  Past the budget (1080p batches of more than ~1000 frames, 4K of more than
+        // ~500, with a cap of 128) two chunks per strip on average, at least 4096: frames usually defer a handful of
+        // entries per strip, and a batch that needs more reports kStatusMaskedFull instead of drawing wrong pixels.
         constexpr size_t kMaskedArenaBudget = (size_t)1 << 30;
         const size_t strips = (size_t)(view->width + 31) / 32;
-        d.masked_cap = strip_masked_cap(d.nmids, d.nsprites);
-        const size_t per_strip = ((size_t)d.masked_cap + kMaskedChunk - 1) / kMaskedChunk;
+        const size_t per_strip = ((size_t)masked_cap + kMaskedChunk - 1) / kMaskedChunk;
         const size_t worst = strips * (size_t)max_batch * per_strip;
         size_t chunks = worst;
         if (sizeof(uint32_t) * 33 * kMaskedChunk * worst > kMaskedArenaBudget) {
@@ -681,104 +879,69 @@ int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, in
         }
         if (const char *env = getenv("B2D_MASKED_CHUNKS")) chunks = (size_t)strtoull(env, nullptr, 0);   // tests: force exhaustion
         if (chunks < 1) chunks = 1;
-        d.masked_chunks = (uint32_t)chunks;
+        masked_chunks = (uint32_t)chunks;
         CU(allocate(r->d_masked, sizeof(uint32_t) * 33 * kMaskedChunk * chunks));
         CU(allocate(r->d_masked_counter, sizeof(uint32_t)));
         CU(cudaMemset(r->d_masked_counter.get(), 0, sizeof(uint32_t)));
         CU(event_create(r->masked_done));
         CU(cudaEventRecord(r->masked_done.get(), nullptr));
-        d.masked_list = r->d_masked.get();
-        d.masked_counter = r->d_masked_counter.get();
     }
-    d.texels = db + h[H_OFF_TEXELS];
-    d.flats = db + h[H_OFF_FLATS];
-    d.colormap = db + h[H_OFF_COLORMAP];
-    d.palette = reinterpret_cast<const uint32_t *>(db + h[H_OFF_PALETTE]);
-    {   // pre-lit texel and flat planes: 32 x (texel bytes + flat bytes)
-        const size_t tstride = (h[H_TEXEL_BYTES] + 255u) & ~(size_t)255, fstride = (size_t)h[H_NFLATS] * 4096u;
-        if (tstride * 33 > 0xFFFFFFFFull || fstride * 32 > 0xFFFFFFFFull) return fail(B2D_ERR_INVALID_ARG, "level textures too large");
-        CU(allocate(r->d_lit, 33 * tstride + 256));                    // plane 32 of the texels: opacity
-        r->d_lit_flats = alloc_aligned_4g(device, 32 * fstride + 256);
-        if (!r->d_lit_flats) return fail(B2D_ERR_NO_MEMORY, "no 4 GiB aligned device memory for the pre-lit flats");
-        CU(launch_prelight_textures(d.colormap, d.texels, d.tex, (int)h[H_NTEX], r->d_lit.get(), tstride, nullptr));
-        CU(launch_prelight(d.colormap, d.flats, r->d_lit_flats.get(), fstride, fstride, nullptr));
-        CU(cudaDeviceSynchronize());
-        d.lit_texels = r->d_lit.get(); d.lit_flats = r->d_lit_flats.get();     // low 32 address bits of lit_flats are zero
-        d.lit_texel_stride = (uint32_t)tstride; d.lit_flat_stride = (uint32_t)fstride;
-    }
-    d.yslope = r->d_yslope.get();
-    d.skyrow = r->d_skyrow.get();
-    CU(allocate(r->d_status, sizeof(int32_t)));
-    CU(cudaMemset(r->d_status.get(), 0, sizeof(int32_t)));
-    d.status_flag = r->d_status.get();
-    d.nverts = (int32_t)h[H_NVERTS]; d.nnodes = (int32_t)h[H_NNODES]; d.nss = (int32_t)h[H_NSSECTORS];
-    d.nsegs = (int32_t)h[H_NSEGS]; d.nsectors = (int32_t)h[H_NSECTORS]; d.ntex = (int32_t)h[H_NTEX];
-    d.nflats = (int32_t)h[H_NFLATS]; d.sky_tex = (int32_t)h[H_SKY_TEX];
-    d.root = h[H_ROOT];
-    d.invF = (uint32_t)(4294967296ULL / (uint64_t)view->F);
-    if (d.nsegs + d.nsprites > 65535) return fail(B2D_ERR_INVALID_ARG, "level has more than 65535 segs + sprites");
-    if (walk_smem_per_warp(d) > 227 * 1024) return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory");
-    if (scene_is_timed(s->blob.data())) {
-        r->h_blob = s->blob;
-        try {
-            r->layout = state_layout(r->h_blob.data());
-        } catch (const std::exception &ex) {
-            return fail(B2D_ERR_INVALID_ARG, ex.what());
+    // per-frame levels: [DeviceScene per level | compact state per timed level | frame levels] in each slot's level buffer
+    size_t off = (r->lv.size() * sizeof(DeviceScene) + 15) & ~(size_t)15;
+    for (LevelRes &lv : r->lv) {
+        DeviceScene &d = lv.ds;
+        d.yslope = r->d_yslope.get();
+        d.status_flag = r->d_status.get();
+        if (d.masked_cap > 0) {
+            d.masked_list = r->d_masked.get();
+            d.masked_counter = r->d_masked_counter.get();
+            d.masked_chunks = masked_chunks;
         }
-        const uint8_t *blob = r->h_blob.data();
-        const StateLayout &L = r->layout;
-        const size_t words = L.words, mb = (size_t)max_batch;
-        // the state rule reads the blob's rest-state sections and the two slot maps
-        CU(allocate(r->d_slot_maps, 4 * (L.sector_slots.size() + L.mid_seg.size()) + 4));
-        CU(cudaMemcpy(r->d_slot_maps.get(), L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(r->d_slot_maps.get() + L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
-        StateSrc &src = r->src = state_src(blob, L);
-        auto on_device = [&](auto p) { return reinterpret_cast<decltype(p)>(db + (reinterpret_cast<const uint8_t *>(p) - blob)); };
-        src.tex = on_device(src.tex); src.sectors = on_device(src.sectors); src.segs = on_device(src.segs);
-        src.sprites = on_device(src.sprites); src.mids = on_device(src.mids); src.anim = on_device(src.anim);
-        src.flat_anim = on_device(src.flat_anim); src.segdyn = on_device(src.segdyn);
-        src.sector_slots = r->d_slot_maps.get();
-        src.mid_seg = reinterpret_cast<const int32_t *>(r->d_slot_maps.get() + L.sector_slots.size());
-        StateTables &t = r->state_tables;              // one table set: [tex | sectors | segs | sprites | mids], 256 B aligned
-        t.slot_bytes = (uint32_t)((state_table_bytes(blob) + 255) & ~(size_t)255);
-        t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
-        t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
-        t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
-        t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
+        lv.stage_off = off;
+        off += 4 * lv.layout.words;
+    }
+    r->levels_frames_off = (off + 15) & ~(size_t)15;
+    if (!r->lv[0].h_blob.empty()) {
+        // level 0's per-frame states and the restates of its plain batches: compact states + set indices and their staging
+        const size_t words = r->lv[0].layout.words, mb = (size_t)max_batch;
         for (WorkSlot &sl : r->slot) {
-            CU(allocate(sl.tables, t.slot_bytes));
             CU(allocate(sl.states, 4 * mb * (words + 1)));
             CU(allocate(sl.h_states, 4 * mb * (words + 1)));
             CU(event_create(sl.states_copied));
         }
-        // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306).  The
-        // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0.
-        r->state.assign(words, 0);
-        compact_state(blob, L, 0, nullptr, nullptr, r->state.data());
-        CU(cudaMemcpy(r->slot[0].states.get(), r->state.data(), 4 * words, cudaMemcpyHostToDevice));
-        for (WorkSlot &sl : r->slot) {
-            CU(launch_state_tables(r->src, r->slot[0].states.get(), (uint32_t)words, 1, sl.tables.get(), t, nullptr));
-            sl.state = r->state;
-        }
-        CU(cudaDeviceSynchronize());
     }
     CU(allocate(r->d_poses, sizeof(Pose) * (size_t)max_batch));
-    int rc = ensure_slot(r.get(), r->slot[0]);
+    rc = ensure_slot(r.get(), r->slot[0]);
     if (rc == B2D_OK) *out = r.release();
     return rc;
+}
+
+int b2d_renderer_create_levels(const b2d_scene *const *scenes, size_t n_levels, const b2d_view *view, int device, int max_batch,
+                               b2d_renderer **out) {
+    return create_renderer(scenes, n_levels, view, device, max_batch, out, true);
+}
+
+int b2d_renderer_create(const b2d_scene *s, const b2d_view *view, int device, int max_batch, b2d_renderer **out) {
+    if (!s) return fail(B2D_ERR_INVALID_ARG, "bad renderer arguments");
+    return create_renderer(&s, 1, view, device, max_batch, out, false);
 }
 
 void b2d_renderer_destroy(b2d_renderer *r) { delete r; }
 
 // The renderer's own state is host data: the setters enqueue nothing (the stream is kept for ABI compatibility), and the
-// next plain batch of each worklist slot expands it into the slot's table set.
+// next batch of each worklist slot that uses a level expands the level's state into the level's table set of the slot.
+// The time is every level's.
 int b2d_renderer_set_time(b2d_renderer *r, uint32_t tics) {
     if (!r) return fail(B2D_ERR_INVALID_ARG, "null renderer");
-    if (r->h_blob.empty()) { r->tics = tics; return B2D_OK; }
     return guarded([&] {
-        std::vector<uint32_t> s(r->layout.words);
-        state_at(r, tics, s.data());
-        r->state.swap(s);
+        std::vector<std::vector<uint32_t>> st(r->lv.size());
+        for (size_t k = 0; k < r->lv.size(); k++) {
+            if (r->lv[k].h_blob.empty()) continue;
+            st[k].resize(r->lv[k].layout.words);
+            state_at(r->lv[k], tics, st[k].data());
+        }
+        for (size_t k = 0; k < r->lv.size(); k++)
+            if (!r->lv[k].h_blob.empty()) r->lv[k].state.swap(st[k]);
         r->tics = tics;
         return B2D_OK;
     });
@@ -786,23 +949,29 @@ int b2d_renderer_set_time(b2d_renderer *r, uint32_t tics) {
 
 int b2d_renderer_set_time_async(b2d_renderer *r, uint32_t tics, void *) { return b2d_renderer_set_time(r, tics); }
 
-int b2d_renderer_set_sector_moves(b2d_renderer *r, const b2d_sector_move *moves, size_t n) {
+int b2d_renderer_set_level_sector_moves(b2d_renderer *r, int level, const b2d_sector_move *moves, size_t n) {
     if (!r || (n && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (r->h_blob.empty()) {
+    if (level < 0 || (size_t)level >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "level index out of range");
+    LevelRes &lv = r->lv[(size_t)level];
+    if (lv.h_blob.empty()) {
         if (n == 0) return B2D_OK;
         return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
     }
     static_assert(sizeof(b2d_sector_move) == sizeof(SectorMove), "ABI record");
     return guarded([&] {
         std::vector<int32_t> fo, co;
-        if (const char *why = expand_moves(r->h_blob.data(), reinterpret_cast<const SectorMove *>(moves), n, fo, co))
+        if (const char *why = expand_moves(lv.h_blob.data(), reinterpret_cast<const SectorMove *>(moves), n, fo, co))
             return fail(B2D_ERR_INVALID_ARG, why);
         bool moved = false;
         for (size_t i = 0; i < fo.size() && !moved; i++) moved = fo[i] != 0 || co[i] != 0;      // all zero: at rest
-        compact_state(r->h_blob.data(), r->layout, r->tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
-                      r->state.data());
+        compact_state(lv.h_blob.data(), lv.layout, r->tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
+                      lv.state.data());
         return B2D_OK;
     });
+}
+
+int b2d_renderer_set_sector_moves(b2d_renderer *r, const b2d_sector_move *moves, size_t n) {
+    return b2d_renderer_set_level_sector_moves(r, 0, moves, n);
 }
 
 int b2d_renderer_set_sector_moves_async(b2d_renderer *r, const b2d_sector_move *moves, size_t n, void *) {
@@ -830,14 +999,14 @@ int b2d_render_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, uint8_
                           static_cast<cudaStream_t>(cuda_stream));
 }
 
-// frames_states (nullable, r->layout.words words per frame): walk + raster of n device poses in batches of max_batch
+// frames_states (nullable, level 0's layout.words words per frame): walk + raster of n device poses in batches of max_batch
 static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, size_t n, const uint32_t *frame_states, uint8_t *d_index_fb,
                            uint32_t *d_rgba_fb, cudaStream_t st) {
     const size_t npix = (size_t)r->view.W * r->view.H;
     for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
         const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
         int rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, (int)cnt, d_index_fb + i * npix,
-                                d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st, frame_states ? frame_states + i * r->layout.words : nullptr);
+                                d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st, frame_states ? frame_states + i * r->lv[0].layout.words : nullptr);
         if (rc != B2D_OK) return rc;
     }
     return B2D_OK;
@@ -893,9 +1062,57 @@ int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint
     return raster_from_slot(r, ticket, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
-// Host poses in, host frames out; frame_states as in enqueue_frames (for all n frames)
+// Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
+// per-frame-level walk (a b2d_renderer_create renderer may not; checked before anything is enqueued)
+static int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
+    if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
+    if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
+        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
+    for (size_t i = 0; i < n; i++)
+        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    return B2D_OK;
+}
+
+// walk -> raster of a batch with per-frame levels on `stream`
+static int enqueue_level_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, int n, uint8_t *d_index,
+                                uint32_t *d_rgba, cudaStream_t stream) {
+    int64_t ticket = -1;
+    int rc = walk_levels_into_slot(r, d_poses, levels, n, stream, &ticket, false);
+    if (rc != B2D_OK) return rc;
+    return raster_from_slot(r, ticket, d_index, d_rgba, stream);
+}
+
+int b2d_render_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, uint8_t *d_index_fb,
+                             uint32_t *d_rgba_fb, void *cuda_stream) {
+    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    int rc = check_levels(r, levels, n);
+    if (rc != B2D_OK || n == 0) return rc;
+    CU(cudaSetDevice(r->device));
+    const size_t npix = (size_t)r->view.W * r->view.H;
+    for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
+        const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
+        rc = enqueue_level_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, levels + i, (int)cnt, d_index_fb + i * npix,
+                                  d_rgba_fb ? d_rgba_fb + i * npix : nullptr, static_cast<cudaStream_t>(cuda_stream));
+        if (rc != B2D_OK) return rc;
+    }
+    return B2D_OK;
+}
+
+int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, void *cuda_stream,
+                           int64_t *ticket_out) {
+    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
+    int rc = check_levels(r, levels, n);
+    if (rc != B2D_OK) return rc;
+    CU(cudaSetDevice(r->device));
+    return walk_levels_into_slot(r, reinterpret_cast<const Pose *>(d_poses), levels, (int)n, static_cast<cudaStream_t>(cuda_stream),
+                                 ticket_out, true);
+}
+
+// Host poses in, host frames out; frame_states as in enqueue_frames (for all n frames), or (exclusive with it) frame_levels:
+// the level of each of the n frames
 static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const uint32_t *frame_states, uint8_t *index_fb,
-                       uint32_t *rgba_fb) {
+                       uint32_t *rgba_fb, const uint32_t *frame_levels = nullptr) {
     if (n == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
@@ -930,8 +1147,11 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const u
         std::memcpy(hp, poses + done, sizeof(Pose) * (size_t)cnt);
         cudaStream_t rs = hs.render_stream.get(), cs = hs.copy_stream[buf].get();
         CU(cudaMemcpyAsync(r->d_poses.get(), hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, rs));
-        int rc = enqueue_frames(r, r->d_poses.get(), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs,
-                                frame_states ? frame_states + done * r->layout.words : nullptr);
+        int rc = frame_levels
+                     ? enqueue_level_frames(r, r->d_poses.get(), frame_levels + done, cnt, hs.index[buf].get(),
+                                            rgba_fb ? hs.rgba[buf].get() : nullptr, rs)
+                     : enqueue_frames(r, r->d_poses.get(), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs,
+                                      frame_states ? frame_states + done * r->lv[0].layout.words : nullptr);
         if (rc != B2D_OK) return rc;
         CU(cudaEventRecord(hs.rendered[buf].get(), rs));
         CU(cudaStreamWaitEvent(cs, hs.rendered[buf].get(), 0));
@@ -982,10 +1202,18 @@ int b2d_render_states(b2d_renderer *r, const b2d_pose *poses, const b2d_frame_st
     return render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
 }
 
+int b2d_render_levels(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, size_t n, uint8_t *index_fb,
+                      uint32_t *rgba_fb) {
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    int rc = check_levels(r, levels, n);
+    if (rc != B2D_OK) return rc;
+    return render_host(r, poses, n, nullptr, index_fb, rgba_fb, levels);
+}
+
 int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_rgba, size_t n_pixels, void *cuda_stream) {
     if (!r || !d_index || !d_rgba) return fail(B2D_ERR_INVALID_ARG, "null argument");
     CU(cudaSetDevice(r->device));
-    CU(launch_palette(r->ds.palette, d_index, d_rgba, n_pixels, static_cast<cudaStream_t>(cuda_stream)));
+    CU(launch_palette(r->lv[0].ds.palette, d_index, d_rgba, n_pixels, static_cast<cudaStream_t>(cuda_stream)));
     r->launches += 1;
     return B2D_OK;
 }
@@ -1047,17 +1275,18 @@ int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
 
 int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capacity, size_t *size_out) {
     if (!r) return fail(B2D_ERR_INVALID_ARG, "null renderer");
-    if (r->h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
+    const LevelRes &lv = r->lv[0];
+    if (lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
     const WorkSlot &s = r->slot[r->last_slot];
     if (s.ticket < 0) return fail(B2D_ERR_INVALID_ARG, "no batch has been walked");
     if (set >= (s.per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
-    const size_t need = state_table_bytes(r->h_blob.data());
+    const size_t need = state_table_bytes(lv.h_blob.data());
     if (size_out) *size_out = need;
     if (!out) return B2D_OK;
     if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
-    const uint8_t *src = s.per_frame ? s.arena.get() + set * (size_t)r->state_tables.slot_bytes : s.tables.get();
+    const uint8_t *src = s.per_frame ? s.arena.get() + set * (size_t)lv.state_tables.slot_bytes : lv.slot[r->last_slot].tables.get();
     CU(cudaMemcpy(out, src, need, cudaMemcpyDeviceToHost));
     return B2D_OK;
 }

@@ -86,10 +86,14 @@ struct WorkSlot {
     int64_t ticket = -1;
     bool rastered = true;
     bool per_frame = false;                               // the batch was walked with per-frame states
+    bool per_level = false;                               // ... or with per-frame levels
     int sets = 0;                                         // ... into this many table sets of the arena (distinct states)
-    // timed scenes: the table set the slot's plain batches read and the compact state it was expanded from
-    DeviceBuf<uint8_t> tables;
-    std::vector<uint32_t> state;
+    // per-frame levels (b2d_render_levels & co.; allocated by the first such call): [the DeviceScene of every level as this
+    // slot's batches read it | the compact states of the levels whose table sets a batch re-expands | each frame's level]
+    // on the device, and its pinned staging
+    DeviceBuf<uint8_t> levels;
+    PinnedBuf<uint8_t> h_levels;
+    Event levels_copied;                                  // h_levels has been read by its copy
     // per-frame states (b2d_render_states & co.): an arena of up to max_batch expanded table sets (allocated by the first
     // such call), and the compact states + per-frame set indices on the device and their pinned staging, shared with the
     // expansion of the slot's own table set
@@ -108,38 +112,53 @@ struct HostStaging {
     std::array<DeviceBuf<uint32_t>, 2> rgba;              // created by the first call that asks for RGBA frames
 };
 
-struct b2d_renderer {
-    int device = 0;
-    View view{};
-    int max_batch = 0;
-    int stride = 0;                 // worklist entries per frame (= n_segs + n_sprites)
+// One level of a renderer (b2d_renderer_create_levels; b2d_renderer_create makes a set of one): the scene on the device
+// and what the kernels read of it.
+struct LevelRes {
     DeviceBuf<uint8_t> d_blob;
-    DeviceBuf<uint32_t> d_yslope;
-    DeviceBuf<uint16_t> d_skyrow;
-    DeviceBuf<int32_t> d_status;
-    DeviceBuf<uint32_t> d_masked;
+    DeviceBuf<uint16_t> d_skyrow;                         // sky texture row of each screen row (the level's sky height)
     DeviceBuf<uint8_t> d_lit;       // colormap-applied copies of the texels (32 light rows + the opacity plane)
     // ... and of the flats, in a region whose address is a multiple of 4 GiB: the raster then forms a flat texel's address
     // as {high word, 32-bit offset} without a 64-bit add (one instruction per flat pixel).  Reserved + mapped through the
     // driver's virtual-memory API (cuMemAddressReserve takes an alignment); an over-sized cudaMalloc is the fall-back.
     Aligned4G d_lit_flats;
-    DeviceScene ds{};
-    DeviceBuf<Pose> d_poses;
-    WorkSlot slot[2];
-    int64_t next_ticket = 0;
-    int last_slot = 0;
-    std::unique_ptr<HostStaging> host;
     DeviceBuf<uint8_t> d_walk_static;                     // node / subsector tables as the walk kernel's shared memory holds them
+    DeviceScene ds{};
     // Scenes with time-dependent content or dynamic sectors (DESIGN.md §3 "State arena"); the rest stays empty.  The
     // device blob is never written after creation: the state rule reads its rest-state sections, and every batch reads
     // its five state-dependent tables from a table set expanded on the device from a compact state.
     std::vector<uint8_t> h_blob;                          // host copy of the scene
     StateLayout layout;
-    uint32_t tics = 0;
-    std::vector<uint32_t> state;                          // the renderer's own compact state (set_time, set_sector_moves)
+    std::vector<uint32_t> state;                          // the level's own compact state (set_time, set_*sector_moves)
     DeviceBuf<uint32_t> d_slot_maps;                      // StateLayout::sector_slots, then ::mid_seg
     StateSrc src{};                                       // device pointers into d_blob and d_slot_maps
     StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
+    size_t stage_off = 0;                                 // byte offset of its compact state in WorkSlot::levels
+    // per worklist slot: the table set the slot's batches read and the compact state it was expanded from
+    struct Slot {
+        DeviceBuf<uint8_t> tables;
+        std::vector<uint32_t> state;
+    } slot[2];
+};
+
+struct b2d_renderer {
+    int device = 0;
+    View view{};
+    int max_batch = 0;
+    int stride = 0;                 // worklist entries per frame (= the largest n_segs + n_sprites of the levels)
+    size_t walk_smem = 0;           // the largest walk_smem_per_warp of the levels
+    // the levels; every entry point without a level argument acts on level 0
+    std::vector<LevelRes> lv;
+    size_t levels_frames_off = 0;   // byte offset of the frame levels in WorkSlot::levels
+    DeviceBuf<uint32_t> d_yslope;
+    DeviceBuf<int32_t> d_status;
+    DeviceBuf<uint32_t> d_masked;   // one arena of deferred masked entries for every level with masked content
+    DeviceBuf<Pose> d_poses;
+    WorkSlot slot[2];
+    int64_t next_ticket = 0;
+    int last_slot = 0;
+    std::unique_ptr<HostStaging> host;
+    uint32_t tics = 0;
     Event masked_done;                                    // last raster that used the masked-entry arena
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;

@@ -123,10 +123,12 @@ __device__ __forceinline__ const T *state_table(const T *plain, const uint8_t *t
     return kStates ? reinterpret_cast<const T *>(tb + off) : plain;
 }
 
-template <bool kStates>
+template <bool kStates, bool kLevels>
 __global__ void __launch_bounds__(128, 7)     // 7 CTAs/SM (72 registers): 924 frames resident on an H100's 132 SMs
-b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const Pose *__restrict__ poses, int n,
-                FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride, const __grid_constant__ StateTables st) {
+b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant__ View vw, const Pose *__restrict__ poses, int n,
+                FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride, const __grid_constant__ StateTables st,
+                const __grid_constant__ LevelTables lt) {
+    static_assert(!(kStates && kLevels), "per-frame states and per-frame levels are exclusive");
     // One CTA per frame.  The per-frame setup (steps 1-3) and the worklist records (step 5) are data-parallel and
     // use all 128 threads; the traversal itself (step 4) is sequential and runs in warp 0 with the lanes working
     // on the segs of a subsector / the words of the column mask.  The kernel is latency-bound (one frame = one
@@ -134,7 +136,15 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tid = threadIdx.x, nthr = blockDim.x;
-    const WalkSmem L = walk_layout(sc.nverts, sc.nsegs, sc.nnodes, sc.nss, sc.nsprites);
+    // Per-frame levels: the scene of the level resident in this CTA (copied from lt.scenes when a frame's level differs
+    // from it); the shared-memory layout below and the traversal tables in it are that level's.
+    DeviceScene *s_level = nullptr;
+    if constexpr (kLevels) {
+        __shared__ DeviceScene s_lv;
+        s_level = &s_lv;
+    }
+    const DeviceScene &sc = kLevels ? *s_level : scene;
+    WalkSmem L = kLevels ? WalkSmem{} : walk_layout(sc.nverts, sc.nsegs, sc.nnodes, sc.nss, sc.nsprites);   // levels: per frame
     uint8_t *base = smem;
     __shared__ int s_count, s_status;
     __shared__ __align__(8) uint64_t s_bar;
@@ -154,9 +164,16 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
     // under another batch's raster -- a CTA per SM keeps the walk's footprint at 1/8 of the register file while it takes
     // a few frame latencies, all hidden behind the raster (launch_walk).
     // The traversal tables (node partition lines + children, subsector records) do not depend on the frame: one bulk copy
-    // per CTA brings them into shared memory while the threads are busy with steps 1-3 of the first frame.
-    const uint32_t static_bytes = 32u * (uint32_t)sc.nnodes + 16u * (uint32_t)sc.nss;
+    // per CTA brings them into shared memory while the threads are busy with steps 1-3 of the first frame.  With per-frame
+    // levels they are copied again whenever a frame's level differs from the resident one (each copy completes one phase
+    // of the mbarrier: `parity` is the phase the next wait is for).
+    uint32_t static_bytes = 0, parity = 0, resident = 0xFFFFFFFFu;
     bool static_pending = false;
+    if constexpr (kLevels) {
+        if (tid == 0) mbar_init(&s_bar, 1);
+    } else {
+        static_bytes = 32u * (uint32_t)sc.nnodes + 16u * (uint32_t)sc.nss;
+    }
     if (static_bytes) {
         if (tid == 0) mbar_init(&s_bar, 1);
         __syncthreads();
@@ -164,6 +181,36 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
         static_pending = true;
     }
     for (int frame = blockIdx.x; frame < n; frame += gridDim.x) {
+    if constexpr (kLevels) {
+        const uint32_t level = lt.frame_level[frame];
+        if (level != resident) {
+            // The previous frame ended in __syncthreads(): nothing reads the old scene or tables any more.  Generic-proxy
+            // accesses to the shared memory the bulk copy overwrites are ordered before it (fence.proxy.async).
+            const uint32_t *src = reinterpret_cast<const uint32_t *>(lt.scenes + level);
+            uint32_t *dst = reinterpret_cast<uint32_t *>(s_level);
+            for (int i = tid; i < (int)(sizeof(DeviceScene) / 4); i += nthr) dst[i] = src[i];
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncthreads();
+            L = walk_layout(sc.nverts, sc.nsegs, sc.nnodes, sc.nss, sc.nsprites);
+            tx = reinterpret_cast<int32_t *>(base + L.off_tx);
+            tz = reinterpret_cast<int32_t *>(base + L.off_tz);
+            segr = reinterpret_cast<uint32_t *>(base + L.off_segr);
+            boxr = reinterpret_cast<uint32_t *>(base + L.off_boxr);
+            node_s = reinterpret_cast<int4 *>(base + L.off_node);
+            ssec_s = reinterpret_cast<int4 *>(base + L.off_ssec);
+            sprr = reinterpret_cast<uint32_t *>(base + L.off_sprr);
+            sprz = reinterpret_cast<int32_t *>(base + L.off_sprz);
+            mask = reinterpret_cast<uint32_t *>(base + L.off_mask);
+            stack = reinterpret_cast<uint32_t *>(base + L.off_stack);
+            list = reinterpret_cast<uint16_t *>(base + L.off_list);
+            static_bytes = 32u * (uint32_t)sc.nnodes + 16u * (uint32_t)sc.nss;
+            if (static_bytes) {
+                if (tid == 0) bulk_copy_g2s(node_s, sc.walk_static, static_bytes, &s_bar);
+                static_pending = true;
+            }
+            resident = level;
+        }
+    }
     FrameConst fc;
     frame_setup(poses[frame], fc);
     uint32_t slot = 0;                  // per-frame states: this frame's slot of the arena
@@ -203,9 +250,10 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
         int lo, hi;
         boxr[i] = box_range(fc, vw, b4, lo, hi) ? pack_range(lo, hi, kVisBit) : 0u;
     }
-    if (static_pending) {                        // first frame of this CTA: the bulk copy has had steps 1-3 to land
-        if (!mbar_wait(&s_bar, 0)) __trap();
+    if (static_pending) {                        // first frame of this CTA (or level): the bulk copy has had steps 1-3 to land
+        if (!mbar_wait(&s_bar, kLevels ? parity : 0u)) __trap();
         static_pending = false;
+        if (kLevels) parity ^= 1u;
     }
     for (int i = tid; i < sc.nsprites; i += nthr) {          // decoration sprites: exact column interval
         const SpriteRec &P = state_table<kStates>(sc.sprites, tb, st.off_sprites)[i];
@@ -344,6 +392,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ 
 #pragma unroll
         for (int i = 0; i < 6; i++) fc.pad[i] = 0;
         if (kStates) fc.pad[0] = (int32_t)slot;      // the raster reads the frame's tables from the same slot
+        if (kLevels) fc.pad[1] = (int32_t)resident;  // ... and the frame's scene from its level
         frames[frame] = fc;
     }
     __syncthreads();                              // the next frame of this CTA reuses the shared-memory tables
@@ -660,9 +709,9 @@ __device__ __forceinline__ uint32_t *masked_push(const DeviceScene &sc, uint32_t
 // holds the worklist index and, per lane, the clip window [ya, yb) that was open behind the seg when the
 // front-to-back walk reached it (the per-column silhouette of everything nearer).  Texels whose opacity plane
 // is 0 leave the pixel as the solid pass drew it (static.frag:21-22).  Kept out of line so that the
-// register allocation of the solid pass is not affected.  kStates only gives each raster variant its own copy (one caller
-// each, so that what the compiler propagates into it from its caller stays as it is).
-template <bool kRgba, int kW, bool kStates>
+// register allocation of the solid pass is not affected.  kStates and kLevels only give each raster variant its own copy
+// (one caller each, so that what the compiler propagates into it from its caller stays as it is).
+template <bool kRgba, int kW, bool kStates, bool kLevels>
 __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, int32_t pose_z, uint8_t *fb,
                                          uint32_t *rgba, uint32_t pal_s, int x, int lane,
                                          const SegFrame *wl, const uint32_t *chunks, int count) {
@@ -779,15 +828,18 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
 // Warps per raster CTA: the four 32-column strips of one 128-column line group (for widths that are a multiple of 128).
 constexpr int kRasterWarps = 4;
 
-template <bool kRgba, int kW, bool kMasked, bool kStates>
+template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels>
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
-                  uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st) {
-    __shared__ uint32_t s_pal[kRgba ? 256 : 1];
+                  uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st,
+                  const __grid_constant__ LevelTables lt) {
+    static_assert(!(kStates && kLevels), "per-frame states and per-frame levels are exclusive");
+    // per-frame levels: a palette per warp (the four warps of a CTA may draw frames of levels from different WADs)
+    __shared__ uint32_t s_pal[kRgba ? (kLevels ? 256 * kRasterWarps : 256) : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
     __shared__ uint32_t s_chunks[kRasterWarps][kMasked ? kMaskedCapMax / kMaskedChunk : 1];
-    if (kRgba) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
+    if (kRgba && !kLevels) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
         for (int i = threadIdx.x; i < 256; i += blockDim.x) s_pal[i] = sc.palette[i];
         __syncthreads();
     }
@@ -822,22 +874,39 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         __syncwarp();
         scp = d;
     }
-    const DeviceScene &ts = *scp;      // = sc without per-frame states
+    if constexpr (kLevels) {
+        // per-frame levels: this warp's copy of the scene of the frame's level (the walk passed the level on in
+        // FrameConst::pad[1]), and that level's palette
+        __shared__ DeviceScene s_lv[kRasterWarps];
+        DeviceScene *d = &s_lv[threadIdx.x >> 5];
+        const DeviceScene *lsrc = lt.scenes + (uint32_t)fc.pad[1];
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(lsrc);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(d);
+        for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
+        if (kRgba) {
+            const uint32_t *pal = lsrc->palette;
+            for (int i = lane; i < 256; i += 32) s_pal[256 * (threadIdx.x >> 5) + i] = pal[i];
+        }
+        __syncwarp();
+        scp = d;
+    }
+    const DeviceScene &ts = *scp;      // = sc without per-frame states or levels
+    const DeviceScene &ls = kLevels ? ts : sc;     // the level's own fields (sky, masked-entry cap): = sc but per-frame levels
     RasterCtx c;
     c.sc = &ts;
-    c.pal_s = (uint32_t)__cvta_generic_to_shared(s_pal);
+    c.pal_s = (uint32_t)__cvta_generic_to_shared(kLevels ? s_pal + 256 * (threadIdx.x >> 5) : s_pal);
     c.rowz = s_rowz[threadIdx.x >> 5];
-    c.dir = plane_dir(fc, vw, inside ? x : 0, sc.invF);
+    c.dir = plane_dir(fc, vw, inside ? x : 0, ls.invF);
     c.fb = index_fb + (size_t)frame * W * H + (inside ? x : 0);
     c.rgba = kRgba ? rgba_fb + (size_t)frame * W * H + (inside ? x : 0) : nullptr;
     c.W = W; c.H = H; c.x = x; c.lane = lane;
     c.skycol = 0;
-    if (sc.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), ts.tex[sc.sky_tex].w);
+    if (ls.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), ts.tex[ls.sky_tex].w);
 
     int ct = 0, cb = inside ? H : 0;              // open window [ct, cb) of this lane's column
     uint32_t *chunks = s_chunks[threadIdx.x >> 5];
     asm("" : "+l"(chunks));        // a run-time value: propagated into masked_pass as a constant, it makes that pass spill more
-    const bool defer = kMasked && sc.masked_list != nullptr;
+    const bool defer = kMasked && ls.masked_list != nullptr;
     int mcount = 0;
     const SegFrame *wl = work + (size_t)frame * stride;
     const int count = fc.count;
@@ -861,7 +930,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             if (is_sprite_entry(sf)) {
                 // decoration sprite: remember the windows open right now; it is drawn in the masked pass
                 if (defer) {
-                    uint32_t *ml = masked_push(sc, chunks, mcount, lane);
+                    uint32_t *ml = masked_push(ls, chunks, mcount, lane);
                     if (ml) {
                         if (lane == 0) ml[0] = (uint32_t)(k0 + j);
                         ml[1 + lane] = in ? ((uint32_t)ct | ((uint32_t)cb << 16)) : 0u;
@@ -912,7 +981,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
                 // defer the masked middle texture: remember the window that is open behind this seg
                 const bool keep = ok && wr.y2 < wr.y3;
                 if (__any_sync(kFull, keep)) {
-                    uint32_t *ml = masked_push(sc, chunks, mcount, lane);
+                    uint32_t *ml = masked_push(ls, chunks, mcount, lane);
                     if (ml) {
                         if (lane == 0) ml[0] = (uint32_t)(k0 + j);
                         ml[1 + lane] = keep ? ((uint32_t)wr.y2 | ((uint32_t)wr.y3 << 16)) : 0u;
@@ -925,7 +994,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     fill_void_warp<kRgba, kW>(c, inside ? ct : 0, inside ? cb : 0);
     if (kMasked && mcount > 0) {
         __syncwarp();
-        masked_pass<kRgba, kW, kStates>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
+        masked_pass<kRgba, kW, kStates, kLevels>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
     }
 }
 
@@ -974,15 +1043,15 @@ static int device_sms() {
     return sms > 0 ? sms : 1;
 }
 
-cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
-                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background,
-                        const StateTables *states) {
+// The walk's launch: `smem` bytes of dynamic shared memory per CTA (one frame per CTA).
+template <bool kStates, bool kLevels>
+static cudaError_t walk_go(const DeviceScene &sc, size_t smem, const View &vw, const Pose *d_poses, int n, FrameConst *d_frames,
+                           SegFrame *d_work, int stride, cudaStream_t stream, bool background, const StateTables &st,
+                           const LevelTables &lt) {
     if (n <= 0) return cudaSuccess;
-    const size_t smem = walk_smem_per_warp(sc);          // one frame per CTA
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
     if (smem > 48 * 1024) {   // per device and cheap: set it on every launch that needs the opt-in
-        cudaError_t e = states ? cudaFuncSetAttribute(b2d_walk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                               : cudaFuncSetAttribute(b2d_walk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(b2d_walk_kernel<kStates, kLevels>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
     // background (b2d_walk_device: the walk of the NEXT batch, meant to run under another batch's raster): a persistent grid
@@ -990,41 +1059,75 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
     // 7/8, so the raster keeps 16 of its 19 warps per SM while the walk hides behind it.
     const int sms = device_sms();
     const int blocks = (background && n > sms) ? sms : n, warps = 4;
-    const StateTables none{};
-    if (states) b2d_walk_kernel<true><<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride, *states);
-    else b2d_walk_kernel<false><<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride, none);
+    b2d_walk_kernel<kStates, kLevels><<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride, st, lt);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
+                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background,
+                        const StateTables *states) {
+    const size_t smem = walk_smem_per_warp(sc);
+    if (states) return walk_go<true, false>(sc, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, *states, LevelTables{});
+    return walk_go<false, false>(sc, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, StateTables{}, LevelTables{});
+}
+
+size_t walk_levels_static_smem() {
+    static const size_t bytes = [] {
+        cudaFuncAttributes a{};
+        if (cudaFuncGetAttributes(&a, b2d_walk_kernel<false, true>) == cudaSuccess) return a.sharedSizeBytes;
+        cudaGetLastError();
+        return sizeof(DeviceScene) + 16;       // s_lv, s_count, s_status, s_bar
+    }();
+    return bytes;
+}
+
+cudaError_t launch_walk_levels(const LevelTables &levels, size_t smem, const View &vw, const Pose *d_poses, int n,
+                               FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background) {
+    if (smem + walk_levels_static_smem() > kWalkSmemMax) return cudaErrorInvalidValue;
+    // every scene the kernel reads comes from `levels`: its scene parameter is not read
+    return walk_go<false, true>(DeviceScene{}, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, StateTables{}, levels);
+}
+
+// The raster's launch for every frame shape.  Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 4 warps
+// per CTA, so a CTA holds the four strips of a 128-column line group (at 1920 and 3840 columns; a CTA may straddle two
+// frames at other widths).  The four warps that write the sectors of the same 128-byte frame lines then start together on
+// one SM and finish those lines close together in time, so fewer partly written lines sit in L2.  That is worth 6 % of the
+// bench.py c2 step over one-warp CTAs; the slots of a CTA's finished warps idle until its slowest strip is done, and that
+// costs less.  The registers are left to the compiler (cap 128): 86 for the 1080p and 4K index-only kernels, i.e. 5 CTAs
+// = 20 warps per SM (DESIGN.md §6).
+// The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
+template <bool kStates, bool kLevels>
+static cudaError_t raster_go(const DeviceScene &sc, bool masked, const View &vw, const FrameConst *d_frames,
+                             const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
+                             cudaStream_t stream, const StateTables &st, const LevelTables &lt) {
+    if (n <= 0) return cudaSuccess;
+    const int strips = (vw.W + 31) / 32;
+    const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
+#define B2D_RASTER_GO(RGBA, KW) do { \
+    if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, st, lt); \
+    else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, st, lt); \
+    } while (0)
+    if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
+    else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
+    else if (vw.W == 3840) B2D_RASTER_GO(false, 3840);      // BASELINE.json's 4K configuration (index frames only)
+    else B2D_RASTER_GO(false, 0);
+#undef B2D_RASTER_GO
     return cudaGetLastError();
 }
 
 cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameConst *d_frames,
                           const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb,
                           uint32_t *d_rgba, cudaStream_t stream, const StateTables *states) {
-    if (n <= 0) return cudaSuccess;
-    const int strips = (vw.W + 31) / 32;
-    // Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 4 warps per CTA, so a CTA holds the four strips of
-    // a 128-column line group (at 1920 and 3840 columns; a CTA may straddle two frames at other widths).  The four warps
-    // that write the sectors of the same 128-byte frame lines then start together on one SM and finish those lines
-    // close together in time, so fewer partly written lines sit in L2.  That is worth 6 % of the bench.py c2 step over
-    // one-warp CTAs; the slots of a CTA's finished warps idle until its slowest strip is done, and that costs less.
-    // The registers are left to the compiler (cap 128): 86 for the 1080p and 4K index-only kernels, i.e. 5 CTAs = 20
-    // warps per SM (DESIGN.md §6).
-    // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
-    const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
     const bool masked = (sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list;
     // Per-frame states (`states`) take the kStates variant of each shape; the frames are the same pixel for pixel.
-    const StateTables none{};
-#define B2D_RASTER_GO2(RGBA, KW, KS) do { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true, KS><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, KS ? *states : none); \
-    else b2d_raster_kernel<RGBA, KW, false, KS><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, KS ? *states : none); \
-    } while (0)
-#define B2D_RASTER_GO(RGBA, KW) do { if (states) B2D_RASTER_GO2(RGBA, KW, true); else B2D_RASTER_GO2(RGBA, KW, false); } while (0)
-    if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
-    else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
-    else if (vw.W == 3840) B2D_RASTER_GO(false, 3840);      // BASELINE.json's 4K configuration (index frames only)
-    else B2D_RASTER_GO(false, 0);
-#undef B2D_RASTER_GO
-#undef B2D_RASTER_GO2
-    return cudaGetLastError();
+    if (states) return raster_go<true, false>(sc, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, *states, LevelTables{});
+    return raster_go<false, false>(sc, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, StateTables{}, LevelTables{});
+}
+
+cudaError_t launch_raster_levels(const LevelTables &levels, bool masked, const View &vw, const FrameConst *d_frames,
+                                 const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
+                                 cudaStream_t stream) {
+    return raster_go<false, true>(DeviceScene{}, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, StateTables{}, levels);
 }
 
 namespace {

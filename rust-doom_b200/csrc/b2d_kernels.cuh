@@ -54,8 +54,20 @@ struct StateTables {
     uint32_t slot_bytes, off_sectors, off_segs, off_sprites, off_mids, pad;
 };
 
+// Per-frame levels (b2d_render_levels): frame i of a batch is rendered from scenes[frame_level[i]], each the DeviceScene of
+// one level of the renderer as the batch's worklist slot reads it.  The walk copies the frame's scene into shared memory
+// and passes its level on in FrameConst::pad[1]; the raster reads the scene of that level.  Exclusive with StateTables.
+struct LevelTables {
+    const DeviceScene *scenes;
+    const uint32_t *frame_level;
+};
+
 // Bytes of dynamic shared memory the BSP-walk kernel needs per frame (= per CTA) for this scene.
 size_t walk_smem_per_warp(const DeviceScene &sc);
+// Static shared memory of the per-frame-level walk (its copy of the resident level's DeviceScene and the barrier words):
+// its dynamic shared memory may be at most kWalkSmemMax minus this.
+size_t walk_levels_static_smem();
+constexpr size_t kWalkSmemMax = 227 * 1024;      // the largest shared-memory opt-in per block on sm_90a
 
 // Kernel 1: front-to-back BSP walk, one CTA per frame.  Writes frames[i] and up to `stride`
 // worklist entries per frame at work[i*stride ...].
@@ -70,6 +82,14 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
 cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameConst *d_frames,
                           const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb,
                           uint32_t *d_rgba, cudaStream_t stream, const StateTables *states = nullptr);
+
+// The walk and the raster of a batch with per-frame levels.  `smem`: the largest walk_smem_per_warp of the levels;
+// `masked`: some level has masked content (its masked_list is set).  Everything else as launch_walk / launch_raster.
+cudaError_t launch_walk_levels(const LevelTables &levels, size_t smem, const View &vw, const Pose *d_poses, int n,
+                               FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background);
+cudaError_t launch_raster_levels(const LevelTables &levels, bool masked, const View &vw, const FrameConst *d_frames,
+                                 const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
+                                 cudaStream_t stream);
 
 // Expands `nstates` compact states (StateLayout::words words each, b2d_scene.hpp) from `src` (device pointers to the
 // rest-state sections) into slots 0 .. nstates-1 of `arena`: one thread per output record.

@@ -5,8 +5,9 @@
 Runs on a machine without a GPU (cuobjdump + c++filt).  Names are normalised so that a kernel that gained the per-frame
 state flag (`kStates`, DESIGN.md §5) is compared, in its `kStates = false` instantiation, with the kernel of the same name
 in the old build: the trailing `false` template argument and the appended `StateTables` parameter are dropped, and the
-hash of each anonymous namespace is ignored.  Addresses and instruction encodings are dropped; the opcodes and operands
-are compared.  Exits 1 if any function of OLD is missing from NEW or differs.
+hash of each anonymous namespace is ignored.  The per-frame level flag (`kLevels`) that follows it is dropped the same way
+in its `false` instantiations, with its appended `LevelTables` parameter.  Addresses and instruction encodings are
+dropped; the opcodes and operands are compared.  Exits 1 if any function of OLD is missing from NEW or differs.
 """
 import re
 import subprocess
@@ -21,6 +22,10 @@ def functions(path):
     txt = subprocess.run(["c++filt"], input=txt, capture_output=True, text=True, check=True).stdout
     txt = re.sub(r"_GLOBAL__N__[0-9a-f_]+_b2d_[a-z]+_cu_[0-9a-f]+", "ANON", txt)
     txt = txt.replace("(anonymous namespace)", "ANON")
+    txt = re.sub(r"(b2d_walk_kernel<[a-z]+), false>", r"\1>", txt)
+    txt = re.sub(r"(b2d_raster_kernel<[a-z]+, \d+, [a-z]+, [a-z]+), false>", r"\1>", txt)
+    txt = re.sub(r"(masked_pass<[a-z]+, \d+, [a-z]+), false>", r"\1>", txt)
+    txt = re.sub(r", b2d::LevelTables\)", ")", txt)
     txt = re.sub(r"void (b2d::ANON::b2d_walk_kernel)<false>", r"\1", txt)
     txt = re.sub(r"(b2d_raster_kernel<[a-z]+, \d+, [a-z]+), false>", r"\1>", txt)
     txt = re.sub(r"(masked_pass<[a-z]+, \d+), false>", r"\1>", txt)
