@@ -57,7 +57,11 @@ typedef struct b2d_pose {
 
 /* Viewport + projection, all integers so that every consumer sees identical bits.
  * F = round(2*focal_x), FY2 = round(2*focal_y) in pixels, where focal_y = (H/2)/tan(fovy/2) and
- * focal_x = (H/2)/(1.2*tan(fovy/2))  (perspective(fovy, aspect=(W/H)*1.2): player.rs:84-89,339-343). */
+ * focal_x = (H/2)/(1.2*tan(fovy/2))  (perspective(fovy, aspect=(W/H)*1.2): player.rs:84-89,339-343).
+ * b2d_view_init accepts 1 <= width <= 4096, 2 <= height <= 2160 and 1 < fovy < 170 degrees, as long as
+ * width <= 256 * F (a short view at a wide field of view: 4096 x 24 stops at 104 degrees).  The renderers accept
+ * hand-built views with the same bounds and 2 <= F, FY2 <= 262144 (2^18; b2d_view_init's largest is FY2 = 247485);
+ * anything else is B2D_ERR_INVALID_ARG.  DESIGN.md "Pixel contract" gives the reason for each bound. */
 typedef struct b2d_view {
     int32_t width, height, F, FY2;
 } b2d_view;

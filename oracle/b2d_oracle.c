@@ -241,8 +241,9 @@ static void draw_plane(Frame *f, int x, int ya, int yb, int32_t h, int32_t flat,
     const int64_t c2 = 2 * (int64_t)x + 1 - W;
     const int64_t nx = asr64((int64_t)f->cosq * f->vw.F + (int64_t)f->sinq * c2, 4);
     const int64_t ny = asr64((int64_t)f->sinq * f->vw.F - (int64_t)f->cosq * c2, 4);
-    const uint32_t ax = (uint32_t)(int32_t)asr64(nx * (int64_t)f->invF, 40);
-    const uint32_t ay = (uint32_t)(int32_t)asr64(ny * (int64_t)f->invF, 40);
+    /* floor(n * invF / 2^40) exactly: n * invF passes 2^63 once |c2| / F is above about 32 */
+    const uint32_t ax = (uint32_t)(int32_t)(int64_t)(((__int128)nx * f->invF) >> 40);
+    const uint32_t ay = (uint32_t)(int32_t)(int64_t)(((__int128)ny * f->invF) >> 40);
     const uint32_t bu = (uint32_t)f->pose.x << 10, bv = (uint32_t)f->pose.y << 10;
     for (int y = ya; y < yb; y++) {
         uint32_t *pr = f->prow + 2 * (size_t)y;
@@ -358,6 +359,8 @@ static void draw_seg(Frame *f, int si) {
         else scale = (-e) >= 20 ? scale_cap : (int64_t)(prod << (-e));
         if (scale > scale_cap) scale = scale_cap;
         if (scale < 1) continue;
+        /* rows use the scale capped at 2^31 - 1: a wall nearer than FY2/16384 units is placed as if at that depth */
+        const int32_t yscale = scale < 0x7FFFFFFF ? (int32_t)scale : 0x7FFFFFFF;
         int64_t isc = ((int64_t)1 << 38) / scale;
         int32_t iscale = (int32_t)clamp64(isc, 1, 1 << 23);
         int64_t z8l = ((int64_t)iscale * FY2) >> 18;
@@ -367,7 +370,7 @@ static void draw_seg(Frame *f, int si) {
         int32_t ucol = S[4] + (int32_t)(((uint64_t)s24 * (uint32_t)S[5]) >> 36)
                      + ((S[3] & SEG_SCROLL) ? (int32_t)(f->tics & 0xFFFFFF) : 0);
 
-        int yfc = yrow(f, fc, (int32_t)scale), yff = yrow(f, ff, (int32_t)scale);
+        int yfc = yrow(f, fc, yscale), yff = yrow(f, ff, yscale);
         if (!two) {
             int y1 = clamp32(yfc, ct, cb);
             int y2 = clamp32(yff, y1, cb);
@@ -376,7 +379,7 @@ static void draw_seg(Frame *f, int si) {
             if (floor_vis) draw_plane(f, x, y2, cb, ff, SF[2], lit(f, S[2], SF[4]));
             f->ctop[x] = H; f->cbot[x] = 0; f->open_cols--;
         } else {
-            int yot = yrow(f, otop, (int32_t)scale), yob = yrow(f, obot, (int32_t)scale);
+            int yot = yrow(f, otop, yscale), yob = yrow(f, obot, yscale);
             int y1 = clamp32(yfc, ct, cb);
             int y2 = clamp32(yot, y1, cb);
             int y3 = clamp32(yob, y2, cb);
@@ -394,7 +397,7 @@ static void draw_seg(Frame *f, int si) {
                         f->masked = (struct Masked *)realloc(f->masked, (size_t)f->cap_masked * sizeof *f->masked);
                     }
                     const int32_t *M = sc->mids + 8 * S[15];
-                    int mya = yrow(f, M[3], (int32_t)scale), myb = yrow(f, M[2], (int32_t)scale);
+                    int mya = yrow(f, M[3], yscale), myb = yrow(f, M[2], yscale);
                     struct Masked *m = &f->masked[f->n_masked++];
                     m->owner = si; m->x = x; m->row = row;
                     m->ya = mya > y2 ? mya : y2; m->yb = myb < y3 ? myb : y3;
@@ -466,11 +469,12 @@ static void record_sprite(Frame *f, int idx) {
     int64_t scale = (FY2 << 25) / cz;
     if (scale > (FY2 << 17)) scale = FY2 << 17;
     if (scale < 1) return;
+    const int32_t yscale = scale < 0x7FFFFFFF ? (int32_t)scale : 0x7FFFFFFF;      /* as for walls */
     int32_t iscale = (int32_t)clamp64(((int64_t)1 << 38) / scale, 1, 1 << 23);
     int64_t z8l = ((int64_t)iscale * FY2) >> 18;
     int32_t z8 = z8l > 65535 ? 65535 : (int32_t)z8l;
     int row = light_row_sprite(lit(f, SP[5], SP[4]), z8);
-    int ys_a = yrow(f, SP[2] + h, (int32_t)scale), ys_b = yrow(f, SP[2], (int32_t)scale);
+    int ys_a = yrow(f, SP[2] + h, yscale), ys_b = yrow(f, SP[2], yscale);
     for (int x = (int)lo; x <= (int)hi; x++) {
         int ct = f->ctop[x], cb = f->cbot[x];
         if (ct >= cb) continue;
@@ -552,7 +556,8 @@ static void render_frame(const Scene *sc, const b2o_view *vw, const b2o_pose *po
     for (int x = 0; x < W; x++) { f.ctop[x] = 0; f.cbot[x] = H; }
     for (int y = 0; y < H; y++) {
         int32_t r2 = 2 * y + 1 - H; if (r2 < 0) r2 = -r2; if (r2 == 0) r2 = 1;
-        f.yslope[y] = (uint32_t)(((uint64_t)vw->FY2 << 16) / (uint32_t)r2);
+        const uint64_t ys = ((uint64_t)vw->FY2 << 16) / (uint32_t)r2;          /* saturated past 2^32 - 1 */
+        f.yslope[y] = ys > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)ys;
     }
     f.open_cols = W;
     f.masked = NULL; f.n_masked = 0; f.cap_masked = 0;
@@ -576,7 +581,8 @@ int b2o_render_t(const uint8_t *scene_blob, const b2o_view *vw, const b2o_pose *
                  const int16_t *light_ov, uint8_t *index_fb, uint32_t *rgba_fb, int32_t *seg_hits, int nthreads) {
     Scene sc;
     if (scene_bind(&sc, scene_blob) != 0) return -1;
-    if (vw->W < 1 || vw->H < 1 || vw->W > 4096 || vw->H > 2160 || vw->F < 2 || vw->FY2 < 2) return -2;
+    if (vw->W < 1 || vw->H < 1 || vw->W > 4096 || vw->H > 2160 || vw->F < 2 || vw->FY2 < 2
+        || vw->F > (1 << 18) || vw->FY2 > (1 << 18) || vw->W > 256 * vw->F) return -2;
     const size_t npix = (size_t)vw->W * vw->H;
     const size_t scratch_ints = 2 * (size_t)sc.nverts + 2 * (size_t)vw->W + (size_t)vw->H + 16
                               + 5 * (size_t)vw->H + 2 * (size_t)vw->H + 4;      /* + plane-row memo (5 words + one int64 per row) */

@@ -694,6 +694,8 @@ int b2d_view_init(b2d_view *v, int width, int height, double fov_y_degrees) {
     v->FY2 = (int32_t)((double)height / t + 0.5);
     v->F = (int32_t)((double)height / (1.2 * t) + 0.5);     // aspect_ratio_correction (player.rs:87)
     if (v->F < 2 || v->FY2 < 2) return fail(B2D_ERR_INVALID_ARG, "degenerate focal length");
+    if (width > kViewWidthPerF * v->F)
+        return fail(B2D_ERR_INVALID_ARG, "view too wide for its focal length (width > 256 * F: short view at a wide field of view)");
     return B2D_OK;
 }
 
@@ -823,7 +825,8 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
     if (n_levels < 1 || n_levels > B2D_MAX_LEVELS) return fail(B2D_ERR_INVALID_ARG, "n_levels out of range (1 .. B2D_MAX_LEVELS)");
     for (size_t k = 0; k < n_levels; k++)
         if (!scenes[k]) return fail(B2D_ERR_INVALID_ARG, "null scene");
-    if (view->width < 1 || view->width > 4096 || view->height < 2 || view->height > 2160 || view->F < 2 || view->FY2 < 2)
+    if (view->width < 1 || view->width > 4096 || view->height < 2 || view->height > 2160 || view->F < 2 || view->FY2 < 2 ||
+        view->F > kViewFocalMax || view->FY2 > kViewFocalMax || view->width > kViewWidthPerF * view->F)
         return fail(B2D_ERR_INVALID_ARG, "view out of range");
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);

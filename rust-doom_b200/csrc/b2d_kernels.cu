@@ -740,7 +740,7 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
             row = light_row_sprite(P.light, z8);
             tex = P.tex; tA = 0; hA = P.low + sh;
             if (ya < yb) {
-                clip_rows(P.low + sh, P.low, (int32_t)scale, pose_z, c.H, ya, yb);
+                clip_rows(P.low + sh, P.low, row_scale(scale), pose_z, c.H, ya, yb);
                 ucol = sprite_column(sp, vw, c.x, sw);
             }
         } else {

@@ -144,12 +144,26 @@ B2D_HD void constrain(int64_t &lo, int64_t &hi, int64_t a, int64_t b, int64_t c)
     else if (a < c) { hi = lo - 1; }
 }
 
+// Largest focal length (F, FY2) a renderer accepts; b2d_view_init's largest is FY2 = 247 485 (2160 rows, fov just over
+// 1 degree).  With F <= 2^18, M = F * C of seg_frame_setup fits in 63 bits while |C| <= (eye-to-vertex distance) x (seg
+// length) stays below 2^45 in Q8 x Q8, i.e. 2^29 square map units (DESIGN.md "Pixel contract", arithmetic limits).
+constexpr int32_t kViewFocalMax = 1 << 18;
+// Widest view per unit of F a renderer accepts (W <= 256 F).  View space is Q8 (1/256 map unit); a screen-edge pixel spans
+// about 2F / W^2 radians, so past this ratio the rounding of far vertices moves edges and texels by several pixels.
+constexpr int32_t kViewWidthPerF = 256;
+
 struct ColumnEval {
     uint32_t s24;      // seg parameter s in Q24
-    int32_t scale;     // pixels per map unit, Q18
+    int32_t scale;     // pixels per map unit, Q18, for the rows: row_scale() of the column's scale
     int32_t iscale;    // map units per pixel, Q20, clamped to [1, 2^23]
     int32_t z8;        // view depth in 1/8 map units, <= 65535
 };
+
+// The scale the rows are placed with (yrow, clip_rows): capped at 2^31 - 1 (8192 pixels per map unit).  A wall nearer than
+// FY2 / 16384 map units is then placed as if at that depth, where the whole screen spans H / 16384 <= 0.14 map units
+// vertically: only an eye within that distance of one of its edge heights can tell.  Texture step and light keep the
+// full scale.
+B2D_HD int32_t row_scale(int64_t scale) { return scale < 0x7FFFFFFF ? (int32_t)scale : 0x7FFFFFFF; }
 
 // Per-frame projection setup of one seg from its view-space endpoints.  Returns false if the seg is
 // back-facing / degenerate or covers no screen column.
@@ -184,7 +198,7 @@ B2D_HD bool column_eval(const SegFrame &sf, const View &vw, int x, ColumnEval &o
     else scale = (-e) >= 20 ? cap : (int64_t)(prod << (-e));
     if (scale > cap) scale = cap;
     if (scale < 1) return false;
-    out.scale = (int32_t)scale;
+    out.scale = row_scale(scale);
     scale_depth(vw, scale, out.iscale, out.z8);
     return true;
 }
@@ -306,7 +320,9 @@ B2D_HD uint32_t yslope_entry(int y, const View &vw) {
     int32_t r2 = 2 * y + 1 - vw.H;
     if (r2 < 0) r2 = -r2;
     if (r2 == 0) r2 = 1;
-    return (uint32_t)(((uint64_t)vw.FY2 << 16) / (uint32_t)r2);
+    // saturated: past 2^32 - 1 (FY2 > 65535, the centre rows only) plane_row's depth saturates as well for |h - eye| >= 1/2
+    const uint64_t s = ((uint64_t)vw.FY2 << 16) / (uint32_t)r2;
+    return s > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)s;
 }
 
 // |h*2^16 - eye_z| clamped to 2048 map units
@@ -325,12 +341,19 @@ B2D_HD int32_t wall_hrel(int32_t h, int32_t pose_z) {
 struct PlaneDir { int32_t ax, ay; };                     // Q18
 B2D_HD PlaneDir plane_dir(const FrameConst &f, const View &vw, int x, uint32_t invF) {
     const int64_t c2 = 2 * (int64_t)x + 1 - vw.W;
-    // (cos*F + sin*c2) / F and (sin*F - cos*c2) / F, Q30 -> Q18 through invF = floor(2^32 / F); >> 4 first keeps 64 bits
+    // (cos*F + sin*c2) / F and (sin*F - cos*c2) / F, Q30 -> Q18 through invF = floor(2^32 / F): (n * invF) >> 40 as the
+    // high word of n * (invF << 24), since n * invF passes 2^63 once |c2| / F is above about 32 (short, wide views)
     const int64_t nx = ((int64_t)f.cosq * vw.F + (int64_t)f.sinq * c2) >> 4;
     const int64_t ny = ((int64_t)f.sinq * vw.F - (int64_t)f.cosq * c2) >> 4;
+    const int64_t m = (int64_t)invF << 24;
     PlaneDir d;
-    d.ax = (int32_t)((nx * (int64_t)invF) >> 40);
-    d.ay = (int32_t)((ny * (int64_t)invF) >> 40);
+#if defined(__CUDA_ARCH__)
+    d.ax = (int32_t)__mul64hi(nx, m);
+    d.ay = (int32_t)__mul64hi(ny, m);
+#else
+    d.ax = (int32_t)(int64_t)(((__int128)nx * m) >> 64);
+    d.ay = (int32_t)(int64_t)(((__int128)ny * m) >> 64);
+#endif
     return d;
 }
 struct PlaneRow { uint32_t z8q; int32_t z8; };           // depth Q8 (for the texel), depth in 1/8 units (for the light row)
@@ -495,7 +518,7 @@ B2D_HD bool sprite_setup(const FrameConst &f, const View &vw, int32_t x, int32_t
     sp.lo = (int32_t)lo; sp.hi = (int32_t)hi;
     const int64_t scale = sprite_scale(vw, sp.cz);
     if (scale < 1) return false;
-    sp.scale = (int32_t)scale;
+    sp.scale = row_scale(scale);
     scale_depth(vw, scale, sp.iscale, sp.z8);
     return true;
 }

@@ -394,7 +394,7 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
                     scale_depth(vw, scale, iscale, z8);
                     row = light_row_sprite(P.light, z8);
                     tex = P.tex; tA = 0; hA = P.low + sh;
-                    clip_rows(P.low + sh, P.low, (int32_t)scale, fc.pose.z, H, ya, yb);
+                    clip_rows(P.low + sh, P.low, row_scale(scale), fc.pose.z, H, ya, yb);
                     ucol = sprite_column(sp, vw, x, sw);
                 } else {
                     const SegRec &S = sc.segs[sf.seg];

@@ -17,6 +17,9 @@ Three more categories are *deviations*, counted separately and bounded tightly b
                 (within a subsector they are depth-sorted)
   sliver        an edge pixel showing a third surface of which the caster has no pixel nearby, or a one-pixel-wide run
                 (both neighbours across it agree): a surface seen edge-on that one renderer gives a column and the other none
+  near_clamp    only when the caller sets dbg["near_depth"] (the renderer's wall depth clamp, max(1, FY2/16384) map units):
+                the caster shows a wall nearer than that depth, which the renderer places at the clamp depth, so its top or
+                bottom edge shows up to near_depth * H / FY2 map units nearer the eye height than it should (DESIGN.md 4)
 Everything else -- a differing pixel away from any edge that no adjacent sample explains -- is *unexplained* and fails."""
 import numpy as np
 
@@ -73,8 +76,9 @@ def classify(g, o, dbg):
     ys, xs = np.nonzero(g != o)
     surf = dbg["surf"]
     img, uu, vv = dbg["img"], dbg["u"], dbg["v"]
-    res = {"differing": int(len(ys)), "texel": 0, "silhouette": 0, "minified": 0, "sky_hack": 0, "sprite_order": 0, "sliver": 0, "unexplained": []}
+    res = {"differing": int(len(ys)), "texel": 0, "silhouette": 0, "minified": 0, "sky_hack": 0, "sprite_order": 0, "sliver": 0, "near_clamp": 0, "unexplained": []}
     # every value a sprite image can produce (any texel, any colormap row): for the sprite-overlap category
+    near = dbg.get("near_depth")
     sprite_values = None
     if (dbg["kind"] == 4).any():
         sprite_values = set()
@@ -121,7 +125,9 @@ def classify(g, o, dbg):
         # -- known semantic deviations of the column renderer (DESIGN.md 4, "deviations"), counted and bounded by the tests:
         ya, yb, xa, xb = max(0, y - 3), min(H, y + 4), max(0, x - 3), min(W, x + 4)
         sa = dbg["sky_all"]
-        if dbg["kind"][y, x] != 3 and any(int(sa[yy, xx]) == ov for yy in range(y0, y1) for xx in range(x0, x1)):
+        if near is not None and dbg["kind"][y, x] == 1 and dbg["t"][y, x] < near:
+            res["near_clamp"] += 1     # a wall nearer than the depth clamp, drawn at the clamp depth: its edge rows move
+        elif dbg["kind"][y, x] != 3 and any(int(sa[yy, xx]) == ov for yy in range(y0, y1) for xx in range(x0, x1)):
             res["sky_hack"] += 1       # a sky ceiling hides what pokes above it (Doom's sky hack; GL puts the sky poly at max+512)
         elif sprite_values is not None and ((dbg["kind"][y, x] == 4) or (ov in sprite_values and (dbg["kind"][ya:yb, xa:xb] == 4).any())):
             res["sprite_order"] += 1   # billboards are ordered / clipped per subsector and column window, not depth-tested per

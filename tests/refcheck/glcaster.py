@@ -420,6 +420,6 @@ def render(archive: W.Archive, tex: W.TextureDirectory, level_index: int, width:
     if debug:
         sky_all = sky_pixels(np.ones(npx, dtype=bool), record=False).reshape(H_, WC)   # what the sky would show at each pixel
         dbg = {"images": images, "cmaps": cmaps, "sky_all": sky_all, "kind": kind.reshape(H_, WC), "img": d_img.reshape(H_, WC), "u": d_u.reshape(H_, WC), "v": d_v.reshape(H_, WC),
-               "row": d_row.reshape(H_, WC), "surf": d_surf.reshape(H_, WC)}
+               "row": d_row.reshape(H_, WC), "surf": d_surf.reshape(H_, WC), "t": best_t.reshape(H_, WC)}     # t: view depth of the hit
         return out.reshape(H_, WC), kind.reshape(H_, WC), dbg
     return out.reshape(H_, WC), kind.reshape(H_, WC)

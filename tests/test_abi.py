@@ -51,6 +51,15 @@ def test_invalid_arguments(b2d, product_scene):
         b2d.make_view(320, 200, 179.5)
 
 
+def test_hand_built_views_out_of_range_are_refused(b2d, product_scene):
+    """b2d_renderer_create checks a view before it looks for a device: F or FY2 above 2^18, or width above 256 F."""
+    from rust_doom_b200 import _lib
+    for w, h, F, FY2 in ((320, 200, (1 << 18) + 1, 400), (320, 200, 300, (1 << 18) + 1), (4096, 24, 15, 20), (513, 2, 2, 2)):
+        with pytest.raises(b2d.B2dError) as e:
+            b2d.Renderer(product_scene, _lib.View(w, h, F, FY2))
+        assert e.value.code == b2d.ERR_INVALID_ARG and "view out of range" in e.value.message, (w, h, F, FY2)
+
+
 def test_no_cpu_fallback(b2d, product_scene):
     import torch
     if torch.cuda.is_available():

@@ -47,15 +47,18 @@ class Tally:
         self.unexplained += [(what,) + u for u in r["unexplained"]]
         return r
 
-    def check(self, allow=None, sky_hack_bound=2e-4):
+    def check(self, allow=None, sky_hack_bound=2e-4, residue=0.01, near_clamp_bound=0.0):
         """`allow`: deviation counts of another tally (the same poses before a change) that are not held against this one;
         `sky_hack_bound`: share of the pixels the sky-hack deviation may take (it grows with the amount of tall geometry
-        standing behind lower open-air sectors)"""
+        standing behind lower open-air sectors); `residue`: share of the pixels all differing ones may take; `near_clamp_bound`:
+        share the near-clamp deviation may take (only counted when the frames' debug data carry the clamp depth)"""
         s = self.sum
         base = allow.sum if allow is not None else {}
         assert not self.unexplained, "unexplained pixels: %s" % self.unexplained[:10]
-        assert s["texel"] + s["silhouette"] + s["minified"] + s["sky_hack"] + s["sprite_order"] + s["sliver"] == s["differing"]
-        assert s["differing"] < 0.01 * self.px, s                       # rounding residue: well under 1 % of the pixels
+        assert s["texel"] + s["silhouette"] + s["minified"] + s["sky_hack"] + s["sprite_order"] + s["sliver"] + s["near_clamp"] \
+            == s["differing"]
+        assert s["differing"] < residue * self.px, s                    # rounding residue: well under 1 % of the pixels by default
+        assert s["near_clamp"] <= near_clamp_bound * self.px, s
         for k in ("sky_hack", "sliver", "sprite_order"):
             assert s[k] - base.get(k, 0) <= (sky_hack_bound if k == "sky_hack" else 2e-4) * self.px, (k, s, base)
 
