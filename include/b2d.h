@@ -292,8 +292,7 @@ int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint
  * (B2D_ERR_INVALID_ARG) a level whose walk tables leave no room for it, a level b2d_renderer_create still accepts by a few
  * hundred bytes; the level calls on such a renderer are B2D_ERR_INVALID_ARG.
  *
- * Not covered: per-frame states together with per-frame levels (b2d_render_states & co. act on level 0), levels in
- * b2d_render_sharded, and the CLI. */
+ * Not covered: levels in b2d_render_sharded, and the CLI. */
 #define B2D_MAX_LEVELS 64
 int b2d_renderer_create_levels(const b2d_scene *const *scenes, size_t n_levels, const b2d_view *view, int device,
                                int max_batch, b2d_renderer **out);
@@ -304,6 +303,32 @@ int b2d_render_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uin
 int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, void *cuda_stream,
                            int64_t *ticket_out);
 int b2d_renderer_set_level_sector_moves(b2d_renderer *r, int level, const b2d_sector_move *moves, size_t n);
+
+/* Per-frame states with per-frame levels: many agents or cameras, each on its own map and in its own episode (own clock,
+ * own doors and lifts), or a recorded session that changes maps, rendered in one batch.  Frame i is byte-identical, in
+ * index and RGBA (through its level's palette), to frame i of b2d_render_device_states on a b2d_renderer_create renderer
+ * of scene levels[i] with state states[i]; its moves, moves[first_move .. +n_moves), name sectors of ITS level.  `levels`,
+ * `states` and `moves` are HOST arrays; the renderer's own time and every level's own sector moves are neither read nor
+ * changed.  Frames whose (level, compact state) are equal share one table set anywhere in the batch; the same state on two
+ * levels is two sets.  A batch costs one walk, one raster and one launch that expands all its sets, whatever the number of
+ * levels and states it mixes, into the worklist slot's arena (sized by the largest table set of the levels; DESIGN.md §3);
+ * a batch whose frames are all on levels without time-dependent content or dynamic sectors costs two launches.  A level
+ * >= n_levels, a NULL `levels` or `states`, a move range past n_moves, a move of a sector that is not declared dynamic on
+ * the frame's level or outside its range, and a renderer whose level calls are refused (see above) are B2D_ERR_INVALID_ARG,
+ * detected before anything is enqueued.
+ *
+ * b2d_render_levels_states: host poses and frames as b2d_render; b2d_render_device_levels_states: like b2d_render_device,
+ * n may exceed max_batch (split into batches).  b2d_walk_device_levels_states: like b2d_walk_device (1..max_batch poses);
+ * the ticket is rastered by b2d_raster_device.  Before a batch is written into the worklist slot's pinned staging, the host
+ * waits for the copy that read that staging two batches earlier. */
+int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, const b2d_frame_state *states,
+                             size_t n, const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb);
+int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
+                                    const b2d_frame_state *states, size_t n, const b2d_sector_move *moves,
+                                    size_t n_moves, uint8_t *d_index_fb, uint32_t *d_rgba_fb, void *cuda_stream);
+int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
+                                  const b2d_frame_state *states, size_t n, const b2d_sector_move *moves,
+                                  size_t n_moves, void *cuda_stream, int64_t *ticket_out);
 
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
@@ -365,13 +390,17 @@ int b2d_device_download(int device, void *host_dst, const void *d_src, size_t by
 int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *seg_ids_out, size_t stride);
 
 /* Introspection for tests: the table-set slot of frames 0..n-1 of the LAST walked batch, which must have been walked with
- * per-frame states (frames with equal compact states share a slot). */
+ * per-frame states (frames with equal compact states share a slot).  With per-frame levels as well, frames with equal
+ * (level, compact state) share a set, sets are numbered in order of first appearance, and a frame on a level without
+ * time-dependent content or dynamic sectors has none (0xFFFFFFFF). */
 int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out);
 
 /* Introspection for tests: the expanded table set `set` of the LAST walked batch, in b2d_scene_tables_at's layout
  * [textures | sectors | segs | sprites | mids] and size (without the device copy's padding).  A batch walked with
  * per-frame states has one set per distinct state (`set` below their number, as b2d_debug_state_slots numbers them); a
- * plain batch has one, the set its worklist slot read (`set` = 0).  With out = NULL only *size_out is written.
+ * plain batch has one, the set its worklist slot read (`set` = 0).  A batch with per-frame states and levels has one per
+ * distinct (level, state), each in the layout and size of b2d_scene_tables_at of ITS level.  With out = NULL only
+ * *size_out is written.
  * Synchronises the device.  B2D_ERR_INVALID_ARG for a scene without time-dependent content or dynamic sectors, a set
  * out of range, or a renderer that has walked no batch. */
 int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capacity, size_t *size_out);

@@ -451,6 +451,38 @@ class Renderer:
         _check(_lib.load().b2d_walk_device_levels(self._h, poses_ptr, lv.ctypes.data, n, stream or None, ctypes.byref(t)))
         return int(t.value)
 
+    def render_levels_states(self, poses: np.ndarray, levels, tics, moves_per_pose=None, rgba: bool = False):
+        """b2d_render_levels_states: pose i rendered from level levels[i] at level time tics[i] with the sector moves
+        moves_per_pose[i] of that level (None = every pose at rest), without touching the renderer's own time and moves."""
+        poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
+        n = len(poses)
+        lv = _levels_array(levels, n)
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        out_index = np.empty((n, self.height, self.width), dtype=np.uint8)
+        out_rgba = np.empty((n, self.height, self.width), dtype=np.uint32) if rgba else None
+        _check(_lib.load().b2d_render_levels_states(self._h, poses.ctypes.data, lv.ctypes.data, states, n, arr, nm,
+                                                    out_index.ctypes.data, out_rgba.ctypes.data if rgba else None))
+        return (out_index, out_rgba) if rgba else out_index
+
+    def render_device_levels_states(self, poses_ptr: int, levels, tics, n: int, index_ptr: int, rgba_ptr: int = 0,
+                                    moves_per_pose=None, stream: int = 0):
+        """b2d_render_device_levels_states: device poses / frames, per-frame levels and states as in
+        render_levels_states; n may exceed max_batch."""
+        lv = _levels_array(levels, n)
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        _check(_lib.load().b2d_render_device_levels_states(self._h, poses_ptr, lv.ctypes.data, states, n, arr, nm, index_ptr,
+                                                           rgba_ptr or None, stream or None))
+
+    def walk_device_levels_states(self, poses_ptr: int, levels, tics, n: int, moves_per_pose=None, stream: int = 0) -> int:
+        """b2d_walk_device_levels_states: the walk of a batch (1..max_batch) with per-frame levels and states; returns the
+        ticket for raster_device."""
+        lv = _levels_array(levels, n)
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        t = ctypes.c_int64(-1)
+        _check(_lib.load().b2d_walk_device_levels_states(self._h, poses_ptr, lv.ctypes.data, states, n, arr, nm, stream or None,
+                                                         ctypes.byref(t)))
+        return int(t.value)
+
     def render_ptr(self, poses_ptr: int, n: int, index_ptr: int, rgba_ptr: int = 0):
         """b2d_render on raw host pointers (e.g. pinned torch tensors)."""
         _check(_lib.load().b2d_render(self._h, poses_ptr, n, index_ptr, rgba_ptr or None))
@@ -478,14 +510,15 @@ class Renderer:
         return counts, ids
 
     def state_slots(self, n: int) -> np.ndarray:
-        """b2d_debug_state_slots: table-set slot of each of the first n frames of the last batch walked with per-frame states."""
+        """b2d_debug_state_slots: table-set slot of each of the first n frames of the last batch walked with per-frame states
+        (with per-frame levels as well, 0xFFFFFFFF for a frame on a level without a table set)."""
         out = np.zeros(n, dtype=np.uint32)
         _check(_lib.load().b2d_debug_state_slots(self._h, n, out.ctypes.data))
         return out
 
     def state_tables(self, set: int = 0) -> bytes:
-        """b2d_debug_state_tables: table set `set` of the last walked batch, laid out as Scene.tables_at returns it (a plain
-        batch has the one set 0)."""
+        """b2d_debug_state_tables: table set `set` of the last walked batch, laid out as Scene.tables_at of the set's level
+        returns it (a plain batch has the one set 0)."""
         size = ctypes.c_size_t()
         _check(_lib.load().b2d_debug_state_tables(self._h, set, None, 0, ctypes.byref(size)))
         buf = ctypes.create_string_buffer(max(size.value, 1))

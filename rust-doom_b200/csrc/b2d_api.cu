@@ -147,12 +147,56 @@ int ensure_slot(const b2d_renderer *r, WorkSlot &s) {
     return B2D_OK;
 }
 
-// Per-frame states: the two worklist slots' arenas of max_batch table sets, allocated together by the first such call.
+// Per-frame states: the two worklist slots' arenas of max_batch table sets, allocated together by the first such call.  A
+// set takes its level's slot_bytes; the arena is sized by the largest of the levels, so that it holds max_batch sets of
+// any mix of levels (b2d_render_levels_states) as well as max_batch sets of level 0 (b2d_render_states).
 int ensure_states(b2d_renderer *r) {
     if (r->slot[0].arena) return B2D_OK;
+    size_t slot_bytes = 0;
+    for (const LevelRes &lv : r->lv) slot_bytes = std::max(slot_bytes, (size_t)lv.state_tables.slot_bytes);
     DeviceBuf<uint8_t> arena[2];
-    for (auto &a : arena) CU(allocate(a, (size_t)r->max_batch * r->lv[0].state_tables.slot_bytes));
+    for (auto &a : arena) CU(allocate(a, (size_t)r->max_batch * slot_bytes));
     for (int i = 0; i < 2; i++) r->slot[i].arena = std::move(arena[i]);
+    return B2D_OK;
+}
+
+// The sections of a batch with per-frame states and levels in WorkSlot::states (and h_states), copied to the device in
+// one piece: what the expansion, the walk and the raster of the batch read.  Byte offsets, each section 16-byte aligned.
+struct LevelsStatesBatch {
+    size_t scenes = 0;         // DeviceScene of every level (its own blob tables; each frame's TableSet replaces them)
+    size_t srcs, sets, descs;  // StateSrc of every level | TableSet of every table set, then of every level | StateSet per set
+    size_t frame_level, frame_set, states, end;  // per frame: level, TableSet index | the sets' compact states
+    LevelsStatesBatch(size_t nlev, size_t nsets, size_t n, size_t state_words) {
+        auto up = [](size_t x) { return (x + 15) & ~(size_t)15; };
+        srcs = up(nlev * sizeof(DeviceScene));
+        sets = up(srcs + nlev * sizeof(StateSrc));
+        descs = up(sets + (nsets + nlev) * sizeof(TableSet));
+        frame_level = up(descs + nsets * sizeof(StateSet));
+        frame_set = up(frame_level + 4 * n);
+        states = up(frame_set + 4 * n);
+        end = states + 4 * state_words;
+    }
+};
+
+// Per-frame states and levels: worklist slot `s`'s `states` / `h_states` large enough for a full batch of LevelsStatesBatch
+// sections (grown, once, by the slot's first such batch, after the slot's earlier work that read them), and its event.
+int ensure_levels_states(b2d_renderer *r, WorkSlot &s) {
+    size_t words = 0;
+    for (const LevelRes &lv : r->lv) words = std::max(words, (size_t)lv.layout.words);
+    const size_t bytes = LevelsStatesBatch(r->lv.size(), (size_t)r->max_batch, (size_t)r->max_batch, (size_t)r->max_batch * words).end;
+    if (s.states_bytes >= bytes) return B2D_OK;
+    if (s.states_copied) CU(cudaEventSynchronize(s.states_copied.get()));
+    if (s.raster_done) CU(cudaEventSynchronize(s.raster_done.get()));      // the slot is rastered: nothing else reads them
+    DeviceBuf<uint32_t> d;
+    PinnedBuf<uint32_t> h;
+    Event ev;
+    CU(allocate(d, bytes));
+    CU(allocate(h, bytes));
+    if (!s.states_copied) CU(event_create(ev));
+    s.states = std::move(d);
+    s.h_states = std::move(h);
+    if (ev) s.states_copied = std::move(ev);
+    s.states_bytes = bytes;
     return B2D_OK;
 }
 
@@ -321,7 +365,7 @@ int walk_levels_into_slot(b2d_renderer *r, const Pose *d_poses, const uint32_t *
         CU(cudaEventRecord(ev[0].get(), stream));
     }
     const LevelTables lt{reinterpret_cast<const DeviceScene *>(s.levels.get()),
-                         reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off)};
+                         reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off), nullptr};
     CU(launch_walk_levels(lt, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background));
     if (r->profiling) {
         CU(cudaEventRecord(ev[1].get(), stream));
@@ -333,6 +377,126 @@ int walk_levels_into_slot(b2d_renderer *r, const Pose *d_poses, const uint32_t *
     s.per_frame = false;
     s.per_level = true;
     s.sets = 0;
+    s.ticket = r->next_ticket;
+    s.rastered = false;
+    r->last_slot = slot;
+    r->launches += 1;
+    *ticket_out = r->next_ticket++;
+    return B2D_OK;
+}
+
+// the LevelTables / StateTables of worklist slot `s`'s batch with per-frame states and levels (`b`: its sections)
+LevelTables levels_states_tables(const WorkSlot &s, const LevelsStatesBatch &b, StateTables &st) {
+    const uint8_t *d = reinterpret_cast<const uint8_t *>(s.states.get());
+    st = StateTables{};
+    st.frame_slot = reinterpret_cast<const uint32_t *>(d + b.frame_set);
+    return LevelTables{reinterpret_cast<const DeviceScene *>(d + b.scenes), reinterpret_cast<const uint32_t *>(d + b.frame_level),
+                       reinterpret_cast<const TableSet *>(d + b.sets)};
+}
+
+// BSP walk of a batch with per-frame states and levels into the next worklist slot, as walk_into_slot.  `levels` and
+// `frame_states` / `starts` as check_levels and build_states left them: frame f's compact state (of its level's layout) is
+// frame_states[starts[f] ..], none on a level without time-dependent content or dynamic sectors.  Frames whose (level,
+// compact state) are equal share a table set; sets are numbered in order of first appearance and packed into the slot's
+// arena, each at its level's slot_bytes.  The batch's LevelsStatesBatch sections go to the device in one copy, then one
+// expansion launch fills every set (none if the batch has no set) and the walk runs.
+int walk_levels_states_into_slot(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *frame_states,
+                                 const size_t *starts, int n, cudaStream_t stream, int64_t *ticket_out, bool background) {
+    const int slot = (int)(r->next_ticket & 1);
+    WorkSlot &s = r->slot[slot];
+    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
+    int rc = ensure_states(r);
+    if (rc == B2D_OK) rc = ensure_slot(r, s);
+    if (rc == B2D_OK) rc = ensure_levels_states(r, s);
+    if (rc != B2D_OK) return rc;
+    const size_t nlev = r->lv.size();
+    // table sets: (level, compact state) -> index, in order of first appearance
+    std::vector<uint32_t> frame_set((size_t)n), first_frame;
+    std::unordered_map<std::string, uint32_t> seen;
+    seen.reserve((size_t)n);
+    size_t state_words = 0;
+    for (int f = 0; f < n; f++) {
+        const LevelRes &lv = r->lv[levels[f]];
+        if (lv.h_blob.empty()) continue;          // no set: the frame reads its level's blob tables
+        std::string key(reinterpret_cast<const char *>(&levels[f]), 4);
+        key.append(reinterpret_cast<const char *>(frame_states + starts[f]), 4 * lv.layout.words);
+        auto it = seen.emplace(std::move(key), (uint32_t)first_frame.size());
+        if (it.second) {
+            first_frame.push_back((uint32_t)f);
+            state_words += lv.layout.words;
+        }
+        frame_set[(size_t)f] = it.first->second;
+    }
+    const size_t nsets = first_frame.size();
+    const LevelsStatesBatch b(nlev, nsets, (size_t)n, state_words);
+    CU(cudaEventSynchronize(s.states_copied.get()));     // the copy issued two batches ago has read the staging
+    uint8_t *h = reinterpret_cast<uint8_t *>(s.h_states.get());
+    DeviceScene *scenes = reinterpret_cast<DeviceScene *>(h + b.scenes);
+    StateSrc *srcs = reinterpret_cast<StateSrc *>(h + b.srcs);
+    TableSet *sets = reinterpret_cast<TableSet *>(h + b.sets);
+    StateSet *descs = reinterpret_cast<StateSet *>(h + b.descs);
+    uint32_t *h_level = reinterpret_cast<uint32_t *>(h + b.frame_level), *h_set = reinterpret_cast<uint32_t *>(h + b.frame_set);
+    uint32_t *h_words = reinterpret_cast<uint32_t *>(h + b.states);
+    for (size_t k = 0; k < nlev; k++) {
+        const LevelRes &lv = r->lv[k];
+        scenes[k] = lv.ds;
+        srcs[k] = lv.src;
+        sets[nsets + k] = TableSet{lv.ds.tex, lv.ds.sectors, lv.ds.segs, lv.ds.sprites, lv.ds.mids};
+    }
+    s.set_level.resize(nsets);
+    s.set_off.resize(nsets);
+    const uint8_t *arena = s.arena.get();
+    size_t aoff = 0, woff = 0, records = 0;
+    for (size_t k = 0; k < nsets; k++) {
+        const int f = (int)first_frame[k];
+        const uint32_t level = levels[f];
+        const LevelRes &lv = r->lv[level];
+        const StateTables &t = lv.state_tables;
+        const uint8_t *set = arena + aoff;
+        sets[k] = TableSet{reinterpret_cast<const TexRec *>(set), reinterpret_cast<const SectorRec *>(set + t.off_sectors),
+                           reinterpret_cast<const SegRec *>(set + t.off_segs), reinterpret_cast<const SpriteRec *>(set + t.off_sprites),
+                           reinterpret_cast<const MidRec *>(set + t.off_mids)};
+        descs[k] = StateSet{level, (uint32_t)woff, (uint32_t)records, 0};
+        std::memcpy(h_words + woff, frame_states + starts[f], 4 * lv.layout.words);
+        s.set_level[k] = level;
+        s.set_off[k] = aoff;
+        aoff += t.slot_bytes;
+        woff += lv.layout.words;
+        records += (size_t)lv.src.ntex + lv.src.nsectors + lv.src.nsegs + lv.src.nsprites + lv.src.nmids;
+    }
+    if (records > 0x7FFFFFFFu) return fail(B2D_ERR_INVALID_ARG, "the batch's table sets hold more than 2^31 records");
+    for (int f = 0; f < n; f++) {
+        h_level[f] = levels[f];
+        h_set[f] = r->lv[levels[f]].h_blob.empty() ? (uint32_t)(nsets + levels[f]) : frame_set[(size_t)f];
+    }
+    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
+    CU(cudaMemcpyAsync(s.states.get(), h, b.end, cudaMemcpyHostToDevice, stream));
+    CU(cudaEventRecord(s.states_copied.get(), stream));
+    StateTables st;
+    const LevelTables lt = levels_states_tables(s, b, st);
+    if (nsets) {
+        const uint8_t *d = reinterpret_cast<const uint8_t *>(s.states.get());
+        CU(launch_state_sets(reinterpret_cast<const StateSrc *>(d + b.srcs), reinterpret_cast<const StateSet *>(d + b.descs), lt.sets,
+                             reinterpret_cast<const uint32_t *>(d + b.states), (int)nsets, (uint32_t)records, stream));
+        r->launches += 1;
+    }
+    Event ev[2];
+    if (r->profiling) {
+        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
+        CU(cudaEventRecord(ev[0].get(), stream));
+    }
+    CU(launch_walk_levels_states(lt, st, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream,
+                                 background));
+    if (r->profiling) {
+        CU(cudaEventRecord(ev[1].get(), stream));
+        for (auto &e : ev) r->prof_events.push_back(std::move(e));
+        r->prof_kinds.push_back(0);
+    }
+    CU(cudaEventRecord(s.walk_done.get(), stream));
+    s.n = n;
+    s.per_frame = true;
+    s.per_level = true;
+    s.sets = (int)nsets;
     s.ticket = r->next_ticket;
     s.rastered = false;
     r->last_slot = slot;
@@ -357,9 +521,14 @@ int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t
         for (auto &e : ev) CU(event_create(e, cudaEventDefault));
         CU(cudaEventRecord(ev[0].get(), stream));
     }
-    if (s.per_level) {
+    if (s.per_level && s.per_frame) {
+        StateTables st;
+        const LevelTables lt = levels_states_tables(s, LevelsStatesBatch(r->lv.size(), (size_t)s.sets, (size_t)s.n, 0), st);
+        CU(launch_raster_levels_states(lt, st, r->d_masked != nullptr, r->view, s.frames.get(), s.work.get(), r->stride, s.n,
+                                       d_index, d_rgba, stream));
+    } else if (s.per_level) {
         const LevelTables lt{reinterpret_cast<const DeviceScene *>(s.levels.get()),
-                             reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off)};
+                             reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off), nullptr};
         CU(launch_raster_levels(lt, r->d_masked != nullptr, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index,
                                 d_rgba, stream));
     } else {
@@ -403,26 +572,34 @@ void state_at(const LevelRes &lv, uint32_t tics, uint32_t *out) {
     std::copy(lv.state.begin() + 1, lv.state.begin() + 2 + 2 * (ptrdiff_t)lv.layout.dyn_sectors.size(), out + 1);
 }
 
-// The compact state of every frame of a b2d_render_states-style call into `out` (level 0's layout.words words per frame), checking
-// everything first: nothing is enqueued for a call with an invalid frame.  `out` stays empty for a scene without
-// time-dependent content or dynamic sectors: its frames all render with the per-batch tables.
-int build_states(const b2d_renderer *r, const b2d_frame_state *states, size_t n, const b2d_sector_move *moves, size_t n_moves,
-                 std::vector<uint32_t> &out) {
+// The compact state of every frame of a b2d_render_states-style call into `out`, checking everything first: nothing is
+// enqueued for a call with an invalid frame.  Frame i is on level levels[i] (levels == nullptr: every frame on level 0;
+// the caller has checked the levels) and its state takes that level's layout.words words, from out[starts[i]] (starts:
+// nullable); a frame on a level without time-dependent content or dynamic sectors has none, and renders with its level's
+// tables.  With every frame on level 0, `out` is n * layout.words words, or empty for such a scene.
+int build_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n, const b2d_sector_move *moves,
+                 size_t n_moves, std::vector<uint32_t> &out, std::vector<size_t> *starts = nullptr) {
     out.clear();
     if (!states || (n_moves && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
     for (size_t i = 0; i < n; i++)
         if (states[i].first_move > n_moves || states[i].n_moves > n_moves - states[i].first_move)
             return fail(B2D_ERR_INVALID_ARG, "a frame's move range runs past the end of the move list");
-    const LevelRes &lv = r->lv[0];
-    if (lv.h_blob.empty()) {
-        for (size_t i = 0; i < n; i++)
-            if (states[i].n_moves) return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
-        return B2D_OK;
-    }
-    const size_t words = lv.layout.words;
-    out.resize(n * words);
-    std::vector<int32_t> fo, co;
+    size_t total = 0;
+    if (starts) starts->assign(n, 0);
     for (size_t i = 0; i < n; i++) {
+        const LevelRes &lv = r->lv[levels ? levels[i] : 0];
+        if (lv.h_blob.empty()) {
+            if (states[i].n_moves) return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
+            continue;
+        }
+        if (starts) (*starts)[i] = total;
+        total += lv.layout.words;
+    }
+    out.resize(total);
+    std::vector<int32_t> fo, co;
+    for (size_t i = 0, at = 0; i < n; i++) {
+        const LevelRes &lv = r->lv[levels ? levels[i] : 0];
+        if (lv.h_blob.empty()) continue;
         bool moved = false;
         if (states[i].n_moves) {
             if (const char *why = expand_moves(lv.h_blob.data(), reinterpret_cast<const SectorMove *>(moves) + states[i].first_move,
@@ -433,7 +610,8 @@ int build_states(const b2d_renderer *r, const b2d_frame_state *states, size_t n,
             for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
         }
         compact_state(lv.h_blob.data(), lv.layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
-                      out.data() + i * words);
+                      out.data() + at);
+        at += lv.layout.words;
     }
     return B2D_OK;
 }
@@ -911,6 +1089,7 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
             CU(allocate(sl.states, 4 * mb * (words + 1)));
             CU(allocate(sl.h_states, 4 * mb * (words + 1)));
             CU(event_create(sl.states_copied));
+            sl.states_bytes = 4 * mb * (words + 1);
         }
     }
     CU(allocate(r->d_poses, sizeof(Pose) * (size_t)max_batch));
@@ -1034,7 +1213,7 @@ int b2d_render_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d
                              void *cuda_stream) {
     if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { return build_states(r, states, n, moves, n_moves, fs); });
+    int rc = guarded([&] { return build_states(r, nullptr, states, n, moves, n_moves, fs); });
     if (rc != B2D_OK || n == 0) return rc;
     CU(cudaSetDevice(r->device));
     return enqueue_batches(r, d_poses, n, fs.empty() ? nullptr : fs.data(), d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
@@ -1045,7 +1224,7 @@ int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_f
     if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { return build_states(r, states, n, moves, n_moves, fs); });
+    int rc = guarded([&] { return build_states(r, nullptr, states, n, moves, n_moves, fs); });
     if (rc != B2D_OK) return rc;
     CU(cudaSetDevice(r->device));
     return walk_into_slot(r, reinterpret_cast<const Pose *>(d_poses), (int)n, static_cast<cudaStream_t>(cuda_stream), ticket_out, true,
@@ -1112,10 +1291,62 @@ int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint3
                                  ticket_out, true);
 }
 
+// Per-frame states and levels: the levels checked as check_levels, then each frame's compact state built with its level's
+// layout (build_states: frame i's from fs[starts[i]])
+static int build_levels_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n,
+                               const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts) {
+    int rc = check_levels(r, levels, n);
+    if (rc != B2D_OK) return rc;
+    return guarded([&] { return build_states(r, levels, states, n, moves, n_moves, fs, &starts); });
+}
+
+// walk -> raster of a batch with per-frame states and levels on `stream`
+static int enqueue_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *frame_states,
+                                        const size_t *starts, int n, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
+    int64_t ticket = -1;
+    int rc = walk_levels_states_into_slot(r, d_poses, levels, frame_states, starts, n, stream, &ticket, false);
+    if (rc != B2D_OK) return rc;
+    return raster_from_slot(r, ticket, d_index, d_rgba, stream);
+}
+
+int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
+                                    size_t n, const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb,
+                                    uint32_t *d_rgba_fb, void *cuda_stream) {
+    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
+    if (rc != B2D_OK || n == 0) return rc;
+    CU(cudaSetDevice(r->device));
+    const size_t npix = (size_t)r->view.W * r->view.H;
+    for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
+        const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
+        rc = enqueue_levels_states_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, levels + i, fs.data(), starts.data() + i,
+                                          (int)cnt, d_index_fb + i * npix, d_rgba_fb ? d_rgba_fb + i * npix : nullptr,
+                                          static_cast<cudaStream_t>(cuda_stream));
+        if (rc != B2D_OK) return rc;
+    }
+    return B2D_OK;
+}
+
+int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
+                                  size_t n, const b2d_sector_move *moves, size_t n_moves, void *cuda_stream, int64_t *ticket_out) {
+    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
+    if (rc != B2D_OK) return rc;
+    CU(cudaSetDevice(r->device));
+    return walk_levels_states_into_slot(r, reinterpret_cast<const Pose *>(d_poses), levels, fs.data(), starts.data(), (int)n,
+                                        static_cast<cudaStream_t>(cuda_stream), ticket_out, true);
+}
+
 // Host poses in, host frames out; frame_states as in enqueue_frames (for all n frames), or (exclusive with it) frame_levels:
-// the level of each of the n frames
+// the level of each of the n frames.  With both and `starts`: per-frame states and levels (frame i's state from
+// frame_states[starts[i]], as build_states left them).
 static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const uint32_t *frame_states, uint8_t *index_fb,
-                       uint32_t *rgba_fb, const uint32_t *frame_levels = nullptr) {
+                       uint32_t *rgba_fb, const uint32_t *frame_levels = nullptr, const size_t *starts = nullptr) {
     if (n == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
@@ -1150,7 +1381,10 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const u
         std::memcpy(hp, poses + done, sizeof(Pose) * (size_t)cnt);
         cudaStream_t rs = hs.render_stream.get(), cs = hs.copy_stream[buf].get();
         CU(cudaMemcpyAsync(r->d_poses.get(), hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, rs));
-        int rc = frame_levels
+        int rc = starts
+                     ? enqueue_levels_states_frames(r, r->d_poses.get(), frame_levels + done, frame_states, starts + done, cnt,
+                                                    hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs)
+                 : frame_levels
                      ? enqueue_level_frames(r, r->d_poses.get(), frame_levels + done, cnt, hs.index[buf].get(),
                                             rgba_fb ? hs.rgba[buf].get() : nullptr, rs)
                      : enqueue_frames(r, r->d_poses.get(), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs,
@@ -1200,7 +1434,7 @@ int b2d_render_states(b2d_renderer *r, const b2d_pose *poses, const b2d_frame_st
                       const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { return build_states(r, states, n, moves, n_moves, fs); });
+    int rc = guarded([&] { return build_states(r, nullptr, states, n, moves, n_moves, fs); });
     if (rc != B2D_OK) return rc;
     return render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
 }
@@ -1211,6 +1445,16 @@ int b2d_render_levels(b2d_renderer *r, const b2d_pose *poses, const uint32_t *le
     int rc = check_levels(r, levels, n);
     if (rc != B2D_OK) return rc;
     return render_host(r, poses, n, nullptr, index_fb, rgba_fb, levels);
+}
+
+int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, const b2d_frame_state *states, size_t n,
+                             const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
+    if (rc != B2D_OK) return rc;
+    return render_host(r, poses, n, fs.data(), index_fb, rgba_fb, levels, starts.data());
 }
 
 int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_rgba, size_t n_pixels, void *cuda_stream) {
@@ -1272,15 +1516,26 @@ int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
         return fail(B2D_ERR_INVALID_ARG, "the last walked batch has no per-frame states or fewer than n frames");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
+    const WorkSlot &s = r->slot[slot];
+    if (s.per_level) {
+        // per-frame states and levels: a frame on a level without a table set (TableSet index >= sets) has none
+        StateTables st;
+        levels_states_tables(s, LevelsStatesBatch(r->lv.size(), (size_t)s.sets, (size_t)s.n, 0), st);
+        CU(cudaMemcpy(slots_out, st.frame_slot, 4 * n, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < n; i++)
+            if (slots_out[i] >= (uint32_t)s.sets) slots_out[i] = 0xFFFFFFFFu;
+        return B2D_OK;
+    }
     CU(cudaMemcpy(slots_out, slot_tables(r, slot).frame_slot, 4 * n, cudaMemcpyDeviceToHost));
     return B2D_OK;
 }
 
 int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capacity, size_t *size_out) {
     if (!r) return fail(B2D_ERR_INVALID_ARG, "null renderer");
-    const LevelRes &lv = r->lv[0];
-    if (lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
     const WorkSlot &s = r->slot[r->last_slot];
+    const bool both = s.per_frame && s.per_level;      // per-frame states and levels: the set's level, at its arena offset
+    const LevelRes &lv = r->lv[both && set < (size_t)s.sets ? s.set_level[set] : 0];
+    if (!both && lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
     if (s.ticket < 0) return fail(B2D_ERR_INVALID_ARG, "no batch has been walked");
     if (set >= (s.per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
     const size_t need = state_table_bytes(lv.h_blob.data());
@@ -1289,7 +1544,8 @@ int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capaci
     if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
-    const uint8_t *src = s.per_frame ? s.arena.get() + set * (size_t)lv.state_tables.slot_bytes : lv.slot[r->last_slot].tables.get();
+    const uint8_t *src = both ? s.arena.get() + s.set_off[set]
+                         : s.per_frame ? s.arena.get() + set * (size_t)lv.state_tables.slot_bytes : lv.slot[r->last_slot].tables.get();
     CU(cudaMemcpy(out, src, need, cudaMemcpyDeviceToHost));
     return B2D_OK;
 }

@@ -86,7 +86,7 @@ struct WorkSlot {
     int64_t ticket = -1;
     bool rastered = true;
     bool per_frame = false;                               // the batch was walked with per-frame states
-    bool per_level = false;                               // ... or with per-frame levels
+    bool per_level = false;                               // ... or with per-frame levels (both: b2d_render_levels_states)
     int sets = 0;                                         // ... into this many table sets of the arena (distinct states)
     // per-frame levels (b2d_render_levels & co.; allocated by the first such call): [the DeviceScene of every level as this
     // slot's batches read it | the compact states of the levels whose table sets a batch re-expands | each frame's level]
@@ -101,6 +101,11 @@ struct WorkSlot {
     DeviceBuf<uint32_t> states;                           // max_batch compact states, then max_batch set indices
     PinnedBuf<uint32_t> h_states;                         // same layout
     Event states_copied;                                  // h_states has been read by its copy
+    // per-frame states and levels (b2d_render_levels_states & co.): `states` and `h_states` then hold the batch's
+    // LevelsStatesBatch sections (b2d_api.cu), in states_bytes bytes (grown by the first such call of the slot)
+    size_t states_bytes = 0;
+    std::vector<uint32_t> set_level;                      // level of each table set
+    std::vector<size_t> set_off;                          // byte offset of each table set in the arena
 };
 
 // Host-path staging (created by the first b2d_render & co.): double-buffered frame outputs.

@@ -122,13 +122,18 @@ template <bool kStates, typename T>
 __device__ __forceinline__ const T *state_table(const T *plain, const uint8_t *tb, uint32_t off) {
     return kStates ? reinterpret_cast<const T *>(tb + off) : plain;
 }
+// ... and with per-frame levels as well, the table of the frame's TableSet (`set`)
+template <bool kStates, bool kLevels, typename T>
+__device__ __forceinline__ const T *frame_table(const T *plain, const uint8_t *tb, uint32_t off, const T *set) {
+    if constexpr (kStates && kLevels) return set;
+    else return state_table<kStates>(plain, tb, off);
+}
 
 template <bool kStates, bool kLevels>
 __global__ void __launch_bounds__(128, 7)     // 7 CTAs/SM (72 registers): 924 frames resident on an H100's 132 SMs
 b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant__ View vw, const Pose *__restrict__ poses, int n,
                 FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride, const __grid_constant__ StateTables st,
                 const __grid_constant__ LevelTables lt) {
-    static_assert(!(kStates && kLevels), "per-frame states and per-frame levels are exclusive");
     // One CTA per frame.  The per-frame setup (steps 1-3) and the worklist records (step 5) are data-parallel and
     // use all 128 threads; the traversal itself (step 4) is sequential and runs in warp 0 with the lanes working
     // on the segs of a subsector / the words of the column mask.  The kernel is latency-bound (one frame = one
@@ -215,9 +220,11 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
     frame_setup(poses[frame], fc);
     uint32_t slot = 0;                  // per-frame states: this frame's slot of the arena
     const uint8_t *tb = nullptr;
+    TableSet fs{};                      // ... and levels: this frame's tables (slot = its TableSet)
     if (kStates) {
         slot = st.frame_slot[frame];
-        tb = st.base + (size_t)slot * st.slot_bytes;
+        if constexpr (kLevels) fs = lt.sets[slot];
+        else tb = st.base + (size_t)slot * st.slot_bytes;
     }
 
     // 1. all vertices into view space (lane-parallel)
@@ -231,7 +238,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
 
     // 2. per-seg exact column interval + static/solid flags (lane-parallel, 64-bit setup)
     for (int i = tid; i < sc.nsegs; i += nthr) {
-        const SegRec &S = state_table<kStates>(sc.segs, tb, st.off_segs)[i];
+        const SegRec &S = frame_table<kStates, kLevels>(sc.segs, tb, st.off_segs, fs.segs)[i];
         uint32_t packed = 0;
         int32_t flags = S.flags;
         if (!(flags & kSegInvalid)) {
@@ -256,11 +263,11 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
         if (kLevels) parity ^= 1u;
     }
     for (int i = tid; i < sc.nsprites; i += nthr) {          // decoration sprites: exact column interval
-        const SpriteRec &P = state_table<kStates>(sc.sprites, tb, st.off_sprites)[i];
+        const SpriteRec &P = frame_table<kStates, kLevels>(sc.sprites, tb, st.off_sprites, fs.sprites)[i];
         SpriteFrame sp;
         uint32_t packed = 0;
         sp.cz = 0;
-        if (P.tex >= 0 && P.tex < sc.ntex && sprite_setup(fc, vw, P.x, P.y, (int32_t)state_table<kStates>(sc.tex, tb, 0u)[P.tex].w, sp))
+        if (P.tex >= 0 && P.tex < sc.ntex && sprite_setup(fc, vw, P.x, P.y, (int32_t)frame_table<kStates, kLevels>(sc.tex, tb, 0u, fs.tex)[P.tex].w, sp))
             packed = pack_range(sp.lo, sp.hi, kVisBit);
         sprr[i] = packed;
         sprz[i] = (int32_t)sp.cz;
@@ -373,14 +380,14 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
         SegFrame sf;
         if (si >= sc.nsegs) {
             const int pi = si - sc.nsegs;
-            const SpriteRec &P = state_table<kStates>(sc.sprites, tb, st.off_sprites)[pi];
+            const SpriteRec &P = frame_table<kStates, kLevels>(sc.sprites, tb, st.off_sprites, fs.sprites)[pi];
             SpriteFrame sp;
-            sprite_setup(fc, vw, P.x, P.y, (int32_t)state_table<kStates>(sc.tex, tb, 0u)[P.tex].w, sp);
+            sprite_setup(fc, vw, P.x, P.y, (int32_t)frame_table<kStates, kLevels>(sc.tex, tb, 0u, fs.tex)[P.tex].w, sp);
             sprite_entry(pi, sp, sf);
             work[(size_t)frame * stride + k] = sf;
             continue;
         }
-        const SegRec &S = state_table<kStates>(sc.segs, tb, st.off_segs)[si];
+        const SegRec &S = frame_table<kStates, kLevels>(sc.segs, tb, st.off_segs, fs.segs)[si];
         seg_frame_setup(vw, tx[S.v1], tz[S.v1], tx[S.v2], tz[S.v2], sf, false);
         sf.seg = si;
         work[(size_t)frame * stride + k] = sf;
@@ -834,7 +841,6 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st,
                   const __grid_constant__ LevelTables lt) {
-    static_assert(!(kStates && kLevels), "per-frame states and per-frame levels are exclusive");
     // per-frame levels: a palette per warp (the four warps of a CTA may draw frames of levels from different WADs)
     __shared__ uint32_t s_pal[kRgba ? (kLevels ? 256 * kRasterWarps : 256) : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
@@ -854,7 +860,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
 
     const FrameConst fc = frames[frame];
     const DeviceScene *scp = &sc;
-    if constexpr (kStates) {
+    if constexpr (kStates && !kLevels) {
         // per-frame states: this warp's copy of the scene description, its five state-dependent tables pointed into the
         // frame's arena slot (the walk passed the slot on in FrameConst::pad[0]); every table read below goes through it
         __shared__ DeviceScene s_sc[kRasterWarps];
@@ -888,6 +894,14 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             for (int i = lane; i < 256; i += 32) s_pal[256 * (threadIdx.x >> 5) + i] = pal[i];
         }
         __syncwarp();
+        if constexpr (kStates) {
+            // ... with per-frame states: its five state-dependent tables pointed at the frame's TableSet (FrameConst::pad[0])
+            if (lane == 0) {
+                const TableSet t = lt.sets[(uint32_t)fc.pad[0]];
+                d->tex = t.tex; d->sectors = t.sectors; d->segs = t.segs; d->sprites = t.sprites; d->mids = t.mids;
+            }
+            __syncwarp();
+        }
         scp = d;
     }
     const DeviceScene &ts = *scp;      // = sc without per-frame states or levels
@@ -1073,8 +1087,11 @@ cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_pos
 
 size_t walk_levels_static_smem() {
     static const size_t bytes = [] {
-        cudaFuncAttributes a{};
-        if (cudaFuncGetAttributes(&a, b2d_walk_kernel<false, true>) == cudaSuccess) return a.sharedSizeBytes;
+        // the larger of the two per-frame-level walks (with and without per-frame states)
+        cudaFuncAttributes a{}, b{};
+        if (cudaFuncGetAttributes(&a, b2d_walk_kernel<false, true>) == cudaSuccess &&
+            cudaFuncGetAttributes(&b, b2d_walk_kernel<true, true>) == cudaSuccess)
+            return a.sharedSizeBytes > b.sharedSizeBytes ? a.sharedSizeBytes : b.sharedSizeBytes;
         cudaGetLastError();
         return sizeof(DeviceScene) + 16;       // s_lv, s_count, s_status, s_bar
     }();
@@ -1086,6 +1103,13 @@ cudaError_t launch_walk_levels(const LevelTables &levels, size_t smem, const Vie
     if (smem + walk_levels_static_smem() > kWalkSmemMax) return cudaErrorInvalidValue;
     // every scene the kernel reads comes from `levels`: its scene parameter is not read
     return walk_go<false, true>(DeviceScene{}, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, StateTables{}, levels);
+}
+
+cudaError_t launch_walk_levels_states(const LevelTables &levels, const StateTables &states, size_t smem, const View &vw,
+                                      const Pose *d_poses, int n, FrameConst *d_frames, SegFrame *d_work, int stride,
+                                      cudaStream_t stream, bool background) {
+    if (smem + walk_levels_static_smem() > kWalkSmemMax) return cudaErrorInvalidValue;
+    return walk_go<true, true>(DeviceScene{}, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, states, levels);
 }
 
 // The raster's launch for every frame shape.  Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 4 warps
@@ -1128,6 +1152,12 @@ cudaError_t launch_raster_levels(const LevelTables &levels, bool masked, const V
                                  const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
                                  cudaStream_t stream) {
     return raster_go<false, true>(DeviceScene{}, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, StateTables{}, levels);
+}
+
+cudaError_t launch_raster_levels_states(const LevelTables &levels, const StateTables &states, bool masked, const View &vw,
+                                        const FrameConst *d_frames, const SegFrame *d_work, int stride, int n,
+                                        uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream) {
+    return raster_go<true, true>(DeviceScene{}, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, states, levels);
 }
 
 namespace {
@@ -1209,7 +1239,45 @@ b2d_state_tables_kernel(const __grid_constant__ StateSrc src, const uint32_t *__
         reinterpret_cast<MidRec *>(out + L.off_mids)[i] = mid_at(src, st, i);
     }
 }
+
+// Per-frame states and levels: one thread per output record of every set of the batch, whatever its level.  The sets
+// number their records one after the other (StateSet::first, ascending): a thread finds its set by binary search.
+__global__ void __launch_bounds__(256)
+b2d_state_sets_kernel(const StateSrc *__restrict__ srcs, const StateSet *__restrict__ sets, const TableSet *__restrict__ out,
+                      const uint32_t *__restrict__ states, int nsets, uint32_t records) {
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < records; g += gridDim.x * blockDim.x) {
+        int lo = 0, hi = nsets - 1;          // the last set with first <= g
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (sets[mid].first <= g) lo = mid; else hi = mid - 1;
+        }
+        const StateSet S = sets[lo];
+        const StateSrc &src = srcs[S.level];
+        const TableSet o = out[lo];
+        const StateIn st = state_in(states + S.state, src.ndyn);
+        uint32_t i = g - S.first;
+        if (i < src.ntex) { const_cast<TexRec *>(o.tex)[i] = tex_at(src, st, i); continue; }
+        i -= src.ntex;
+        if (i < src.nsectors) { const_cast<SectorRec *>(o.sectors)[i] = sector_at(src, st, i); continue; }
+        i -= src.nsectors;
+        if (i < src.nsegs) { const_cast<SegRec *>(o.segs)[i] = seg_at(src, st, i); continue; }
+        i -= src.nsegs;
+        if (i < src.nsprites) { const_cast<SpriteRec *>(o.sprites)[i] = sprite_at(src, st, i); continue; }
+        i -= src.nsprites;
+        const_cast<MidRec *>(o.mids)[i] = mid_at(src, st, i);
+    }
+}
 }  // namespace
+
+cudaError_t launch_state_sets(const StateSrc *d_srcs, const StateSet *d_sets, const TableSet *d_out, const uint32_t *d_states,
+                              int nsets, uint32_t records, cudaStream_t stream) {
+    if (nsets <= 0 || records == 0) return cudaSuccess;
+    size_t blocks = ((size_t)records + 255) / 256;
+    const size_t cap = (size_t)device_sms() * 16;
+    if (blocks > cap) blocks = cap;
+    b2d_state_sets_kernel<<<(int)blocks, 256, 0, stream>>>(d_srcs, d_sets, d_out, d_states, nsets, records);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_state_tables(const StateSrc &src, const uint32_t *d_states, uint32_t words, int nstates, uint8_t *d_arena,
                                 const StateTables &layout, cudaStream_t stream) {

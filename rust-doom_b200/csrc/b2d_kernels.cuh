@@ -54,12 +54,32 @@ struct StateTables {
     uint32_t slot_bytes, off_sectors, off_segs, off_sprites, off_mids, pad;
 };
 
+// The five state-dependent tables of one frame of a batch with per-frame states and levels: an expanded table set of the
+// frame's level in the state arena, or, on a level without time-dependent content or dynamic sectors, its blob tables.
+struct TableSet {
+    const TexRec *tex;
+    const SectorRec *sectors;
+    const SegRec *segs;
+    const SpriteRec *sprites;
+    const MidRec *mids;
+};
+
 // Per-frame levels (b2d_render_levels): frame i of a batch is rendered from scenes[frame_level[i]], each the DeviceScene of
 // one level of the renderer as the batch's worklist slot reads it.  The walk copies the frame's scene into shared memory
-// and passes its level on in FrameConst::pad[1]; the raster reads the scene of that level.  Exclusive with StateTables.
+// and passes its level on in FrameConst::pad[1]; the raster reads the scene of that level.
+// With per-frame states as well (b2d_render_levels_states), frame i reads its five tables from sets[StateTables::frame_slot[i]]
+// (passed on in FrameConst::pad[0]) instead of its scene's; the other fields of StateTables are not read.
 struct LevelTables {
     const DeviceScene *scenes;
     const uint32_t *frame_level;
+    const TableSet *sets;
+};
+
+// One table set to expand in a batch with per-frame states and levels (launch_state_sets): level `level`'s rule at the
+// compact state at word `state` of the batch's states, into the tables of TableSet `set`.  `first`: the set's first record
+// in the expansion's numbering of all records of the batch (the record counts of the sets before it, summed).
+struct StateSet {
+    uint32_t level, state, first, pad;
 };
 
 // Bytes of dynamic shared memory the BSP-walk kernel needs per frame (= per CTA) for this scene.
@@ -90,6 +110,20 @@ cudaError_t launch_walk_levels(const LevelTables &levels, size_t smem, const Vie
 cudaError_t launch_raster_levels(const LevelTables &levels, bool masked, const View &vw, const FrameConst *d_frames,
                                  const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
                                  cudaStream_t stream);
+
+// The walk and the raster of a batch with per-frame states and levels: `levels.sets` and `states.frame_slot` set, as above.
+cudaError_t launch_walk_levels_states(const LevelTables &levels, const StateTables &states, size_t smem, const View &vw,
+                                      const Pose *d_poses, int n, FrameConst *d_frames, SegFrame *d_work, int stride,
+                                      cudaStream_t stream, bool background);
+cudaError_t launch_raster_levels_states(const LevelTables &levels, const StateTables &states, bool masked, const View &vw,
+                                        const FrameConst *d_frames, const SegFrame *d_work, int stride, int n,
+                                        uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream);
+
+// Expands the `nsets` table sets of a batch with per-frame states and levels in one grid: set k by the rule of level
+// sets[k].level (srcs[level]: device pointers to that level's rest-state sections) into the tables of out[k].  `records`:
+// the records of all sets together (sets[k].first counts them up).
+cudaError_t launch_state_sets(const StateSrc *d_srcs, const StateSet *d_sets, const TableSet *d_out, const uint32_t *d_states,
+                              int nsets, uint32_t records, cudaStream_t stream);
 
 // Expands `nstates` compact states (StateLayout::words words each, b2d_scene.hpp) from `src` (device pointers to the
 // rest-state sections) into slots 0 .. nstates-1 of `arena`: one thread per output record.
