@@ -250,7 +250,7 @@ int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint
 int b2d_render_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, uint8_t *d_index_fb,
                       uint32_t *d_rgba_fb, void *cuda_stream);
 
-/* Kernel 3 on its own: palette lookup index -> RGBA8 for n_pixels device bytes. */
+/* Kernel 3 on its own: palette lookup index -> RGBA8 for n_pixels device bytes, through level 0's palette. */
 int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_rgba, size_t n_pixels,
                            void *cuda_stream);
 
@@ -292,7 +292,8 @@ int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint
  * (B2D_ERR_INVALID_ARG) a level whose walk tables leave no room for it, a level b2d_renderer_create still accepts by a few
  * hundred bytes; the level calls on such a renderer are B2D_ERR_INVALID_ARG.
  *
- * Not covered: levels in b2d_render_sharded, and the CLI. */
+ * b2d_render_sharded_levels_states (below) shards a level set with per-frame states across GPUs, and
+ * b2d_palette_lut_levels_device turns index frames of several levels into RGBA, each through its own level's palette. */
 #define B2D_MAX_LEVELS 64
 int b2d_renderer_create_levels(const b2d_scene *const *scenes, size_t n_levels, const b2d_view *view, int device,
                                int max_batch, b2d_renderer **out);
@@ -329,6 +330,17 @@ int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, co
 int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
                                   const b2d_frame_state *states, size_t n, const b2d_sector_move *moves,
                                   size_t n_moves, void *cuda_stream, int64_t *ticket_out);
+
+/* Kernel 3 with a palette per frame: frame f of the n_frames contiguous W x H index frames at d_index (W x H: the
+ * renderer's view) goes through the palette of level levels[f] into d_rgba, as the RGBA output of b2d_render_levels
+ * colours it; on a set of one level it is b2d_palette_lut_device over n_frames * W * H pixels.  For gathered frames of a
+ * level set (b2d_render_sharded_levels_states), whose levels may come from archives with different PLAYPALs.  `levels`
+ * is a HOST array, staged through the renderer's pinned memory: before it is rewritten the host waits for the copy of
+ * the previous call, and the copy waits on `cuda_stream` for the previous call's kernel; the device is not synchronised
+ * (a call with more frames than any before it allocates larger staging first).  A NULL argument or a level >= n_levels
+ * is B2D_ERR_INVALID_ARG, detected before anything is enqueued. */
+int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames,
+                                  uint32_t *d_rgba, void *cuda_stream);
 
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
@@ -373,6 +385,22 @@ typedef void (*b2d_chunk_fn)(void *user, int chunk_index, size_t first_local_pos
  * stats_out->registration names what was used.  Synchronous: returns when this rank's part is complete. */
 int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames,
                        int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out);
+
+/* b2d_render_sharded over a level set with per-frame states: collective, with the same block split, chunking, buffer
+ * layout, transports, modes, callback contract and stats.  `poses`, `levels`, `states` and `moves` are HOST arrays, the
+ * same whole-job lists on every rank; pose i is rendered from level levels[i] with state states[i], whose moves name
+ * sectors of its own level, as in b2d_render_levels_states.  Frame j of rank q in a gathered chunk is byte-identical to
+ * frame q*per + first_local_pose + j of b2d_render_device_levels_states over the whole list on a renderer over the same
+ * scenes; a short last block is padded by repeating the last pose with its level and state.  The renderer's own time and
+ * every level's own moves are neither read nor changed.  The WHOLE list is checked before any collective or launch (a
+ * level out of range, a NULL array, a move range past n_moves, a move of an undeclared sector or out of its range on the
+ * frame's level, a renderer whose level calls are refused): every rank returns the same B2D_ERR_INVALID_ARG and none is
+ * left waiting for a peer.  Each chunk costs the walk, raster and one state-set expansion of b2d_walk_device_levels_states;
+ * the walk of chunk k+1 runs under the raster of chunk k as in b2d_render_sharded. */
+int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
+                                     const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves,
+                                     size_t n_moves, size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user,
+                                     b2d_sharded_stats *stats_out);
 
 /* One 32-bit checksum per frame on the device: sum_i (p[i] + 1) * (i * 0x9E3779B1 + 0x7F4A7C15) mod 2^32
  * (position sensitive, order independent).  Used to validate gathered frames without moving them to the host. */

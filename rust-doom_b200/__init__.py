@@ -310,6 +310,21 @@ def _levels_array(levels, n: int) -> np.ndarray:
     return np.ascontiguousarray(lv & 0xFFFFFFFF, dtype=np.uint32)
 
 
+def _chunk_fn(on_chunk):
+    """the b2d_chunk_fn of a sharded call: on_chunk(chunk_index, first_local_pose, frames_per_rank, device_ptr, ranks, stream)"""
+    def tramp(_user, k, first, cnt, ptr, ranks, stream):
+        if on_chunk is not None:
+            on_chunk(int(k), int(first), int(cnt), int(ptr or 0), int(ranks), int(stream or 0))
+    return _lib.CHUNK_FN(tramp)
+
+
+def _sharded_stats(st) -> dict:
+    return {"total_ms": st.total_ms, "render_ms": st.render_ms, "gather_ms": st.gather_ms,
+            "frames_local": int(st.frames_local), "frames_gathered": int(st.frames_gathered),
+            "chunks": int(st.chunks), "chunk_frames": int(st.chunk_frames), "bytes_received": int(st.bytes_received),
+            "registration": st.registration.decode("ascii", "replace")}
+
+
 class Renderer:
     """Bound to one CUDA device; owns the scene copy in HBM and the per-batch work buffers."""
 
@@ -503,6 +518,12 @@ class Renderer:
     def palette_lut_device(self, index_ptr: int, rgba_ptr: int, n_pixels: int, stream: int = 0):
         _check(_lib.load().b2d_palette_lut_device(self._h, index_ptr, rgba_ptr, n_pixels, stream or None))
 
+    def palette_lut_levels_device(self, index_ptr: int, levels, n_frames: int, rgba_ptr: int, stream: int = 0):
+        """b2d_palette_lut_levels_device: frame f of the n_frames contiguous index frames at index_ptr through the palette of
+        level levels[f] (host list) into rgba_ptr (device pointers)."""
+        lv = _levels_array(levels, n_frames)
+        _check(_lib.load().b2d_palette_lut_levels_device(self._h, index_ptr, lv.ctypes.data, n_frames, rgba_ptr, stream or None))
+
     def worklist(self, n: int):
         counts = np.zeros(n, dtype=np.int32)
         ids = np.full((n, self.worklist_stride), -1, dtype=np.int32)
@@ -547,17 +568,23 @@ class Renderer:
         poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
         st = _lib.ShardedStats()
 
-        def tramp(_user, k, first, cnt, ptr, ranks, stream):
-            if on_chunk is not None:
-                on_chunk(int(k), int(first), int(cnt), int(ptr or 0), int(ranks), int(stream or 0))
-
-        cb = _lib.CHUNK_FN(tramp)
         _check(_lib.load().b2d_render_sharded(self._h, comm._h, poses.ctypes.data, len(poses), int(chunk_frames), int(mode),
-                                              cb, None, ctypes.byref(st)))
-        return {"total_ms": st.total_ms, "render_ms": st.render_ms, "gather_ms": st.gather_ms,
-                "frames_local": int(st.frames_local), "frames_gathered": int(st.frames_gathered),
-                "chunks": int(st.chunks), "chunk_frames": int(st.chunk_frames), "bytes_received": int(st.bytes_received),
-                "registration": st.registration.decode("ascii", "replace")}
+                                              _chunk_fn(on_chunk), None, ctypes.byref(st)))
+        return _sharded_stats(st)
+
+    def render_sharded_levels_states(self, comm: "Comm", poses: np.ndarray, levels, tics, moves_per_pose=None,
+                                     chunk_frames: int = 256, mode: int = _lib.SHARD_RENDER_GATHER, on_chunk=None) -> dict:
+        """b2d_render_sharded_levels_states: render_sharded over the renderer's level set, pose i rendered from level
+        levels[i] at level time tics[i] with the sector moves moves_per_pose[i] of that level (None = every pose at rest),
+        as render_levels_states renders it.  The whole job's lists, identical on every rank."""
+        poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
+        n = len(poses)
+        lv = _levels_array(levels, n)
+        states, arr, nm = _frame_states(tics, moves_per_pose, n)
+        st = _lib.ShardedStats()
+        _check(_lib.load().b2d_render_sharded_levels_states(self._h, comm._h, poses.ctypes.data, lv.ctypes.data, states, n, arr, nm,
+                                                            int(chunk_frames), int(mode), _chunk_fn(on_chunk), None, ctypes.byref(st)))
+        return _sharded_stats(st)
 
     def close(self):
         if self._h:

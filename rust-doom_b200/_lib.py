@@ -54,6 +54,7 @@ EXPORTS = [
     "b2d_raster_device", "b2d_palette_lut_device",
     "b2d_debug_worklist", "b2d_debug_state_slots", "b2d_debug_state_tables", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
     "b2d_comm_unique_id", "b2d_comm_create", "b2d_comm_destroy", "b2d_comm_info", "b2d_render_sharded",
+    "b2d_render_sharded_levels_states", "b2d_palette_lut_levels_device",
     "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_download",
 ]
 
@@ -183,6 +184,9 @@ def load() -> ctypes.CDLL:
     L.b2d_comm_destroy.restype = None
     L.b2d_comm_info.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)]
     L.b2d_render_sharded.argtypes = [vp, vp, vp, cs, cs, ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
+    L.b2d_render_sharded_levels_states.argtypes = [vp, vp, vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, cs,
+                                                   ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
+    L.b2d_palette_lut_levels_device.argtypes = [vp, vp, vp, cs, vp, vp]
     L.b2d_frame_checksums_device.argtypes = [vp, cs, cs, vp, vp]
     _lib = L
     return L

@@ -2,13 +2,21 @@
 
     python -m rust_doom_b200.cli --iwad doom1.wad --level 0 --resolution 1920x1080 [--fov 65]
                                  [--poses N] [--dump frame.ppm] [--device 0]
+    python -m rust_doom_b200.cli --iwad doom1.wad --levels 0,2,5 --poses N [--tics T] [--dump f.ppm] [--stream s.ppm]
+                                 [--world W --rank R --id-file PATH [--chunk C]]
     python -m rust_doom_b200.cli --iwad doom1.wad list-levels
     python -m rust_doom_b200.cli --iwad doom1.wad check
 
 `list-levels` prints "<index> <name>" per level (main.rs:116-121); `check` loads and compiles every level
 (the reference's smoke test, main.rs:99-115 / game/src/game.rs:118-129) without needing a GPU.  Without
 --iwad a synthetic IWAD is generated (no WAD ships with either project).  Unlike the reference, --fov is
-honoured (its value is parsed but never read there: main.rs:131 vs game/src/game.rs:72)."""
+honoured (its value is parsed but never read there: main.rs:131 vs game/src/game.rs:72).
+
+--levels renders a level set through one renderer, as the compiled CLI does: the look-around from each listed level's
+start, --poses per level, pose i at tic T + i.  --dump NAME.EXT writes NAME.L.EXT, the first frame of level L.  With
+--world the poses are sharded over one process per GPU (b2d_render_sharded_levels_states; rank 0 writes the NCCL unique id
+to --id-file, the others read it) and rank 0 colours every gathered frame with its own level's palette on the device
+(b2d_palette_lut_levels_device) before it writes the --stream."""
 from __future__ import annotations
 
 import argparse
@@ -91,6 +99,117 @@ def _main_sharded(b2d, scene, view, poses, args, w, h, world) -> int:
         dist.destroy_process_group()
 
 
+def parse_levels(text: str, n_levels: int):
+    """--levels: `all` or comma-separated level indices below n_levels; ValueError otherwise"""
+    if text == "all":
+        return list(range(n_levels))
+    out = [int(v) for v in text.split(",")]
+    if not out or any(v < 0 or v >= n_levels for v in out):
+        raise ValueError(text)
+    return out
+
+
+def level_set_job(b2d, scenes, per_level: int, tics: int):
+    """(poses, levels, tics) of --levels: the look-around from each scene's start, per_level poses each, pose i at tics + i"""
+    poses = np.concatenate([np.repeat(sc.start_pose, per_level) for sc in scenes])
+    turn = (np.arange(per_level, dtype=np.uint64) << np.uint64(32)) // np.uint64(per_level)
+    poses["angle"] = (poses["angle"].astype(np.uint64) + np.tile(turn, len(scenes))).astype(np.uint32)
+    levels = np.repeat(np.arange(len(scenes), dtype=np.uint32), per_level)
+    return poses, levels, (tics + np.arange(len(poses), dtype=np.int64)) & 0xFFFFFFFF
+
+
+def _dump_name(dump: str, level: int) -> str:
+    stem, ext = os.path.splitext(dump)
+    return "%s.%d%s" % (stem, level, ext or ".ppm")
+
+
+def _write_image(path: str, rgb: np.ndarray):
+    with open(path, "wb") as f:
+        f.write(encode_png(rgb) if path.lower().endswith(".png") else encode_ppm(rgb))
+
+
+def _comm_from_file(b2d, id_file: str, rank: int, world: int):
+    if rank == 0:
+        with open(id_file + ".tmp", "wb") as f:
+            f.write(b2d.Comm.unique_id())
+        os.replace(id_file + ".tmp", id_file)
+    else:
+        for _ in range(600):
+            if os.path.exists(id_file):
+                break
+            time.sleep(0.1)
+    with open(id_file, "rb") as f:
+        uid = f.read()
+    return b2d.Comm(uid, rank, world, rank)
+
+
+def _main_levels(b2d, arch, set_, view, args, w, h) -> int:
+    scenes = [b2d.Scene(arch, i) for i in set_]
+    if any(sc.start_pose is None for sc in scenes):
+        print("Fatal error: a level has no player-1 start", file=sys.stderr)
+        return 1
+    per_level = max(args.poses, 1)
+    poses, levels, tics = level_set_job(b2d, scenes, per_level, args.tics)
+    n = len(poses)
+    if not args.world:
+        r = b2d.Renderer.from_levels(scenes, view, device=args.device, max_batch=min(n, 64))
+        rgba = r.render_levels_states(poses, levels, tics, rgba=True)[1]
+        print("rendered %d frame(s) %dx%d of %d level(s)" % (n, w, h, len(set_)))
+        if args.dump:
+            for k, lvl in enumerate(set_):
+                _write_image(_dump_name(args.dump, lvl), rgba_to_rgb(rgba[k * per_level]))
+        if args.stream:
+            with open(args.stream, "wb") as f:
+                for i in range(n):
+                    f.write(encode_ppm(rgba_to_rgb(rgba[i])))
+        return 0
+    import torch
+    from rust_doom_b200 import _lib
+    rank, world = args.rank, args.world
+    torch.cuda.set_device(rank)
+    r = b2d.Renderer.from_levels(scenes, view, device=rank, max_batch=min(n, 64))
+    comm = _comm_from_file(b2d, args.id_file, rank, world)
+    per = (n + world - 1) // world
+    frame_bytes = len(encode_ppm(np.zeros((h, w, 3), np.uint8)))
+    out = open(args.stream, "wb") if (args.stream and rank == 0) else None
+    if out is not None:
+        out.truncate(n * frame_bytes)
+    firsts = {}
+
+    def sink(k, first, cnt, ptr, ranks, stream):
+        # every gathered frame through its own level's palette on the device, then to its place in the stream
+        g = [q * per + first + j for q in range(ranks) for j in range(cnt)]
+        rgba = torch.empty((len(g), h, w), dtype=torch.int32, device="cuda")
+        r.palette_lut_levels_device(ptr, [levels[min(i, n - 1)] for i in g], len(g), rgba.data_ptr(), stream)
+        with torch.cuda.stream(torch.cuda.ExternalStream(stream)):
+            host = rgba.cpu().numpy().view(np.uint32)
+        for i, frame in zip(g, host):
+            if i < n:
+                out.seek(i * frame_bytes)
+                out.write(encode_ppm(rgba_to_rgb(frame)))
+                if args.dump and i % per_level == 0:
+                    firsts[int(levels[i])] = frame
+
+    try:
+        t0 = time.perf_counter()
+        st = r.render_sharded_levels_states(comm, poses, levels, tics, None, args.chunk, _lib.SHARD_RENDER_GATHER,
+                                            sink if out is not None else None)
+        dt = time.perf_counter() - t0
+        bits = r.status()
+        if bits:
+            print("Fatal error: frames incomplete (status %d)" % bits, file=sys.stderr)
+            return 1
+        print("rank %d/%d: %d frames gathered in %d chunk(s) of %d level(s), %.2f ms" % (rank, world, st["frames_gathered"],
+                                                                                      st["chunks"], len(set_), dt * 1e3))
+        for k, frame in firsts.items():
+            _write_image(_dump_name(args.dump, set_[k]), rgba_to_rgb(frame))
+        return 0
+    finally:
+        if out is not None:
+            out.close()
+        comm.close()
+
+
 def main(argv=None) -> int:
     import rust_doom_b200 as b2d
     from rust_doom_b200 import poses as P
@@ -110,6 +229,12 @@ def main(argv=None) -> int:
                     help="advance the level time by this many tics (1/35 s) per frame: animated flats / walls, "
                          "scrolling walls, light effects")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--levels", default=None, help="render a level set: `all` or comma-separated level indices")
+    ap.add_argument("--tics", type=int, default=0, help="with --levels: pose i at level time T + i")
+    ap.add_argument("--world", type=int, default=0, help="with --levels: shard over this many processes, one per GPU")
+    ap.add_argument("--rank", type=int, default=0)
+    ap.add_argument("--id-file", default=None, help="with --world: the file rank 0 writes the NCCL unique id to")
+    ap.add_argument("--chunk", type=int, default=16, help="with --world: frames per rank and chunk")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 
@@ -130,6 +255,19 @@ def main(argv=None) -> int:
                 print("Level %d (%s): %d segs, %d subsectors, %d sectors, %d textures: ok"
                       % (i, name, sc.info.n_segs, sc.info.n_ssectors, sc.info.n_sectors, sc.info.n_textures))
             return 0
+        if args.levels is not None:
+            try:
+                set_ = parse_levels(args.levels, arch.num_levels())
+            except ValueError:
+                print("--levels takes `all` or comma-separated level indices below %d" % arch.num_levels(), file=sys.stderr)
+                return 2
+            if args.world and not args.id_file:
+                print("--id-file PATH is required with --world", file=sys.stderr)
+                return 2
+            return _main_levels(b2d, arch, set_, b2d.make_view(w, h, args.fov), args, w, h)
+        if args.world:
+            print("--world takes --levels (a single level shards under torchrun)", file=sys.stderr)
+            return 2
         scene = b2d.Scene(arch, args.level)
         view = b2d.make_view(w, h, args.fov)
         if args.poses <= 1:

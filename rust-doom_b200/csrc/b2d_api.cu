@@ -634,6 +634,10 @@ int b2d::walk_frames(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t s
 int b2d::raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
     return raster_from_slot(r, ticket, d_index, d_rgba, stream);
 }
+int b2d::walk_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *fs,
+                                   const size_t *starts, int n, cudaStream_t stream, int64_t *ticket_out, bool background) {
+    return walk_levels_states_into_slot(r, d_poses, levels, fs, starts, n, stream, ticket_out, background);
+}
 
 // walk -> raster on the caller's stream
 int b2d::enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba,
@@ -642,6 +646,26 @@ int b2d::enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_
     int rc = walk_into_slot(r, d_poses, n, stream, &ticket, false, frame_states);
     if (rc != B2D_OK) return rc;
     return raster_from_slot(r, ticket, d_index, d_rgba, stream);
+}
+
+// Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
+// per-frame-level walk (a b2d_renderer_create renderer may not; checked before anything is enqueued)
+static int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
+    if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
+    if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
+        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
+    for (size_t i = 0; i < n; i++)
+        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    return B2D_OK;
+}
+
+// Per-frame states and levels: the levels checked as check_levels, then each frame's compact state built with its level's
+// layout (build_states: frame i's from fs[starts[i]])
+int b2d::build_levels_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n,
+                             const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts) {
+    int rc = check_levels(r, levels, n);
+    if (rc != B2D_OK) return rc;
+    return guarded([&] { return build_states(r, levels, states, n, moves, n_moves, fs, &starts); });
 }
 
 extern "C" {
@@ -1082,6 +1106,10 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
         off += 4 * lv.layout.words;
     }
     r->levels_frames_off = (off + 15) & ~(size_t)15;
+    // every level's palette side by side (b2d_palette_lut_levels_device): at most B2D_MAX_LEVELS x 1 KB
+    CU(allocate(r->d_palettes, r->lv.size() * 256 * sizeof(uint32_t)));
+    for (size_t k = 0; k < r->lv.size(); k++)
+        CU(cudaMemcpy(r->d_palettes.get() + k * 256, r->lv[k].ds.palette, 256 * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
     if (!r->lv[0].h_blob.empty()) {
         // level 0's per-frame states and the restates of its plain batches: compact states + set indices and their staging
         const size_t words = r->lv[0].layout.words, mb = (size_t)max_batch;
@@ -1244,17 +1272,6 @@ int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint
     return raster_from_slot(r, ticket, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
-// Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
-// per-frame-level walk (a b2d_renderer_create renderer may not; checked before anything is enqueued)
-static int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
-    if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
-    if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
-        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
-    for (size_t i = 0; i < n; i++)
-        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
-    return B2D_OK;
-}
-
 // walk -> raster of a batch with per-frame levels on `stream`
 static int enqueue_level_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, int n, uint8_t *d_index,
                                 uint32_t *d_rgba, cudaStream_t stream) {
@@ -1289,15 +1306,6 @@ int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint3
     CU(cudaSetDevice(r->device));
     return walk_levels_into_slot(r, reinterpret_cast<const Pose *>(d_poses), levels, (int)n, static_cast<cudaStream_t>(cuda_stream),
                                  ticket_out, true);
-}
-
-// Per-frame states and levels: the levels checked as check_levels, then each frame's compact state built with its level's
-// layout (build_states: frame i's from fs[starts[i]])
-static int build_levels_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n,
-                               const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts) {
-    int rc = check_levels(r, levels, n);
-    if (rc != B2D_OK) return rc;
-    return guarded([&] { return build_states(r, levels, states, n, moves, n_moves, fs, &starts); });
 }
 
 // walk -> raster of a batch with per-frame states and levels on `stream`
@@ -1461,6 +1469,42 @@ int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_
     if (!r || !d_index || !d_rgba) return fail(B2D_ERR_INVALID_ARG, "null argument");
     CU(cudaSetDevice(r->device));
     CU(launch_palette(r->lv[0].ds.palette, d_index, d_rgba, n_pixels, static_cast<cudaStream_t>(cuda_stream)));
+    r->launches += 1;
+    return B2D_OK;
+}
+
+int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, uint32_t *d_rgba,
+                                  void *cuda_stream) {
+    if (!r || !d_index || !levels || !d_rgba) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    for (size_t i = 0; i < n_frames; i++)
+        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    if (n_frames == 0) return B2D_OK;
+    CU(cudaSetDevice(r->device));
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    if (r->lut_levels_cap < n_frames) {
+        // created whole, or not at all; the old buffers go once the last call's kernel has read them
+        size_t cap = r->lut_levels_cap ? r->lut_levels_cap : 1024;
+        while (cap < n_frames) cap *= 2;
+        DeviceBuf<uint32_t> d;
+        PinnedBuf<uint32_t> h;
+        Event copied, done;
+        CU(allocate(d, cap * sizeof(uint32_t)));
+        CU(allocate(h, cap * sizeof(uint32_t)));
+        CU(event_create(copied));
+        CU(event_create(done));
+        if (r->lut_done) CU(cudaEventSynchronize(r->lut_done.get()));
+        r->d_lut_levels = std::move(d); r->h_lut_levels = std::move(h);
+        r->lut_levels_copied = std::move(copied); r->lut_done = std::move(done);
+        r->lut_levels_cap = cap;
+    } else {
+        CU(cudaEventSynchronize(r->lut_levels_copied.get()));     // the previous call's copy has read the staging
+        CU(cudaStreamWaitEvent(st, r->lut_done.get(), 0));        // ... and its kernel the device copy
+    }
+    std::memcpy(r->h_lut_levels.get(), levels, n_frames * sizeof(uint32_t));
+    CU(cudaMemcpyAsync(r->d_lut_levels.get(), r->h_lut_levels.get(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(r->lut_levels_copied.get(), st));
+    CU(launch_palette_levels(r->d_palettes.get(), r->d_lut_levels.get(), d_index, d_rgba, n_frames, (size_t)r->view.W * r->view.H, st));
+    CU(cudaEventRecord(r->lut_done.get(), st));
     r->launches += 1;
     return B2D_OK;
 }

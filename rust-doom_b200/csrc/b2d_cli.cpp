@@ -7,6 +7,11 @@
 // Multi-GPU (one process per GPU): --rank R --world N --id-file PATH --chunk C renders the pose list through
 // b2d_render_sharded -- rank 0 writes the NCCL unique id to PATH, the others read it -- with the frame all-gather on, and
 // prints one checksum line per rank over all gathered frames (every rank must print the same value).
+// Level sets: --levels LIST (comma-separated level indices, or `all`) renders the look-around from every listed level's
+// start, --poses per level, pose i at tic T + i (--tics T), through one b2d_renderer_create_levels renderer:
+// b2d_render_levels_states in one process (--dump NAME writes NAME.L.ppm, the first frame of level L), and
+// b2d_render_sharded_levels_states with --world.
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +24,26 @@
 #include "../../include/b2d.h"
 
 namespace {
+
+// "all" or comma-separated level indices into `out`; false on anything else
+bool parse_levels(const std::string &text, int nlevels, std::vector<int> &out) {
+    out.clear();
+    if (text == "all") {
+        for (int i = 0; i < nlevels; i++) out.push_back(i);
+        return nlevels > 0;
+    }
+    size_t at = 0;
+    while (at <= text.size()) {
+        const size_t comma = std::min(text.find(',', at), text.size());
+        const std::string item = text.substr(at, comma - at);
+        char *end = nullptr;
+        const long v = std::strtol(item.c_str(), &end, 10);
+        if (item.empty() || *end || v < 0 || v >= nlevels) return false;
+        out.push_back((int)v);
+        at = comma + 1;
+    }
+    return !out.empty();
+}
 
 int fail(const char *what) {
     std::fprintf(stderr, "Fatal error: %s: %s\n", what, b2d_last_error());
@@ -49,13 +74,125 @@ void on_chunk(void *user, int, size_t first, size_t cnt, const uint8_t *d_frames
         b2d_frame_checksums_device(d_frames + (size_t)q * cnt * s->npix, cnt, s->npix, s->d_sums + (size_t)q * s->per + first, stream);
 }
 
+// the communicator of an --id-file job: rank 0 writes the NCCL unique id to the file, the others read it
+int make_comm(const std::string &id_file, int rank, int world, b2d_comm **comm) {
+    uint8_t id[B2D_COMM_ID_BYTES];
+    if (id_file.empty()) { std::fprintf(stderr, "--id-file PATH is required with --world\n"); return 2; }
+    if (rank == 0) {
+        if (b2d_comm_unique_id(id) != B2D_OK) return fail("unique id");
+        const std::string tmp = id_file + ".tmp";
+        std::FILE *f = std::fopen(tmp.c_str(), "wb");
+        if (!f || std::fwrite(id, 1, sizeof id, f) != sizeof id) { std::perror(tmp.c_str()); return 1; }
+        std::fclose(f);
+        std::rename(tmp.c_str(), id_file.c_str());
+    } else {
+        std::FILE *f = nullptr;
+        for (int tries = 0; tries < 600 && !(f = std::fopen(id_file.c_str(), "rb")); tries++) usleep(100000);
+        if (!f || std::fread(id, 1, sizeof id, f) != sizeof id) { std::fprintf(stderr, "cannot read %s\n", id_file.c_str()); return 1; }
+        std::fclose(f);
+    }
+    if (b2d_comm_create(id, rank, world, rank, comm) != B2D_OK) return fail("communicator");
+    return 0;
+}
+
+// after a sharded render: the renderer's status, then one checksum line over every gathered frame; frees the sink's table
+int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st, int rank, int world) {
+    int32_t bits = 0;
+    if (b2d_renderer_status(r, &bits) != B2D_OK) return fail("status");
+    if (bits) { std::fprintf(stderr, "Fatal error: frames incomplete (status %d)\n", bits); return 1; }
+    std::vector<uint32_t> sums(sink.per * (size_t)world);
+    if (b2d_device_download(rank, sums.data(), sink.d_sums, sums.size() * sizeof(uint32_t)) != B2D_OK) return fail("download");
+    uint32_t all = 0;
+    for (size_t i = 0; i < sums.size(); i++) all = all * 31u + sums[i];
+    std::printf("rank %d/%d: %lld frames gathered in %lld chunk(s), %.3f ms, checksum %08x, buffers %s\n", rank, world,
+                (long long)st.frames_gathered, (long long)st.chunks, st.total_ms, all, st.registration);
+    b2d_device_free(rank, sink.d_sums);
+    return 0;
+}
+
+// --levels: the look-around of every level of `set` from its start, nposes per level, pose i at tic tics + i
+int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
+                     const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file) {
+    std::vector<b2d_scene *> scenes;
+    struct Scenes {
+        std::vector<b2d_scene *> &v;
+        ~Scenes() { for (b2d_scene *s : v) b2d_scene_destroy(s); }
+    } owner{scenes};
+    const size_t per_level = (size_t)nposes, n = per_level * set.size();
+    std::vector<b2d_pose> poses(n);
+    std::vector<uint32_t> levels(n);
+    std::vector<b2d_frame_state> states(n);
+    for (size_t k = 0; k < set.size(); k++) {
+        b2d_scene *sc = nullptr;
+        if (b2d_scene_create(arch, set[k], &sc) != B2D_OK) return fail("level");
+        scenes.push_back(sc);
+        b2d_scene_info info;
+        b2d_scene_info_get(sc, &info);
+        if (!info.has_start) { std::fprintf(stderr, "Fatal error: level %d has no player-1 start\n", set[k]); return 1; }
+        for (size_t i = 0; i < per_level; i++) {        // look around from the spawn point
+            b2d_pose &p = poses[k * per_level + i];
+            p = info.start;
+            p.angle = info.start.angle + (uint32_t)(((uint64_t)i << 32) / (uint64_t)per_level);
+            levels[k * per_level + i] = (uint32_t)k;
+        }
+    }
+    for (size_t i = 0; i < n; i++) states[i] = b2d_frame_state{tics + (uint32_t)i, 0, 0};
+    b2d_view view;
+    if (b2d_view_init(&view, width, height, fov) != B2D_OK) return fail("view");
+    b2d_renderer *r = nullptr;
+    if (b2d_renderer_create_levels(scenes.data(), scenes.size(), &view, world > 0 ? rank : 0, n < 64 ? (int)n : 64, &r) != B2D_OK)
+        return fail("renderer");
+    struct Renderer {
+        b2d_renderer *r;
+        ~Renderer() { b2d_renderer_destroy(r); }
+    } rown{r};
+    const size_t npix = (size_t)width * height;
+    if (world > 0) {
+        b2d_comm *comm = nullptr;
+        if (int rc = make_comm(id_file, rank, world, &comm)) return rc;
+        const size_t per = (n + (size_t)world - 1) / (size_t)world;
+        ShardSink sink{nullptr, per, npix};
+        if (b2d_device_alloc(rank, sizeof(uint32_t) * per * (size_t)world, reinterpret_cast<void **>(&sink.d_sums)) != B2D_OK) return fail("device memory");
+        b2d_sharded_stats st;
+        if (b2d_render_sharded_levels_states(r, comm, poses.data(), levels.data(), states.data(), n, nullptr, 0, (size_t)chunk,
+                                             B2D_SHARD_RENDER_GATHER, on_chunk, &sink, &st) != B2D_OK)
+            return fail("sharded render");
+        const int rc = report_sharded(r, sink, st, rank, world);
+        b2d_comm_destroy(comm);
+        return rc;
+    }
+    std::vector<uint8_t> index(npix * n);
+    std::vector<uint32_t> rgba(npix * n);
+    if (b2d_render_levels_states(r, poses.data(), levels.data(), states.data(), n, nullptr, 0, index.data(), rgba.data()) != B2D_OK)
+        return fail("render");
+    std::printf("rendered %zu frame(s) %dx%d of %zu level(s)\n", n, width, height, set.size());
+    if (!dump.empty()) {
+        const std::string stem = dump.size() > 4 && dump.compare(dump.size() - 4, 4, ".ppm") == 0 ? dump.substr(0, dump.size() - 4) : dump;
+        for (size_t k = 0; k < set.size(); k++) {
+            const std::string name = stem + "." + std::to_string(set[k]) + ".ppm";
+            std::FILE *f = std::fopen(name.c_str(), "wb");
+            if (!f) { std::perror(name.c_str()); return 1; }
+            write_ppm(f, rgba.data() + npix * k * per_level, width, height);
+            std::fclose(f);
+        }
+    }
+    if (!stream.empty()) {
+        std::FILE *f = std::fopen(stream.c_str(), "wb");
+        if (!f) { std::perror(stream.c_str()); return 1; }
+        for (size_t i = 0; i < n; i++) write_ppm(f, rgba.data() + npix * i, width, height);
+        std::fclose(f);
+    }
+    return 0;
+}
+
 }  // namespace
 
 int main(int argc, char **argv) {
-    std::string iwad, dump, stream, command, id_file;
+    std::string iwad, dump, stream, command, id_file, levels_arg;
     int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16;
     double fov = 65.0;
     unsigned long tics = 0;
+    bool with_levels = false;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
         auto next = [&](const char *name) -> const char * {
@@ -65,6 +202,7 @@ int main(int argc, char **argv) {
         if (a == "-i" || a == "--iwad") iwad = next("--iwad");
         else if (a == "-m" || a == "--metadata") next("--metadata");           // accepted; the sky table is built in
         else if (a == "-l" || a == "--level") level = std::atoi(next("--level"));
+        else if (a == "--levels") { levels_arg = next("--levels"); with_levels = true; }
         else if (a == "-f" || a == "--fov") fov = std::atof(next("--fov"));
         else if (a == "-r" || a == "--resolution") {
             if (std::sscanf(next("--resolution"), "%dx%d", &width, &height) != 2) {
@@ -113,6 +251,16 @@ int main(int argc, char **argv) {
         return 0;
     }
 
+    if (with_levels) {
+        std::vector<int> set;
+        if (!parse_levels(levels_arg, nlevels, set)) {
+            std::fprintf(stderr, "--levels takes `all` or comma-separated level indices below %d\n", nlevels);
+            return 2;
+        }
+        const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file);
+        b2d_archive_close(arch);
+        return rc;
+    }
     b2d_scene *sc = nullptr;
     if (b2d_scene_create(arch, level, &sc) != B2D_OK) { b2d_archive_close(arch); return fail("level"); }
     b2d_scene_info info;
@@ -130,39 +278,15 @@ int main(int argc, char **argv) {
     const size_t npix = (size_t)width * height;
     if (world > 0) {
         // ---- sharded: every rank runs this with the same pose list
-        uint8_t id[B2D_COMM_ID_BYTES];
-        if (id_file.empty()) { std::fprintf(stderr, "--id-file PATH is required with --world\n"); return 2; }
-        if (rank == 0) {
-            if (b2d_comm_unique_id(id) != B2D_OK) return fail("unique id");
-            const std::string tmp = id_file + ".tmp";
-            std::FILE *f = std::fopen(tmp.c_str(), "wb");
-            if (!f || std::fwrite(id, 1, sizeof id, f) != sizeof id) { std::perror(tmp.c_str()); return 1; }
-            std::fclose(f);
-            std::rename(tmp.c_str(), id_file.c_str());
-        } else {
-            std::FILE *f = nullptr;
-            for (int tries = 0; tries < 600 && !(f = std::fopen(id_file.c_str(), "rb")); tries++) usleep(100000);
-            if (!f || std::fread(id, 1, sizeof id, f) != sizeof id) { std::fprintf(stderr, "cannot read %s\n", id_file.c_str()); return 1; }
-            std::fclose(f);
-        }
         b2d_comm *comm = nullptr;
-        if (b2d_comm_create(id, rank, world, rank, &comm) != B2D_OK) return fail("communicator");
+        if (int rc = make_comm(id_file, rank, world, &comm)) return rc;
         const size_t per = ((size_t)nposes + (size_t)world - 1) / (size_t)world;
         ShardSink sink{nullptr, per, npix};
         if (b2d_device_alloc(rank, sizeof(uint32_t) * per * (size_t)world, reinterpret_cast<void **>(&sink.d_sums)) != B2D_OK) return fail("device memory");
         b2d_sharded_stats st;
         if (b2d_render_sharded(r, comm, poses.data(), (size_t)nposes, (size_t)chunk, B2D_SHARD_RENDER_GATHER, on_chunk, &sink, &st) != B2D_OK)
             return fail("sharded render");
-        int32_t bits = 0;
-        if (b2d_renderer_status(r, &bits) != B2D_OK) return fail("status");
-        if (bits) { std::fprintf(stderr, "Fatal error: frames incomplete (status %d)\n", bits); return 1; }
-        std::vector<uint32_t> sums(per * (size_t)world);
-        if (b2d_device_download(rank, sums.data(), sink.d_sums, sums.size() * sizeof(uint32_t)) != B2D_OK) return fail("download");
-        uint32_t all = 0;
-        for (size_t i = 0; i < sums.size(); i++) all = all * 31u + sums[i];
-        std::printf("rank %d/%d: %lld frames gathered in %lld chunk(s), %.3f ms, checksum %08x, buffers %s\n", rank, world,
-                    (long long)st.frames_gathered, (long long)st.chunks, st.total_ms, all, st.registration);
-        b2d_device_free(rank, sink.d_sums);
+        if (int rc = report_sharded(r, sink, st, rank, world)) return rc;
         b2d_comm_destroy(comm);
         b2d_renderer_destroy(r);
         b2d_scene_destroy(sc);

@@ -22,6 +22,13 @@ int enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index
 // the two halves (b2d_walk_device / b2d_raster_device): a background walk into a worklist slot, the raster of a ticket
 int walk_frames(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background);
 int raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);
+// per-frame states and levels (b2d_render_levels_states & co.): the n HOST levels and states checked and each frame's compact
+// state built with its level's layout (frame i's from fs[starts[i]]); nothing is enqueued
+int build_levels_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n,
+                        const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts);
+// the walk of such a batch (levels, fs and starts of its n frames as build_levels_states left them) into a worklist slot
+int walk_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *fs, const size_t *starts,
+                              int n, cudaStream_t stream, int64_t *ticket_out, bool background);
 
 // Owners of CUDA resources.  They release on the current device: ~b2d_renderer and b2d_comm_destroy select theirs first.
 struct DeviceFree { void operator()(void *p) const { cudaFree(p); } };
@@ -165,6 +172,13 @@ struct b2d_renderer {
     std::unique_ptr<HostStaging> host;
     uint32_t tics = 0;
     Event masked_done;                                    // last raster that used the masked-entry arena
+    // b2d_palette_lut_levels_device: every level's palette, [n_levels][256], and the frame levels of a call on the device
+    // with their pinned staging (grown by a call with more frames than it holds)
+    DeviceBuf<uint32_t> d_palettes;
+    DeviceBuf<uint32_t> d_lut_levels;
+    PinnedBuf<uint32_t> h_lut_levels;
+    size_t lut_levels_cap = 0;
+    Event lut_levels_copied, lut_done;                    // the staging has been read by its copy; the kernel has read the copy
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;
     bool profiling = false;

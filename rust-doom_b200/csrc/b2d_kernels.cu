@@ -9,7 +9,8 @@
 //                        draws wall columns, floor/ceiling spans and sky from texel planes that already
 //                        carry the light->colormap lookup; every pixel is written exactly once.
 //   b2d_prelight_*     : build those planes once per renderer (32 light rows x texels / flats).
-//   b2d_palette_kernel : index -> RGBA8 with the 256-entry palette in shared memory, 128-bit I/O.
+//   b2d_palette_kernel : index -> RGBA8 with the 256-entry palette in shared memory, 128-bit I/O;
+//   b2d_palette_levels_kernel the same with a palette per frame (a level set's frames).
 //
 // There is no dense contraction anywhere on this path, so no tensor-core (wgmma) work: the
 // kernels are integer/LSU/latency bound and are tuned against the HBM write roofline (DESIGN.md).
@@ -1044,6 +1045,42 @@ b2d_palette_kernel(const uint32_t *__restrict__ palette, const uint8_t *__restri
         rgba[p] = s_pal[index[p]];
 }
 
+// Kernel 3 with a palette per frame: `parts` CTAs per frame (blockIdx.x = frame * parts + part), each loading the palette of
+// its frame's level, palettes[levels[frame]], into shared memory and streaming a contiguous 1/parts of the frame.
+__global__ void __launch_bounds__(256)
+b2d_palette_levels_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__restrict__ levels,
+                          const uint8_t *__restrict__ index, uint32_t *__restrict__ rgba, size_t npix, int parts) {
+    __shared__ uint32_t s_pal[256];
+    const size_t frame = blockIdx.x / parts;
+    const int part = blockIdx.x % parts;
+    s_pal[threadIdx.x] = palettes[(size_t)levels[frame] * 256 + threadIdx.x];
+    __syncthreads();
+    const uint8_t *in = index + frame * npix;
+    uint32_t *out = rgba + frame * npix;
+    // 128-bit path when every frame starts 16-byte aligned in both buffers
+    const bool aligned = npix % 16 == 0 && ((reinterpret_cast<uintptr_t>(index) | reinterpret_cast<uintptr_t>(rgba)) & 15) == 0;
+    const size_t n = aligned ? npix / 16 : npix;
+    const size_t per = (n + parts - 1) / parts, lo = (size_t)part * per, hi = lo + per < n ? lo + per : n;
+    if (aligned) {
+        for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+            const uint4 q = __ldcs(reinterpret_cast<const uint4 *>(in) + i);
+            const uint32_t wds[4] = {q.x, q.y, q.z, q.w};
+            uint4 *o4 = reinterpret_cast<uint4 *>(out) + 4 * i;
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                uint4 o;
+                o.x = s_pal[wds[k] & 0xFF];
+                o.y = s_pal[(wds[k] >> 8) & 0xFF];
+                o.z = s_pal[(wds[k] >> 16) & 0xFF];
+                o.w = s_pal[wds[k] >> 24];
+                __stcs(o4 + k, o);
+            }
+        }
+    } else {
+        for (size_t p = lo + threadIdx.x; p < hi; p += blockDim.x) out[p] = s_pal[in[p]];
+    }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1287,6 +1324,16 @@ cudaError_t launch_state_tables(const StateSrc &src, const uint32_t *d_states, u
     const size_t cap = (size_t)device_sms() * 16;
     if (blocks > cap) blocks = cap;
     b2d_state_tables_kernel<<<(int)blocks, 256, 0, stream>>>(src, d_states, words, nstates, d_arena, layout);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, uint32_t *d_rgba,
+                                  size_t n_frames, size_t npix, cudaStream_t stream) {
+    if (n_frames == 0 || npix == 0) return cudaSuccess;
+    // ~32 KB of a frame's index bytes per CTA (8 128-bit loads per thread): 64 CTAs per 1080p frame
+    const size_t parts = (npix + 32767) / 32768;
+    if (n_frames * parts > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    b2d_palette_levels_kernel<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_levels, d_index, d_rgba, npix, (int)parts);
     return cudaGetLastError();
 }
 

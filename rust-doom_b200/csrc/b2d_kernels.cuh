@@ -141,5 +141,8 @@ cudaError_t launch_prelight_textures(const uint8_t *d_colormap, const uint8_t *d
 // Kernel 3: palette LUT on its own (index -> RGBA8), 16 pixels per thread.
 cudaError_t launch_palette(const uint32_t *d_palette, const uint8_t *d_index, uint32_t *d_rgba,
                            size_t n_pixels, cudaStream_t stream);
+// ... with a palette per frame: frame f of the n_frames contiguous npix-pixel frames through palettes[levels[f] * 256 ..].
+cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, uint32_t *d_rgba,
+                                  size_t n_frames, size_t npix, cudaStream_t stream);
 
 }  // namespace b2d

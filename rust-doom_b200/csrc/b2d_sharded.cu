@@ -17,7 +17,9 @@
 // hand-off this stands in for is `frame.finish()` in engine/src/renderer.rs:160-167.
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <vector>
 
@@ -370,12 +372,26 @@ int b2d_frame_checksums_device(const uint8_t *d_frames, size_t n_frames, size_t 
     return B2D_OK;
 }
 
-int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode,
-                       b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+}  // extern "C"
+
+namespace {
+
+// the walk of one chunk of a sharded call: local poses [first, first + n) of the rank's block, at d_poses
+using ChunkWalk = std::function<int(const Pose *d_poses, size_t first, int n, cudaStream_t stream, int64_t *ticket_out)>;
+
+int check_sharded(const b2d_renderer *r, const b2d_comm *c, const b2d_pose *poses, int mode) {
     if (!r || !c || !poses) return b2d::fail(B2D_ERR_INVALID_ARG, "null argument");
     if (mode < B2D_SHARD_RENDER_ONLY || mode > B2D_SHARD_GATHER_ONLY) return b2d::fail(B2D_ERR_INVALID_ARG, "unknown mode");
     if (r->device != c->device) return b2d::fail(B2D_ERR_INVALID_ARG, "renderer and communicator are on different devices");
-    if (n_total == 0) return B2D_OK;
+    return B2D_OK;
+}
+
+// The chunk loop of the sharded calls, after their arguments have been checked (check_sharded and the caller's checks of
+// the whole job: a rank that refused its input here would leave its peers waiting in a collective).  `walk` enqueues the
+// BSP walk of local poses [first, first + n) of this rank's padded block, read from d_poses, as a background grid on
+// `stream` and returns its ticket.
+int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode, b2d_chunk_fn fn,
+                 void *user, b2d_sharded_stats *stats_out, const ChunkWalk &walk) {
     B2D_CU(cudaSetDevice(c->device));
     Nccl &n = nccl();
     const size_t world = (size_t)c->world, rank = (size_t)c->rank;
@@ -412,7 +428,7 @@ int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size
     auto chunk_count = [&](size_t k) { const size_t f = k * chunk; return (per - f) < chunk ? (per - f) : chunk; };
     int64_t ticket = -1;
     if (do_render) {
-        int wrc = b2d::walk_frames(r, c->d_poses.get(), (int)chunk_count(0), walk_stream, &ticket, true);
+        int wrc = walk(c->d_poses.get(), 0, (int)chunk_count(0), walk_stream, &ticket);
         if (wrc != B2D_OK) return wrc;
     }
 
@@ -442,7 +458,7 @@ int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size
             result = b2d::raster_frames(r, ticket, slice, nullptr, render_stream);
             if (result != B2D_OK) break;
             if (k + 1 < nchunks) {
-                result = b2d::walk_frames(r, c->d_poses.get() + (k + 1) * chunk, (int)chunk_count(k + 1), walk_stream, &ticket, true);
+                result = walk(c->d_poses.get() + (k + 1) * chunk, (k + 1) * chunk, (int)chunk_count(k + 1), walk_stream, &ticket);
                 if (result != B2D_OK) break;
             }
         }
@@ -492,6 +508,48 @@ int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size
         *stats_out = st;
     }
     return result;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode,
+                       b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    int rc = check_sharded(r, c, poses, mode);
+    if (rc != B2D_OK || n_total == 0) return rc;
+    return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
+                        [r](const Pose *d_poses, size_t, int n, cudaStream_t stream, int64_t *ticket) {
+                            return b2d::walk_frames(r, d_poses, n, stream, ticket, true);
+                        });
+}
+
+int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
+                                     const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves, size_t n_moves,
+                                     size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    int rc = check_sharded(r, c, poses, mode);
+    if (rc != B2D_OK) return rc;
+    // the whole list, identical on every rank, is checked and its compact states built before anything else: every rank
+    // then refuses the same input, before any collective
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    rc = b2d::build_levels_states(r, levels, states, n_total, moves, n_moves, fs, starts);
+    if (rc != B2D_OK || n_total == 0) return rc;
+    // this rank's block, padded like its poses by repeating the last entry (level and state with it); its states stay
+    // where build_levels_states put them
+    const size_t world = (size_t)c->world, rank = (size_t)c->rank, per = (n_total + world - 1) / world;
+    std::vector<uint32_t> block_levels(per);
+    std::vector<size_t> block_starts(per);
+    for (size_t i = 0; i < per; i++) {
+        const size_t g = std::min(rank * per + i, n_total - 1);
+        block_levels[i] = levels[g];
+        block_starts[i] = starts[g];
+    }
+    return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
+                        [&](const Pose *d_poses, size_t first, int n, cudaStream_t stream, int64_t *ticket) {
+                            return b2d::walk_levels_states_frames(r, d_poses, block_levels.data() + first, fs.data(),
+                                                                  block_starts.data() + first, n, stream, ticket, true);
+                        });
 }
 
 }  // extern "C"

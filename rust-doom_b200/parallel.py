@@ -52,10 +52,23 @@ def sharded_schedule(n_total: int, world: int, chunk_frames: int, max_batch: int
 def padded_block(poses: np.ndarray, rank: int, world: int) -> np.ndarray:
     """Rank `rank`'s block of the job as b2d_render_sharded renders it: poses[rank*per + i], indices past the end
     clamped to the last pose."""
-    n = len(poses)
-    per = (n + world - 1) // world
-    idx = np.minimum(rank * per + np.arange(per), n - 1)
-    return poses[idx]
+    return poses[padded_block_indices(len(poses), rank, world)]
+
+
+def padded_block_indices(n_total: int, rank: int, world: int) -> np.ndarray:
+    """Indices into the whole job of rank `rank`'s padded block (padded_block): rank*per + i, clamped to the last entry."""
+    per = (n_total + world - 1) // world
+    return np.minimum(rank * per + np.arange(per), n_total - 1)
+
+
+def padded_block_levels_states(poses: np.ndarray, levels, tics, rank: int, world: int, moves_per_pose=None):
+    """Rank `rank`'s block of a level-set job as b2d_render_sharded_levels_states renders it: (poses, levels, tics,
+    moves_per_pose or None) of the job's entries rank*per + i, a short last block padded by repeating the last pose
+    WITH its level, time and moves.  Chunk k of the block is sharded_schedule's chunk k, as for b2d_render_sharded."""
+    idx = padded_block_indices(len(poses), rank, world)
+    per_pose = None if moves_per_pose is None else list(moves_per_pose)
+    moves = None if per_pose is None else [per_pose[i] for i in idx.tolist()]
+    return poses[idx], np.asarray(levels)[idx], np.asarray(tics)[idx], moves
 
 
 def sharded_gather_emulated(local_frames, n_total: int, chunk_frames: int, on_chunk, group=None):
