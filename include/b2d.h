@@ -262,7 +262,11 @@ int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_
  * looping over the frames): it then takes several frame latencies instead of one but leaves
  * 7/8 of the registers to the raster it runs under.  Rasters of consecutive batches may go to two alternating
  * streams (and output buffers): the first CTAs of batch k+1 then fill the SMs the last CTAs of batch k leave idle.  At
- * most two batches can be walked and not yet rastered; tickets are rastered once.  d_poses is read by the walk
+ * most two batches can be walked and not yet rastered; tickets are rastered once.  The one-call renders (b2d_render,
+ * b2d_render_device and their _timed, _states, _levels and _levels_states forms, b2d_render_sharded*) walk into the same
+ * two slots: a call of one batch (n <= max_batch, or one chunk) into the next slot, a longer call into both.  While a
+ * slot such a call needs holds a ticket that was walked but not rastered, the call is B2D_ERR_INVALID_ARG, detected
+ * before anything is enqueued; a single batch that fits the free slot renders as usual.  d_poses is read by the walk
  * only.  Levels with masked middle textures or sprites share one arena of deferred entries per renderer: their rasters are
  * ordered one after the other through an event, whatever streams they are enqueued on.  Replaces nothing in the reference (its render loop is synchronous, engine/src/renderer.rs:62-175). */
 int b2d_walk_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, void *cuda_stream, int64_t *ticket_out);
@@ -321,7 +325,8 @@ int b2d_renderer_set_level_sector_moves(b2d_renderer *r, int level, const b2d_se
  * b2d_render_levels_states: host poses and frames as b2d_render; b2d_render_device_levels_states: like b2d_render_device,
  * n may exceed max_batch (split into batches).  b2d_walk_device_levels_states: like b2d_walk_device (1..max_batch poses);
  * the ticket is rastered by b2d_raster_device.  Before a batch is written into the worklist slot's pinned staging, the host
- * waits for the copy that read that staging two batches earlier. */
+ * waits for the copy that read that staging two batches earlier; a slot's first such batch first grows the slot's staging
+ * and its device copy, after the host has waited for the slot's earlier copy and raster. */
 int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, const b2d_frame_state *states,
                              size_t n, const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb);
 int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
@@ -382,7 +387,10 @@ typedef void (*b2d_chunk_fn)(void *user, int chunk_index, size_t first_local_pos
  * peers' buffers with the copy engines over CUDA-IPC mappings (ordered across ranks by two 4-byte ncclAllReduce per
  * chunk); if any rank cannot map a peer's buffer all ranks fall back, together, to an in-place ncclAllGather, which
  * B2D_GATHER=nccl also selects (buffers then from ncclMemAlloc, registered with the communicator where NCCL offers it).
- * stats_out->registration names what was used.  Synchronous: returns when this rank's part is complete. */
+ * stats_out->registration names what was used.  Synchronous: returns when this rank's part is complete.  The chunks
+ * walk into the renderer's worklist slots as the one-call renders do (see b2d_raster_device): a rank whose slot holds a
+ * walked, unrastered ticket refuses the call, and that is local to the rank, so raster every ticket on every rank before
+ * a collective call, or the other ranks wait in the collective for the one that refused. */
 int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames,
                        int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out);
 

@@ -639,6 +639,16 @@ int b2d::walk_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const u
     return walk_levels_states_into_slot(r, d_poses, levels, fs, starts, n, stream, ticket_out, background);
 }
 
+int b2d::check_slots_free(const b2d_renderer *r, size_t batches) {
+    for (size_t k = 0; k < batches && k < 2; k++)
+        if (!r->slot[(r->next_ticket + (int64_t)k) & 1].rastered)
+            return fail(B2D_ERR_INVALID_ARG, "a worklist slot this call needs holds a batch that was walked but not rastered yet");
+    return B2D_OK;
+}
+
+// batches of at most max_batch frames in n frames
+static size_t batch_count(const b2d_renderer *r, size_t n) { return (n + (size_t)r->max_batch - 1) / (size_t)r->max_batch; }
+
 // walk -> raster on the caller's stream
 int b2d::enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba,
                         cudaStream_t stream, const uint32_t *frame_states) {
@@ -1212,6 +1222,8 @@ int b2d_render_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, uint8_
 // frames_states (nullable, level 0's layout.words words per frame): walk + raster of n device poses in batches of max_batch
 static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, size_t n, const uint32_t *frame_states, uint8_t *d_index_fb,
                            uint32_t *d_rgba_fb, cudaStream_t st) {
+    const int rc = check_slots_free(r, batch_count(r, n));
+    if (rc != B2D_OK) return rc;
     const size_t npix = (size_t)r->view.W * r->view.H;
     for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
         const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
@@ -1285,6 +1297,7 @@ int b2d_render_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uin
                              uint32_t *d_rgba_fb, void *cuda_stream) {
     if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK && n) rc = check_slots_free(r, batch_count(r, n));
     if (rc != B2D_OK || n == 0) return rc;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
@@ -1324,6 +1337,7 @@ int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, co
     std::vector<uint32_t> fs;
     std::vector<size_t> starts;
     int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
+    if (rc == B2D_OK && n) rc = check_slots_free(r, batch_count(r, n));
     if (rc != B2D_OK || n == 0) return rc;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
@@ -1356,6 +1370,7 @@ int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, cons
 static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const uint32_t *frame_states, uint8_t *index_fb,
                        uint32_t *rgba_fb, const uint32_t *frame_levels = nullptr, const size_t *starts = nullptr) {
     if (n == 0) return B2D_OK;
+    if (check_slots_free(r, batch_count(r, n)) != B2D_OK) return B2D_ERR_INVALID_ARG;
     CU(cudaSetDevice(r->device));
     const size_t npix = (size_t)r->view.W * r->view.H;
     if (!r->host) {       // created whole, or not at all
@@ -1430,8 +1445,10 @@ int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tic
     if (!tics) return b2d_render(r, poses, n, index_fb, rgba_fb);
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0) return B2D_OK;
+    int rc = check_slots_free(r, batch_count(r, n));          // refused before the time changes as well
+    if (rc != B2D_OK) return rc;
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { timed_states(r, tics, n, fs); return B2D_OK; });
+    rc = guarded([&] { timed_states(r, tics, n, fs); return B2D_OK; });
     if (rc != B2D_OK) return rc;
     rc = render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
     const int trc = b2d_renderer_set_time(r, tics[n - 1]);                // the renderer is left at the last pose's time

@@ -19,6 +19,9 @@ int cuda_fail(cudaError_t e, const char *what);
 // (nullable): n compact states (r->layout.words words each), frame i rendered at its own state.
 int enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
                    const uint32_t *frame_states = nullptr);
+// A one-call render of `batches` batches walks the first into the next worklist slot and alternates slots from there: it
+// is refused (B2D_ERR_INVALID_ARG) before anything is enqueued while a slot it would use holds a walked, unrastered batch.
+int check_slots_free(const b2d_renderer *r, size_t batches);
 // the two halves (b2d_walk_device / b2d_raster_device): a background walk into a worklist slot, the raster of a ticket
 int walk_frames(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background);
 int raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);

@@ -403,7 +403,8 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
     const size_t npix = (size_t)r->view.W * r->view.H;
     const bool do_render = mode != B2D_SHARD_GATHER_ONLY, do_gather = mode != B2D_SHARD_RENDER_ONLY;
 
-    int rc = ensure_buffers(c, world * chunk * npix);
+    int rc = do_render ? b2d::check_slots_free(r, nchunks) : B2D_OK;
+    if (rc == B2D_OK) rc = ensure_buffers(c, world * chunk * npix);
     if (rc != B2D_OK) return rc;
     // this rank's block of poses, padded by repeating the last pose of the list, on the device in one copy
     if (c->poses_cap < per) {
