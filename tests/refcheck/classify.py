@@ -20,6 +20,10 @@ Three more categories are *deviations*, counted separately and bounded tightly b
   near_clamp    only when the caller sets dbg["near_depth"] (the renderer's wall depth clamp, max(1, FY2/16384) map units):
                 the caster shows a wall nearer than that depth, which the renderer places at the clamp depth, so its top or
                 bottom edge shows up to near_depth * H / FY2 map units nearer the eye height than it should (DESIGN.md 4)
+  far_step      only when the caller sets dbg["far_depth"] (4 FY2 map units, where iscale reaches its cap of 8 units per
+                row): the caster shows a wall farther than that, which the renderer textures at 8 texels per row instead
+                of its true step (and lights at that depth), so the oracle shows a texel of the same texture columns at
+                another height (DESIGN.md 4)
 Everything else -- a differing pixel away from any edge that no adjacent sample explains -- is *unexplained* and fails."""
 import numpy as np
 
@@ -70,15 +74,37 @@ def _footprint(dbg, y, x, H, W):
     return vals
 
 
+def _texture_band(dbg, y, x, H, W):
+    """Lit values of the texels in the texture columns the 3x3 neighbourhood (same surface) spans, +-1, at any height and
+    colormap row +-1: what a column of the same surface shows whatever its vertical texture step."""
+    i = int(dbg["img"][y, x])
+    if i < 0:
+        return set()
+    img = dbg["images"][i]
+    h, w = img.shape
+    u, r = int(dbg["u"][y, x]), int(dbg["row"][y, x])
+    dus = [0]
+    for yy in range(max(0, y - 1), min(H, y + 2)):
+        for xx in range(max(0, x - 1), min(W, x + 2)):
+            if dbg["surf"][yy, xx] == dbg["surf"][y, x]:
+                dus.append((int(dbg["u"][yy, xx]) - u + w // 2) % w - w // 2)
+    cols = [(u + du) % w for du in range(min(dus) - 1, max(dus) + 2)]
+    t = img[:, cols]
+    texels = np.unique(t[(t >> 8) == 0] & 0xFF).astype(np.int64)
+    return set(np.unique(dbg["cmaps"][max(0, r - 1):min(31, r + 1) + 1][:, texels]).tolist())
+
+
 def classify(g, o, dbg):
     """Returns dict(differing, texel, silhouette, unexplained=[(y, x, caster value, oracle value), ...])."""
     H, W = g.shape
     ys, xs = np.nonzero(g != o)
     surf = dbg["surf"]
     img, uu, vv = dbg["img"], dbg["u"], dbg["v"]
-    res = {"differing": int(len(ys)), "texel": 0, "silhouette": 0, "minified": 0, "sky_hack": 0, "sprite_order": 0, "sliver": 0, "near_clamp": 0, "unexplained": []}
+    res = {"differing": int(len(ys)), "texel": 0, "silhouette": 0, "minified": 0, "sky_hack": 0, "sprite_order": 0, "sliver": 0,
+           "near_clamp": 0, "far_step": 0, "unexplained": []}
     # every value a sprite image can produce (any texel, any colormap row): for the sprite-overlap category
     near = dbg.get("near_depth")
+    far = dbg.get("far_depth")
     sprite_values = None
     if (dbg["kind"] == 4).any():
         sprite_values = set()
@@ -127,6 +153,8 @@ def classify(g, o, dbg):
         sa = dbg["sky_all"]
         if near is not None and dbg["kind"][y, x] == 1 and dbg["t"][y, x] < near:
             res["near_clamp"] += 1     # a wall nearer than the depth clamp, drawn at the clamp depth: its edge rows move
+        elif far is not None and dbg["kind"][y, x] == 1 and dbg["t"][y, x] > far and ov in _texture_band(dbg, y, x, H, W):
+            res["far_step"] += 1       # a wall farther than 4 FY2 units: its texture step is capped at 8 texels per row
         elif dbg["kind"][y, x] != 3 and any(int(sa[yy, xx]) == ov for yy in range(y0, y1) for xx in range(x0, x1)):
             res["sky_hack"] += 1       # a sky ceiling hides what pokes above it (Doom's sky hack; GL puts the sky poly at max+512)
         elif sprite_values is not None and ((dbg["kind"][y, x] == 4) or (ov in sprite_values and (dbg["kind"][ya:yb, xa:xb] == 4).any())):

@@ -33,7 +33,7 @@ def _sector_at_vec(level: W.Level, px: np.ndarray, py: np.ndarray) -> np.ndarray
     nx, ny = nodes["x"].astype(np.float64), nodes["y"].astype(np.float64)
     ndx, ndy = nodes["dx"].astype(np.float64), nodes["dy"].astype(np.float64)
     right, left = nodes["right"].astype(np.int64), nodes["left"].astype(np.int64)
-    for _ in range(64):
+    for _ in range(len(nodes) + 1):                        # a tree may be as deep as it has nodes
         act = ~leaf
         if not act.any():
             break

@@ -184,6 +184,21 @@ def test_wide_views_are_refused_at_the_width_bound(b2d):
     assert render.make_view(4096, 24, 105.0).F == 15
 
 
+def projection_bound(blob: bytes, eyes) -> float:
+    """The largest (eye-to-vertex distance) x (seg length) in square map units over the blob's segs and the given eye
+    positions (map units).  seg_frame_setup's |C| <= that x 2^16 in Q8 x Q8, so M = F * C fits in 63 bits at every F a
+    renderer accepts (<= 2^18) while this stays below 2^29."""
+    verts = scene.section(blob, "verts").astype(np.float64)
+    segs = scene.section(blob, "segs")
+    a, b = verts[segs[:, 0]], verts[segs[:, 1]]
+    seglen = np.hypot(*(b - a).T)
+    worst = 0.0
+    for ex, ey in eyes:
+        d = np.maximum(np.hypot(a[:, 0] - ex, a[:, 1] - ey), np.hypot(b[:, 0] - ex, b[:, 1] - ey))
+        worst = max(worst, float((d * seglen).max()))
+    return worst
+
+
 def test_focal_lengths_fit_the_largest_generated_level(b2d):
     """seg_frame_setup's M = F * C in 63 bits: |C| <= (eye-to-vertex distance) * (seg length) in Q8 x Q8, for an eye anywhere a
     pose can put it (|x|, |y| < 32768 units: Q16 in int32), on the largest generated level, at the largest F a renderer accepts
@@ -196,6 +211,7 @@ def test_focal_lengths_fit_the_largest_generated_level(b2d):
     seglen = max(math.hypot(*(verts[s[1]] - verts[s[0]])) for s in segs) * 256
     assert b2d.make_view(4096, 2160, 1.0001).FY2 < (1 << 18)
     assert (1 << 18) * diag * seglen < 2.0 ** 63
+    assert projection_bound(blob, [(x, y) for x in (-32768, 32767) for y in (-32768, 32767)]) < 2.0 ** 29
 
 
 # ---- the same grid through the kernels ----------------------------------------------------------------------------------
