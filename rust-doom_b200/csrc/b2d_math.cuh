@@ -378,7 +378,10 @@ B2D_HD uint32_t flat_offset(uint32_t cm6, uint32_t U, uint32_t V) {
 }
 
 // wall texture row: t(y) = tbase + y*tstep (Q16); row index = floor-mod of t>>16 by the height,
-// evaluated with the per-texture magic reciprocal (exact for |t>>16| < 2^14, h <= 4096).
+// evaluated with the per-texture magic reciprocal hmagic = floor(2^32 / h) + 1 (mod 2^32): exact for 1 <= h <= 4096 and
+// |t>>16| < 2^14, which every wall, masked middle and sprite column stays inside (tests/test_texture_sizes.py derives the
+// bound).  For h = 1 the magic wraps to 1 and the quotient to 0; the final select maps that case (and, defensively, any
+// t outside the domain) to a row inside the texture.
 B2D_HD int32_t wall_tbase(int32_t tA, int32_t hA, int32_t pose_z, int32_t H, int32_t iscale) {
     int64_t t = ((int64_t)tA << 16) + wall_hrel(hA, pose_z) + (((int64_t)(1 - H) * iscale) >> 5);
     return (int32_t)t;
@@ -386,7 +389,8 @@ B2D_HD int32_t wall_tbase(int32_t tA, int32_t hA, int32_t pose_z, int32_t H, int
 B2D_HD uint32_t wall_row(int32_t t, uint32_t h, uint32_t hmagic, uint32_t hbias) {
     uint32_t n = ((uint32_t)t + (hbias << 16)) >> 16;
     uint32_t q = umulhi32(n, hmagic);
-    return n - q * h;
+    const uint32_t r = n - q * h;
+    return r < h ? r : 0u;
 }
 
 // ---- pre-lit texel planes (product-side data layout; results are the same bytes as colormap[row][texel]) -------

@@ -196,6 +196,27 @@ void walk(const HostScene &sc, const View &vw, const Pose &pose, FrameConst &fc,
 
 struct Lane { int ct, cb; uint32_t skycol; };
 
+// Probes of the raster mirror (read by tests through hostcheck_probe): texel reads that leave the texture's own texels,
+// its opacity plane or the flat they belong to (counted, and read as 0 instead), and per wall path the number of column
+// pieces drawn on it, by texture height (index min(h, 4096)).  The paths are draw_wall_warp's and masked_pass's.
+enum Path { kPathFast16, kPathFast8, kPathWord8, kPathSplit44, kPathBytes, kPathRowMajor, kPathMaskedInter, kPathMaskedRowMajor,
+            kPaths };
+constexpr int kProbeHeights = 4097;
+struct Probe {
+    long long oob = 0;
+    std::vector<long long> cov = std::vector<long long>((size_t)kPaths * kProbeHeights, 0);
+    void path(int p, uint32_t h) { cov[(size_t)p * kProbeHeights + (h < 4096u ? h : 4096u)]++; }
+};
+Probe g_probe;
+
+// n bytes at offset off of a texture's plane (texel_off based), or 0 (and counted) past its w*h texels
+uint32_t tex_read(const uint8_t *pl, const TexRec &T, uint64_t off, int n) {
+    if (off + (uint64_t)n > (uint64_t)T.w * T.h) { g_probe.oob++; return 0u; }
+    uint32_t v = 0;
+    std::memcpy(&v, pl + off, (size_t)n);
+    return v;
+}
+
 // mirrors b2d_raster_kernel, lanes executed one after the other
 struct RasterStats { long long iters = 0, pixels = 0, entries = 0, evals = 0; };
 
@@ -211,7 +232,7 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
         const uint8_t *px = sc.lit_texels + T.texel_off;                       // light row 0
         for (int y = ya; y < yb; y++) {
             int v = sky_row(y, H, (int32_t)T.h);
-            put(x, y, px[lit_index(inter, T.w, (uint32_t)v, ln.skycol)]);
+            put(x, y, (uint8_t)tex_read(px, T, lit_index(inter, T.w, (uint32_t)v, ln.skycol), 1));
         }
     };
     auto draw_plane = [&](int x, const Lane &ln, int ya, int yb, int32_t h, int32_t flat, int lightb, bool visible) {
@@ -224,8 +245,12 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
         const PlaneDir dir = plane_dir(fc, vw, x, invF);
         for (int y = ya; y < yb; y++) {
             PlaneRow pr = plane_row(habs, yslope[(size_t)y]);
-            const uint32_t cm6 = (sc.lit_flat_stride >> 6) * (uint32_t)light_row(lightb, pr.z8) + 64u * (uint32_t)flat;
-            put(x, y, px[flat_offset(cm6, plane_u(fc.pose.x, pr.z8q, dir.ax), plane_u(fc.pose.y, pr.z8q, dir.ay))]);
+            const int lr = light_row(lightb, pr.z8);
+            const uint32_t cm6 = (sc.lit_flat_stride >> 6) * (uint32_t)lr + 64u * (uint32_t)flat;
+            const uint32_t off = flat_offset(cm6, plane_u(fc.pose.x, pr.z8q, dir.ax), plane_u(fc.pose.y, pr.z8q, dir.ay));
+            const uint32_t own = (uint32_t)lr * sc.lit_flat_stride + 4096u * (uint32_t)flat;   // this flat in this light plane
+            if (off - own >= 4096u) { g_probe.oob++; put(x, y, 0); continue; }
+            put(x, y, px[off]);
         }
     };
     auto draw_wall = [&](int x, int ya, int yb, int32_t tex, int32_t tA, int32_t hA, int32_t ucol, int32_t iscale, int row) {
@@ -237,7 +262,9 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
         const uint32_t tstep = (uint32_t)(iscale >> 4);
         uint32_t t = (uint32_t)wall_tbase(tA, hA, fc.pose.z, H, iscale) + (uint32_t)ya * tstep;
         if (!tex_interleaved(T.h, T.texel_off)) {
-            for (int y = ya; y < yb; y++, t += tstep) put(x, y, pl[wall_row((int32_t)t, T.h, T.hmagic, T.hbias) * T.w + col]);
+            g_probe.path(kPathRowMajor, T.h);
+            for (int y = ya; y < yb; y++, t += tstep)
+                put(x, y, (uint8_t)tex_read(pl, T, wall_row((int32_t)t, T.h, T.hmagic, T.hbias) * T.w + col, 1));
             return;
         }
         if (T.h >= 8u && tstep <= kWallFast8) {
@@ -245,6 +272,7 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
             // lane, alternating between the 16- and the 8-row form, and starting a few rows above ya the way a lane whose
             // neighbours start higher does)
             const int R = (tstep <= kWallFast16 && (x & 1) == 0) ? 16 : 8;
+            g_probe.path(R == 16 ? kPathFast16 : kPathFast8, T.h);
             const int y0 = std::max(0, ya - (x % 5) * 3);
             const uint32_t t0 = (uint32_t)wall_tbase(tA, hA, fc.pose.z, H, iscale) + (uint32_t)y0 * tstep;
             const uint32_t r0 = wall_row((int32_t)t0, T.h, T.hmagic, T.hbias);
@@ -252,9 +280,8 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
             const uint32_t ts29 = tstep << 13, nq = T.h >> 2, w4f = 4u * T.w;
             for (int y = y0; y < yb; y += R) {
                 const uint32_t q1 = q + 1u == nq ? 0u : q + 1u;
-                uint32_t w0, w1;
-                std::memcpy(&w0, pl + 4u * col + (size_t)q * w4f, 4);
-                std::memcpy(&w1, pl + 4u * col + (size_t)q1 * w4f, 4);
+                const uint32_t w0 = tex_read(pl, T, 4u * col + (uint64_t)q * w4f, 4);
+                const uint32_t w1 = tex_read(pl, T, 4u * col + (uint64_t)q1 * w4f, 4);
                 const uint32_t m = row_mask(y, ya, yb, R);
                 for (int k = 0; k < R; k++)
                     if ((m >> k) & 1u) put(x, y + k, (uint8_t)(pick_byte(w0, w1, wall_sel(acc, ts29, (uint32_t)k)) & 0xFFu));
@@ -266,40 +293,41 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
         // consecutive row quads, eight byte fetches otherwise (the kernel decides per warp, here per lane: both
         // forms must give the same bytes, which is what the comparison with the oracle checks)
         const uint32_t colb = 4u * col, w4 = 4u * T.w;
+        uint32_t used = 0;
         for (int y = ya; y < yb; y += 8, t += 8u * tstep) {
             const uint32_t r0 = wall_row((int32_t)t, T.h, T.hmagic, T.hbias);
             const uint32_t acc = wall_acc(t, r0);
             uint32_t v[8];
             if (((acc + 7u * tstep) >> 16) < 8u) {
+                used |= 1u << kPathWord8;
                 const uint32_t q0 = r0 >> 2, q1 = next_quad(q0, T.h);
-                uint32_t w0, w1;
-                std::memcpy(&w0, pl + (q0 * w4 + colb), 4);
-                std::memcpy(&w1, pl + (q1 * w4 + colb), 4);
+                const uint32_t w0 = tex_read(pl, T, q0 * w4 + colb, 4), w1 = tex_read(pl, T, q1 * w4 + colb, 4);
                 for (uint32_t k = 0; k < 8; k++) v[k] = pick_byte(w0, w1, (acc + k * tstep) >> 16) & 0xFFu;
             } else {
                 const uint32_t t4 = t + 4u * tstep;
                 const uint32_t r4 = wall_row((int32_t)t4, T.h, T.hmagic, T.hbias);
                 const uint32_t acc4 = wall_acc(t4, r4);
                 if (((acc + 3u * tstep) >> 16) < 8u && ((acc4 + 3u * tstep) >> 16) < 8u) {   // two 4-row halves
+                    used |= 1u << kPathSplit44;
                     const uint32_t q0 = r0 >> 2, q4 = r4 >> 2;
-                    uint32_t a0, a1, b0, b1;
-                    std::memcpy(&a0, pl + (q0 * w4 + colb), 4);
-                    std::memcpy(&a1, pl + (next_quad(q0, T.h) * w4 + colb), 4);
-                    std::memcpy(&b0, pl + (q4 * w4 + colb), 4);
-                    std::memcpy(&b1, pl + (next_quad(q4, T.h) * w4 + colb), 4);
+                    const uint32_t a0 = tex_read(pl, T, q0 * w4 + colb, 4), a1 = tex_read(pl, T, next_quad(q0, T.h) * w4 + colb, 4);
+                    const uint32_t b0 = tex_read(pl, T, q4 * w4 + colb, 4), b1 = tex_read(pl, T, next_quad(q4, T.h) * w4 + colb, 4);
                     for (uint32_t k = 0; k < 4; k++) {
                         v[k] = pick_byte(a0, a1, (acc + k * tstep) >> 16) & 0xFFu;
                         v[k + 4] = pick_byte(b0, b1, (acc4 + k * tstep) >> 16) & 0xFFu;
                     }
                 } else {
+                    used |= 1u << kPathBytes;
                     for (uint32_t k = 0; k < 8; k++) {
                         const uint32_t rk = wall_row((int32_t)(t + k * tstep), T.h, T.hmagic, T.hbias);
-                        v[k] = pl[(rk >> 2) * w4 + colb + (rk & 3u)];
+                        v[k] = tex_read(pl, T, (rk >> 2) * w4 + colb + (rk & 3u), 1);
                     }
                 }
             }
             for (int k = 0; k < 8 && y + k < yb; k++) put(x, y + k, (uint8_t)v[k]);
         }
+        for (int p = kPathWord8; p <= kPathBytes; p++)
+            if ((used >> p) & 1u) g_probe.path(p, T.h);
     };
 
     const int strips = (W + SW - 1) / SW;
@@ -416,10 +444,12 @@ void raster(const HostScene &sc, const View &vw, const FrameConst &fc, const std
                 const bool has_mask = T.mask_off != 0xFFFFFFFFu;
                 const uint8_t *pm = sc.lit_texels + (size_t)32 * sc.lit_texel_stride + T.texel_off;   // opacity plane
                 int32_t tbase = wall_tbase(tA, hA, fc.pose.z, H, iscale), tstep = iscale >> 4;
+                if (ya < yb) g_probe.path(inter ? kPathMaskedInter : kPathMaskedRowMajor, T.h);
                 for (int y = ya; y < yb; y++) {
                     const uint32_t r = wall_row(tbase + y * tstep, T.h, T.hmagic, T.hbias);
-                    if (has_mask && !pm[lit_index(inter, T.w, r, col)]) continue;
-                    put(x, y, px[lit_index(inter, T.w, r, col)]);
+                    const uint32_t off = lit_index(inter, T.w, r, col);
+                    if (has_mask && !tex_read(pm, T, off, 1)) continue;
+                    put(x, y, (uint8_t)tex_read(px, T, off, 1));
                 }
             }
         }
@@ -494,6 +524,21 @@ extern "C" void hostcheck_lights(const uint8_t *blob, uint32_t tics, int16_t *ou
 }
 
 extern "C" void hostcheck_sincos(uint32_t angle, int32_t *c, int32_t *s) { sincos_q30(angle, *c, *s); }
+
+// the product's wall_row for texture rows u = u0 .. u0 + n - 1 (t = u * 2^16 + frac) of a texture of height h
+extern "C" void hostcheck_wall_rows(uint32_t h, uint32_t hmagic, uint32_t hbias, int32_t u0, int32_t n, uint32_t frac,
+                                    uint32_t *out) {
+    for (int32_t i = 0; i < n; i++)
+        out[i] = wall_row((int32_t)(((uint32_t)(u0 + i) << 16) | (frac & 0xFFFFu)), h, hmagic, hbias);
+}
+
+// the raster mirror's probes since the last reset: out-of-texture reads, and the [kPaths][4097] path counts
+extern "C" int hostcheck_probe(int reset, long long *oob, long long *cov) {
+    if (oob) *oob = g_probe.oob;
+    if (cov) std::memcpy(cov, g_probe.cov.data(), g_probe.cov.size() * sizeof(long long));
+    if (reset) g_probe = Probe();
+    return kPaths;
+}
 
 // lock-step iteration statistics for a strip width (design exploration; test-only)
 extern "C" int hostcheck_stats(const uint8_t *blob, const View *vw, const Pose *poses, int n, int strip_width,
