@@ -347,6 +347,35 @@ int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, cons
 int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames,
                                   uint32_t *d_rgba, void *cuda_stream);
 
+/* Kernel 4, resolve: index frames to box-filtered colour or grey frames at 1/factor of the render size (DESIGN.md C17), for
+ * consumers that take small observations (many agents or cameras per launch) and for anti-aliased images (render at
+ * factor x the size, resolve to 1x).  Replaces nothing in the reference (its GL path samples each pixel once: nearest
+ * filtering, no MSAA).  Frame f of the n_frames contiguous W x H index frames at d_index (W x H: the renderer's view)
+ * becomes a (W/factor) x (H/factor) frame at d_out: each output channel is the half-up rounded mean,
+ * (sum + factor^2/2) / factor^2, of its factor x factor block's entries of level levels[f]'s palette, or of that palette's
+ * luma Y = (77 R + 150 G + 29 B + 128) >> 8 for B2D_RESOLVE_GRAY8, averaged in the palette's encoded values.  Formats, row
+ * major, top row first:
+ *   B2D_RESOLVE_RGBA8        u32 per pixel packed as rgba_fb (alpha 0xFF), [n][H/k][W/k]; factor 1 is byte-identical to
+ *                            b2d_palette_lut_levels_device and to the raster's rgba_fb
+ *   B2D_RESOLVE_RGB8         3 x u8 per pixel, [n][H/k][W/k][3]
+ *   B2D_RESOLVE_RGB8_PLANAR  u8, [n][3][H/k][W/k] (the layout a convolution reads)
+ *   B2D_RESOLVE_GRAY8        u8, [n][H/k][W/k]
+ * b2d_resolve_frame_bytes gives the bytes of one output frame.  d_index and d_out may have any alignment (16-byte aligned
+ * frames take 128-bit loads).  The call is enqueued on `cuda_stream` and does not synchronise the device.  `levels` is a
+ * HOST array, or NULL for level 0 on every frame (nothing is staged then).  It is staged through pinned memory of this
+ * call's own (not shared with b2d_palette_lut_levels_device): before it is rewritten the host waits for the copy of the
+ * previous call that had levels, and the copy waits on `cuda_stream` for that call's kernel (a call with more frames than
+ * any before it allocates larger staging first).  A NULL d_index or d_out, a factor outside 1..8 or not dividing W and H,
+ * an unknown format and a level >= n_levels are B2D_ERR_INVALID_ARG, detected before anything is enqueued; n_frames = 0
+ * enqueues nothing. */
+#define B2D_RESOLVE_RGBA8 0
+#define B2D_RESOLVE_RGB8 1
+#define B2D_RESOLVE_RGB8_PLANAR 2
+#define B2D_RESOLVE_GRAY8 3
+int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, int factor,
+                       int format, void *d_out, void *cuda_stream);
+int b2d_resolve_frame_bytes(const b2d_renderer *r, int factor, int format, size_t *bytes_out);
+
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
  * per-frame `frame.finish()` of engine/src/renderer.rs:160-167.  One process per GPU.  NCCL (libnccl.so.2) is bound
@@ -416,9 +445,11 @@ int b2d_frame_checksums_device(const uint8_t *d_frames, size_t n_frames, size_t 
                                void *cuda_stream);
 
 /* Device memory for hosts that do not link a CUDA library themselves (the compiled CLI; a Rust binding would use its
- * cuda-sys crate instead): allocate / free on `device`, and a synchronous device -> host copy. */
+ * cuda-sys crate instead): allocate / free on `device`, a synchronous host -> device copy and a synchronous device -> host
+ * copy. */
 int b2d_device_alloc(int device, size_t bytes, void **d_out);
 int b2d_device_free(int device, void *d_ptr);
+int b2d_device_upload(int device, void *d_dst, const void *host_src, size_t bytes);
 int b2d_device_download(int device, void *host_dst, const void *d_src, size_t bytes);
 
 /* Introspection for tests/profiling: copies the BSP-walk worklist of the LAST b2d_render_device

@@ -302,6 +302,10 @@ def make_view(width: int, height: int, fov_deg: float = DEFAULT_FOV_DEG) -> "_li
 
 MAX_LEVELS = 64                 # B2D_MAX_LEVELS
 
+RESOLVE_RGBA8, RESOLVE_RGB8, RESOLVE_RGB8_PLANAR, RESOLVE_GRAY8 = (_lib.RESOLVE_RGBA8, _lib.RESOLVE_RGB8, _lib.RESOLVE_RGB8_PLANAR,
+                                                                   _lib.RESOLVE_GRAY8)
+RESOLVE_FORMATS = {"rgba": RESOLVE_RGBA8, "rgb": RESOLVE_RGB8, "rgb_planar": RESOLVE_RGB8_PLANAR, "gray": RESOLVE_GRAY8}
+
 
 def _levels_array(levels, n: int) -> np.ndarray:
     """the uint32 level array of n poses (the library refuses an index out of range)"""
@@ -523,6 +527,39 @@ class Renderer:
         level levels[f] (host list) into rgba_ptr (device pointers)."""
         lv = _levels_array(levels, n_frames)
         _check(_lib.load().b2d_palette_lut_levels_device(self._h, index_ptr, lv.ctypes.data, n_frames, rgba_ptr, stream or None))
+
+    def resolve_device(self, index_ptr: int, n: int, factor: int, fmt: int, out_ptr: int, levels=None, stream: int = 0):
+        """b2d_resolve_device: frame f of the n contiguous index frames at index_ptr, box-filtered by `factor` (1..8, dividing
+        the view's sides) through the palette of level levels[f] (host list; None = level 0) into out_ptr in format `fmt`
+        (RESOLVE_RGBA8 / RESOLVE_RGB8 / RESOLVE_RGB8_PLANAR / RESOLVE_GRAY8; device pointers)."""
+        lv = None if levels is None else _levels_array(levels, n)
+        _check(_lib.load().b2d_resolve_device(self._h, index_ptr, None if lv is None else lv.ctypes.data, n, int(factor), int(fmt),
+                                              out_ptr, stream or None))
+
+    def resolve_frame_bytes(self, factor: int, fmt: int) -> int:
+        """b2d_resolve_frame_bytes: bytes of one resolved frame."""
+        out = ctypes.c_size_t()
+        _check(_lib.load().b2d_resolve_frame_bytes(self._h, int(factor), int(fmt), ctypes.byref(out)))
+        return int(out.value)
+
+    def resolve(self, index, factor: int = 2, fmt: str = "rgb_planar", levels=None):
+        """The resolve of a CUDA uint8 tensor [n, H, W] of index frames into a new CUDA tensor, on the current torch stream:
+        fmt "rgba" -> int32 [n, H/k, W/k] (RGBA8 words), "rgb" -> uint8 [n, H/k, W/k, 3], "rgb_planar" -> uint8
+        [n, 3, H/k, W/k], "gray" -> uint8 [n, H/k, W/k]; `levels` as in resolve_device."""
+        import torch
+        code = RESOLVE_FORMATS[fmt]
+        if not (index.is_cuda and index.dtype == torch.uint8 and index.dim() == 3 and tuple(index.shape[1:]) == (self.height, self.width)):
+            raise ValueError("resolve takes a CUDA uint8 tensor [n, %d, %d]" % (self.height, self.width))
+        index = index.contiguous()
+        n, k = int(index.shape[0]), int(factor)
+        oh, ow = (self.height // k, self.width // k) if 1 <= k <= 8 else (0, 0)      # the library refuses other factors
+        shape = {_lib.RESOLVE_RGBA8: (n, oh, ow), _lib.RESOLVE_RGB8: (n, oh, ow, 3), _lib.RESOLVE_RGB8_PLANAR: (n, 3, oh, ow),
+                 _lib.RESOLVE_GRAY8: (n, oh, ow)}[code]
+        out = torch.empty(shape, dtype=torch.int32 if code == _lib.RESOLVE_RGBA8 else torch.uint8, device=index.device)
+        with torch.cuda.device(index.device):
+            stream = torch.cuda.current_stream().cuda_stream
+        self.resolve_device(index.data_ptr(), n, k, code, out.data_ptr(), levels, stream)
+        return out
 
     def worklist(self, n: int):
         counts = np.zeros(n, dtype=np.int32)

@@ -55,10 +55,12 @@ EXPORTS = [
     "b2d_debug_worklist", "b2d_debug_state_slots", "b2d_debug_state_tables", "b2d_launch_count", "b2d_profile_enable", "b2d_profile_read",
     "b2d_comm_unique_id", "b2d_comm_create", "b2d_comm_destroy", "b2d_comm_info", "b2d_render_sharded",
     "b2d_render_sharded_levels_states", "b2d_palette_lut_levels_device",
-    "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_download",
+    "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_upload", "b2d_device_download",
+    "b2d_resolve_device", "b2d_resolve_frame_bytes",
 ]
 
 COMM_ID_BYTES = 128
+RESOLVE_RGBA8, RESOLVE_RGB8, RESOLVE_RGB8_PLANAR, RESOLVE_GRAY8 = 0, 1, 2, 3      # B2D_RESOLVE_*
 SHARD_RENDER_ONLY, SHARD_RENDER_GATHER, SHARD_GATHER_ONLY = 0, 1, 2
 
 
@@ -188,5 +190,7 @@ def load() -> ctypes.CDLL:
                                                    ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
     L.b2d_palette_lut_levels_device.argtypes = [vp, vp, vp, cs, vp, vp]
     L.b2d_frame_checksums_device.argtypes = [vp, cs, cs, vp, vp]
+    L.b2d_resolve_device.argtypes = [vp, vp, vp, cs, ci, ci, vp, vp]
+    L.b2d_resolve_frame_bytes.argtypes = [vp, ci, ci, ctypes.POINTER(cs)]
     _lib = L
     return L

@@ -1,7 +1,7 @@
 """`b2d` command line, mirroring rs_doom's flags (reference src/main.rs:17-80,89-124):
 
     python -m rust_doom_b200.cli --iwad doom1.wad --level 0 --resolution 1920x1080 [--fov 65]
-                                 [--poses N] [--dump frame.ppm] [--device 0]
+                                 [--poses N] [--dump frame.ppm] [--device 0] [--supersample K]
     python -m rust_doom_b200.cli --iwad doom1.wad --levels 0,2,5 --poses N [--tics T] [--dump f.ppm] [--stream s.ppm]
                                  [--world W --rank R --id-file PATH [--chunk C]]
     python -m rust_doom_b200.cli --iwad doom1.wad list-levels
@@ -16,7 +16,12 @@ honoured (its value is parsed but never read there: main.rs:131 vs game/src/game
 start, --poses per level, pose i at tic T + i.  --dump NAME.EXT writes NAME.L.EXT, the first frame of level L.  With
 --world the poses are sharded over one process per GPU (b2d_render_sharded_levels_states; rank 0 writes the NCCL unique id
 to --id-file, the others read it) and rank 0 colours every gathered frame with its own level's palette on the device
-(b2d_palette_lut_levels_device) before it writes the --stream."""
+(b2d_palette_lut_levels_device) before it writes the --stream.
+
+--supersample K (1..8) renders every frame at K times the resolution with the same field of view and resolves each K x K
+block to one pixel of the --resolution frame on the device (b2d_resolve_device, C17: the half-up rounded mean of the
+block's palette colours, each frame through its own level's palette): an anti-aliased --dump and --stream.  Not with
+--world."""
 from __future__ import annotations
 
 import argparse
@@ -128,6 +133,14 @@ def _write_image(path: str, rgb: np.ndarray):
         f.write(encode_png(rgb) if path.lower().endswith(".png") else encode_ppm(rgb))
 
 
+def resolve_rgb(r, index: np.ndarray, factor: int, levels=None) -> np.ndarray:
+    """(n, H, W, 3) uint8: the host index frames of renderer r resolved by `factor` on its device (b2d_resolve_device)"""
+    import torch
+    dev = torch.device("cuda", r.device)
+    with torch.cuda.device(dev):
+        return r.resolve(torch.from_numpy(np.ascontiguousarray(index)).to(dev), factor, "rgb", levels).cpu().numpy()
+
+
 def _comm_from_file(b2d, id_file: str, rank: int, world: int):
     if rank == 0:
         with open(id_file + ".tmp", "wb") as f:
@@ -153,15 +166,21 @@ def _main_levels(b2d, arch, set_, view, args, w, h) -> int:
     n = len(poses)
     if not args.world:
         r = b2d.Renderer.from_levels(scenes, view, device=args.device, max_batch=min(n, 64))
-        rgba = r.render_levels_states(poses, levels, tics, rgba=True)[1]
-        print("rendered %d frame(s) %dx%d of %d level(s)" % (n, w, h, len(set_)))
+        if args.supersample > 1:
+            rgb = resolve_rgb(r, r.render_levels_states(poses, levels, tics), args.supersample, levels)
+            print("rendered %d frame(s) %dx%d of %d level(s), supersampled %dx" % (n, w, h, len(set_), args.supersample))
+            frame = lambda i: rgb[i]    # noqa: E731
+        else:
+            rgba = r.render_levels_states(poses, levels, tics, rgba=True)[1]
+            print("rendered %d frame(s) %dx%d of %d level(s)" % (n, w, h, len(set_)))
+            frame = lambda i: rgba_to_rgb(rgba[i])    # noqa: E731
         if args.dump:
             for k, lvl in enumerate(set_):
-                _write_image(_dump_name(args.dump, lvl), rgba_to_rgb(rgba[k * per_level]))
+                _write_image(_dump_name(args.dump, lvl), frame(k * per_level))
         if args.stream:
             with open(args.stream, "wb") as f:
                 for i in range(n):
-                    f.write(encode_ppm(rgba_to_rgb(rgba[i])))
+                    f.write(encode_ppm(frame(i)))
         return 0
     import torch
     from rust_doom_b200 import _lib
@@ -235,6 +254,8 @@ def main(argv=None) -> int:
     ap.add_argument("--rank", type=int, default=0)
     ap.add_argument("--id-file", default=None, help="with --world: the file rank 0 writes the NCCL unique id to")
     ap.add_argument("--chunk", type=int, default=16, help="with --world: frames per rank and chunk")
+    ap.add_argument("--supersample", type=int, default=1,
+                    help="render at K times the resolution (1..8) and resolve every K x K block to one output pixel")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 
@@ -242,6 +263,13 @@ def main(argv=None) -> int:
         w, h = (int(v) for v in args.resolution.lower().split("x"))
     except ValueError:
         print("resolution format is WIDTHxHEIGHT", file=sys.stderr)
+        return 2
+    ss = args.supersample
+    if not 1 <= ss <= 8:
+        print("--supersample takes a factor in 1..8", file=sys.stderr)
+        return 2
+    if ss > 1 and (args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        print("--supersample does not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
         return 2
     try:
         arch = b2d.Archive.open(args.iwad) if args.iwad else b2d.Archive.from_bytes(synthwad.build_iwad(1, synthwad.E1_MAPS[:3]))
@@ -264,12 +292,12 @@ def main(argv=None) -> int:
             if args.world and not args.id_file:
                 print("--id-file PATH is required with --world", file=sys.stderr)
                 return 2
-            return _main_levels(b2d, arch, set_, b2d.make_view(w, h, args.fov), args, w, h)
+            return _main_levels(b2d, arch, set_, b2d.make_view(ss * w, ss * h, args.fov), args, w, h)
         if args.world:
             print("--world takes --levels (a single level shards under torchrun)", file=sys.stderr)
             return 2
         scene = b2d.Scene(arch, args.level)
-        view = b2d.make_view(w, h, args.fov)
+        view = b2d.make_view(ss * w, ss * h, args.fov)
         if args.poses <= 1:
             poses = scene.start_pose if scene.start_pose is not None else P.random_poses(scene, 1, 1)
         else:
@@ -279,23 +307,35 @@ def main(argv=None) -> int:
             return _main_sharded(b2d, scene, view, poses, args, w, h, world)
         r = b2d.Renderer(scene, view, device=args.device, max_batch=min(len(poses), 256))
         t0 = time.perf_counter()
-        if args.tics_per_frame > 0:          # time is a per-batch input: one batch per frame
+        if ss > 1:
+            index = np.empty((len(poses), ss * h, ss * w), dtype=np.uint8)
+            if args.tics_per_frame > 0:
+                for i in range(len(poses)):
+                    r.set_time(i * args.tics_per_frame)
+                    index[i] = r.render(poses[i:i + 1])[0]
+            else:
+                r.render(poses, out_index=index)
+            rgb = resolve_rgb(r, index, ss)
+            frame = lambda i: rgb[i]    # noqa: E731
+        elif args.tics_per_frame > 0:          # time is a per-batch input: one batch per frame
             rgba = np.empty((len(poses), h, w), dtype=np.uint32)
             for i in range(len(poses)):
                 r.set_time(i * args.tics_per_frame)
                 rgba[i] = r.render(poses[i:i + 1], rgba=True)[1][0]
         else:
             rgba = r.render(poses, rgba=True)[1]
+        if ss == 1:
+            frame = lambda i: rgba_to_rgb(rgba[i])    # noqa: E731
         dt = time.perf_counter() - t0
         print("rendered %d frame(s) %dx%d in %.2f ms (%.0f frames/s end to end)" % (len(poses), w, h, dt * 1e3, len(poses) / dt))
         if args.dump:
-            rgb = rgba_to_rgb(rgba[0])
+            rgb0 = frame(0)
             with open(args.dump, "wb") as f:
-                f.write(encode_png(rgb) if args.dump.lower().endswith(".png") else encode_ppm(rgb))
+                f.write(encode_png(rgb0) if args.dump.lower().endswith(".png") else encode_ppm(rgb0))
         if args.stream:
             with open(args.stream, "wb") as f:
-                for i in range(len(rgba)):
-                    f.write(encode_ppm(rgba_to_rgb(rgba[i])))
+                for i in range(len(poses)):
+                    f.write(encode_ppm(frame(i)))
         return 0
     except b2d.B2dError as e:
         print("Fatal error: %s" % e, file=sys.stderr)

@@ -1526,6 +1526,64 @@ int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const
     return B2D_OK;
 }
 
+// the resolve's arguments against the renderer's view: B2D_OK or B2D_ERR_INVALID_ARG with the message set
+static int check_resolve(const b2d_renderer *r, int factor, int format) {
+    if (factor < 1 || factor > 8 || r->view.W % factor || r->view.H % factor)
+        return fail(B2D_ERR_INVALID_ARG, "resolve factor must be in 1..8 and divide the view's width and height");
+    if (format < B2D_RESOLVE_RGBA8 || format > B2D_RESOLVE_GRAY8) return fail(B2D_ERR_INVALID_ARG, "unknown resolve format");
+    return B2D_OK;
+}
+
+int b2d_resolve_frame_bytes(const b2d_renderer *r, int factor, int format, size_t *bytes_out) {
+    if (!r || !bytes_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (int rc = check_resolve(r, factor, format)) return rc;
+    const size_t bpp = format == B2D_RESOLVE_RGBA8 ? 4 : format == B2D_RESOLVE_GRAY8 ? 1 : 3;
+    *bytes_out = (size_t)(r->view.W / factor) * (size_t)(r->view.H / factor) * bpp;
+    return B2D_OK;
+}
+
+int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, int factor, int format,
+                       void *d_out, void *cuda_stream) {
+    if (!r || !d_index || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (int rc = check_resolve(r, factor, format)) return rc;
+    if (levels)
+        for (size_t i = 0; i < n_frames; i++)
+            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    if (n_frames == 0) return B2D_OK;
+    CU(cudaSetDevice(r->device));
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    const uint32_t *d_levels = nullptr;          // NULL levels: every frame through level 0's palette, nothing to stage
+    if (levels) {
+        if (r->resolve_levels_cap < n_frames) {
+            // created whole, or not at all; the old buffers go once the last call's kernel has read them
+            size_t cap = r->resolve_levels_cap ? r->resolve_levels_cap : 1024;
+            while (cap < n_frames) cap *= 2;
+            DeviceBuf<uint32_t> d;
+            PinnedBuf<uint32_t> h;
+            Event copied, done;
+            CU(allocate(d, cap * sizeof(uint32_t)));
+            CU(allocate(h, cap * sizeof(uint32_t)));
+            CU(event_create(copied));
+            CU(event_create(done));
+            if (r->resolve_done) CU(cudaEventSynchronize(r->resolve_done.get()));
+            r->d_resolve_levels = std::move(d); r->h_resolve_levels = std::move(h);
+            r->resolve_levels_copied = std::move(copied); r->resolve_done = std::move(done);
+            r->resolve_levels_cap = cap;
+        } else {
+            CU(cudaEventSynchronize(r->resolve_levels_copied.get()));     // the previous call's copy has read the staging
+            CU(cudaStreamWaitEvent(st, r->resolve_done.get(), 0));        // ... and its kernel the device copy
+        }
+        std::memcpy(r->h_resolve_levels.get(), levels, n_frames * sizeof(uint32_t));
+        CU(cudaMemcpyAsync(r->d_resolve_levels.get(), r->h_resolve_levels.get(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        CU(cudaEventRecord(r->resolve_levels_copied.get(), st));
+        d_levels = r->d_resolve_levels.get();
+    }
+    CU(launch_resolve(r->d_palettes.get(), d_levels, d_index, d_out, n_frames, r->view.W, r->view.H, factor, format, st));
+    if (levels) CU(cudaEventRecord(r->resolve_done.get(), st));
+    r->launches += 1;
+    return B2D_OK;
+}
+
 int b2d_device_alloc(int device, size_t bytes, void **d_out) {
     if (!d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     CU(cudaSetDevice(device));
@@ -1537,6 +1595,13 @@ int b2d_device_alloc(int device, size_t bytes, void **d_out) {
 int b2d_device_free(int device, void *d_ptr) {
     CU(cudaSetDevice(device));
     CU(cudaFree(d_ptr));
+    return B2D_OK;
+}
+
+int b2d_device_upload(int device, void *d_dst, const void *host_src, size_t bytes) {
+    if (!d_dst || !host_src) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    CU(cudaSetDevice(device));
+    CU(cudaMemcpy(d_dst, host_src, bytes, cudaMemcpyHostToDevice));
     return B2D_OK;
 }
 

@@ -11,6 +11,9 @@
 // start, --poses per level, pose i at tic T + i (--tics T), through one b2d_renderer_create_levels renderer:
 // b2d_render_levels_states in one process (--dump NAME writes NAME.L.ppm, the first frame of level L), and
 // b2d_render_sharded_levels_states with --world.
+// --supersample K (1..8) renders at K times the resolution with the same field of view and resolves every frame to
+// --resolution RGB on the device (b2d_resolve_device, each frame through its own level's palette) for --dump and --stream;
+// not with --world.
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -60,6 +63,45 @@ void write_ppm(std::FILE *f, const uint32_t *rgba, int w, int h) {
         }
         std::fwrite(row.data(), 1, row.size(), f);
     }
+}
+
+void write_ppm_rgb(std::FILE *f, const uint8_t *rgb, int w, int h) {
+    std::fprintf(f, "P6\n%d %d\n255\n", w, h);
+    std::fwrite(rgb, 1, (size_t)w * h * 3, f);
+}
+
+// --supersample: render the n poses (levels: per-frame levels and states, else the renderer's own state) into device index
+// frames at the renderer's view, resolve them by `factor` to RGB8 and download them into `rgb` (n x (W/factor) x (H/factor) x 3)
+int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, size_t max_batch,
+                        const uint32_t *levels, const b2d_frame_state *states, int factor, std::vector<uint8_t> &rgb) {
+    const size_t n = poses.size(), npix = (size_t)view.width * view.height;
+    size_t frame_bytes = 0;
+    if (b2d_resolve_frame_bytes(r, factor, B2D_RESOLVE_RGB8, &frame_bytes) != B2D_OK) return fail("resolve");
+    void *d_poses = nullptr, *d_index = nullptr, *d_rgb = nullptr;
+    struct Bufs {
+        int device;
+        void **p[3];
+        ~Bufs() { for (void **q : p) if (*q) b2d_device_free(device, *q); }
+    } owner{device, {&d_poses, &d_index, &d_rgb}};
+    if (b2d_device_alloc(device, sizeof(b2d_pose) * n, &d_poses) != B2D_OK || b2d_device_alloc(device, npix * n, &d_index) != B2D_OK ||
+        b2d_device_alloc(device, frame_bytes * n, &d_rgb) != B2D_OK)
+        return fail("device memory");
+    if (b2d_device_upload(device, d_poses, poses.data(), sizeof(b2d_pose) * n) != B2D_OK) return fail("upload");
+    const b2d_pose *dp = static_cast<const b2d_pose *>(d_poses);
+    uint8_t *di = static_cast<uint8_t *>(d_index);
+    if (levels) {
+        if (b2d_render_device_levels_states(r, dp, levels, states, n, nullptr, 0, di, nullptr, nullptr) != B2D_OK) return fail("render");
+    } else {
+        for (size_t i = 0; i < n; i += max_batch)
+            if (b2d_render_device(r, dp + i, std::min(max_batch, n - i), di + npix * i, nullptr, nullptr) != B2D_OK) return fail("render");
+    }
+    if (b2d_resolve_device(r, di, levels, n, factor, B2D_RESOLVE_RGB8, d_rgb, nullptr) != B2D_OK) return fail("resolve");
+    int32_t bits = 0;
+    if (b2d_renderer_status(r, &bits) != B2D_OK) return fail("status");
+    if (bits) { std::fprintf(stderr, "Fatal error: frames incomplete (status %d)\n", bits); return 1; }
+    rgb.resize(frame_bytes * n);
+    if (b2d_device_download(device, rgb.data(), d_rgb, rgb.size()) != B2D_OK) return fail("download");
+    return 0;
 }
 
 // b2d_render_sharded consumer: per-frame checksums of every gathered chunk into a device table (the table lives in device memory
@@ -112,7 +154,8 @@ int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st
 
 // --levels: the look-around of every level of `set` from its start, nposes per level, pose i at tic tics + i
 int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
-                     const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file) {
+                     const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file,
+                     int supersample) {
     std::vector<b2d_scene *> scenes;
     struct Scenes {
         std::vector<b2d_scene *> &v;
@@ -138,7 +181,7 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
     }
     for (size_t i = 0; i < n; i++) states[i] = b2d_frame_state{tics + (uint32_t)i, 0, 0};
     b2d_view view;
-    if (b2d_view_init(&view, width, height, fov) != B2D_OK) return fail("view");
+    if (b2d_view_init(&view, width * supersample, height * supersample, fov) != B2D_OK) return fail("view");
     b2d_renderer *r = nullptr;
     if (b2d_renderer_create_levels(scenes.data(), scenes.size(), &view, world > 0 ? rank : 0, n < 64 ? (int)n : 64, &r) != B2D_OK)
         return fail("renderer");
@@ -161,25 +204,36 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
         b2d_comm_destroy(comm);
         return rc;
     }
-    std::vector<uint8_t> index(npix * n);
-    std::vector<uint32_t> rgba(npix * n);
-    if (b2d_render_levels_states(r, poses.data(), levels.data(), states.data(), n, nullptr, 0, index.data(), rgba.data()) != B2D_OK)
-        return fail("render");
-    std::printf("rendered %zu frame(s) %dx%d of %zu level(s)\n", n, width, height, set.size());
+    std::vector<uint8_t> index, rgb;
+    std::vector<uint32_t> rgba;
+    if (supersample > 1) {
+        if (int rc = render_supersampled(r, 0, view, poses, n < 64 ? n : 64, levels.data(), states.data(), supersample, rgb)) return rc;
+        std::printf("rendered %zu frame(s) %dx%d of %zu level(s), supersampled %dx\n", n, width, height, set.size(), supersample);
+    } else {
+        index.resize(npix * n);
+        rgba.resize(npix * n);
+        if (b2d_render_levels_states(r, poses.data(), levels.data(), states.data(), n, nullptr, 0, index.data(), rgba.data()) != B2D_OK)
+            return fail("render");
+        std::printf("rendered %zu frame(s) %dx%d of %zu level(s)\n", n, width, height, set.size());
+    }
+    auto write_frame = [&](std::FILE *f, size_t i) {
+        if (supersample > 1) write_ppm_rgb(f, rgb.data() + npix * 3 * i, width, height);
+        else write_ppm(f, rgba.data() + npix * i, width, height);
+    };
     if (!dump.empty()) {
         const std::string stem = dump.size() > 4 && dump.compare(dump.size() - 4, 4, ".ppm") == 0 ? dump.substr(0, dump.size() - 4) : dump;
         for (size_t k = 0; k < set.size(); k++) {
             const std::string name = stem + "." + std::to_string(set[k]) + ".ppm";
             std::FILE *f = std::fopen(name.c_str(), "wb");
             if (!f) { std::perror(name.c_str()); return 1; }
-            write_ppm(f, rgba.data() + npix * k * per_level, width, height);
+            write_frame(f, k * per_level);
             std::fclose(f);
         }
     }
     if (!stream.empty()) {
         std::FILE *f = std::fopen(stream.c_str(), "wb");
         if (!f) { std::perror(stream.c_str()); return 1; }
-        for (size_t i = 0; i < n; i++) write_ppm(f, rgba.data() + npix * i, width, height);
+        for (size_t i = 0; i < n; i++) write_frame(f, i);
         std::fclose(f);
     }
     return 0;
@@ -189,7 +243,7 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
 
 int main(int argc, char **argv) {
     std::string iwad, dump, stream, command, id_file, levels_arg;
-    int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16;
+    int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16, supersample = 1;
     double fov = 65.0;
     unsigned long tics = 0;
     bool with_levels = false;
@@ -217,11 +271,14 @@ int main(int argc, char **argv) {
         else if (a == "--world") world = std::atoi(next("--world"));
         else if (a == "--chunk") chunk = std::atoi(next("--chunk"));
         else if (a == "--id-file") id_file = next("--id-file");
+        else if (a == "--supersample") supersample = std::atoi(next("--supersample"));
         else if (a == "list-levels" || a == "check") command = a;
         else { std::fprintf(stderr, "unknown argument %s\n", a.c_str()); return 2; }
     }
     if (iwad.empty()) { std::fprintf(stderr, "--iwad FILE is required\n"); return 2; }
     if (nposes < 1) nposes = 1;
+    if (supersample < 1 || supersample > 8) { std::fprintf(stderr, "--supersample takes a factor in 1..8\n"); return 2; }
+    if (supersample > 1 && world > 0) { std::fprintf(stderr, "--supersample does not combine with --world\n"); return 2; }
 
     b2d_archive *arch = nullptr;
     if (b2d_archive_open(iwad.c_str(), &arch) != B2D_OK) return fail("open");
@@ -257,7 +314,8 @@ int main(int argc, char **argv) {
             std::fprintf(stderr, "--levels takes `all` or comma-separated level indices below %d\n", nlevels);
             return 2;
         }
-        const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file);
+        const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file,
+                                        supersample);
         b2d_archive_close(arch);
         return rc;
     }
@@ -267,7 +325,7 @@ int main(int argc, char **argv) {
     b2d_scene_info_get(sc, &info);
     if (!info.has_start) { std::fprintf(stderr, "Fatal error: the level has no player-1 start\n"); return 1; }
     b2d_view view;
-    if (b2d_view_init(&view, width, height, fov) != B2D_OK) return fail("view");
+    if (b2d_view_init(&view, width * supersample, height * supersample, fov) != B2D_OK) return fail("view");
     b2d_renderer *r = nullptr;
     if (b2d_renderer_create(sc, &view, world > 0 ? rank : 0, nposes < 64 ? nposes : 64, &r) != B2D_OK) return fail("renderer");
     if (b2d_renderer_set_time(r, (uint32_t)tics) != B2D_OK) return fail("time");
@@ -276,6 +334,27 @@ int main(int argc, char **argv) {
     for (int i = 0; i < nposes; i++)          // look around from the spawn point
         poses[(size_t)i].angle = info.start.angle + (uint32_t)(((uint64_t)i << 32) / (uint64_t)nposes);
     const size_t npix = (size_t)width * height;
+    if (supersample > 1) {
+        std::vector<uint8_t> rgb;
+        if (int rc = render_supersampled(r, 0, view, poses, nposes < 64 ? nposes : 64, nullptr, nullptr, supersample, rgb)) return rc;
+        std::printf("rendered %d frame(s) %dx%d, supersampled %dx\n", nposes, width, height, supersample);
+        if (!dump.empty()) {
+            std::FILE *f = std::fopen(dump.c_str(), "wb");
+            if (!f) { std::perror(dump.c_str()); return 1; }
+            write_ppm_rgb(f, rgb.data(), width, height);
+            std::fclose(f);
+        }
+        if (!stream.empty()) {
+            std::FILE *f = std::fopen(stream.c_str(), "wb");
+            if (!f) { std::perror(stream.c_str()); return 1; }
+            for (int i = 0; i < nposes; i++) write_ppm_rgb(f, rgb.data() + npix * 3 * (size_t)i, width, height);
+            std::fclose(f);
+        }
+        b2d_renderer_destroy(r);
+        b2d_scene_destroy(sc);
+        b2d_archive_close(arch);
+        return 0;
+    }
     if (world > 0) {
         // ---- sharded: every rank runs this with the same pose list
         b2d_comm *comm = nullptr;

@@ -182,6 +182,11 @@ struct b2d_renderer {
     PinnedBuf<uint32_t> h_lut_levels;
     size_t lut_levels_cap = 0;
     Event lut_levels_copied, lut_done;                    // the staging has been read by its copy; the kernel has read the copy
+    // b2d_resolve_device: its own frame levels on the device and their pinned staging, with the same rules
+    DeviceBuf<uint32_t> d_resolve_levels;
+    PinnedBuf<uint32_t> h_resolve_levels;
+    size_t resolve_levels_cap = 0;
+    Event resolve_levels_copied, resolve_done;
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;
     bool profiling = false;

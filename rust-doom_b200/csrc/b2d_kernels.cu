@@ -11,6 +11,8 @@
 //   b2d_prelight_*     : build those planes once per renderer (32 light rows x texels / flats).
 //   b2d_palette_kernel : index -> RGBA8 with the 256-entry palette in shared memory, 128-bit I/O;
 //   b2d_palette_levels_kernel the same with a palette per frame (a level set's frames).
+//   b2d_resolve_kernel : k x k box filter of index frames through a palette (or its luma) per frame into RGBA, RGB,
+//                        planar RGB or grey frames at 1/k of the size (C17).
 //
 // There is no dense contraction anywhere on this path, so no tensor-core (wgmma) work: the
 // kernels are integer/LSU/latency bound and are tuned against the HBM write roofline (DESIGN.md).
@@ -1081,6 +1083,167 @@ b2d_palette_levels_kernel(const uint32_t *__restrict__ palettes, const uint32_t 
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Kernel 4: resolve (C17) -- k x k box filter of index frames through a palette per frame
+// ------------------------------------------------------------------------------------------------
+// Output formats, the values of B2D_RESOLVE_* in include/b2d.h.
+constexpr int kResolveRgba = 0, kResolveRgb = 1, kResolvePlanar = 2, kResolveGray = 3;
+
+// `N` bytes, packed little-endian in w[], to dst with the widest stores its alignment allows.
+template <int N>
+__device__ __forceinline__ void store_run(uint8_t *dst, const uint32_t (&w)[(N + 3) / 4]) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dst);
+    if constexpr (N % 16 == 0) {
+        if ((a & 15) == 0) {
+#pragma unroll
+            for (int q = 0; q < N / 16; q++) __stcs(reinterpret_cast<uint4 *>(dst) + q, make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]));
+            return;
+        }
+    }
+    if constexpr (N % 8 == 0) {
+        if ((a & 7) == 0) {
+#pragma unroll
+            for (int q = 0; q < N / 8; q++) __stcs(reinterpret_cast<uint2 *>(dst) + q, make_uint2(w[2 * q], w[2 * q + 1]));
+            return;
+        }
+    }
+    if constexpr (N % 4 == 0) {
+        if ((a & 3) == 0) {
+#pragma unroll
+            for (int q = 0; q < N / 4; q++) __stcs(reinterpret_cast<unsigned int *>(dst) + q, w[q]);
+            return;
+        }
+    }
+    if constexpr (N % 2 == 0) {
+        if ((a & 1) == 0) {
+#pragma unroll
+            for (int q = 0; q < N / 2; q++) reinterpret_cast<uint16_t *>(dst)[q] = (uint16_t)(w[q / 2] >> (16 * (q % 2)));
+            return;
+        }
+    }
+#pragma unroll
+    for (int b = 0; b < N; b++) dst[b] = (uint8_t)(w[b / 4] >> (8 * (b % 4)));
+}
+
+// Writes the P output pixels (x0 .. x0+P-1, y) of one frame from their k x k sums: acc0 = {R | B << 16} (grey: Y) and
+// acc1 = G, each rounded half up, (sum + k*k/2) / (k*k).  `o` is the frame's output, OW x OH pixels.
+template <int K, int FMT, int P>
+__device__ __forceinline__ void resolve_emit(uint8_t *o, size_t opix, int OW, int y, int x0, const uint32_t (&acc0)[P],
+                                             const uint32_t (&acc1)[P]) {
+    constexpr uint32_t kk = K * K, half = K * K / 2;
+    const size_t at = (size_t)y * OW + x0;
+    if constexpr (FMT == kResolveGray) {
+        uint32_t w[(P + 3) / 4] = {};
+#pragma unroll
+        for (int p = 0; p < P; p++) w[p / 4] |= ((acc0[p] + half) / kk) << (8 * (p % 4));
+        store_run<P>(o + at, w);
+    } else {
+        uint32_t r[P], g[P], b[P];
+#pragma unroll
+        for (int p = 0; p < P; p++) {
+            r[p] = ((acc0[p] & 0xFFFFu) + half) / kk;
+            b[p] = ((acc0[p] >> 16) + half) / kk;
+            g[p] = (acc1[p] + half) / kk;
+        }
+        if constexpr (FMT == kResolveRgba) {
+            uint32_t w[P];
+#pragma unroll
+            for (int p = 0; p < P; p++) w[p] = r[p] | (g[p] << 8) | (b[p] << 16) | 0xFF000000u;
+            store_run<4 * P>(o + 4 * at, w);
+        } else if constexpr (FMT == kResolveRgb) {
+            uint32_t w[(3 * P + 3) / 4] = {};
+#pragma unroll
+            for (int p = 0; p < P; p++) {
+                w[(3 * p) / 4] |= r[p] << (8 * ((3 * p) % 4));
+                w[(3 * p + 1) / 4] |= g[p] << (8 * ((3 * p + 1) % 4));
+                w[(3 * p + 2) / 4] |= b[p] << (8 * ((3 * p + 2) % 4));
+            }
+            store_run<3 * P>(o + 3 * at, w);
+        } else {   // planar: R plane, G plane, B plane
+            uint32_t wr[(P + 3) / 4] = {}, wg[(P + 3) / 4] = {}, wb[(P + 3) / 4] = {};
+#pragma unroll
+            for (int p = 0; p < P; p++) {
+                wr[p / 4] |= r[p] << (8 * (p % 4));
+                wg[p / 4] |= g[p] << (8 * (p % 4));
+                wb[p / 4] |= b[p] << (8 * (p % 4));
+            }
+            store_run<P>(o + at, wr);
+            store_run<P>(o + opix + at, wg);
+            store_run<P>(o + 2 * opix + at, wb);
+        }
+    }
+}
+
+// `parts` CTAs per frame (blockIdx.x = frame * parts + part), each loading its frame's palette -- as {R | B << 16, G}, or
+// the luma Y = (77 R + 150 G + 29 B + 128) >> 8 for grey -- into shared memory and resolving a contiguous 1/parts of the
+// frame's work items (sums of up to 64 entries stay below 2^14, so R and B share a word).  Vector path (`vec`: W a
+// multiple of P * K and the index frames 16-byte aligned): an item is P = 16 / gcd(K, 16) output pixels of one output row,
+// read as P * K / 16 128-bit streaming loads from each of its K input rows, so every byte's output pixel is a
+// compile-time constant.  Otherwise an item is one output pixel, read byte by byte.  Stores: store_run.
+template <int K, int FMT>
+__global__ void __launch_bounds__(256)
+b2d_resolve_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__restrict__ levels, const uint8_t *__restrict__ index,
+                   uint8_t *__restrict__ out, int W, int H, int parts, bool vec) {
+    constexpr int P = K == 1 ? 16 : K == 2 ? 8 : K == 4 ? 4 : K == 6 ? 8 : K == 8 ? 2 : 16;     // 16 / gcd(K, 16)
+    constexpr int kBpp = FMT == kResolveRgba ? 4 : FMT == kResolveGray ? 1 : 3;
+    __shared__ uint2 s_tab[256];
+    const size_t frame = blockIdx.x / parts;
+    const int part = blockIdx.x % parts;
+    {
+        const uint32_t c = palettes[(size_t)(levels ? levels[frame] : 0u) * 256 + threadIdx.x];
+        const uint32_t R = c & 0xFF, G = (c >> 8) & 0xFF, B = (c >> 16) & 0xFF;
+        s_tab[threadIdx.x] = FMT == kResolveGray ? make_uint2((77 * R + 150 * G + 29 * B + 128) >> 8, 0u) : make_uint2(R | (B << 16), G);
+    }
+    __syncthreads();
+    const int OW = W / K, OH = H / K;
+    const size_t opix = (size_t)OW * OH;
+    const uint8_t *in = index + frame * (size_t)W * H;
+    uint8_t *o = out + frame * opix * kBpp;
+    if (vec) {
+        const int groups = OW / P;
+        const size_t n = (size_t)OH * groups, per = (n + parts - 1) / parts, lo = (size_t)part * per, hi = lo + per < n ? lo + per : n;
+        for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+            const int y = (int)(i / groups), x0 = (int)(i % groups) * P;
+            const uint8_t *src = in + (size_t)y * K * W + (size_t)x0 * K;
+            uint32_t acc0[P], acc1[P];
+#pragma unroll
+            for (int p = 0; p < P; p++) acc0[p] = acc1[p] = 0;
+#pragma unroll
+            for (int j = 0; j < K; j++) {
+#pragma unroll
+                for (int q = 0; q < P * K / 16; q++) {
+                    const uint4 v = __ldcs(reinterpret_cast<const uint4 *>(src + (size_t)j * W) + q);
+                    const uint32_t wds[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int b = 0; b < 16; b++) {
+                        const uint2 t = s_tab[(wds[b / 4] >> (8 * (b % 4))) & 0xFF];
+                        acc0[(16 * q + b) / K] += t.x;
+                        if (FMT != kResolveGray) acc1[(16 * q + b) / K] += t.y;
+                    }
+                }
+            }
+            resolve_emit<K, FMT, P>(o, opix, OW, y, x0, acc0, acc1);
+        }
+    } else {
+        const size_t n = opix, per = (n + parts - 1) / parts, lo = (size_t)part * per, hi = lo + per < n ? lo + per : n;
+        for (size_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+            const int y = (int)(i / OW), x = (int)(i % OW);
+            const uint8_t *src = in + (size_t)y * K * W + (size_t)x * K;
+            uint32_t acc0[1] = {0}, acc1[1] = {0};
+#pragma unroll
+            for (int j = 0; j < K; j++) {
+#pragma unroll
+                for (int b = 0; b < K; b++) {
+                    const uint2 t = s_tab[__ldcs(src + (size_t)j * W + b)];
+                    acc0[0] += t.x;
+                    if (FMT != kResolveGray) acc1[0] += t.y;
+                }
+            }
+            resolve_emit<K, FMT, 1>(o, opix, OW, y, x, acc0, acc1);
+        }
+    }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1334,6 +1497,45 @@ cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_
     const size_t parts = (npix + 32767) / 32768;
     if (n_frames * parts > 0x7FFFFFFFull) return cudaErrorInvalidValue;
     b2d_palette_levels_kernel<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_levels, d_index, d_rgba, npix, (int)parts);
+    return cudaGetLastError();
+}
+
+using ResolveFn = void (*)(const uint32_t *, const uint32_t *, const uint8_t *, uint8_t *, int, int, int, bool);
+
+template <int K>
+static ResolveFn resolve_kernel_of(int format) {
+    switch (format) {
+    case kResolveRgba: return b2d_resolve_kernel<K, kResolveRgba>;
+    case kResolveRgb: return b2d_resolve_kernel<K, kResolveRgb>;
+    case kResolvePlanar: return b2d_resolve_kernel<K, kResolvePlanar>;
+    case kResolveGray: return b2d_resolve_kernel<K, kResolveGray>;
+    default: return nullptr;
+    }
+}
+
+cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, void *d_out,
+                           size_t n_frames, int W, int H, int factor, int format, cudaStream_t stream) {
+    if (n_frames == 0) return cudaSuccess;
+    ResolveFn fn = nullptr;
+    switch (factor) {
+    case 1: fn = resolve_kernel_of<1>(format); break;
+    case 2: fn = resolve_kernel_of<2>(format); break;
+    case 3: fn = resolve_kernel_of<3>(format); break;
+    case 4: fn = resolve_kernel_of<4>(format); break;
+    case 5: fn = resolve_kernel_of<5>(format); break;
+    case 6: fn = resolve_kernel_of<6>(format); break;
+    case 7: fn = resolve_kernel_of<7>(format); break;
+    case 8: fn = resolve_kernel_of<8>(format); break;
+    }
+    if (!fn || W % factor || H % factor) return cudaErrorInvalidValue;
+    // output pixels per vector item: 16 / gcd(factor, 16), as in the kernel
+    const int P = factor == 2 || factor == 6 ? 8 : factor == 4 ? 4 : factor == 8 ? 2 : 16;
+    const bool vec = W % (P * factor) == 0 && (reinterpret_cast<uintptr_t>(d_index) & 15) == 0;
+    // ~32 KB of a frame's index bytes per CTA, as K3 per level
+    const size_t parts = ((size_t)W * H + 32767) / 32768;
+    if (n_frames * parts > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    fn<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_levels, d_index, static_cast<uint8_t *>(d_out), W, H,
+                                                         (int)parts, vec);
     return cudaGetLastError();
 }
 

@@ -144,5 +144,9 @@ cudaError_t launch_palette(const uint32_t *d_palette, const uint8_t *d_index, ui
 // ... with a palette per frame: frame f of the n_frames contiguous npix-pixel frames through palettes[levels[f] * 256 ..].
 cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, uint32_t *d_rgba,
                                   size_t n_frames, size_t npix, cudaStream_t stream);
+// Kernel 4: C17 resolve of the n_frames contiguous W x H index frames at d_index, frame f through palettes[levels[f] * 256 ..]
+// (d_levels NULL: level 0), box-filtered by `factor` (1..8, dividing W and H) into d_out in B2D_RESOLVE_* `format`.
+cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, void *d_out,
+                           size_t n_frames, int W, int H, int factor, int format, cudaStream_t stream);
 
 }  // namespace b2d
