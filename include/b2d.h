@@ -402,7 +402,7 @@ typedef struct b2d_sharded_stats {
 } b2d_sharded_stats;
 
 /* Called on the host once per chunk, right after the chunk's work has been ENQUEUED: d_frames holds `ranks` x
- * frames_per_rank finished index frames (rank-major; frame j of rank q is pose q*per + first_local_pose + j, with
+ * frames_per_rank finished index frames (resolved frames in the *_resolved calls; rank-major; frame j of rank q is pose q*per + first_local_pose + j, with
  * per = ceil(n_total/world)), valid for work enqueued on `cuda_stream`, which is ordered after the gather.  The
  * buffer is reused two chunks later, after everything the callback enqueued on that stream. */
 typedef void (*b2d_chunk_fn)(void *user, int chunk_index, size_t first_local_pose, size_t frames_per_rank,
@@ -438,6 +438,31 @@ int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pos
                                      const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves,
                                      size_t n_moves, size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user,
                                      b2d_sharded_stats *stats_out);
+
+/* The two sharded calls with the resolve (Kernel 4, b2d_resolve_device) applied on each rank before the exchange: for
+ * many agents or cameras, whose consumers want small observations, and for anti-aliased frames (render at factor x the
+ * size, resolve by factor).  The same job as the unresolved call: block split, padding, chunking, transports, modes and
+ * the walk of chunk k+1 under the raster of chunk k.  Each rank rasters a chunk into a rank-local index staging buffer
+ * (chunk x W x H bytes, owned by the communicator) and resolves it on the same stream straight into its slice of the
+ * exchange buffer, so the exchange carries resolved frames and every rank resolves only its own.
+ *   What the consumer gets: in a gathered chunk, frame j of rank q is byte-identical to b2d_resolve_device(factor, format)
+ *   applied to the index frame the unresolved call gathers at that position, through the palette of levels[pose] in the
+ *   level-set call and of level 0 in the plain call.
+ *   Callback: d_frames holds ranks x frames_per_rank such frames, rank-major and contiguous, each
+ *   b2d_resolve_frame_bytes(r, factor, format) bytes (frames are not aligned beyond that).
+ *   Refusals: factor and format are checked by b2d_resolve_device's rule (factor in 1..8 dividing the view's width and
+ *   height, a B2D_RESOLVE_* format) together with the unresolved call's whole-job checks, before any collective or launch,
+ *   so every rank returns the same B2D_ERR_INVALID_ARG.
+ *   Stats: bytes_received counts resolved bytes, (world-1) x per x frame bytes; render_ms covers raster plus resolve; the
+ *   struct is unchanged.  B2D_SHARD_GATHER_ONLY gathers resolved-size chunks without rendering, to time the exchange
+ *   alone at the size it carries.
+ * Each chunk costs the unresolved call's launches plus one resolve. */
+int b2d_render_sharded_resolved(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames,
+                                int factor, int format, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out);
+int b2d_render_sharded_levels_states_resolved(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
+                                              const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves,
+                                              size_t n_moves, size_t chunk_frames, int factor, int format, int mode,
+                                              b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out);
 
 /* One 32-bit checksum per frame on the device: sum_i (p[i] + 1) * (i * 0x9E3779B1 + 0x7F4A7C15) mod 2^32
  * (position sensitive, order independent).  Used to validate gathered frames without moving them to the host. */

@@ -598,29 +598,46 @@ class Renderer:
 
     # -- multi-GPU ------------------------------------------------------------------------------------
     def render_sharded(self, comm: "Comm", poses: np.ndarray, chunk_frames: int = 256, mode: int = _lib.SHARD_RENDER_GATHER,
-                       on_chunk=None) -> dict:
+                       on_chunk=None, resolve=None) -> dict:
         """b2d_render_sharded: collective over the communicator.  `poses` is the whole job's pose list (identical on
         every rank); on_chunk(chunk_index, first_local_pose, frames_per_rank, device_ptr, ranks, stream) is called on
-        the host after each chunk has been enqueued (work it enqueues on `stream` sees the gathered frames)."""
+        the host after each chunk has been enqueued (work it enqueues on `stream` sees the gathered frames).
+        resolve=(factor, fmt), fmt a key of RESOLVE_FORMATS: b2d_render_sharded_resolved, every rank resolves its own
+        frames before the exchange and the callback sees resolved frames of resolve_frame_bytes(factor, code) bytes each."""
         poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
         st = _lib.ShardedStats()
-
-        _check(_lib.load().b2d_render_sharded(self._h, comm._h, poses.ctypes.data, len(poses), int(chunk_frames), int(mode),
-                                              _chunk_fn(on_chunk), None, ctypes.byref(st)))
+        if resolve is None:
+            _check(_lib.load().b2d_render_sharded(self._h, comm._h, poses.ctypes.data, len(poses), int(chunk_frames), int(mode),
+                                                  _chunk_fn(on_chunk), None, ctypes.byref(st)))
+        else:
+            factor, fmt = resolve
+            _check(_lib.load().b2d_render_sharded_resolved(self._h, comm._h, poses.ctypes.data, len(poses), int(chunk_frames),
+                                                           int(factor), RESOLVE_FORMATS[fmt], int(mode), _chunk_fn(on_chunk), None,
+                                                           ctypes.byref(st)))
         return _sharded_stats(st)
 
     def render_sharded_levels_states(self, comm: "Comm", poses: np.ndarray, levels, tics, moves_per_pose=None,
-                                     chunk_frames: int = 256, mode: int = _lib.SHARD_RENDER_GATHER, on_chunk=None) -> dict:
+                                     chunk_frames: int = 256, mode: int = _lib.SHARD_RENDER_GATHER, on_chunk=None,
+                                     resolve=None) -> dict:
         """b2d_render_sharded_levels_states: render_sharded over the renderer's level set, pose i rendered from level
         levels[i] at level time tics[i] with the sector moves moves_per_pose[i] of that level (None = every pose at rest),
-        as render_levels_states renders it.  The whole job's lists, identical on every rank."""
+        as render_levels_states renders it.  The whole job's lists, identical on every rank.  resolve=(factor, fmt):
+        b2d_render_sharded_levels_states_resolved, as in render_sharded, each frame through its own level's palette."""
         poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
         n = len(poses)
         lv = _levels_array(levels, n)
         states, arr, nm = _frame_states(tics, moves_per_pose, n)
         st = _lib.ShardedStats()
-        _check(_lib.load().b2d_render_sharded_levels_states(self._h, comm._h, poses.ctypes.data, lv.ctypes.data, states, n, arr, nm,
-                                                            int(chunk_frames), int(mode), _chunk_fn(on_chunk), None, ctypes.byref(st)))
+        if resolve is None:
+            _check(_lib.load().b2d_render_sharded_levels_states(self._h, comm._h, poses.ctypes.data, lv.ctypes.data, states, n, arr,
+                                                                nm, int(chunk_frames), int(mode), _chunk_fn(on_chunk), None,
+                                                                ctypes.byref(st)))
+        else:
+            factor, fmt = resolve
+            _check(_lib.load().b2d_render_sharded_levels_states_resolved(self._h, comm._h, poses.ctypes.data, lv.ctypes.data, states,
+                                                                         n, arr, nm, int(chunk_frames), int(factor),
+                                                                         RESOLVE_FORMATS[fmt], int(mode), _chunk_fn(on_chunk),
+                                                                         None, ctypes.byref(st)))
         return _sharded_stats(st)
 
     def close(self):

@@ -56,7 +56,7 @@ EXPORTS = [
     "b2d_comm_unique_id", "b2d_comm_create", "b2d_comm_destroy", "b2d_comm_info", "b2d_render_sharded",
     "b2d_render_sharded_levels_states", "b2d_palette_lut_levels_device",
     "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_upload", "b2d_device_download",
-    "b2d_resolve_device", "b2d_resolve_frame_bytes",
+    "b2d_resolve_device", "b2d_resolve_frame_bytes", "b2d_render_sharded_resolved", "b2d_render_sharded_levels_states_resolved",
 ]
 
 COMM_ID_BYTES = 128
@@ -192,5 +192,8 @@ def load() -> ctypes.CDLL:
     L.b2d_frame_checksums_device.argtypes = [vp, cs, cs, vp, vp]
     L.b2d_resolve_device.argtypes = [vp, vp, vp, cs, ci, ci, vp, vp]
     L.b2d_resolve_frame_bytes.argtypes = [vp, ci, ci, ctypes.POINTER(cs)]
+    L.b2d_render_sharded_resolved.argtypes = [vp, vp, vp, cs, cs, ci, ci, ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
+    L.b2d_render_sharded_levels_states_resolved.argtypes = [vp, vp, vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove),
+                                                            cs, cs, ci, ci, ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
     _lib = L
     return L

@@ -4,7 +4,8 @@
 // replicated; the only exchange the path has is BASELINE.json's "all-gather of finished frames".  It is built so that it
 // costs no extra pass over HBM and hides under rendering:
 //   * a chunk of frames is rastered straight into this rank's slice of the all-gather receive buffer (the buffer IS the
-//     NCCL send buffer: in-place ncclAllGather, no staging copy);
+//     NCCL send buffer: in-place ncclAllGather, no staging copy); the resolved calls raster it into a rank-local staging
+//     buffer instead and resolve it (K4) from there into the slice, so the exchange carries the smaller resolved frames;
 //   * the gather of chunk k runs on its own stream while chunk k+1 is rendered into the other buffer; a third stream
 //     runs the consumer of gathered chunk k (the caller's callback: checksum, encoder, sink), so the gather stream goes
 //     back to back;
@@ -160,6 +161,12 @@ struct b2d_comm {
     DeviceBuf<int32_t> d_token;
     DeviceBuf<Pose> d_poses; PinnedBuf<Pose> h_poses;
     size_t poses_cap = 0;
+    // resolved calls (b2d_render_sharded*_resolved): the rank-local index frames of one chunk, which K4 reads, and the
+    // frame levels of the rank's block with their pinned staging, uploaded once per call next to the poses
+    DeviceBuf<uint8_t> d_stage;
+    size_t stage_bytes = 0;
+    DeviceBuf<uint32_t> d_levels; PinnedBuf<uint32_t> h_levels;
+    size_t levels_cap = 0;
 };
 
 namespace {
@@ -386,12 +393,22 @@ int check_sharded(const b2d_renderer *r, const b2d_comm *c, const b2d_pose *pose
     return B2D_OK;
 }
 
+// The resolve step of a resolved sharded call: K4 by `factor` into `format`, frame_bytes bytes per resolved frame;
+// block_levels (HOST, nullable = level 0 on every frame) holds the level of each entry of this rank's padded block.
+struct ShardResolve {
+    int factor = 1, format = B2D_RESOLVE_RGBA8;
+    size_t frame_bytes = 0;
+    const uint32_t *block_levels = nullptr;
+};
+
 // The chunk loop of the sharded calls, after their arguments have been checked (check_sharded and the caller's checks of
 // the whole job: a rank that refused its input here would leave its peers waiting in a collective).  `walk` enqueues the
 // BSP walk of local poses [first, first + n) of this rank's padded block, read from d_poses, as a background grid on
-// `stream` and returns its ticket.
+// `stream` and returns its ticket.  With `res` (nullable) each chunk is rastered into the comm's index staging and
+// resolved from there into this rank's slice of the exchange buffer, on the render stream: the raster of chunk k+1 follows
+// the resolve of chunk k there, so one staging buffer serves every chunk.  Without it, chunks are rastered into the slice.
 int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode, b2d_chunk_fn fn,
-                 void *user, b2d_sharded_stats *stats_out, const ChunkWalk &walk) {
+                 void *user, b2d_sharded_stats *stats_out, const ChunkWalk &walk, const ShardResolve *res = nullptr) {
     B2D_CU(cudaSetDevice(c->device));
     Nccl &n = nccl();
     const size_t world = (size_t)c->world, rank = (size_t)c->rank;
@@ -401,11 +418,24 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
     if (chunk > per) chunk = per;
     const size_t nchunks = (per + chunk - 1) / chunk;
     const size_t npix = (size_t)r->view.W * r->view.H;
+    const size_t frame_bytes = res ? res->frame_bytes : npix;            // of one frame in the exchange buffers
     const bool do_render = mode != B2D_SHARD_GATHER_ONLY, do_gather = mode != B2D_SHARD_RENDER_ONLY;
+    const bool do_resolve = res && do_render;
 
     int rc = do_render ? b2d::check_slots_free(r, nchunks) : B2D_OK;
-    if (rc == B2D_OK) rc = ensure_buffers(c, world * chunk * npix);
+    if (rc == B2D_OK) rc = ensure_buffers(c, world * chunk * frame_bytes);
     if (rc != B2D_OK) return rc;
+    if (do_resolve && c->stage_bytes < chunk * npix) {
+        c->stage_bytes = 0; c->d_stage.reset();
+        B2D_CU(allocate(c->d_stage, chunk * npix));
+        c->stage_bytes = chunk * npix;
+    }
+    if (do_resolve && res->block_levels && c->levels_cap < per) {
+        c->levels_cap = 0; c->d_levels.reset(); c->h_levels.reset();
+        B2D_CU(allocate(c->d_levels, per * sizeof(uint32_t)));
+        B2D_CU(allocate(c->h_levels, per * sizeof(uint32_t)));
+        c->levels_cap = per;
+    }
     // this rank's block of poses, padded by repeating the last pose of the list, on the device in one copy
     if (c->poses_cap < per) {
         c->poses_cap = 0; c->d_poses.reset(); c->h_poses.reset();
@@ -425,6 +455,12 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
     B2D_CU(event_create(poses_up));
     B2D_CU(cudaEventRecord(poses_up.get(), render_stream));
     B2D_CU(cudaStreamWaitEvent(walk_stream, poses_up.get(), 0));
+    const uint32_t *d_levels = nullptr;                                  // the resolve's frame levels; NULL: level 0
+    if (do_resolve && res->block_levels) {
+        std::memcpy(c->h_levels.get(), res->block_levels, per * sizeof(uint32_t));
+        B2D_CU(cudaMemcpyAsync(c->d_levels.get(), c->h_levels.get(), per * sizeof(uint32_t), cudaMemcpyHostToDevice, render_stream));
+        d_levels = c->d_levels.get();
+    }
     // the BSP walk of chunk k+1 runs as a background grid on its own stream under the raster of chunk k
     auto chunk_count = [&](size_t k) { const size_t f = k * chunk; return (per - f) < chunk ? (per - f) : chunk; };
     int64_t ticket = -1;
@@ -452,12 +488,17 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
         const int b = (int)(k & 1);
         const size_t first = k * chunk;
         const size_t cnt = (per - first) < chunk ? (per - first) : chunk;
-        uint8_t *slice = c->buf[b] + rank * cnt * npix;                  // in-place all-gather: rank-major slices of cnt frames
+        uint8_t *slice = c->buf[b] + rank * cnt * frame_bytes;           // in-place all-gather: rank-major slices of cnt frames
         if (k >= 2) B2D_CU(cudaStreamWaitEvent(render_stream, consumed[b].get(), 0));     // chunk k-2 has left this buffer
         B2D_CU(cudaEventRecord(rt[2 * k].get(), render_stream));
         if (do_render) {
-            result = b2d::raster_frames(r, ticket, slice, nullptr, render_stream);
+            result = b2d::raster_frames(r, ticket, do_resolve ? c->d_stage.get() : slice, nullptr, render_stream);
             if (result != B2D_OK) break;
+            if (do_resolve) {
+                B2D_CU(launch_resolve(r->d_palettes.get(), d_levels ? d_levels + first : nullptr, c->d_stage.get(), slice, cnt,
+                                      r->view.W, r->view.H, res->factor, res->format, render_stream));
+                r->launches += 1;
+            }
             if (k + 1 < nchunks) {
                 result = walk(c->d_poses.get() + (k + 1) * chunk, (k + 1) * chunk, (int)chunk_count(k + 1), walk_stream, &ticket);
                 if (result != B2D_OK) break;
@@ -469,10 +510,10 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
             B2D_CU(cudaStreamWaitEvent(gather_stream, rendered[b].get(), 0));
             B2D_CU(cudaEventRecord(gt[2 * k].get(), gather_stream));
             if (c->ce) {
-                result = ce_gather(c, b, rank * cnt * npix, cnt * npix);
+                result = ce_gather(c, b, rank * cnt * frame_bytes, cnt * frame_bytes);
                 if (result != B2D_OK) break;
             } else {
-                int nrc = n.AllGather(slice, c->buf[b], cnt * npix, kNcclUint8, c->comm, gather_stream);
+                int nrc = n.AllGather(slice, c->buf[b], cnt * frame_bytes, kNcclUint8, c->comm, gather_stream);
                 if (nrc != 0) { result = nccl_fail(nrc, "ncclAllGather"); break; }
             }
             B2D_CU(cudaEventRecord(gt[2 * k + 1].get(), gather_stream));
@@ -504,31 +545,32 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
         st.frames_gathered = do_gather ? (int64_t)(per * world) : 0;
         st.chunks = (int64_t)nchunks;
         st.chunk_frames = (int64_t)chunk;
-        st.bytes_received = do_gather ? (int64_t)((world - 1) * per * npix) : 0;
+        st.bytes_received = do_gather ? (int64_t)((world - 1) * per * frame_bytes) : 0;
         std::strncpy(st.registration, c->registration, sizeof st.registration - 1);
         *stats_out = st;
     }
     return result;
 }
 
-}  // namespace
-
-extern "C" {
-
-int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode,
-                       b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+// The two sharded calls, unresolved (res = NULL) or resolved (res: factor and format set).  A resolved call's factor and
+// format are checked by the rule of b2d_resolve_device with the other whole-job checks, before any collective or launch.
+int render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode,
+                   b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out, ShardResolve *res) {
     int rc = check_sharded(r, c, poses, mode);
+    if (rc == B2D_OK && res) rc = b2d_resolve_frame_bytes(r, res->factor, res->format, &res->frame_bytes);
     if (rc != B2D_OK || n_total == 0) return rc;
     return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
                         [r](const Pose *d_poses, size_t, int n, cudaStream_t stream, int64_t *ticket) {
                             return b2d::walk_frames(r, d_poses, n, stream, ticket, true);
-                        });
+                        }, res);
 }
 
-int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
-                                     const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves, size_t n_moves,
-                                     size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
+                                 const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves, size_t n_moves,
+                                 size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out,
+                                 ShardResolve *res) {
     int rc = check_sharded(r, c, poses, mode);
+    if (rc == B2D_OK && res) rc = b2d_resolve_frame_bytes(r, res->factor, res->format, &res->frame_bytes);
     if (rc != B2D_OK) return rc;
     // the whole list, identical on every rank, is checked and its compact states built before anything else: every rank
     // then refuses the same input, before any collective
@@ -546,11 +588,45 @@ int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pos
         block_levels[i] = levels[g];
         block_starts[i] = starts[g];
     }
+    if (res) res->block_levels = block_levels.data();
     return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
                         [&](const Pose *d_poses, size_t first, int n, cudaStream_t stream, int64_t *ticket) {
                             return b2d::walk_levels_states_frames(r, d_poses, block_levels.data() + first, fs.data(),
                                                                   block_starts.data() + first, n, stream, ticket, true);
-                        });
+                        }, res);
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode,
+                       b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    return render_sharded(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out, nullptr);
+}
+
+int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
+                                     const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves, size_t n_moves,
+                                     size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    return render_sharded_levels_states(r, c, poses, levels, states, n_total, moves, n_moves, chunk_frames, mode, fn, user,
+                                        stats_out, nullptr);
+}
+
+int b2d_render_sharded_resolved(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames,
+                                int factor, int format, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    ShardResolve res;
+    res.factor = factor; res.format = format;
+    return render_sharded(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out, &res);
+}
+
+int b2d_render_sharded_levels_states_resolved(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
+                                              const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves,
+                                              size_t n_moves, size_t chunk_frames, int factor, int format, int mode,
+                                              b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    ShardResolve res;
+    res.factor = factor; res.format = format;
+    return render_sharded_levels_states(r, c, poses, levels, states, n_total, moves, n_moves, chunk_frames, mode, fn, user,
+                                        stats_out, &res);
 }
 
 }  // extern "C"
