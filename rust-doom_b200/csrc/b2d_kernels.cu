@@ -835,8 +835,9 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
     }
 }
 
-// Warps per raster CTA: the four 32-column strips of one 128-column line group (for widths that are a multiple of 128).
-constexpr int kRasterWarps = 4;
+// Warps per raster CTA: the eight 32-column strips of two adjacent 128-column line groups (for widths that are a multiple
+// of 256; at 1920 columns every other CTA straddles two frames).
+constexpr int kRasterWarps = 8;
 
 template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels>
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
@@ -844,7 +845,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st,
                   const __grid_constant__ LevelTables lt) {
-    // per-frame levels: a palette per warp (the four warps of a CTA may draw frames of levels from different WADs)
+    // per-frame levels: a palette per warp (the warps of a CTA may draw frames of levels from different WADs)
     __shared__ uint32_t s_pal[kRgba ? (kLevels ? 256 * kRasterWarps : 256) : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
     __shared__ uint32_t s_chunks[kRasterWarps][kMasked ? kMaskedCapMax / kMaskedChunk : 1];
@@ -1312,13 +1313,14 @@ cudaError_t launch_walk_levels_states(const LevelTables &levels, const StateTabl
     return walk_go<true, true>(DeviceScene{}, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, states, levels);
 }
 
-// The raster's launch for every frame shape.  Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 4 warps
-// per CTA, so a CTA holds the four strips of a 128-column line group (at 1920 and 3840 columns; a CTA may straddle two
-// frames at other widths).  The four warps that write the sectors of the same 128-byte frame lines then start together on
-// one SM and finish those lines close together in time, so fewer partly written lines sit in L2.  That is worth 6 % of the
-// bench.py c2 step over one-warp CTAs; the slots of a CTA's finished warps idle until its slowest strip is done, and that
-// costs less.  The registers are left to the compiler (cap 128): 86 for the 1080p and 4K index-only kernels, i.e. 5 CTAs
-// = 20 warps per SM (DESIGN.md §6).
+// The raster's launch for every frame shape.  Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 8 warps
+// per CTA, so a CTA holds the eight strips of two adjacent 128-column line groups (a CTA may straddle two frames at 1920
+// columns and at other widths).  The warps that write the sectors of the same 128-byte frame lines, and of the next lines
+// of the same rows, then start together on one SM and finish those lines close together in time, so fewer partly written
+// lines sit in L2.  Against four-warp CTAs (one line group) that is worth 3.8 % of the bench.py c2 step and 5.9 % at 4K,
+// although residency falls from 20 to 16 warps per SM and the slots of a CTA's finished warps idle until its slowest strip
+// is done.  The registers are left to the compiler (cap 128): 86 for the 1080p and 4K index-only kernels, i.e. 2 CTAs
+// = 16 warps per SM (DESIGN.md §6).
 // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
 template <bool kStates, bool kLevels>
 static cudaError_t raster_go(const DeviceScene &sc, bool masked, const View &vw, const FrameConst *d_frames,
