@@ -223,7 +223,8 @@ int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_
  * max_batch (split into batches).  b2d_walk_device_states: like b2d_walk_device (1..max_batch poses); the ticket is
  * rastered by b2d_raster_device, and its table sets live in the ticket's worklist slot until then.  The device-resident
  * calls do not synchronise the device, but before a batch's compact states are written into the worklist slot's pinned
- * staging, the host waits for the copy that read that staging two batches earlier (normally finished long before). */
+ * staging (sized for a full batch when the renderer is created), the host waits for the copy that read that staging two
+ * batches earlier (normally finished long before). */
 typedef struct b2d_frame_state {
     uint32_t tics;                    /* level time */
     uint32_t first_move, n_moves;     /* moves[first_move .. first_move + n_moves) of the call's list; n_moves = 0: all at rest */
@@ -324,9 +325,9 @@ int b2d_renderer_set_level_sector_moves(b2d_renderer *r, int level, const b2d_se
  *
  * b2d_render_levels_states: host poses and frames as b2d_render; b2d_render_device_levels_states: like b2d_render_device,
  * n may exceed max_batch (split into batches).  b2d_walk_device_levels_states: like b2d_walk_device (1..max_batch poses);
- * the ticket is rastered by b2d_raster_device.  Before a batch is written into the worklist slot's pinned staging, the host
- * waits for the copy that read that staging two batches earlier; a slot's first such batch first grows the slot's staging
- * and its device copy, after the host has waited for the slot's earlier copy and raster. */
+ * the ticket is rastered by b2d_raster_device.  Before a batch is written into the worklist slot's pinned staging (sized
+ * for a full batch when the renderer is created), the host waits for the copy that read that staging two batches
+ * earlier. */
 int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, const b2d_frame_state *states,
                              size_t n, const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb);
 int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,

@@ -160,393 +160,70 @@ int ensure_states(b2d_renderer *r) {
     return B2D_OK;
 }
 
-// The sections of a batch with per-frame states and levels in WorkSlot::states (and h_states), copied to the device in
-// one piece: what the expansion, the walk and the raster of the batch read.  Byte offsets, each section 16-byte aligned.
-struct LevelsStatesBatch {
-    size_t scenes = 0;         // DeviceScene of every level (its own blob tables; each frame's TableSet replaces them)
-    size_t srcs, sets, descs;  // StateSrc of every level | TableSet of every table set, then of every level | StateSet per set
-    size_t frame_level, frame_set, states, end;  // per frame: level, TableSet index | the sets' compact states
-    LevelsStatesBatch(size_t nlev, size_t nsets, size_t n, size_t state_words) {
+// The sections of a batch in its worklist slot's staging (WorkSlot::stage, h_stage), copied to the device in one piece:
+// what the batch's expansions, walk and raster read.  Byte offsets, each section 16-byte aligned; a section the batch
+// does not use is empty.
+struct StageLayout {
+    size_t scenes = 0;         // with per-frame levels: the DeviceScene of every level
+    size_t srcs, sets, descs;  // StateSrc of every level | TableSet of every set to expand, then, with per-frame states, of
+                               // every level's blob tables | StateSet of every set to expand
+    size_t frame_level, frame_set, states, end;  // per frame: level | TableSet index (per-frame states) | the sets' states
+    StageLayout(size_t nlev, size_t nsets, size_t n, size_t state_words, bool per_frame, bool per_level) {
         auto up = [](size_t x) { return (x + 15) & ~(size_t)15; };
-        srcs = up(nlev * sizeof(DeviceScene));
+        srcs = up((per_level ? nlev : 0) * sizeof(DeviceScene));
         sets = up(srcs + nlev * sizeof(StateSrc));
-        descs = up(sets + (nsets + nlev) * sizeof(TableSet));
+        descs = up(sets + (nsets + (per_frame ? nlev : 0)) * sizeof(TableSet));
         frame_level = up(descs + nsets * sizeof(StateSet));
-        frame_set = up(frame_level + 4 * n);
-        states = up(frame_set + 4 * n);
+        frame_set = up(frame_level + (per_level ? 4 * n : 0));
+        states = up(frame_set + (per_frame ? 4 * n : 0));
         end = states + 4 * state_words;
     }
 };
 
-// Per-frame states and levels: worklist slot `s`'s `states` / `h_states` large enough for a full batch of LevelsStatesBatch
-// sections (grown, once, by the slot's first such batch, after the slot's earlier work that read them), and its event.
-int ensure_levels_states(b2d_renderer *r, WorkSlot &s) {
-    size_t words = 0;
-    for (const LevelRes &lv : r->lv) words = std::max(words, (size_t)lv.layout.words);
-    const size_t bytes = LevelsStatesBatch(r->lv.size(), (size_t)r->max_batch, (size_t)r->max_batch, (size_t)r->max_batch * words).end;
-    if (s.states_bytes >= bytes) return B2D_OK;
-    if (s.states_copied) CU(cudaEventSynchronize(s.states_copied.get()));
-    if (s.raster_done) CU(cudaEventSynchronize(s.raster_done.get()));      // the slot is rastered: nothing else reads them
-    DeviceBuf<uint32_t> d;
-    PinnedBuf<uint32_t> h;
-    Event ev;
-    CU(allocate(d, bytes));
-    CU(allocate(h, bytes));
-    if (!s.states_copied) CU(event_create(ev));
-    s.states = std::move(d);
-    s.h_states = std::move(h);
-    if (ev) s.states_copied = std::move(ev);
-    s.states_bytes = bytes;
-    return B2D_OK;
+// the five tables of the table set at `set`, laid out as `t` says
+TableSet table_set(const uint8_t *set, const StateTables &t) {
+    return TableSet{reinterpret_cast<const TexRec *>(set), reinterpret_cast<const SectorRec *>(set + t.off_sectors),
+                    reinterpret_cast<const SegRec *>(set + t.off_segs), reinterpret_cast<const SpriteRec *>(set + t.off_sprites),
+                    reinterpret_cast<const MidRec *>(set + t.off_mids)};
 }
 
-// Per-frame levels: both worklist slots' scene arrays, level staging and events, allocated together by the first such call.
-int ensure_levels(b2d_renderer *r) {
-    if (r->slot[0].levels) return B2D_OK;
-    const size_t bytes = r->levels_frames_off + 4 * (size_t)r->max_batch;
-    DeviceBuf<uint8_t> d[2];
-    PinnedBuf<uint8_t> h[2];
-    Event ev[2];
-    for (int i = 0; i < 2; i++) {
-        CU(allocate(d[i], bytes));
-        CU(allocate(h[i], bytes));
-        CU(event_create(ev[i]));
-    }
-    for (int i = 0; i < 2; i++) {
-        r->slot[i].levels = std::move(d[i]);
-        r->slot[i].h_levels = std::move(h[i]);
-        r->slot[i].levels_copied = std::move(ev[i]);
-    }
-    return B2D_OK;
-}
-
-// the arena view of worklist slot `slot` (after ensure_states)
-StateTables slot_tables(const b2d_renderer *r, int slot) {
-    StateTables t = r->lv[0].state_tables;
-    t.base = r->slot[slot].arena.get();
-    t.frame_slot = r->slot[slot].states.get() + (size_t)r->max_batch * r->lv[0].layout.words;
-    return t;
-}
+// records of one table set of a level (the threads of its expansion)
+size_t set_records(const LevelRes &lv) { return (size_t)lv.src.ntex + lv.src.nsectors + lv.src.nsegs + lv.src.nsprites + lv.src.nmids; }
 
 // a level's scene as the kernels of worklist slot `slot` read it: on a timed scene, the five state-dependent tables are the
 // level's table set of that slot
 DeviceScene slot_scene(const LevelRes &lv, int slot) {
     DeviceScene d = lv.ds;
-    const uint8_t *set = lv.slot[slot].tables.get();
-    if (!set) return d;
-    const StateTables &t = lv.state_tables;
-    d.tex = reinterpret_cast<const TexRec *>(set);
-    d.sectors = reinterpret_cast<const SectorRec *>(set + t.off_sectors);
-    d.segs = reinterpret_cast<const SegRec *>(set + t.off_segs);
-    d.sprites = reinterpret_cast<const SpriteRec *>(set + t.off_sprites);
-    d.mids = reinterpret_cast<const MidRec *>(set + t.off_mids);
+    if (const uint8_t *set = lv.slot[slot].tables.get()) {
+        const TableSet t = table_set(set, lv.state_tables);
+        d.tex = t.tex; d.sectors = t.sectors; d.segs = t.segs; d.sprites = t.sprites; d.mids = t.mids;
+    }
     return d;
 }
 
-// BSP walk of a batch into the next worklist slot, on `stream`.  The slot's previous raster (if any, on whatever
-// stream) is awaited through an event, so a caller may run walks and rasters on two streams and have the walk of
-// batch k+1 overlap the raster of batch k.  `frame_states` (nullable): one compact state per frame; the batch's distinct
-// states are expanded into the slot's arena on `stream` first (frames with equal states share one table set).  A plain
-// batch on a timed scene reads the slot's own table set, which is re-expanded on `stream` when the renderer's state
-// differs from the one the set holds: the walk and the raster of a ticket read one state whatever is set in between.
-int walk_into_slot(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background = false,
-                   const uint32_t *frame_states = nullptr) {
-    const int slot = (int)(r->next_ticket & 1);
-    WorkSlot &s = r->slot[slot];
-    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
-    int rc = frame_states ? ensure_states(r) : B2D_OK;
-    if (rc == B2D_OK) rc = ensure_slot(r, s);
-    if (rc != B2D_OK) return rc;
-    LevelRes &lv = r->lv[0];
-    const bool restate = !frame_states && lv.slot[slot].tables && lv.slot[slot].state != lv.state;
-    const size_t words = lv.layout.words;
-    int nstates = 0;
-    if (frame_states || restate) {
-        CU(cudaEventSynchronize(s.states_copied.get()));     // the copy issued two batches ago has read the staging
-        uint32_t *hs = s.h_states.get(), *hslot = hs + (size_t)r->max_batch * words;
-        if (restate) {
-            std::memcpy(hs, lv.state.data(), 4 * words);
-            nstates = 1;
-        } else {
-            // distinct states -> slots 0, 1, ... in order of first appearance, anywhere in the batch
-            std::unordered_map<std::string, uint32_t> seen;
-            seen.reserve((size_t)n);
-            for (int f = 0; f < n; f++) {
-                const uint32_t *w = frame_states + (size_t)f * words;
-                auto it = seen.emplace(std::string(reinterpret_cast<const char *>(w), 4 * words), (uint32_t)nstates);
-                if (it.second) std::memcpy(hs + (size_t)nstates++ * words, w, 4 * words);
-                hslot[f] = it.first->second;
-            }
-        }
-    }
-    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
-    const StateTables stt = frame_states ? slot_tables(r, slot) : StateTables{};
-    if (nstates) {
-        uint32_t *hs = s.h_states.get();
-        CU(cudaMemcpyAsync(s.states.get(), hs, 4 * words * (size_t)nstates, cudaMemcpyHostToDevice, stream));
-        if (frame_states)
-            CU(cudaMemcpyAsync(const_cast<uint32_t *>(stt.frame_slot), hs + (size_t)r->max_batch * words, 4 * (size_t)n,
-                               cudaMemcpyHostToDevice, stream));
-        CU(cudaEventRecord(s.states_copied.get(), stream));
-        uint8_t *sets = (frame_states ? s.arena : lv.slot[slot].tables).get();
-        CU(launch_state_tables(lv.src, s.states.get(), (uint32_t)words, nstates, sets, lv.state_tables, stream));
-        r->launches += 1;
-        if (restate) lv.slot[slot].state = lv.state;
-    }
+// `launch` on `stream`, between two timing events while the renderer profiles (b2d_profile_read): kind 0 = walk, 1 = raster
+template <typename Launch>
+int profiled(b2d_renderer *r, cudaStream_t stream, int kind, Launch launch) {
     Event ev[2];
     if (r->profiling) {
         for (auto &e : ev) CU(event_create(e, cudaEventDefault));
         CU(cudaEventRecord(ev[0].get(), stream));
     }
-    CU(launch_walk(slot_scene(lv, slot), r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background,
-                   frame_states ? &stt : nullptr));
+    CU(launch());
     if (r->profiling) {
         CU(cudaEventRecord(ev[1].get(), stream));
         for (auto &e : ev) r->prof_events.push_back(std::move(e));
-        r->prof_kinds.push_back(0);
+        r->prof_kinds.push_back(kind);
     }
-    CU(cudaEventRecord(s.walk_done.get(), stream));
-    s.n = n;
-    s.per_frame = frame_states != nullptr;
-    s.per_level = false;
-    s.sets = frame_states ? nstates : 0;
-    s.ticket = r->next_ticket;
-    s.rastered = false;
-    r->last_slot = slot;
-    r->launches += 1;
-    *ticket_out = r->next_ticket++;
     return B2D_OK;
 }
 
-// BSP walk of a batch with per-frame levels (levels[i] < r->lv.size(), checked by the caller) into the next worklist slot,
-// as walk_into_slot.  The frame levels, the DeviceScene of every level as the slot reads it and the compact states of the
-// timed levels the batch uses whose table set of the slot is stale go to the device in one copy; each stale set is then
-// re-expanded (one launch per such level) before the walk.
-int walk_levels_into_slot(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, int n, cudaStream_t stream,
-                          int64_t *ticket_out, bool background) {
-    const int slot = (int)(r->next_ticket & 1);
-    WorkSlot &s = r->slot[slot];
-    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
-    int rc = ensure_levels(r);
-    if (rc == B2D_OK) rc = ensure_slot(r, s);
-    if (rc != B2D_OK) return rc;
-    CU(cudaEventSynchronize(s.levels_copied.get()));     // the copy issued two batches ago has read the staging
-    uint8_t *h = s.h_levels.get();
-    DeviceScene *scenes = reinterpret_cast<DeviceScene *>(h);
-    uint32_t *frame_level = reinterpret_cast<uint32_t *>(h + r->levels_frames_off);
-    const size_t nlev = r->lv.size();
-    std::vector<char> used(nlev, 0);
-    for (int f = 0; f < n; f++) {
-        frame_level[f] = levels[f];
-        used[levels[f]] = 1;
-    }
-    std::vector<size_t> stale;
-    for (size_t k = 0; k < nlev; k++) {
-        LevelRes &lv = r->lv[k];
-        scenes[k] = slot_scene(lv, slot);
-        if (used[k] && lv.slot[slot].tables && lv.slot[slot].state != lv.state) {
-            std::memcpy(h + lv.stage_off, lv.state.data(), 4 * lv.layout.words);
-            stale.push_back(k);
-        }
-    }
-    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
-    CU(cudaMemcpyAsync(s.levels.get(), h, r->levels_frames_off + 4 * (size_t)n, cudaMemcpyHostToDevice, stream));
-    CU(cudaEventRecord(s.levels_copied.get(), stream));
-    for (size_t k : stale) {
-        LevelRes &lv = r->lv[k];
-        CU(launch_state_tables(lv.src, reinterpret_cast<const uint32_t *>(s.levels.get() + lv.stage_off), (uint32_t)lv.layout.words,
-                               1, lv.slot[slot].tables.get(), lv.state_tables, stream));
-        r->launches += 1;
-        lv.slot[slot].state = lv.state;
-    }
-    Event ev[2];
-    if (r->profiling) {
-        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
-        CU(cudaEventRecord(ev[0].get(), stream));
-    }
-    const LevelTables lt{reinterpret_cast<const DeviceScene *>(s.levels.get()),
-                         reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off), nullptr};
-    CU(launch_walk_levels(lt, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background));
-    if (r->profiling) {
-        CU(cudaEventRecord(ev[1].get(), stream));
-        for (auto &e : ev) r->prof_events.push_back(std::move(e));
-        r->prof_kinds.push_back(0);
-    }
-    CU(cudaEventRecord(s.walk_done.get(), stream));
-    s.n = n;
-    s.per_frame = false;
-    s.per_level = true;
-    s.sets = 0;
-    s.ticket = r->next_ticket;
-    s.rastered = false;
-    r->last_slot = slot;
-    r->launches += 1;
-    *ticket_out = r->next_ticket++;
-    return B2D_OK;
-}
-
-// the LevelTables / StateTables of worklist slot `s`'s batch with per-frame states and levels (`b`: its sections)
-LevelTables levels_states_tables(const WorkSlot &s, const LevelsStatesBatch &b, StateTables &st) {
-    const uint8_t *d = reinterpret_cast<const uint8_t *>(s.states.get());
-    st = StateTables{};
-    st.frame_slot = reinterpret_cast<const uint32_t *>(d + b.frame_set);
-    return LevelTables{reinterpret_cast<const DeviceScene *>(d + b.scenes), reinterpret_cast<const uint32_t *>(d + b.frame_level),
-                       reinterpret_cast<const TableSet *>(d + b.sets)};
-}
-
-// BSP walk of a batch with per-frame states and levels into the next worklist slot, as walk_into_slot.  `levels` and
-// `frame_states` / `starts` as check_levels and build_states left them: frame f's compact state (of its level's layout) is
-// frame_states[starts[f] ..], none on a level without time-dependent content or dynamic sectors.  Frames whose (level,
-// compact state) are equal share a table set; sets are numbered in order of first appearance and packed into the slot's
-// arena, each at its level's slot_bytes.  The batch's LevelsStatesBatch sections go to the device in one copy, then one
-// expansion launch fills every set (none if the batch has no set) and the walk runs.
-int walk_levels_states_into_slot(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *frame_states,
-                                 const size_t *starts, int n, cudaStream_t stream, int64_t *ticket_out, bool background) {
-    const int slot = (int)(r->next_ticket & 1);
-    WorkSlot &s = r->slot[slot];
-    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
-    int rc = ensure_states(r);
-    if (rc == B2D_OK) rc = ensure_slot(r, s);
-    if (rc == B2D_OK) rc = ensure_levels_states(r, s);
-    if (rc != B2D_OK) return rc;
-    const size_t nlev = r->lv.size();
-    // table sets: (level, compact state) -> index, in order of first appearance
-    std::vector<uint32_t> frame_set((size_t)n), first_frame;
-    std::unordered_map<std::string, uint32_t> seen;
-    seen.reserve((size_t)n);
-    size_t state_words = 0;
-    for (int f = 0; f < n; f++) {
-        const LevelRes &lv = r->lv[levels[f]];
-        if (lv.h_blob.empty()) continue;          // no set: the frame reads its level's blob tables
-        std::string key(reinterpret_cast<const char *>(&levels[f]), 4);
-        key.append(reinterpret_cast<const char *>(frame_states + starts[f]), 4 * lv.layout.words);
-        auto it = seen.emplace(std::move(key), (uint32_t)first_frame.size());
-        if (it.second) {
-            first_frame.push_back((uint32_t)f);
-            state_words += lv.layout.words;
-        }
-        frame_set[(size_t)f] = it.first->second;
-    }
-    const size_t nsets = first_frame.size();
-    const LevelsStatesBatch b(nlev, nsets, (size_t)n, state_words);
-    CU(cudaEventSynchronize(s.states_copied.get()));     // the copy issued two batches ago has read the staging
-    uint8_t *h = reinterpret_cast<uint8_t *>(s.h_states.get());
-    DeviceScene *scenes = reinterpret_cast<DeviceScene *>(h + b.scenes);
-    StateSrc *srcs = reinterpret_cast<StateSrc *>(h + b.srcs);
-    TableSet *sets = reinterpret_cast<TableSet *>(h + b.sets);
-    StateSet *descs = reinterpret_cast<StateSet *>(h + b.descs);
-    uint32_t *h_level = reinterpret_cast<uint32_t *>(h + b.frame_level), *h_set = reinterpret_cast<uint32_t *>(h + b.frame_set);
-    uint32_t *h_words = reinterpret_cast<uint32_t *>(h + b.states);
-    for (size_t k = 0; k < nlev; k++) {
-        const LevelRes &lv = r->lv[k];
-        scenes[k] = lv.ds;
-        srcs[k] = lv.src;
-        sets[nsets + k] = TableSet{lv.ds.tex, lv.ds.sectors, lv.ds.segs, lv.ds.sprites, lv.ds.mids};
-    }
-    s.set_level.resize(nsets);
-    s.set_off.resize(nsets);
-    const uint8_t *arena = s.arena.get();
-    size_t aoff = 0, woff = 0, records = 0;
-    for (size_t k = 0; k < nsets; k++) {
-        const int f = (int)first_frame[k];
-        const uint32_t level = levels[f];
-        const LevelRes &lv = r->lv[level];
-        const StateTables &t = lv.state_tables;
-        const uint8_t *set = arena + aoff;
-        sets[k] = TableSet{reinterpret_cast<const TexRec *>(set), reinterpret_cast<const SectorRec *>(set + t.off_sectors),
-                           reinterpret_cast<const SegRec *>(set + t.off_segs), reinterpret_cast<const SpriteRec *>(set + t.off_sprites),
-                           reinterpret_cast<const MidRec *>(set + t.off_mids)};
-        descs[k] = StateSet{level, (uint32_t)woff, (uint32_t)records, 0};
-        std::memcpy(h_words + woff, frame_states + starts[f], 4 * lv.layout.words);
-        s.set_level[k] = level;
-        s.set_off[k] = aoff;
-        aoff += t.slot_bytes;
-        woff += lv.layout.words;
-        records += (size_t)lv.src.ntex + lv.src.nsectors + lv.src.nsegs + lv.src.nsprites + lv.src.nmids;
-    }
-    if (records > 0x7FFFFFFFu) return fail(B2D_ERR_INVALID_ARG, "the batch's table sets hold more than 2^31 records");
-    for (int f = 0; f < n; f++) {
-        h_level[f] = levels[f];
-        h_set[f] = r->lv[levels[f]].h_blob.empty() ? (uint32_t)(nsets + levels[f]) : frame_set[(size_t)f];
-    }
-    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
-    CU(cudaMemcpyAsync(s.states.get(), h, b.end, cudaMemcpyHostToDevice, stream));
-    CU(cudaEventRecord(s.states_copied.get(), stream));
-    StateTables st;
-    const LevelTables lt = levels_states_tables(s, b, st);
-    if (nsets) {
-        const uint8_t *d = reinterpret_cast<const uint8_t *>(s.states.get());
-        CU(launch_state_sets(reinterpret_cast<const StateSrc *>(d + b.srcs), reinterpret_cast<const StateSet *>(d + b.descs), lt.sets,
-                             reinterpret_cast<const uint32_t *>(d + b.states), (int)nsets, (uint32_t)records, stream));
-        r->launches += 1;
-    }
-    Event ev[2];
-    if (r->profiling) {
-        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
-        CU(cudaEventRecord(ev[0].get(), stream));
-    }
-    CU(launch_walk_levels_states(lt, st, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream,
-                                 background));
-    if (r->profiling) {
-        CU(cudaEventRecord(ev[1].get(), stream));
-        for (auto &e : ev) r->prof_events.push_back(std::move(e));
-        r->prof_kinds.push_back(0);
-    }
-    CU(cudaEventRecord(s.walk_done.get(), stream));
-    s.n = n;
-    s.per_frame = true;
-    s.per_level = true;
-    s.sets = (int)nsets;
-    s.ticket = r->next_ticket;
-    s.rastered = false;
-    r->last_slot = slot;
-    r->launches += 1;
-    *ticket_out = r->next_ticket++;
-    return B2D_OK;
-}
-
-int raster_from_slot(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
-    const int slot = (int)(ticket & 1);
-    WorkSlot &s = r->slot[slot];
-    if (ticket < 0 || s.ticket != ticket || s.rastered) return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
-    CU(cudaStreamWaitEvent(stream, s.walk_done.get(), 0));
-    if (r->d_masked) {
-        // one arena of deferred masked entries per renderer: rasters that use it run one after the other (each fills the
-        // machine on its own, so nothing is lost), whatever streams they were enqueued on
-        CU(cudaStreamWaitEvent(stream, r->masked_done.get(), 0));
-        CU(cudaMemsetAsync(r->d_masked_counter.get(), 0, sizeof(uint32_t), stream));
-    }
-    Event ev[2];
-    if (r->profiling) {
-        for (auto &e : ev) CU(event_create(e, cudaEventDefault));
-        CU(cudaEventRecord(ev[0].get(), stream));
-    }
-    if (s.per_level && s.per_frame) {
-        StateTables st;
-        const LevelTables lt = levels_states_tables(s, LevelsStatesBatch(r->lv.size(), (size_t)s.sets, (size_t)s.n, 0), st);
-        CU(launch_raster_levels_states(lt, st, r->d_masked != nullptr, r->view, s.frames.get(), s.work.get(), r->stride, s.n,
-                                       d_index, d_rgba, stream));
-    } else if (s.per_level) {
-        const LevelTables lt{reinterpret_cast<const DeviceScene *>(s.levels.get()),
-                             reinterpret_cast<const uint32_t *>(s.levels.get() + r->levels_frames_off), nullptr};
-        CU(launch_raster_levels(lt, r->d_masked != nullptr, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index,
-                                d_rgba, stream));
-    } else {
-        const StateTables stt = s.per_frame ? slot_tables(r, slot) : StateTables{};
-        CU(launch_raster(slot_scene(r->lv[0], slot), r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba,
-                         stream, s.per_frame ? &stt : nullptr));
-    }
-    if (r->profiling) {
-        CU(cudaEventRecord(ev[1].get(), stream));
-        for (auto &e : ev) r->prof_events.push_back(std::move(e));
-        r->prof_kinds.push_back(1);
-    }
-    CU(cudaEventRecord(s.raster_done.get(), stream));
-    if (r->d_masked) CU(cudaEventRecord(r->masked_done.get(), stream));
-    s.rastered = true;
-    r->launches += 1;
-    return B2D_OK;
-}
+// A table set a batch expands: level `level` at the compact state `state` (host) into the tables at `tables`.
+struct Expansion {
+    uint32_t level;
+    const uint32_t *state;
+    uint8_t *tables;
+};
 
 // the state-dependent tables (level time `tics`, sector offsets), laid out [tex | sectors | segs | sprites | mids]
 size_t state_table_bytes(const uint8_t *blob) {
@@ -572,71 +249,62 @@ void state_at(const LevelRes &lv, uint32_t tics, uint32_t *out) {
     std::copy(lv.state.begin() + 1, lv.state.begin() + 2 + 2 * (ptrdiff_t)lv.layout.dyn_sectors.size(), out + 1);
 }
 
-// The compact state of every frame of a b2d_render_states-style call into `out`, checking everything first: nothing is
-// enqueued for a call with an invalid frame.  Frame i is on level levels[i] (levels == nullptr: every frame on level 0;
-// the caller has checked the levels) and its state takes that level's layout.words words, from out[starts[i]] (starts:
-// nullable); a frame on a level without time-dependent content or dynamic sectors has none, and renders with its level's
-// tables.  With every frame on level 0, `out` is n * layout.words words, or empty for such a scene.
-int build_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n, const b2d_sector_move *moves,
-                 size_t n_moves, std::vector<uint32_t> &out, std::vector<size_t> *starts = nullptr) {
-    out.clear();
-    if (!states || (n_moves && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    for (size_t i = 0; i < n; i++)
-        if (states[i].first_move > n_moves || states[i].n_moves > n_moves - states[i].first_move)
-            return fail(B2D_ERR_INVALID_ARG, "a frame's move range runs past the end of the move list");
-    size_t total = 0;
-    if (starts) starts->assign(n, 0);
-    for (size_t i = 0; i < n; i++) {
-        const LevelRes &lv = r->lv[levels ? levels[i] : 0];
-        if (lv.h_blob.empty()) {
-            if (states[i].n_moves) return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
-            continue;
-        }
-        if (starts) (*starts)[i] = total;
-        total += lv.layout.words;
-    }
-    out.resize(total);
-    std::vector<int32_t> fo, co;
-    for (size_t i = 0, at = 0; i < n; i++) {
-        const LevelRes &lv = r->lv[levels ? levels[i] : 0];
-        if (lv.h_blob.empty()) continue;
-        bool moved = false;
-        if (states[i].n_moves) {
-            if (const char *why = expand_moves(lv.h_blob.data(), reinterpret_cast<const SectorMove *>(moves) + states[i].first_move,
-                                               states[i].n_moves, fo, co)) {
-                out.clear();
-                return fail(B2D_ERR_INVALID_ARG, why);
-            }
-            for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
-        }
-        compact_state(lv.h_blob.data(), lv.layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
-                      out.data() + at);
-        at += lv.layout.words;
-    }
-    return B2D_OK;
-}
-
-// b2d_render_timed: tics[i] with the renderer's current moves
-void timed_states(const b2d_renderer *r, const uint32_t *tics, size_t n, std::vector<uint32_t> &out) {
-    out.clear();
-    const LevelRes &lv = r->lv[0];
-    if (lv.h_blob.empty()) return;
-    const size_t words = lv.layout.words;
-    out.resize(n * words);
-    for (size_t i = 0; i < n; i++) state_at(lv, tics[i], out.data() + i * words);
-}
-
 }  // namespace
 
-int b2d::walk_frames(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background) {
-    return walk_into_slot(r, d_poses, n, stream, ticket_out, background);
+int b2d::build_states(const b2d_renderer *r, const b2d_frame_state *states, const uint32_t *tics, size_t n,
+                      const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts,
+                      Frames &out) {
+    if (!tics) {
+        if (!states || (n_moves && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
+        for (size_t i = 0; i < n; i++)
+            if (states[i].first_move > n_moves || states[i].n_moves > n_moves - states[i].first_move)
+                return fail(B2D_ERR_INVALID_ARG, "a frame's move range runs past the end of the move list");
+    }
+    return guarded([&] {
+        const uint32_t *levels = out.levels;
+        size_t total = 0;
+        starts.assign(n, 0);
+        for (size_t i = 0; i < n; i++) {
+            const LevelRes &lv = r->lv[levels ? levels[i] : 0];
+            if (lv.h_blob.empty()) {
+                if (!tics && states[i].n_moves) return fail(B2D_ERR_INVALID_ARG, "the scene declares no dynamic sectors");
+                continue;
+            }
+            starts[i] = total;
+            total += lv.layout.words;
+        }
+        fs.assign(total, 0);
+        std::vector<int32_t> fo, co;
+        for (size_t i = 0; i < n; i++) {
+            const LevelRes &lv = r->lv[levels ? levels[i] : 0];
+            if (lv.h_blob.empty()) continue;
+            if (tics) {
+                state_at(lv, tics[i], fs.data() + starts[i]);
+                continue;
+            }
+            bool moved = false;
+            if (states[i].n_moves) {
+                if (const char *why = expand_moves(lv.h_blob.data(), reinterpret_cast<const SectorMove *>(moves) + states[i].first_move,
+                                                   states[i].n_moves, fo, co))
+                    return fail(B2D_ERR_INVALID_ARG, why);
+                for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
+            }
+            compact_state(lv.h_blob.data(), lv.layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
+                          fs.data() + starts[i]);
+        }
+        out.fs = fs.data();
+        out.starts = !levels && r->lv[0].h_blob.empty() ? nullptr : starts.data();
+        return B2D_OK;
+    });
 }
-int b2d::raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
-    return raster_from_slot(r, ticket, d_index, d_rgba, stream);
-}
-int b2d::walk_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *fs,
-                                   const size_t *starts, int n, cudaStream_t stream, int64_t *ticket_out, bool background) {
-    return walk_levels_states_into_slot(r, d_poses, levels, fs, starts, n, stream, ticket_out, background);
+
+int b2d::check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
+    if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
+    if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
+        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
+    for (size_t i = 0; i < n; i++)
+        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    return B2D_OK;
 }
 
 int b2d::check_slots_free(const b2d_renderer *r, size_t batches) {
@@ -646,36 +314,186 @@ int b2d::check_slots_free(const b2d_renderer *r, size_t batches) {
     return B2D_OK;
 }
 
-// batches of at most max_batch frames in n frames
-static size_t batch_count(const b2d_renderer *r, size_t n) { return (n + (size_t)r->max_batch - 1) / (size_t)r->max_batch; }
-
-// walk -> raster on the caller's stream
-int b2d::enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba,
-                        cudaStream_t stream, const uint32_t *frame_states) {
-    int64_t ticket = -1;
-    int rc = walk_into_slot(r, d_poses, n, stream, &ticket, false, frame_states);
+// BSP walk of a batch into the next worklist slot, on `stream`.  The slot's previous raster (if any, on whatever stream) is
+// awaited through an event, so a caller may run walks and rasters on two streams and have the walk of batch k+1 overlap the
+// raster of batch k.  The batch's table sets are expanded on `stream` first.  With per-frame states: frames whose (level,
+// compact state) are equal share a set; sets are numbered in order of first appearance and packed into the slot's arena,
+// each at its level's slot_bytes (level 0's sets at level 0's stride, as the per-frame-state kernels without per-frame
+// levels read them), and one launch expands them all.  Without: the slot's own table set of each timed level the batch
+// uses is re-expanded, one launch per level, when the level's state differs from the one the set holds, so the walk and
+// the raster of a ticket read one state whatever is set in between.  What the batch stages (StageLayout) goes to the device
+// in one copy; a plain batch at an unchanged state stages nothing and does not wait on the host.
+int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int n, cudaStream_t stream, bool background,
+                    int64_t *ticket_out) {
+    const int slot = (int)(r->next_ticket & 1);
+    WorkSlot &s = r->slot[slot];
+    if (!s.rastered) return fail(B2D_ERR_INVALID_ARG, "both worklist slots hold batches that were walked but not rastered yet");
+    const bool per_frame = fr.starts != nullptr, per_level = fr.levels != nullptr;
+    int rc = per_frame ? ensure_states(r) : B2D_OK;
+    if (rc == B2D_OK) rc = ensure_slot(r, s);
     if (rc != B2D_OK) return rc;
-    return raster_from_slot(r, ticket, d_index, d_rgba, stream);
-}
-
-// Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
-// per-frame-level walk (a b2d_renderer_create renderer may not; checked before anything is enqueued)
-static int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
-    if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
-    if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
-        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
-    for (size_t i = 0; i < n; i++)
-        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    const size_t nlev = r->lv.size();
+    auto level = [&](int f) { return per_level ? fr.levels[f] : 0u; };
+    std::vector<Expansion> plan;
+    std::vector<uint32_t> frame_set;
+    size_t state_words = 0;
+    if (per_frame) {
+        frame_set.resize((size_t)n);
+        std::unordered_map<std::string, uint32_t> seen;
+        seen.reserve((size_t)n);
+        size_t aoff = 0;
+        for (int f = 0; f < n; f++) {
+            const uint32_t k = level(f);
+            const LevelRes &lv = r->lv[k];
+            if (lv.h_blob.empty()) {                  // no set: the frame reads its level's blob tables
+                frame_set[(size_t)f] = (uint32_t)-1;
+                continue;
+            }
+            const uint32_t *w = fr.fs + fr.starts[f];
+            std::string key(reinterpret_cast<const char *>(&k), 4);
+            key.append(reinterpret_cast<const char *>(w), 4 * lv.layout.words);
+            auto it = seen.emplace(std::move(key), (uint32_t)plan.size());
+            if (it.second) {
+                plan.push_back(Expansion{k, w, s.arena.get() + aoff});
+                aoff += lv.state_tables.slot_bytes;
+                state_words += lv.layout.words;
+            }
+            frame_set[(size_t)f] = it.first->second;
+        }
+    } else {
+        for (uint32_t k = 0; k < nlev; k++) {
+            LevelRes &lv = r->lv[k];
+            if (lv.slot[slot].tables && lv.slot[slot].state != lv.state &&
+                (per_level ? std::find(fr.levels, fr.levels + n, k) != fr.levels + n : k == 0)) {
+                plan.push_back(Expansion{k, lv.state.data(), lv.slot[slot].tables.get()});
+                state_words += lv.layout.words;
+            }
+        }
+    }
+    const size_t nsets = plan.size();
+    const StageLayout L(nlev, nsets, (size_t)n, state_words, per_frame, per_level);
+    const bool stage = per_level || nsets > 0;
+    size_t records = 0;
+    if (stage) {
+        CU(cudaEventSynchronize(s.staged.get()));     // the copy issued two batches ago has read the staging
+        uint8_t *h = s.h_stage.get();
+        StateSrc *srcs = reinterpret_cast<StateSrc *>(h + L.srcs);
+        TableSet *sets = reinterpret_cast<TableSet *>(h + L.sets);
+        StateSet *descs = reinterpret_cast<StateSet *>(h + L.descs);
+        uint32_t *words = reinterpret_cast<uint32_t *>(h + L.states);
+        for (size_t k = 0; k < nlev; k++) {
+            const LevelRes &lv = r->lv[k];
+            if (per_level) reinterpret_cast<DeviceScene *>(h + L.scenes)[k] = per_frame ? lv.ds : slot_scene(lv, slot);
+            srcs[k] = lv.src;
+            if (per_frame) sets[nsets + k] = TableSet{lv.ds.tex, lv.ds.sectors, lv.ds.segs, lv.ds.sprites, lv.ds.mids};
+        }
+        size_t woff = 0;
+        for (size_t k = 0; k < nsets; k++) {
+            const LevelRes &lv = r->lv[plan[k].level];
+            sets[k] = table_set(plan[k].tables, lv.state_tables);
+            // one launch numbers the records of all per-frame sets; a launch of its own per stale set starts at 0
+            descs[k] = StateSet{plan[k].level, (uint32_t)woff, per_frame ? (uint32_t)records : 0u, 0};
+            std::memcpy(words + woff, plan[k].state, 4 * lv.layout.words);
+            woff += lv.layout.words;
+            records += set_records(lv);
+        }
+        if (records > 0x7FFFFFFFu) return fail(B2D_ERR_INVALID_ARG, "the batch's table sets hold more than 2^31 records");
+        for (int f = 0; f < n && per_level; f++) reinterpret_cast<uint32_t *>(h + L.frame_level)[f] = fr.levels[f];
+        for (int f = 0; f < n && per_frame; f++)
+            reinterpret_cast<uint32_t *>(h + L.frame_set)[f] =
+                frame_set[(size_t)f] == (uint32_t)-1 ? (uint32_t)(nsets + level(f)) : frame_set[(size_t)f];
+    }
+    CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
+    const uint8_t *d = s.stage.get();
+    if (stage) {
+        CU(cudaMemcpyAsync(s.stage.get(), s.h_stage.get(), L.end, cudaMemcpyHostToDevice, stream));
+        CU(cudaEventRecord(s.staged.get(), stream));
+    }
+    const StateSrc *d_srcs = reinterpret_cast<const StateSrc *>(d + L.srcs);
+    const TableSet *d_sets = reinterpret_cast<const TableSet *>(d + L.sets);
+    const StateSet *d_descs = reinterpret_cast<const StateSet *>(d + L.descs);
+    const uint32_t *d_words = reinterpret_cast<const uint32_t *>(d + L.states);
+    if (per_frame && nsets) {
+        CU(launch_state_sets(d_srcs, d_descs, d_sets, d_words, (int)nsets, (uint32_t)records, stream));
+        r->launches += 1;
+    }
+    for (size_t k = 0; k < nsets && !per_frame; k++) {
+        LevelRes &lv = r->lv[plan[k].level];
+        CU(launch_state_sets(d_srcs, d_descs + k, d_sets + k, d_words, 1, (uint32_t)set_records(lv), stream));
+        r->launches += 1;
+        lv.slot[slot].state = lv.state;
+    }
+    BatchTables t{};
+    t.per_frame = per_frame;
+    t.per_level = per_level;
+    if (per_level)
+        t.levels = LevelTables{reinterpret_cast<const DeviceScene *>(d + L.scenes), reinterpret_cast<const uint32_t *>(d + L.frame_level),
+                               per_frame ? d_sets : nullptr};
+    else
+        t.scene = slot_scene(r->lv[0], slot);
+    if (per_frame) {
+        if (!per_level) {
+            t.states = r->lv[0].state_tables;
+            t.states.base = s.arena.get();
+        }
+        t.states.frame_slot = reinterpret_cast<const uint32_t *>(d + L.frame_set);
+    }
+    rc = profiled(r, stream, 0, [&] {
+        return launch_walk(t, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background);
+    });
+    if (rc != B2D_OK) return rc;
+    CU(cudaEventRecord(s.walk_done.get(), stream));
+    s.n = n;
+    s.tables = t;
+    s.sets = per_frame ? (int)nsets : 0;
+    s.set_level.resize(s.sets);
+    s.set_off.resize(s.sets);
+    for (int k = 0; k < s.sets; k++) {
+        s.set_level[k] = plan[k].level;
+        s.set_off[k] = (size_t)(plan[k].tables - s.arena.get());
+    }
+    s.ticket = r->next_ticket;
+    s.rastered = false;
+    r->last_slot = slot;
+    r->launches += 1;
+    *ticket_out = r->next_ticket++;
     return B2D_OK;
 }
 
-// Per-frame states and levels: the levels checked as check_levels, then each frame's compact state built with its level's
-// layout (build_states: frame i's from fs[starts[i]])
-int b2d::build_levels_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n,
-                             const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts) {
-    int rc = check_levels(r, levels, n);
+int b2d::raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
+    const int slot = (int)(ticket & 1);
+    WorkSlot &s = r->slot[slot];
+    if (ticket < 0 || s.ticket != ticket || s.rastered) return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
+    CU(cudaStreamWaitEvent(stream, s.walk_done.get(), 0));
+    if (r->d_masked) {
+        // one arena of deferred masked entries per renderer: rasters that use it run one after the other (each fills the
+        // machine on its own, so nothing is lost), whatever streams they were enqueued on
+        CU(cudaStreamWaitEvent(stream, r->masked_done.get(), 0));
+        CU(cudaMemsetAsync(r->d_masked_counter.get(), 0, sizeof(uint32_t), stream));
+    }
+    // masked content in a level the frames read: with per-frame levels, any level's
+    const bool masked = r->d_masked && (s.tables.per_level || s.tables.scene.masked_list);
+    const int rc = profiled(r, stream, 1, [&] {
+        return launch_raster(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba, stream);
+    });
     if (rc != B2D_OK) return rc;
-    return guarded([&] { return build_states(r, levels, states, n, moves, n_moves, fs, &starts); });
+    CU(cudaEventRecord(s.raster_done.get(), stream));
+    if (r->d_masked) CU(cudaEventRecord(r->masked_done.get(), stream));
+    s.rastered = true;
+    r->launches += 1;
+    return B2D_OK;
+}
+
+// batches of at most max_batch frames in n frames
+static size_t batch_count(const b2d_renderer *r, size_t n) { return (n + (size_t)r->max_batch - 1) / (size_t)r->max_batch; }
+
+// walk -> raster of one batch on `stream`
+static int enqueue_frames(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int n, uint8_t *d_index, uint32_t *d_rgba,
+                          cudaStream_t stream) {
+    int64_t ticket = -1;
+    int rc = walk_batch(r, d_poses, fr, n, stream, false, &ticket);
+    if (rc != B2D_OK) return rc;
+    return raster_batch(r, ticket, d_index, d_rgba, stream);
 }
 
 extern "C" {
@@ -1012,16 +830,26 @@ int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
         t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
         for (auto &sl : lv.slot) CU(allocate(sl.tables, t.slot_bytes));
         // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306).  The
-        // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0.
+        // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0,
+        // expanded by one launch.
         lv.state.assign(words, 0);
         compact_state(blob, L, 0, nullptr, nullptr, lv.state.data());
-        DeviceBuf<uint32_t> d_state;
-        CU(allocate(d_state, 4 * words));
-        CU(cudaMemcpy(d_state.get(), lv.state.data(), 4 * words, cudaMemcpyHostToDevice));
-        for (auto &sl : lv.slot) {
-            CU(launch_state_tables(lv.src, d_state.get(), (uint32_t)words, 1, sl.tables.get(), t, nullptr));
-            sl.state = lv.state;
+        const StageLayout S(1, 2, 0, words, false, false);
+        const uint32_t records = (uint32_t)set_records(lv);
+        std::vector<uint8_t> stage(S.end);
+        *reinterpret_cast<StateSrc *>(stage.data() + S.srcs) = lv.src;
+        for (uint32_t k = 0; k < 2; k++) {
+            reinterpret_cast<TableSet *>(stage.data() + S.sets)[k] = table_set(lv.slot[k].tables.get(), t);
+            reinterpret_cast<StateSet *>(stage.data() + S.descs)[k] = StateSet{0, 0, k * records, 0};
+            lv.slot[k].state = lv.state;
         }
+        std::memcpy(stage.data() + S.states, lv.state.data(), 4 * words);
+        DeviceBuf<uint8_t> d;
+        CU(allocate(d, S.end));
+        CU(cudaMemcpy(d.get(), stage.data(), S.end, cudaMemcpyHostToDevice));
+        CU(launch_state_sets(reinterpret_cast<const StateSrc *>(d.get() + S.srcs), reinterpret_cast<const StateSet *>(d.get() + S.descs),
+                             reinterpret_cast<const TableSet *>(d.get() + S.sets), reinterpret_cast<const uint32_t *>(d.get() + S.states),
+                             2, 2 * records, nullptr));
         CU(cudaDeviceSynchronize());
     }
     return B2D_OK;
@@ -1101,8 +929,7 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
         CU(event_create(r->masked_done));
         CU(cudaEventRecord(r->masked_done.get(), nullptr));
     }
-    // per-frame levels: [DeviceScene per level | compact state per timed level | frame levels] in each slot's level buffer
-    size_t off = (r->lv.size() * sizeof(DeviceScene) + 15) & ~(size_t)15;
+    size_t words = 0;
     for (LevelRes &lv : r->lv) {
         DeviceScene &d = lv.ds;
         d.yslope = r->d_yslope.get();
@@ -1112,23 +939,19 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
             d.masked_counter = r->d_masked_counter.get();
             d.masked_chunks = masked_chunks;
         }
-        lv.stage_off = off;
-        off += 4 * lv.layout.words;
+        words = std::max(words, (size_t)lv.layout.words);
     }
-    r->levels_frames_off = (off + 15) & ~(size_t)15;
     // every level's palette side by side (b2d_palette_lut_levels_device): at most B2D_MAX_LEVELS x 1 KB
     CU(allocate(r->d_palettes, r->lv.size() * 256 * sizeof(uint32_t)));
     for (size_t k = 0; k < r->lv.size(); k++)
         CU(cudaMemcpy(r->d_palettes.get() + k * 256, r->lv[k].ds.palette, 256 * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
-    if (!r->lv[0].h_blob.empty()) {
-        // level 0's per-frame states and the restates of its plain batches: compact states + set indices and their staging
-        const size_t words = r->lv[0].layout.words, mb = (size_t)max_batch;
-        for (WorkSlot &sl : r->slot) {
-            CU(allocate(sl.states, 4 * mb * (words + 1)));
-            CU(allocate(sl.h_states, 4 * mb * (words + 1)));
-            CU(event_create(sl.states_copied));
-            sl.states_bytes = 4 * mb * (words + 1);
-        }
+    // each worklist slot's staging, for the largest batch: max_batch frames with a table set each, or a stale set per level
+    const size_t sets = std::max((size_t)max_batch, r->lv.size());
+    const size_t stage_bytes = StageLayout(r->lv.size(), sets, (size_t)max_batch, sets * words, true, true).end;
+    for (WorkSlot &sl : r->slot) {
+        CU(allocate(sl.stage, stage_bytes));
+        CU(allocate(sl.h_stage, stage_bytes));
+        CU(event_create(sl.staged));
     }
     CU(allocate(r->d_poses, sizeof(Pose) * (size_t)max_batch));
     rc = ensure_slot(r.get(), r->slot[0]);
@@ -1215,20 +1038,20 @@ int b2d_render_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, uint8_
     if (n == 0) return B2D_OK;
     if (n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n exceeds max_batch");
     CU(cudaSetDevice(r->device));
-    return enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses), (int)n, d_index_fb, d_rgba_fb,
+    return enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses), Frames{}, (int)n, d_index_fb, d_rgba_fb,
                           static_cast<cudaStream_t>(cuda_stream));
 }
 
-// frames_states (nullable, level 0's layout.words words per frame): walk + raster of n device poses in batches of max_batch
-static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, size_t n, const uint32_t *frame_states, uint8_t *d_index_fb,
+// walk + raster of the n frames `fr` (device poses) in batches of max_batch on `st`
+static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, const Frames &fr, size_t n, uint8_t *d_index_fb,
                            uint32_t *d_rgba_fb, cudaStream_t st) {
-    const int rc = check_slots_free(r, batch_count(r, n));
+    int rc = check_slots_free(r, batch_count(r, n));
     if (rc != B2D_OK) return rc;
     const size_t npix = (size_t)r->view.W * r->view.H;
     for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
         const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
-        int rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, (int)cnt, d_index_fb + i * npix,
-                                d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st, frame_states ? frame_states + i * r->lv[0].layout.words : nullptr);
+        rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, fr.from(i), (int)cnt, d_index_fb + i * npix,
+                            d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st);
         if (rc != B2D_OK) return rc;
     }
     return B2D_OK;
@@ -1239,11 +1062,11 @@ int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint
     if (!r || !d_poses || !d_index_fb || !tics) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
-    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { timed_states(r, tics, n, fs); return B2D_OK; });
-    if (rc != B2D_OK) return rc;
-    rc = enqueue_batches(r, d_poses, n, fs.empty() ? nullptr : fs.data(), d_index_fb, d_rgba_fb, st);
+    std::vector<size_t> starts;
+    Frames fr;
+    int rc = build_states(r, nullptr, tics, n, nullptr, 0, fs, starts, fr);
+    if (rc == B2D_OK) rc = enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
     if (rc != B2D_OK) return rc;
     return b2d_renderer_set_time(r, tics[n - 1]);                          // the renderer is left at the last pose's time
 }
@@ -1253,10 +1076,12 @@ int b2d_render_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d
                              void *cuda_stream) {
     if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { return build_states(r, nullptr, states, n, moves, n_moves, fs); });
+    std::vector<size_t> starts;
+    Frames fr;
+    int rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK || n == 0) return rc;
     CU(cudaSetDevice(r->device));
-    return enqueue_batches(r, d_poses, n, fs.empty() ? nullptr : fs.data(), d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+    return enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
@@ -1264,70 +1089,46 @@ int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_f
     if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { return build_states(r, nullptr, states, n, moves, n_moves, fs); });
+    std::vector<size_t> starts;
+    Frames fr;
+    int rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK) return rc;
     CU(cudaSetDevice(r->device));
-    return walk_into_slot(r, reinterpret_cast<const Pose *>(d_poses), (int)n, static_cast<cudaStream_t>(cuda_stream), ticket_out, true,
-                          fs.empty() ? nullptr : fs.data());
+    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
 }
 
 int b2d_walk_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, void *cuda_stream, int64_t *ticket_out) {
     if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
     CU(cudaSetDevice(r->device));
-    return walk_into_slot(r, reinterpret_cast<const Pose *>(d_poses), (int)n, static_cast<cudaStream_t>(cuda_stream), ticket_out, true);
+    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), Frames{}, (int)n, static_cast<cudaStream_t>(cuda_stream), true,
+                      ticket_out);
 }
 
 int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint32_t *d_rgba_fb, void *cuda_stream) {
     if (!r || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     CU(cudaSetDevice(r->device));
-    return raster_from_slot(r, ticket, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
-}
-
-// walk -> raster of a batch with per-frame levels on `stream`
-static int enqueue_level_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, int n, uint8_t *d_index,
-                                uint32_t *d_rgba, cudaStream_t stream) {
-    int64_t ticket = -1;
-    int rc = walk_levels_into_slot(r, d_poses, levels, n, stream, &ticket, false);
-    if (rc != B2D_OK) return rc;
-    return raster_from_slot(r, ticket, d_index, d_rgba, stream);
+    return raster_batch(r, ticket, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int b2d_render_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, uint8_t *d_index_fb,
                              uint32_t *d_rgba_fb, void *cuda_stream) {
     if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK && n) rc = check_slots_free(r, batch_count(r, n));
+    const int rc = check_levels(r, levels, n);
     if (rc != B2D_OK || n == 0) return rc;
     CU(cudaSetDevice(r->device));
-    const size_t npix = (size_t)r->view.W * r->view.H;
-    for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
-        const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
-        rc = enqueue_level_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, levels + i, (int)cnt, d_index_fb + i * npix,
-                                  d_rgba_fb ? d_rgba_fb + i * npix : nullptr, static_cast<cudaStream_t>(cuda_stream));
-        if (rc != B2D_OK) return rc;
-    }
-    return B2D_OK;
+    return enqueue_batches(r, d_poses, Frames{levels}, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, void *cuda_stream,
                            int64_t *ticket_out) {
     if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
-    int rc = check_levels(r, levels, n);
+    const int rc = check_levels(r, levels, n);
     if (rc != B2D_OK) return rc;
     CU(cudaSetDevice(r->device));
-    return walk_levels_into_slot(r, reinterpret_cast<const Pose *>(d_poses), levels, (int)n, static_cast<cudaStream_t>(cuda_stream),
-                                 ticket_out, true);
-}
-
-// walk -> raster of a batch with per-frame states and levels on `stream`
-static int enqueue_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *frame_states,
-                                        const size_t *starts, int n, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
-    int64_t ticket = -1;
-    int rc = walk_levels_states_into_slot(r, d_poses, levels, frame_states, starts, n, stream, &ticket, false);
-    if (rc != B2D_OK) return rc;
-    return raster_from_slot(r, ticket, d_index, d_rgba, stream);
+    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), Frames{levels}, (int)n, static_cast<cudaStream_t>(cuda_stream),
+                      true, ticket_out);
 }
 
 int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
@@ -1336,19 +1137,12 @@ int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, co
     if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     std::vector<uint32_t> fs;
     std::vector<size_t> starts;
-    int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
-    if (rc == B2D_OK && n) rc = check_slots_free(r, batch_count(r, n));
+    Frames fr{levels};
+    int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK || n == 0) return rc;
     CU(cudaSetDevice(r->device));
-    const size_t npix = (size_t)r->view.W * r->view.H;
-    for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
-        const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
-        rc = enqueue_levels_states_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, levels + i, fs.data(), starts.data() + i,
-                                          (int)cnt, d_index_fb + i * npix, d_rgba_fb ? d_rgba_fb + i * npix : nullptr,
-                                          static_cast<cudaStream_t>(cuda_stream));
-        if (rc != B2D_OK) return rc;
-    }
-    return B2D_OK;
+    return enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
@@ -1357,18 +1151,16 @@ int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, cons
     if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
     std::vector<uint32_t> fs;
     std::vector<size_t> starts;
-    int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
+    Frames fr{levels};
+    int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK) return rc;
     CU(cudaSetDevice(r->device));
-    return walk_levels_states_into_slot(r, reinterpret_cast<const Pose *>(d_poses), levels, fs.data(), starts.data(), (int)n,
-                                        static_cast<cudaStream_t>(cuda_stream), ticket_out, true);
+    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
 }
 
-// Host poses in, host frames out; frame_states as in enqueue_frames (for all n frames), or (exclusive with it) frame_levels:
-// the level of each of the n frames.  With both and `starts`: per-frame states and levels (frame i's state from
-// frame_states[starts[i]], as build_states left them).
-static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const uint32_t *frame_states, uint8_t *index_fb,
-                       uint32_t *rgba_fb, const uint32_t *frame_levels = nullptr, const size_t *starts = nullptr) {
+// Host poses in, host frames out: the n frames `fr` in batches of max_batch.
+static int render_host(b2d_renderer *r, const b2d_pose *poses, const Frames &fr, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
     if (n == 0) return B2D_OK;
     if (check_slots_free(r, batch_count(r, n)) != B2D_OK) return B2D_ERR_INVALID_ARG;
     CU(cudaSetDevice(r->device));
@@ -1404,14 +1196,7 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const u
         std::memcpy(hp, poses + done, sizeof(Pose) * (size_t)cnt);
         cudaStream_t rs = hs.render_stream.get(), cs = hs.copy_stream[buf].get();
         CU(cudaMemcpyAsync(r->d_poses.get(), hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, rs));
-        int rc = starts
-                     ? enqueue_levels_states_frames(r, r->d_poses.get(), frame_levels + done, frame_states, starts + done, cnt,
-                                                    hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs)
-                 : frame_levels
-                     ? enqueue_level_frames(r, r->d_poses.get(), frame_levels + done, cnt, hs.index[buf].get(),
-                                            rgba_fb ? hs.rgba[buf].get() : nullptr, rs)
-                     : enqueue_frames(r, r->d_poses.get(), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs,
-                                      frame_states ? frame_states + done * r->lv[0].layout.words : nullptr);
+        int rc = enqueue_frames(r, r->d_poses.get(), fr.from(done), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs);
         if (rc != B2D_OK) return rc;
         CU(cudaEventRecord(hs.rendered[buf].get(), rs));
         CU(cudaStreamWaitEvent(cs, hs.rendered[buf].get(), 0));
@@ -1438,7 +1223,7 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, size_t n, const u
 
 int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    return render_host(r, poses, n, nullptr, index_fb, rgba_fb);
+    return render_host(r, poses, Frames{}, n, index_fb, rgba_fb);
 }
 
 int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tics, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
@@ -1448,9 +1233,11 @@ int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tic
     int rc = check_slots_free(r, batch_count(r, n));          // refused before the time changes as well
     if (rc != B2D_OK) return rc;
     std::vector<uint32_t> fs;
-    rc = guarded([&] { timed_states(r, tics, n, fs); return B2D_OK; });
+    std::vector<size_t> starts;
+    Frames fr;
+    rc = build_states(r, nullptr, tics, n, nullptr, 0, fs, starts, fr);
     if (rc != B2D_OK) return rc;
-    rc = render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
+    rc = render_host(r, poses, fr, n, index_fb, rgba_fb);
     const int trc = b2d_renderer_set_time(r, tics[n - 1]);                // the renderer is left at the last pose's time
     return rc != B2D_OK ? rc : trc;
 }
@@ -1459,9 +1246,11 @@ int b2d_render_states(b2d_renderer *r, const b2d_pose *poses, const b2d_frame_st
                       const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     std::vector<uint32_t> fs;
-    int rc = guarded([&] { return build_states(r, nullptr, states, n, moves, n_moves, fs); });
+    std::vector<size_t> starts;
+    Frames fr;
+    int rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK) return rc;
-    return render_host(r, poses, n, fs.empty() ? nullptr : fs.data(), index_fb, rgba_fb);
+    return render_host(r, poses, fr, n, index_fb, rgba_fb);
 }
 
 int b2d_render_levels(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, size_t n, uint8_t *index_fb,
@@ -1469,7 +1258,7 @@ int b2d_render_levels(b2d_renderer *r, const b2d_pose *poses, const uint32_t *le
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     int rc = check_levels(r, levels, n);
     if (rc != B2D_OK) return rc;
-    return render_host(r, poses, n, nullptr, index_fb, rgba_fb, levels);
+    return render_host(r, poses, Frames{levels}, n, index_fb, rgba_fb);
 }
 
 int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, const b2d_frame_state *states, size_t n,
@@ -1477,9 +1266,35 @@ int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint3
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     std::vector<uint32_t> fs;
     std::vector<size_t> starts;
-    int rc = build_levels_states(r, levels, states, n, moves, n_moves, fs, starts);
+    Frames fr{levels};
+    int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK) return rc;
-    return render_host(r, poses, n, fs.data(), index_fb, rgba_fb, levels, starts.data());
+    return render_host(r, poses, fr, n, index_fb, rgba_fb);
+}
+
+// The n frame levels of a call staged in `s` on `st`: into staging grown to hold them (created whole, or not at all; the
+// old buffers go once the last call's kernel has read them), or into the present staging once the previous call's copy
+// has read it and, on `st`, its kernel the device copy.  The caller records s.done after its kernel.
+static int stage_levels(LevelStaging &s, const uint32_t *levels, size_t n, cudaStream_t st) {
+    if (s.cap < n) {
+        LevelStaging g;
+        g.cap = s.cap ? s.cap : 1024;
+        while (g.cap < n) g.cap *= 2;
+        CU(allocate(g.d, g.cap * sizeof(uint32_t)));
+        CU(allocate(g.h, g.cap * sizeof(uint32_t)));
+        CU(event_create(g.copied));
+        CU(event_create(g.done));
+        if (s.done) CU(cudaEventSynchronize(s.done.get()));
+        s = std::move(g);
+    } else {
+        CU(cudaEventSynchronize(s.copied.get()));     // the previous call's copy has read the staging
+        CU(cudaStreamWaitEvent(st, s.done.get(), 0));        // ... and its kernel the device copy
+    }
+    std::memcpy(s.h.get(), levels, n * sizeof(uint32_t));
+    CU(cudaMemcpyAsync(s.d.get(), s.h.get(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(s.copied.get(), st));
+    return B2D_OK;
 }
 
 int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_rgba, size_t n_pixels, void *cuda_stream) {
@@ -1498,30 +1313,9 @@ int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    if (r->lut_levels_cap < n_frames) {
-        // created whole, or not at all; the old buffers go once the last call's kernel has read them
-        size_t cap = r->lut_levels_cap ? r->lut_levels_cap : 1024;
-        while (cap < n_frames) cap *= 2;
-        DeviceBuf<uint32_t> d;
-        PinnedBuf<uint32_t> h;
-        Event copied, done;
-        CU(allocate(d, cap * sizeof(uint32_t)));
-        CU(allocate(h, cap * sizeof(uint32_t)));
-        CU(event_create(copied));
-        CU(event_create(done));
-        if (r->lut_done) CU(cudaEventSynchronize(r->lut_done.get()));
-        r->d_lut_levels = std::move(d); r->h_lut_levels = std::move(h);
-        r->lut_levels_copied = std::move(copied); r->lut_done = std::move(done);
-        r->lut_levels_cap = cap;
-    } else {
-        CU(cudaEventSynchronize(r->lut_levels_copied.get()));     // the previous call's copy has read the staging
-        CU(cudaStreamWaitEvent(st, r->lut_done.get(), 0));        // ... and its kernel the device copy
-    }
-    std::memcpy(r->h_lut_levels.get(), levels, n_frames * sizeof(uint32_t));
-    CU(cudaMemcpyAsync(r->d_lut_levels.get(), r->h_lut_levels.get(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(r->lut_levels_copied.get(), st));
-    CU(launch_palette_levels(r->d_palettes.get(), r->d_lut_levels.get(), d_index, d_rgba, n_frames, (size_t)r->view.W * r->view.H, st));
-    CU(cudaEventRecord(r->lut_done.get(), st));
+    if (int rc = stage_levels(r->lut_levels, levels, n_frames, st)) return rc;
+    CU(launch_palette_levels(r->d_palettes.get(), r->lut_levels.d.get(), d_index, d_rgba, n_frames, (size_t)r->view.W * r->view.H, st));
+    CU(cudaEventRecord(r->lut_levels.done.get(), st));
     r->launches += 1;
     return B2D_OK;
 }
@@ -1554,32 +1348,11 @@ int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     const uint32_t *d_levels = nullptr;          // NULL levels: every frame through level 0's palette, nothing to stage
     if (levels) {
-        if (r->resolve_levels_cap < n_frames) {
-            // created whole, or not at all; the old buffers go once the last call's kernel has read them
-            size_t cap = r->resolve_levels_cap ? r->resolve_levels_cap : 1024;
-            while (cap < n_frames) cap *= 2;
-            DeviceBuf<uint32_t> d;
-            PinnedBuf<uint32_t> h;
-            Event copied, done;
-            CU(allocate(d, cap * sizeof(uint32_t)));
-            CU(allocate(h, cap * sizeof(uint32_t)));
-            CU(event_create(copied));
-            CU(event_create(done));
-            if (r->resolve_done) CU(cudaEventSynchronize(r->resolve_done.get()));
-            r->d_resolve_levels = std::move(d); r->h_resolve_levels = std::move(h);
-            r->resolve_levels_copied = std::move(copied); r->resolve_done = std::move(done);
-            r->resolve_levels_cap = cap;
-        } else {
-            CU(cudaEventSynchronize(r->resolve_levels_copied.get()));     // the previous call's copy has read the staging
-            CU(cudaStreamWaitEvent(st, r->resolve_done.get(), 0));        // ... and its kernel the device copy
-        }
-        std::memcpy(r->h_resolve_levels.get(), levels, n_frames * sizeof(uint32_t));
-        CU(cudaMemcpyAsync(r->d_resolve_levels.get(), r->h_resolve_levels.get(), n_frames * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-        CU(cudaEventRecord(r->resolve_levels_copied.get(), st));
-        d_levels = r->d_resolve_levels.get();
+        if (int rc = stage_levels(r->resolve_levels, levels, n_frames, st)) return rc;
+        d_levels = r->resolve_levels.d.get();
     }
     CU(launch_resolve(r->d_palettes.get(), d_levels, d_index, d_out, n_frames, r->view.W, r->view.H, factor, format, st));
-    if (levels) CU(cudaEventRecord(r->resolve_done.get(), st));
+    if (levels) CU(cudaEventRecord(r->resolve_levels.done.get(), st));
     r->launches += 1;
     return B2D_OK;
 }
@@ -1637,41 +1410,32 @@ int b2d_debug_worklist(b2d_renderer *r, size_t n, int32_t *counts_out, int32_t *
 
 int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
     if (!r || !slots_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    const int slot = r->last_slot;
-    if (!r->slot[slot].per_frame || n > (size_t)r->slot[slot].n)
+    const WorkSlot &s = r->slot[r->last_slot];
+    if (!s.tables.per_frame || n > (size_t)s.n)
         return fail(B2D_ERR_INVALID_ARG, "the last walked batch has no per-frame states or fewer than n frames");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
-    const WorkSlot &s = r->slot[slot];
-    if (s.per_level) {
-        // per-frame states and levels: a frame on a level without a table set (TableSet index >= sets) has none
-        StateTables st;
-        levels_states_tables(s, LevelsStatesBatch(r->lv.size(), (size_t)s.sets, (size_t)s.n, 0), st);
-        CU(cudaMemcpy(slots_out, st.frame_slot, 4 * n, cudaMemcpyDeviceToHost));
-        for (size_t i = 0; i < n; i++)
-            if (slots_out[i] >= (uint32_t)s.sets) slots_out[i] = 0xFFFFFFFFu;
-        return B2D_OK;
-    }
-    CU(cudaMemcpy(slots_out, slot_tables(r, slot).frame_slot, 4 * n, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(slots_out, s.tables.states.frame_slot, 4 * n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; i++)      // a frame on a level without a table set (TableSet index >= sets) has none
+        if (slots_out[i] >= (uint32_t)s.sets) slots_out[i] = 0xFFFFFFFFu;
     return B2D_OK;
 }
 
 int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capacity, size_t *size_out) {
     if (!r) return fail(B2D_ERR_INVALID_ARG, "null renderer");
     const WorkSlot &s = r->slot[r->last_slot];
-    const bool both = s.per_frame && s.per_level;      // per-frame states and levels: the set's level, at its arena offset
-    const LevelRes &lv = r->lv[both && set < (size_t)s.sets ? s.set_level[set] : 0];
-    if (!both && lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
+    const bool per_frame = s.tables.per_frame;        // a per-frame set of the arena, or the slot's own set of level 0
+    const LevelRes &lv = r->lv[per_frame && set < (size_t)s.sets ? s.set_level[set] : 0];
+    if (!per_frame && lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
     if (s.ticket < 0) return fail(B2D_ERR_INVALID_ARG, "no batch has been walked");
-    if (set >= (s.per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
+    if (set >= (per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
     const size_t need = state_table_bytes(lv.h_blob.data());
     if (size_out) *size_out = need;
     if (!out) return B2D_OK;
     if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
-    const uint8_t *src = both ? s.arena.get() + s.set_off[set]
-                         : s.per_frame ? s.arena.get() + set * (size_t)lv.state_tables.slot_bytes : lv.slot[r->last_slot].tables.get();
+    const uint8_t *src = per_frame ? s.arena.get() + s.set_off[set] : lv.slot[r->last_slot].tables.get();
     CU(cudaMemcpy(out, src, need, cudaMemcpyDeviceToHost));
     return B2D_OK;
 }

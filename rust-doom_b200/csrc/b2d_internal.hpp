@@ -15,23 +15,33 @@
 namespace b2d {
 int fail(int code, const std::string &msg);            // sets the thread-local message, returns code
 int cuda_fail(cudaError_t e, const char *what);
-// BSP walk + raster of n device poses into d_index / d_rgba (nullable) on `stream`; not synchronised.  `frame_states`
-// (nullable): n compact states (r->layout.words words each), frame i rendered at its own state.
-int enqueue_frames(b2d_renderer *r, const Pose *d_poses, int n, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
-                   const uint32_t *frame_states = nullptr);
+// The frames of a call, or of one batch of it (HOST arrays).  `levels`: the level of each frame, checked by check_levels
+// (nullptr: every frame on level 0).  `starts`: with per-frame states, frame i's compact state is fs[starts[i] ..] (its
+// level's layout.words words; none on a level without time-dependent content or dynamic sectors); nullptr: every level at
+// the renderer's own state, a plain batch.
+struct Frames {
+    const uint32_t *levels = nullptr;
+    const uint32_t *fs = nullptr;
+    const size_t *starts = nullptr;
+    Frames from(size_t first) const { return {levels ? levels + first : nullptr, fs, starts ? starts + first : nullptr}; }
+};
+// The n per-frame states of a call on the frames of `out` (out.levels set by the caller), checked, and out.fs / out.starts
+// pointing into `fs` / `starts`: with `tics`, frame i at tics[i] with its level's current sector moves; else at
+// states[i] (its time and its range of `moves`).  With every frame on level 0 and a level 0 without time-dependent content
+// or dynamic sectors, the call is a plain one (out.starts stays nullptr).  Nothing is enqueued.
+int build_states(const b2d_renderer *r, const b2d_frame_state *states, const uint32_t *tics, size_t n, const b2d_sector_move *moves,
+                 size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts, Frames &out);
+// Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
+// per-frame-level walk (a b2d_renderer_create renderer may not); B2D_ERR_INVALID_ARG otherwise.
+int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n);
 // A one-call render of `batches` batches walks the first into the next worklist slot and alternates slots from there: it
 // is refused (B2D_ERR_INVALID_ARG) before anything is enqueued while a slot it would use holds a walked, unrastered batch.
 int check_slots_free(const b2d_renderer *r, size_t batches);
-// the two halves (b2d_walk_device / b2d_raster_device): a background walk into a worklist slot, the raster of a ticket
-int walk_frames(b2d_renderer *r, const Pose *d_poses, int n, cudaStream_t stream, int64_t *ticket_out, bool background);
-int raster_frames(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);
-// per-frame states and levels (b2d_render_levels_states & co.): the n HOST levels and states checked and each frame's compact
-// state built with its level's layout (frame i's from fs[starts[i]]); nothing is enqueued
-int build_levels_states(const b2d_renderer *r, const uint32_t *levels, const b2d_frame_state *states, size_t n,
-                        const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts);
-// the walk of such a batch (levels, fs and starts of its n frames as build_levels_states left them) into a worklist slot
-int walk_levels_states_frames(b2d_renderer *r, const Pose *d_poses, const uint32_t *levels, const uint32_t *fs, const size_t *starts,
-                              int n, cudaStream_t stream, int64_t *ticket_out, bool background);
+// The BSP walk of the n frames `frames` (device poses d_poses) into the next worklist slot on `stream`, and the raster of a
+// ticket (b2d_walk_device* / b2d_raster_device); neither is synchronised.
+int walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &frames, int n, cudaStream_t stream, bool background,
+               int64_t *ticket_out);
+int raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);
 
 // Owners of CUDA resources.  They release on the current device: ~b2d_renderer and b2d_comm_destroy select theirs first.
 struct DeviceFree { void operator()(void *p) const { cudaFree(p); } };
@@ -95,27 +105,18 @@ struct WorkSlot {
     int n = 0;                                            // frames walked into the slot
     int64_t ticket = -1;
     bool rastered = true;
-    bool per_frame = false;                               // the batch was walked with per-frame states
-    bool per_level = false;                               // ... or with per-frame levels (both: b2d_render_levels_states)
-    int sets = 0;                                         // ... into this many table sets of the arena (distinct states)
-    // per-frame levels (b2d_render_levels & co.; allocated by the first such call): [the DeviceScene of every level as this
-    // slot's batches read it | the compact states of the levels whose table sets a batch re-expands | each frame's level]
-    // on the device, and its pinned staging
-    DeviceBuf<uint8_t> levels;
-    PinnedBuf<uint8_t> h_levels;
-    Event levels_copied;                                  // h_levels has been read by its copy
-    // per-frame states (b2d_render_states & co.): an arena of up to max_batch expanded table sets (allocated by the first
-    // such call), and the compact states + per-frame set indices on the device and their pinned staging, shared with the
-    // expansion of the slot's own table set
+    BatchTables tables{};                                 // what the batch's walk read and its raster reads
+    // Per-frame states (b2d_render_states & co.): an arena of up to max_batch expanded table sets, allocated by the first
+    // such call; the batch's sets are packed into it, each at its level's slot_bytes
     DeviceBuf<uint8_t> arena;
-    DeviceBuf<uint32_t> states;                           // max_batch compact states, then max_batch set indices
-    PinnedBuf<uint32_t> h_states;                         // same layout
-    Event states_copied;                                  // h_states has been read by its copy
-    // per-frame states and levels (b2d_render_levels_states & co.): `states` and `h_states` then hold the batch's
-    // LevelsStatesBatch sections (b2d_api.cu), in states_bytes bytes (grown by the first such call of the slot)
-    size_t states_bytes = 0;
+    int sets = 0;                                         // table sets of the batch in the arena (distinct states)
     std::vector<uint32_t> set_level;                      // level of each table set
     std::vector<size_t> set_off;                          // byte offset of each table set in the arena
+    // The sections of a batch (StageLayout, b2d_api.cu) on the device and their pinned staging, sized at renderer creation
+    // for the largest batch: what its expansions, walk and raster read besides the poses
+    DeviceBuf<uint8_t> stage;
+    PinnedBuf<uint8_t> h_stage;
+    Event staged;                                         // h_stage has been read by its copy
 };
 
 // Host-path staging (created by the first b2d_render & co.): double-buffered frame outputs.
@@ -125,6 +126,15 @@ struct HostStaging {
     DeviceBuf<uint8_t> index[2];
     PinnedBuf<Pose> poses;                                // two buffers of max_batch poses
     std::array<DeviceBuf<uint32_t>, 2> rgba;              // created by the first call that asks for RGBA frames
+};
+
+// A call's frame levels on the device, with their pinned staging (stage_levels, b2d_api.cu): grown by a call with more
+// frames than they hold.
+struct LevelStaging {
+    DeviceBuf<uint32_t> d;
+    PinnedBuf<uint32_t> h;
+    size_t cap = 0;
+    Event copied, done;                                   // the staging has been read by its copy; the kernel has read the copy
 };
 
 // One level of a renderer (b2d_renderer_create_levels; b2d_renderer_create makes a set of one): the scene on the device
@@ -148,7 +158,6 @@ struct LevelRes {
     DeviceBuf<uint32_t> d_slot_maps;                      // StateLayout::sector_slots, then ::mid_seg
     StateSrc src{};                                       // device pointers into d_blob and d_slot_maps
     StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
-    size_t stage_off = 0;                                 // byte offset of its compact state in WorkSlot::levels
     // per worklist slot: the table set the slot's batches read and the compact state it was expanded from
     struct Slot {
         DeviceBuf<uint8_t> tables;
@@ -164,7 +173,6 @@ struct b2d_renderer {
     size_t walk_smem = 0;           // the largest walk_smem_per_warp of the levels
     // the levels; every entry point without a level argument acts on level 0
     std::vector<LevelRes> lv;
-    size_t levels_frames_off = 0;   // byte offset of the frame levels in WorkSlot::levels
     DeviceBuf<uint32_t> d_yslope;
     DeviceBuf<int32_t> d_status;
     DeviceBuf<uint32_t> d_masked;   // one arena of deferred masked entries for every level with masked content
@@ -175,18 +183,9 @@ struct b2d_renderer {
     std::unique_ptr<HostStaging> host;
     uint32_t tics = 0;
     Event masked_done;                                    // last raster that used the masked-entry arena
-    // b2d_palette_lut_levels_device: every level's palette, [n_levels][256], and the frame levels of a call on the device
-    // with their pinned staging (grown by a call with more frames than it holds)
-    DeviceBuf<uint32_t> d_palettes;
-    DeviceBuf<uint32_t> d_lut_levels;
-    PinnedBuf<uint32_t> h_lut_levels;
-    size_t lut_levels_cap = 0;
-    Event lut_levels_copied, lut_done;                    // the staging has been read by its copy; the kernel has read the copy
-    // b2d_resolve_device: its own frame levels on the device and their pinned staging, with the same rules
-    DeviceBuf<uint32_t> d_resolve_levels;
-    PinnedBuf<uint32_t> h_resolve_levels;
-    size_t resolve_levels_cap = 0;
-    Event resolve_levels_copied, resolve_done;
+    DeviceBuf<uint32_t> d_palettes;                       // every level's palette, [n_levels][256]
+    // the frame levels of a call of b2d_palette_lut_levels_device and of b2d_resolve_device, each call kind with its own
+    LevelStaging lut_levels, resolve_levels;
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;
     bool profiling = false;

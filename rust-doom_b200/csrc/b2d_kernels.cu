@@ -1260,9 +1260,8 @@ static int device_sms() {
 
 // The walk's launch: `smem` bytes of dynamic shared memory per CTA (one frame per CTA).
 template <bool kStates, bool kLevels>
-static cudaError_t walk_go(const DeviceScene &sc, size_t smem, const View &vw, const Pose *d_poses, int n, FrameConst *d_frames,
-                           SegFrame *d_work, int stride, cudaStream_t stream, bool background, const StateTables &st,
-                           const LevelTables &lt) {
+static cudaError_t walk_go(const BatchTables &t, size_t smem, const View &vw, const Pose *d_poses, int n, FrameConst *d_frames,
+                           SegFrame *d_work, int stride, cudaStream_t stream, bool background) {
     if (n <= 0) return cudaSuccess;
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
     if (smem > 48 * 1024) {   // per device and cheap: set it on every launch that needs the opt-in
@@ -1274,16 +1273,9 @@ static cudaError_t walk_go(const DeviceScene &sc, size_t smem, const View &vw, c
     // 7/8, so the raster keeps 16 of its 19 warps per SM while the walk hides behind it.
     const int sms = device_sms();
     const int blocks = (background && n > sms) ? sms : n, warps = 4;
-    b2d_walk_kernel<kStates, kLevels><<<blocks, warps * 32, smem, stream>>>(sc, vw, d_poses, n, d_frames, d_work, stride, st, lt);
+    b2d_walk_kernel<kStates, kLevels><<<blocks, warps * 32, smem, stream>>>(t.scene, vw, d_poses, n, d_frames, d_work, stride,
+                                                                            t.states, t.levels);
     return cudaGetLastError();
-}
-
-cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
-                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background,
-                        const StateTables *states) {
-    const size_t smem = walk_smem_per_warp(sc);
-    if (states) return walk_go<true, false>(sc, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, *states, LevelTables{});
-    return walk_go<false, false>(sc, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, StateTables{}, LevelTables{});
 }
 
 size_t walk_levels_static_smem() {
@@ -1299,18 +1291,13 @@ size_t walk_levels_static_smem() {
     return bytes;
 }
 
-cudaError_t launch_walk_levels(const LevelTables &levels, size_t smem, const View &vw, const Pose *d_poses, int n,
-                               FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background) {
-    if (smem + walk_levels_static_smem() > kWalkSmemMax) return cudaErrorInvalidValue;
-    // every scene the kernel reads comes from `levels`: its scene parameter is not read
-    return walk_go<false, true>(DeviceScene{}, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, StateTables{}, levels);
-}
-
-cudaError_t launch_walk_levels_states(const LevelTables &levels, const StateTables &states, size_t smem, const View &vw,
-                                      const Pose *d_poses, int n, FrameConst *d_frames, SegFrame *d_work, int stride,
-                                      cudaStream_t stream, bool background) {
-    if (smem + walk_levels_static_smem() > kWalkSmemMax) return cudaErrorInvalidValue;
-    return walk_go<true, true>(DeviceScene{}, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background, states, levels);
+cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw, const Pose *d_poses, int n,
+                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background) {
+    if (t.per_level && levels_smem + walk_levels_static_smem() > kWalkSmemMax) return cudaErrorInvalidValue;
+    const size_t smem = t.per_level ? levels_smem : walk_smem_per_warp(t.scene);
+    auto go = t.per_level ? (t.per_frame ? walk_go<true, true> : walk_go<false, true>)
+                          : (t.per_frame ? walk_go<true, false> : walk_go<false, false>);
+    return go(t, smem, vw, d_poses, n, d_frames, d_work, stride, stream, background);
 }
 
 // The raster's launch for every frame shape.  Launch shape: one warp per (frame, 32-column strip), kRasterWarps = 8 warps
@@ -1323,15 +1310,15 @@ cudaError_t launch_walk_levels_states(const LevelTables &levels, const StateTabl
 // = 16 warps per SM (DESIGN.md §6).
 // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
 template <bool kStates, bool kLevels>
-static cudaError_t raster_go(const DeviceScene &sc, bool masked, const View &vw, const FrameConst *d_frames,
+static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
                              const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
-                             cudaStream_t stream, const StateTables &st, const LevelTables &lt) {
+                             cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
     const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
 #define B2D_RASTER_GO(RGBA, KW) do { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, st, lt); \
-    else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(sc, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, st, lt); \
+    if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels); \
+    else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels); \
     } while (0)
     if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
     else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
@@ -1341,25 +1328,12 @@ static cudaError_t raster_go(const DeviceScene &sc, bool masked, const View &vw,
     return cudaGetLastError();
 }
 
-cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameConst *d_frames,
-                          const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb,
-                          uint32_t *d_rgba, cudaStream_t stream, const StateTables *states) {
-    const bool masked = (sc.nmids > 0 || sc.nsprites > 0) && sc.masked_list;
-    // Per-frame states (`states`) take the kStates variant of each shape; the frames are the same pixel for pixel.
-    if (states) return raster_go<true, false>(sc, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, *states, LevelTables{});
-    return raster_go<false, false>(sc, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, StateTables{}, LevelTables{});
-}
-
-cudaError_t launch_raster_levels(const LevelTables &levels, bool masked, const View &vw, const FrameConst *d_frames,
-                                 const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
-                                 cudaStream_t stream) {
-    return raster_go<false, true>(DeviceScene{}, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, StateTables{}, levels);
-}
-
-cudaError_t launch_raster_levels_states(const LevelTables &levels, const StateTables &states, bool masked, const View &vw,
-                                        const FrameConst *d_frames, const SegFrame *d_work, int stride, int n,
-                                        uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream) {
-    return raster_go<true, true>(DeviceScene{}, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, states, levels);
+// Per-frame states take the kStates variant of each shape; the frames are the same pixel for pixel.
+cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
+                          int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream) {
+    auto go = t.per_level ? (t.per_frame ? raster_go<true, true> : raster_go<false, true>)
+                          : (t.per_frame ? raster_go<true, false> : raster_go<false, false>);
+    return go(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream);
 }
 
 namespace {
@@ -1418,32 +1392,10 @@ cudaError_t launch_prelight(const uint8_t *d_colormap, const uint8_t *d_src, uin
 }
 
 namespace {
-// Per-frame states: one thread per output record of every state of the batch -- the state rule of b2d_scene.hpp, the same
-// functions scene_at_time runs on the host.
-__global__ void __launch_bounds__(256)
-b2d_state_tables_kernel(const __grid_constant__ StateSrc src, const uint32_t *__restrict__ states, uint32_t words, int nstates,
-                        uint8_t *__restrict__ arena, const __grid_constant__ StateTables L) {
-    const uint32_t per = src.ntex + src.nsectors + src.nsegs + src.nsprites + src.nmids;
-    const size_t total = (size_t)per * (size_t)nstates;
-    for (size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t k = (uint32_t)(g / per);
-        uint32_t i = (uint32_t)(g - (size_t)k * per);
-        const StateIn st = state_in(states + (size_t)k * words, src.ndyn);
-        uint8_t *out = arena + (size_t)k * L.slot_bytes;
-        if (i < src.ntex) { reinterpret_cast<TexRec *>(out)[i] = tex_at(src, st, i); continue; }
-        i -= src.ntex;
-        if (i < src.nsectors) { reinterpret_cast<SectorRec *>(out + L.off_sectors)[i] = sector_at(src, st, i); continue; }
-        i -= src.nsectors;
-        if (i < src.nsegs) { reinterpret_cast<SegRec *>(out + L.off_segs)[i] = seg_at(src, st, i); continue; }
-        i -= src.nsegs;
-        if (i < src.nsprites) { reinterpret_cast<SpriteRec *>(out + L.off_sprites)[i] = sprite_at(src, st, i); continue; }
-        i -= src.nsprites;
-        reinterpret_cast<MidRec *>(out + L.off_mids)[i] = mid_at(src, st, i);
-    }
-}
-
-// Per-frame states and levels: one thread per output record of every set of the batch, whatever its level.  The sets
-// number their records one after the other (StateSet::first, ascending): a thread finds its set by binary search.
+// Every table set expansion (a batch's per-frame sets, a stale set of a worklist slot, a level's tic-0 sets): one thread
+// per output record of every set of the launch, whatever its level -- the state rule of b2d_scene.hpp, the same functions
+// scene_at_time runs on the host.  The sets number their records one after the other (StateSet::first, ascending): a
+// thread finds its set by binary search.
 __global__ void __launch_bounds__(256)
 b2d_state_sets_kernel(const StateSrc *__restrict__ srcs, const StateSet *__restrict__ sets, const TableSet *__restrict__ out,
                       const uint32_t *__restrict__ states, int nsets, uint32_t records) {
@@ -1478,17 +1430,6 @@ cudaError_t launch_state_sets(const StateSrc *d_srcs, const StateSet *d_sets, co
     const size_t cap = (size_t)device_sms() * 16;
     if (blocks > cap) blocks = cap;
     b2d_state_sets_kernel<<<(int)blocks, 256, 0, stream>>>(d_srcs, d_sets, d_out, d_states, nsets, records);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_state_tables(const StateSrc &src, const uint32_t *d_states, uint32_t words, int nstates, uint8_t *d_arena,
-                                const StateTables &layout, cudaStream_t stream) {
-    const size_t total = (size_t)(src.ntex + src.nsectors + src.nsegs + src.nsprites + src.nmids) * (size_t)nstates;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    const size_t cap = (size_t)device_sms() * 16;
-    if (blocks > cap) blocks = cap;
-    b2d_state_tables_kernel<<<(int)blocks, 256, 0, stream>>>(src, d_states, words, nstates, d_arena, layout);
     return cudaGetLastError();
 }
 

@@ -54,8 +54,9 @@ struct StateTables {
     uint32_t slot_bytes, off_sectors, off_segs, off_sprites, off_mids, pad;
 };
 
-// The five state-dependent tables of one frame of a batch with per-frame states and levels: an expanded table set of the
-// frame's level in the state arena, or, on a level without time-dependent content or dynamic sectors, its blob tables.
+// The five state-dependent tables of one level at one state: an expanded table set (in a state arena, or a level's own set of
+// a worklist slot), or, on a level without time-dependent content or dynamic sectors, its blob tables.  What a frame of a
+// batch with per-frame states and levels reads, and where launch_state_sets writes.
 struct TableSet {
     const TexRec *tex;
     const SectorRec *sectors;
@@ -75,9 +76,9 @@ struct LevelTables {
     const TableSet *sets;
 };
 
-// One table set to expand in a batch with per-frame states and levels (launch_state_sets): level `level`'s rule at the
-// compact state at word `state` of the batch's states, into the tables of TableSet `set`.  `first`: the set's first record
-// in the expansion's numbering of all records of the batch (the record counts of the sets before it, summed).
+// One table set to expand (launch_state_sets): level `level`'s rule at the compact state at word `state` of the launch's
+// states, into the tables of its TableSet.  `first`: the set's first record in the launch's numbering of all its records
+// (the record counts of the sets before it, summed).
 struct StateSet {
     uint32_t level, state, first, pad;
 };
@@ -89,46 +90,33 @@ size_t walk_smem_per_warp(const DeviceScene &sc);
 size_t walk_levels_static_smem();
 constexpr size_t kWalkSmemMax = 227 * 1024;      // the largest shared-memory opt-in per block on sm_90a
 
-// Kernel 1: front-to-back BSP walk, one CTA per frame.  Writes frames[i] and up to `stride`
-// worklist entries per frame at work[i*stride ...].
-// `states` (nullable): per-frame tables.
-cudaError_t launch_walk(const DeviceScene &sc, const View &vw, const Pose *d_poses, int n,
-                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background = false,
-                        const StateTables *states = nullptr);
+// The tables a batch's walk and raster read, and which of their <kStates, kLevels> variants runs.  Without per-frame levels
+// every frame reads `scene` (level 0 as the batch's worklist slot reads it); with them, the scenes of `levels` (and `scene`
+// is not read).  With per-frame states the five state-dependent tables come from `states` (level 0's slot layout; with
+// per-frame levels, only its frame_slot is read, into `levels.sets`).
+struct BatchTables {
+    DeviceScene scene;
+    StateTables states;
+    LevelTables levels;
+    bool per_frame, per_level;
+};
 
-// Kernel 2: wall-column / flat-span / sky rasteriser, one warp per (frame, 32-column strip).
-// Writes every pixel of d_index_fb exactly once; if d_rgba != nullptr also the palette-mapped RGBA8.
-// `states` (nullable): per-frame tables, the arena the walk of these frames read.
-cudaError_t launch_raster(const DeviceScene &sc, const View &vw, const FrameConst *d_frames,
-                          const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb,
-                          uint32_t *d_rgba, cudaStream_t stream, const StateTables *states = nullptr);
+// Kernel 1: front-to-back BSP walk, one CTA per frame.  Writes frames[i] and up to `stride` worklist entries per frame at
+// work[i*stride ...].  `levels_smem`: with per-frame levels, the largest walk_smem_per_warp of the levels.
+cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw, const Pose *d_poses, int n,
+                        FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background);
 
-// The walk and the raster of a batch with per-frame levels.  `smem`: the largest walk_smem_per_warp of the levels;
-// `masked`: some level has masked content (its masked_list is set).  Everything else as launch_walk / launch_raster.
-cudaError_t launch_walk_levels(const LevelTables &levels, size_t smem, const View &vw, const Pose *d_poses, int n,
-                               FrameConst *d_frames, SegFrame *d_work, int stride, cudaStream_t stream, bool background);
-cudaError_t launch_raster_levels(const LevelTables &levels, bool masked, const View &vw, const FrameConst *d_frames,
-                                 const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
-                                 cudaStream_t stream);
+// Kernel 2: wall-column / flat-span / sky rasteriser, one warp per (frame, 32-column strip), of the frames a walk of the same
+// tables wrote.  Writes every pixel of d_index_fb exactly once; if d_rgba != nullptr also the palette-mapped RGBA8.
+// `masked`: some level the frames read has masked content (its masked_list is set).
+cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
+                          int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream);
 
-// The walk and the raster of a batch with per-frame states and levels: `levels.sets` and `states.frame_slot` set, as above.
-cudaError_t launch_walk_levels_states(const LevelTables &levels, const StateTables &states, size_t smem, const View &vw,
-                                      const Pose *d_poses, int n, FrameConst *d_frames, SegFrame *d_work, int stride,
-                                      cudaStream_t stream, bool background);
-cudaError_t launch_raster_levels_states(const LevelTables &levels, const StateTables &states, bool masked, const View &vw,
-                                        const FrameConst *d_frames, const SegFrame *d_work, int stride, int n,
-                                        uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream);
-
-// Expands the `nsets` table sets of a batch with per-frame states and levels in one grid: set k by the rule of level
-// sets[k].level (srcs[level]: device pointers to that level's rest-state sections) into the tables of out[k].  `records`:
-// the records of all sets together (sets[k].first counts them up).
+// Expands the `nsets` table sets of a batch in one grid: set k by the rule of level sets[k].level (srcs[level]: device
+// pointers to that level's rest-state sections) into the tables of out[k].  `records`: the records of all sets together
+// (sets[k].first counts them up).
 cudaError_t launch_state_sets(const StateSrc *d_srcs, const StateSet *d_sets, const TableSet *d_out, const uint32_t *d_states,
                               int nsets, uint32_t records, cudaStream_t stream);
-
-// Expands `nstates` compact states (StateLayout::words words each, b2d_scene.hpp) from `src` (device pointers to the
-// rest-state sections) into slots 0 .. nstates-1 of `arena`: one thread per output record.
-cudaError_t launch_state_tables(const StateSrc &src, const uint32_t *d_states, uint32_t words, int nstates, uint8_t *d_arena,
-                                const StateTables &layout, cudaStream_t stream);
 
 // Pre-light kernels (once per renderer).  Flats: dst[r * stride + i] = colormap[r][src[i]] for r < 32, i < n.
 cudaError_t launch_prelight(const uint8_t *d_colormap, const uint8_t *d_src, uint8_t *d_dst, size_t n, size_t stride,

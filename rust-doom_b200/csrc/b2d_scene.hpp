@@ -128,7 +128,7 @@ inline bool scene_is_timed(const uint8_t *blob) {
 }
 
 // ---- The state rule: one record of the state-dependent tables at one state -------------------------------------------
-// The same functions run on the host (scene_at_time, for b2d_scene_tables_at) and on the device (b2d_state_tables_kernel,
+// The same functions run on the host (scene_at_time, for b2d_scene_tables_at) and on the device (b2d_state_sets_kernel,
 // one thread per record, for every state a renderer draws: its own and per-frame states).
 //
 // A *compact state* holds only what the tables depend on, as 32-bit words (StateLayout::words of them):

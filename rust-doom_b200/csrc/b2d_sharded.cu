@@ -20,7 +20,6 @@
 
 #include <algorithm>
 #include <cstring>
-#include <functional>
 #include <mutex>
 #include <vector>
 
@@ -383,9 +382,6 @@ int b2d_frame_checksums_device(const uint8_t *d_frames, size_t n_frames, size_t 
 
 namespace {
 
-// the walk of one chunk of a sharded call: local poses [first, first + n) of the rank's block, at d_poses
-using ChunkWalk = std::function<int(const Pose *d_poses, size_t first, int n, cudaStream_t stream, int64_t *ticket_out)>;
-
 int check_sharded(const b2d_renderer *r, const b2d_comm *c, const b2d_pose *poses, int mode) {
     if (!r || !c || !poses) return b2d::fail(B2D_ERR_INVALID_ARG, "null argument");
     if (mode < B2D_SHARD_RENDER_ONLY || mode > B2D_SHARD_GATHER_ONLY) return b2d::fail(B2D_ERR_INVALID_ARG, "unknown mode");
@@ -402,13 +398,13 @@ struct ShardResolve {
 };
 
 // The chunk loop of the sharded calls, after their arguments have been checked (check_sharded and the caller's checks of
-// the whole job: a rank that refused its input here would leave its peers waiting in a collective).  `walk` enqueues the
-// BSP walk of local poses [first, first + n) of this rank's padded block, read from d_poses, as a background grid on
-// `stream` and returns its ticket.  With `res` (nullable) each chunk is rastered into the comm's index staging and
+// the whole job: a rank that refused its input here would leave its peers waiting in a collective).  `block`: the frames
+// of this rank's padded block (its poses are padded here the same way); each chunk of it is walked as a background grid
+// on the walk stream.  With `res` (nullable) each chunk is rastered into the comm's index staging and
 // resolved from there into this rank's slice of the exchange buffer, on the render stream: the raster of chunk k+1 follows
 // the resolve of chunk k there, so one staging buffer serves every chunk.  Without it, chunks are rastered into the slice.
 int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames, int mode, b2d_chunk_fn fn,
-                 void *user, b2d_sharded_stats *stats_out, const ChunkWalk &walk, const ShardResolve *res = nullptr) {
+                 void *user, b2d_sharded_stats *stats_out, const Frames &block, const ShardResolve *res = nullptr) {
     B2D_CU(cudaSetDevice(c->device));
     Nccl &n = nccl();
     const size_t world = (size_t)c->world, rank = (size_t)c->rank;
@@ -462,10 +458,14 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
         d_levels = c->d_levels.get();
     }
     // the BSP walk of chunk k+1 runs as a background grid on its own stream under the raster of chunk k
-    auto chunk_count = [&](size_t k) { const size_t f = k * chunk; return (per - f) < chunk ? (per - f) : chunk; };
+    auto walk = [&](size_t k, int64_t *ticket) {
+        const size_t f = k * chunk;
+        return b2d::walk_batch(r, c->d_poses.get() + f, block.from(f), (int)((per - f) < chunk ? (per - f) : chunk), walk_stream,
+                               true, ticket);
+    };
     int64_t ticket = -1;
     if (do_render) {
-        int wrc = walk(c->d_poses.get(), 0, (int)chunk_count(0), walk_stream, &ticket);
+        int wrc = walk(0, &ticket);
         if (wrc != B2D_OK) return wrc;
     }
 
@@ -492,7 +492,7 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
         if (k >= 2) B2D_CU(cudaStreamWaitEvent(render_stream, consumed[b].get(), 0));     // chunk k-2 has left this buffer
         B2D_CU(cudaEventRecord(rt[2 * k].get(), render_stream));
         if (do_render) {
-            result = b2d::raster_frames(r, ticket, do_resolve ? c->d_stage.get() : slice, nullptr, render_stream);
+            result = b2d::raster_batch(r, ticket, do_resolve ? c->d_stage.get() : slice, nullptr, render_stream);
             if (result != B2D_OK) break;
             if (do_resolve) {
                 B2D_CU(launch_resolve(r->d_palettes.get(), d_levels ? d_levels + first : nullptr, c->d_stage.get(), slice, cnt,
@@ -500,7 +500,7 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
                 r->launches += 1;
             }
             if (k + 1 < nchunks) {
-                result = walk(c->d_poses.get() + (k + 1) * chunk, (k + 1) * chunk, (int)chunk_count(k + 1), walk_stream, &ticket);
+                result = walk(k + 1, &ticket);
                 if (result != B2D_OK) break;
             }
         }
@@ -559,10 +559,7 @@ int render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n
     int rc = check_sharded(r, c, poses, mode);
     if (rc == B2D_OK && res) rc = b2d_resolve_frame_bytes(r, res->factor, res->format, &res->frame_bytes);
     if (rc != B2D_OK || n_total == 0) return rc;
-    return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
-                        [r](const Pose *d_poses, size_t, int n, cudaStream_t stream, int64_t *ticket) {
-                            return b2d::walk_frames(r, d_poses, n, stream, ticket, true);
-                        }, res);
+    return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out, Frames{}, res);
 }
 
 int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
@@ -576,10 +573,12 @@ int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *p
     // then refuses the same input, before any collective
     std::vector<uint32_t> fs;
     std::vector<size_t> starts;
-    rc = b2d::build_levels_states(r, levels, states, n_total, moves, n_moves, fs, starts);
+    Frames all{levels};
+    rc = b2d::check_levels(r, levels, n_total);
+    if (rc == B2D_OK) rc = b2d::build_states(r, states, nullptr, n_total, moves, n_moves, fs, starts, all);
     if (rc != B2D_OK || n_total == 0) return rc;
     // this rank's block, padded like its poses by repeating the last entry (level and state with it); its states stay
-    // where build_levels_states put them
+    // where build_states put them
     const size_t world = (size_t)c->world, rank = (size_t)c->rank, per = (n_total + world - 1) / world;
     std::vector<uint32_t> block_levels(per);
     std::vector<size_t> block_starts(per);
@@ -590,10 +589,7 @@ int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *p
     }
     if (res) res->block_levels = block_levels.data();
     return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
-                        [&](const Pose *d_poses, size_t first, int n, cudaStream_t stream, int64_t *ticket) {
-                            return b2d::walk_levels_states_frames(r, d_poses, block_levels.data() + first, fs.data(),
-                                                                  block_starts.data() + first, n, stream, ticket, true);
-                        }, res);
+                        Frames{block_levels.data(), fs.data(), block_starts.data()}, res);
 }
 
 }  // namespace

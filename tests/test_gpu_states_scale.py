@@ -1,5 +1,5 @@
 """-m gpu: per-frame states at the benchmark's batch sizes.  1000-frame 1080p batches pipelined the way bench.py and
-tools/timeline_bench.py run them, with enough distinct states that b2d_state_tables_kernel's grid-stride loop takes more
+tools/timeline_bench.py run them, with enough distinct states that b2d_state_sets_kernel's grid-stride loop takes more
 than one pass; and worklist slots that hold plain and per-frame batches in turn.  Every frame is compared with the oracle
 at its own state, and every expanded table set, read back, with oracle/scene.py tables_at."""
 import numpy as np
@@ -67,7 +67,7 @@ def test_states_pipelined_1000_frame_batches_rich_level(b2d):
     dps = [_dev_poses(p) for p, _, _ in batches]
     outs = [torch.empty((N, HEIGHT, WIDTH), dtype=torch.uint8, device="cuda") for _ in batches]
     s_walk, s_r = torch.cuda.Stream(priority=-1), (torch.cuda.Stream(), torch.cuda.Stream())
-    threads = _sms() * 16 * 256                                     # launch_state_tables' grid cap
+    threads = _sms() * 16 * 256                                     # launch_state_sets' grid cap
     torch.cuda.synchronize()
 
     def walk(k):
