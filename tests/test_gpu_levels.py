@@ -33,7 +33,12 @@ def _other_palette(data: bytes) -> bytes:
 
 @pytest.fixture(scope="module")
 def levels(b2d):
-    """[{scene, blob (oracle), level, dyn, data}] of the four levels; RICH declares dynamic sectors (refcheck moves.pick)"""
+    return make_levels(b2d)
+
+
+def make_levels(b2d):
+    """[{scene, blob (oracle), data, dyn}] of the four levels; RICH declares dynamic sectors (refcheck moves.pick) and
+    carries one moved state of them (moves)"""
     from oracle import scene as S, wad as W
     from rust_doom_b200 import synthwad
     from tests.refcheck import moves as MV
