@@ -161,6 +161,19 @@ int b2d_scene_tables_at(const b2d_scene *s, uint32_t tics, const b2d_sector_move
                         size_t capacity, size_t *size_out);
 
 int b2d_scene_info_get(const b2d_scene *s, b2d_scene_info *out);
+/* The palettes a scene holds for the resolve's per-frame palettes (b2d_resolve_palettes_device): PLAYPAL's 14 in Doom --
+ * 0 normal, 1..8 the red damage flash, 9..12 the yellow bonus-pickup flash, 13 the radiation suit's green (the reference
+ * exposes them as TextureDirectory::palette(i), wad/src/tex.rs:126; its renderer uses palette 0 only).  An archive scene
+ * keeps every PLAYPAL entry; a scene from lumps keeps the one palette it was made with (768 zero bytes without one).  The
+ * blob holds palette 0 only and does not change.
+ * b2d_scene_num_palettes: the number of palettes, 1 or more (B2D_ERR_INVALID_ARG for a NULL scene).
+ * b2d_scene_set_palettes: gives a scene the whole PLAYPAL, n_palettes x 768 bytes (R, G, B per entry), copied -- what a
+ * host that built the scene from lumps has from TextureDirectory::palette(i).  Palette 0 must be byte-equal to the palette
+ * the scene holds now, so nothing the scene renders changes; a NULL argument, n_palettes = 0 and a different palette 0 are
+ * B2D_ERR_INVALID_ARG and leave the scene as it was.  Renderers copy a scene's palettes when they are created: a later
+ * call changes no existing renderer. */
+int b2d_scene_num_palettes(const b2d_scene *s);
+int b2d_scene_set_palettes(b2d_scene *s, const uint8_t *playpal, size_t n_palettes);
 /* Read-only access to the compiled "B2DS" blob (layout in DESIGN.md); valid until destroy. */
 const void *b2d_scene_blob(const b2d_scene *s, size_t *size_out);
 /* LevelWalker::sector_at (visitor.rs:1028-1060): sector id at a map position, -1 if outside. */
@@ -205,7 +218,8 @@ int b2d_renderer_status(b2d_renderer *r, int32_t *bits_out);
 
 /* End-to-end: HOST poses in, HOST frames out (pinned staging + copies inside).  index_fb gets
  * n*W*H palette indices, row-major, top row first; rgba_fb (nullable) gets n*W*H RGBA8
- * (R in the low byte).  n may exceed max_batch; it is processed in batches. */
+ * (R in the low byte), always through palette 0 of the frame's level (tints: b2d_resolve_palettes_device).  n may exceed
+ * max_batch; it is processed in batches. */
 int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_fb, uint32_t *rgba_fb);
 
 /* Per-frame state: every pose carries its own level time and state of the moving sectors (a demo replay, a recorded
@@ -377,6 +391,18 @@ int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *
                        int format, void *d_out, void *cuda_stream);
 int b2d_resolve_frame_bytes(const b2d_renderer *r, int factor, int format, size_t *bytes_out);
 
+/* b2d_resolve_device with a palette per frame: frame f goes through palette palettes[f] of level levels[f] (DESIGN.md
+ * C17: table T_{l,p}) -- Doom's damage, bonus and radiation-suit tints, picked per frame by the host from the player's
+ * state as ST_doPaletteStuff does.  `palettes` is a HOST array, or NULL for palette 0 on every frame; `levels` as in
+ * b2d_resolve_device.  Frames on palette 0 are byte-identical to b2d_resolve_device's, and factor 1 with
+ * B2D_RESOLVE_RGBA8 is the per-frame-palette form of b2d_palette_lut_levels_device.  Each renderer holds every palette its
+ * scenes had when it was created (b2d_scene_num_palettes) in one colour table; a frame's table index, the only per-frame
+ * input of the kernel, is staged as b2d_resolve_device stages its levels, through the same pinned memory and with the
+ * same waits (nothing is staged when both arrays are NULL).  A palette >= the palette count of its frame's level, and
+ * every refusal of b2d_resolve_device, are B2D_ERR_INVALID_ARG, detected before anything is enqueued. */
+int b2d_resolve_palettes_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, const uint32_t *palettes,
+                                size_t n_frames, int factor, int format, void *d_out, void *cuda_stream);
+
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
  * per-frame `frame.finish()` of engine/src/renderer.rs:160-167.  One process per GPU.  NCCL (libnccl.so.2) is bound
@@ -464,6 +490,19 @@ int b2d_render_sharded_levels_states_resolved(b2d_renderer *r, b2d_comm *c, cons
                                               const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves,
                                               size_t n_moves, size_t chunk_frames, int factor, int format, int mode,
                                               b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out);
+/* b2d_render_sharded_levels_states_resolved with a palette per pose: `palettes` (HOST, the same whole-job list on every
+ * rank; NULL = palette 0 everywhere, which is the call without palettes) next to `levels` and `states`.  Frame j of rank q
+ * in a gathered chunk is byte-identical to b2d_resolve_palettes_device applied to the index frame the unresolved call
+ * gathers there, with that pose's level and palette; a short last block repeats the last pose's palette too.  A palette
+ * >= the palette count of its pose's level, anywhere in the job, is refused with the other whole-job checks, before any
+ * collective or launch, so every rank returns the same B2D_ERR_INVALID_ARG.  For tints on one level, pass a level set
+ * of one; b2d_render_sharded_resolved has no palette form. */
+int b2d_render_sharded_levels_states_resolved_palettes(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses,
+                                                       const uint32_t *levels, const uint32_t *palettes,
+                                                       const b2d_frame_state *states, size_t n_total,
+                                                       const b2d_sector_move *moves, size_t n_moves, size_t chunk_frames,
+                                                       int factor, int format, int mode, b2d_chunk_fn fn, void *user,
+                                                       b2d_sharded_stats *stats_out);
 
 /* One 32-bit checksum per frame on the device: sum_i (p[i] + 1) * (i * 0x9E3779B1 + 0x7F4A7C15) mod 2^32
  * (position sensitive, order independent).  Used to validate gathered frames without moving them to the host. */

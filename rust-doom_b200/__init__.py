@@ -196,6 +196,20 @@ class Scene:
         del keep
         return cls(None, 0, _handle=h)
 
+    @property
+    def num_palettes(self) -> int:
+        """b2d_scene_num_palettes: the palettes the scene holds for per-frame palettes (14 for Doom's PLAYPAL)."""
+        return _check(_lib.load().b2d_scene_num_palettes(self._h))
+
+    def set_palettes(self, playpal: bytes):
+        """b2d_scene_set_palettes: give a scene built from lumps the whole PLAYPAL (n x 768 bytes, n >= 1), whose palette 0
+        must equal the one the scene was made with.  Renderers created afterwards see the palettes; existing ones do not."""
+        raw = bytes(playpal)
+        if not raw or len(raw) % 768:
+            raise ValueError("a PLAYPAL is a positive multiple of 768 bytes")
+        buf = ctypes.create_string_buffer(raw, len(raw))
+        _check(_lib.load().b2d_scene_set_palettes(self._h, buf, len(raw) // 768))
+
     def tables_at(self, tics: int = 0, moves=()) -> bytes:
         """b2d_scene_tables_at: the state-dependent tables [textures | sectors | segs | sprites | mids] at level time `tics`
         with `moves` = (sector, floor_offset, ceil_offset) applied (host only)."""
@@ -312,6 +326,11 @@ def _levels_array(levels, n: int) -> np.ndarray:
     lv = np.asarray(levels, dtype=np.int64).reshape(-1)
     assert lv.shape == (n,), "one level per pose"
     return np.ascontiguousarray(lv & 0xFFFFFFFF, dtype=np.uint32)
+
+
+def _palettes_array(palettes, n: int) -> Optional[np.ndarray]:
+    """the uint32 palette array of n frames, or None (palette 0 everywhere); the library refuses a palette out of range"""
+    return None if palettes is None else _levels_array(palettes, n)
 
 
 def _chunk_fn(on_chunk):
@@ -528,13 +547,20 @@ class Renderer:
         lv = _levels_array(levels, n_frames)
         _check(_lib.load().b2d_palette_lut_levels_device(self._h, index_ptr, lv.ctypes.data, n_frames, rgba_ptr, stream or None))
 
-    def resolve_device(self, index_ptr: int, n: int, factor: int, fmt: int, out_ptr: int, levels=None, stream: int = 0):
+    def resolve_device(self, index_ptr: int, n: int, factor: int, fmt: int, out_ptr: int, levels=None, stream: int = 0,
+                       palettes=None):
         """b2d_resolve_device: frame f of the n contiguous index frames at index_ptr, box-filtered by `factor` (1..8, dividing
         the view's sides) through the palette of level levels[f] (host list; None = level 0) into out_ptr in format `fmt`
-        (RESOLVE_RGBA8 / RESOLVE_RGB8 / RESOLVE_RGB8_PLANAR / RESOLVE_GRAY8; device pointers)."""
+        (RESOLVE_RGBA8 / RESOLVE_RGB8 / RESOLVE_RGB8_PLANAR / RESOLVE_GRAY8; device pointers).  palettes[f] (host list):
+        b2d_resolve_palettes_device, frame f through palette palettes[f] of its level (None = palette 0)."""
         lv = None if levels is None else _levels_array(levels, n)
-        _check(_lib.load().b2d_resolve_device(self._h, index_ptr, None if lv is None else lv.ctypes.data, n, int(factor), int(fmt),
-                                              out_ptr, stream or None))
+        pv = _palettes_array(palettes, n)
+        if pv is None:
+            _check(_lib.load().b2d_resolve_device(self._h, index_ptr, None if lv is None else lv.ctypes.data, n, int(factor),
+                                                  int(fmt), out_ptr, stream or None))
+        else:
+            _check(_lib.load().b2d_resolve_palettes_device(self._h, index_ptr, None if lv is None else lv.ctypes.data,
+                                                           pv.ctypes.data, n, int(factor), int(fmt), out_ptr, stream or None))
 
     def resolve_frame_bytes(self, factor: int, fmt: int) -> int:
         """b2d_resolve_frame_bytes: bytes of one resolved frame."""
@@ -542,10 +568,10 @@ class Renderer:
         _check(_lib.load().b2d_resolve_frame_bytes(self._h, int(factor), int(fmt), ctypes.byref(out)))
         return int(out.value)
 
-    def resolve(self, index, factor: int = 2, fmt: str = "rgb_planar", levels=None):
+    def resolve(self, index, factor: int = 2, fmt: str = "rgb_planar", levels=None, palettes=None):
         """The resolve of a CUDA uint8 tensor [n, H, W] of index frames into a new CUDA tensor, on the current torch stream:
         fmt "rgba" -> int32 [n, H/k, W/k] (RGBA8 words), "rgb" -> uint8 [n, H/k, W/k, 3], "rgb_planar" -> uint8
-        [n, 3, H/k, W/k], "gray" -> uint8 [n, H/k, W/k]; `levels` as in resolve_device."""
+        [n, 3, H/k, W/k], "gray" -> uint8 [n, H/k, W/k]; `levels` and `palettes` as in resolve_device."""
         import torch
         code = RESOLVE_FORMATS[fmt]
         if not (index.is_cuda and index.dtype == torch.uint8 and index.dim() == 3 and tuple(index.shape[1:]) == (self.height, self.width)):
@@ -558,7 +584,7 @@ class Renderer:
         out = torch.empty(shape, dtype=torch.int32 if code == _lib.RESOLVE_RGBA8 else torch.uint8, device=index.device)
         with torch.cuda.device(index.device):
             stream = torch.cuda.current_stream().cuda_stream
-        self.resolve_device(index.data_ptr(), n, k, code, out.data_ptr(), levels, stream)
+        self.resolve_device(index.data_ptr(), n, k, code, out.data_ptr(), levels, stream, palettes)
         return out
 
     def worklist(self, n: int):
@@ -618,17 +644,27 @@ class Renderer:
 
     def render_sharded_levels_states(self, comm: "Comm", poses: np.ndarray, levels, tics, moves_per_pose=None,
                                      chunk_frames: int = 256, mode: int = _lib.SHARD_RENDER_GATHER, on_chunk=None,
-                                     resolve=None) -> dict:
+                                     resolve=None, palettes=None) -> dict:
         """b2d_render_sharded_levels_states: render_sharded over the renderer's level set, pose i rendered from level
         levels[i] at level time tics[i] with the sector moves moves_per_pose[i] of that level (None = every pose at rest),
         as render_levels_states renders it.  The whole job's lists, identical on every rank.  resolve=(factor, fmt):
-        b2d_render_sharded_levels_states_resolved, as in render_sharded, each frame through its own level's palette."""
+        b2d_render_sharded_levels_states_resolved, as in render_sharded, each frame through its own level's palette.
+        palettes (with resolve only): b2d_render_sharded_levels_states_resolved_palettes, pose i through palette
+        palettes[i] of its level."""
+        if palettes is not None and resolve is None:
+            raise ValueError("palettes= colours resolved frames: pass resolve=(factor, fmt) with it")
         poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
         n = len(poses)
         lv = _levels_array(levels, n)
+        pv = _palettes_array(palettes, n)
         states, arr, nm = _frame_states(tics, moves_per_pose, n)
         st = _lib.ShardedStats()
-        if resolve is None:
+        if pv is not None:
+            factor, fmt = resolve
+            _check(_lib.load().b2d_render_sharded_levels_states_resolved_palettes(
+                self._h, comm._h, poses.ctypes.data, lv.ctypes.data, pv.ctypes.data, states, n, arr, nm, int(chunk_frames),
+                int(factor), RESOLVE_FORMATS[fmt], int(mode), _chunk_fn(on_chunk), None, ctypes.byref(st)))
+        elif resolve is None:
             _check(_lib.load().b2d_render_sharded_levels_states(self._h, comm._h, poses.ctypes.data, lv.ctypes.data, states, n, arr,
                                                                 nm, int(chunk_frames), int(mode), _chunk_fn(on_chunk), None,
                                                                 ctypes.byref(st)))

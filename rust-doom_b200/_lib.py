@@ -57,6 +57,8 @@ EXPORTS = [
     "b2d_render_sharded_levels_states", "b2d_palette_lut_levels_device",
     "b2d_frame_checksums_device", "b2d_device_alloc", "b2d_device_free", "b2d_device_upload", "b2d_device_download",
     "b2d_resolve_device", "b2d_resolve_frame_bytes", "b2d_render_sharded_resolved", "b2d_render_sharded_levels_states_resolved",
+    "b2d_scene_num_palettes", "b2d_scene_set_palettes", "b2d_resolve_palettes_device",
+    "b2d_render_sharded_levels_states_resolved_palettes",
 ]
 
 COMM_ID_BYTES = 128
@@ -195,5 +197,11 @@ def load() -> ctypes.CDLL:
     L.b2d_render_sharded_resolved.argtypes = [vp, vp, vp, cs, cs, ci, ci, ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
     L.b2d_render_sharded_levels_states_resolved.argtypes = [vp, vp, vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove),
                                                             cs, cs, ci, ci, ci, CHUNK_FN, vp, ctypes.POINTER(ShardedStats)]
+    L.b2d_scene_num_palettes.argtypes = [vp]
+    L.b2d_scene_set_palettes.argtypes = [vp, vp, cs]
+    L.b2d_resolve_palettes_device.argtypes = [vp, vp, vp, vp, cs, ci, ci, vp, vp]
+    L.b2d_render_sharded_levels_states_resolved_palettes.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(FrameState), cs,
+                                                                     ctypes.POINTER(SectorMove), cs, cs, ci, ci, ci, CHUNK_FN, vp,
+                                                                     ctypes.POINTER(ShardedStats)]
     _lib = L
     return L

@@ -1,7 +1,7 @@
 """`b2d` command line, mirroring rs_doom's flags (reference src/main.rs:17-80,89-124):
 
     python -m rust_doom_b200.cli --iwad doom1.wad --level 0 --resolution 1920x1080 [--fov 65]
-                                 [--poses N] [--dump frame.ppm] [--device 0] [--supersample K]
+                                 [--poses N] [--dump frame.ppm] [--device 0] [--supersample K] [--palette P]
     python -m rust_doom_b200.cli --iwad doom1.wad --levels 0,2,5 --poses N [--tics T] [--dump f.ppm] [--stream s.ppm]
                                  [--world W --rank R --id-file PATH [--chunk C]]
     python -m rust_doom_b200.cli --iwad doom1.wad list-levels
@@ -21,7 +21,11 @@ to --id-file, the others read it) and rank 0 colours every gathered frame with i
 --supersample K (1..8) renders every frame at K times the resolution with the same field of view and resolves each K x K
 block to one pixel of the --resolution frame on the device (b2d_resolve_device, C17: the half-up rounded mean of the
 block's palette colours, each frame through its own level's palette): an anti-aliased --dump and --stream.  Not with
---world."""
+--world.
+
+--palette P colours the dumped and streamed frames through PLAYPAL palette P of each frame's level instead of palette 0
+(b2d_resolve_palettes_device; in Doom 1..8 are the damage flash, 9..12 the bonus flash, 13 the radiation suit), through
+the resolve at the --supersample factor (1 by default).  With --levels too; not with --world."""
 from __future__ import annotations
 
 import argparse
@@ -133,12 +137,23 @@ def _write_image(path: str, rgb: np.ndarray):
         f.write(encode_png(rgb) if path.lower().endswith(".png") else encode_ppm(rgb))
 
 
-def resolve_rgb(r, index: np.ndarray, factor: int, levels=None) -> np.ndarray:
-    """(n, H, W, 3) uint8: the host index frames of renderer r resolved by `factor` on its device (b2d_resolve_device)"""
+def resolve_rgb(r, index: np.ndarray, factor: int, levels=None, palette: int = 0) -> np.ndarray:
+    """(n, H, W, 3) uint8: the host index frames of renderer r resolved by `factor` on its device through palette `palette`
+    of each frame's level (b2d_resolve_device, b2d_resolve_palettes_device)"""
     import torch
     dev = torch.device("cuda", r.device)
+    palettes = [palette] * len(index) if palette else None
     with torch.cuda.device(dev):
-        return r.resolve(torch.from_numpy(np.ascontiguousarray(index)).to(dev), factor, "rgb", levels).cpu().numpy()
+        return r.resolve(torch.from_numpy(np.ascontiguousarray(index)).to(dev), factor, "rgb", levels, palettes).cpu().numpy()
+
+
+def _palette_out_of_range(scenes, palette: int) -> bool:
+    """--palette: P at or past a scene's palette count is a usage error, reported here"""
+    n = min(sc.num_palettes for sc in scenes)
+    if palette < n:
+        return False
+    print("--palette takes a palette index below %d" % n, file=sys.stderr)
+    return True
 
 
 def _comm_from_file(b2d, id_file: str, rank: int, world: int):
@@ -161,14 +176,17 @@ def _main_levels(b2d, arch, set_, view, args, w, h) -> int:
     if any(sc.start_pose is None for sc in scenes):
         print("Fatal error: a level has no player-1 start", file=sys.stderr)
         return 1
+    if _palette_out_of_range(scenes, args.palette):
+        return 2
     per_level = max(args.poses, 1)
     poses, levels, tics = level_set_job(b2d, scenes, per_level, args.tics)
     n = len(poses)
     if not args.world:
         r = b2d.Renderer.from_levels(scenes, view, device=args.device, max_batch=min(n, 64))
-        if args.supersample > 1:
-            rgb = resolve_rgb(r, r.render_levels_states(poses, levels, tics), args.supersample, levels)
-            print("rendered %d frame(s) %dx%d of %d level(s), supersampled %dx" % (n, w, h, len(set_), args.supersample))
+        if args.supersample > 1 or args.palette:
+            rgb = resolve_rgb(r, r.render_levels_states(poses, levels, tics), args.supersample, levels, args.palette)
+            print("rendered %d frame(s) %dx%d of %d level(s), supersampled %dx, palette %d" % (n, w, h, len(set_), args.supersample,
+                                                                                             args.palette))
             frame = lambda i: rgb[i]    # noqa: E731
         else:
             rgba = r.render_levels_states(poses, levels, tics, rgba=True)[1]
@@ -256,6 +274,8 @@ def main(argv=None) -> int:
     ap.add_argument("--chunk", type=int, default=16, help="with --world: frames per rank and chunk")
     ap.add_argument("--supersample", type=int, default=1,
                     help="render at K times the resolution (1..8) and resolve every K x K block to one output pixel")
+    ap.add_argument("--palette", type=int, default=0,
+                    help="colour the frames through PLAYPAL palette P (Doom: 1..8 damage, 9..12 bonus, 13 radiation suit)")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 
@@ -270,6 +290,12 @@ def main(argv=None) -> int:
         return 2
     if ss > 1 and (args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1):
         print("--supersample does not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
+        return 2
+    if args.palette < 0:
+        print("--palette takes a palette index", file=sys.stderr)
+        return 2
+    if args.palette and (args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        print("--palette does not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
         return 2
     try:
         arch = b2d.Archive.open(args.iwad) if args.iwad else b2d.Archive.from_bytes(synthwad.build_iwad(1, synthwad.E1_MAPS[:3]))
@@ -297,6 +323,8 @@ def main(argv=None) -> int:
             print("--world takes --levels (a single level shards under torchrun)", file=sys.stderr)
             return 2
         scene = b2d.Scene(arch, args.level)
+        if _palette_out_of_range([scene], args.palette):
+            return 2
         view = b2d.make_view(ss * w, ss * h, args.fov)
         if args.poses <= 1:
             poses = scene.start_pose if scene.start_pose is not None else P.random_poses(scene, 1, 1)
@@ -307,7 +335,7 @@ def main(argv=None) -> int:
             return _main_sharded(b2d, scene, view, poses, args, w, h, world)
         r = b2d.Renderer(scene, view, device=args.device, max_batch=min(len(poses), 256))
         t0 = time.perf_counter()
-        if ss > 1:
+        if ss > 1 or args.palette:
             index = np.empty((len(poses), ss * h, ss * w), dtype=np.uint8)
             if args.tics_per_frame > 0:
                 for i in range(len(poses)):
@@ -315,7 +343,7 @@ def main(argv=None) -> int:
                     index[i] = r.render(poses[i:i + 1])[0]
             else:
                 r.render(poses, out_index=index)
-            rgb = resolve_rgb(r, index, ss)
+            rgb = resolve_rgb(r, index, ss, palette=args.palette)
             frame = lambda i: rgb[i]    # noqa: E731
         elif args.tics_per_frame > 0:          # time is a per-batch input: one batch per frame
             rgba = np.empty((len(poses), h, w), dtype=np.uint32)
@@ -324,7 +352,7 @@ def main(argv=None) -> int:
                 rgba[i] = r.render(poses[i:i + 1], rgba=True)[1][0]
         else:
             rgba = r.render(poses, rgba=True)[1]
-        if ss == 1:
+        if ss == 1 and not args.palette:
             frame = lambda i: rgba_to_rgb(rgba[i])    # noqa: E731
         dt = time.perf_counter() - t0
         print("rendered %d frame(s) %dx%d in %.2f ms (%.0f frames/s end to end)" % (len(poses), w, h, dt * 1e3, len(poses) / dt))

@@ -307,6 +307,14 @@ int b2d::check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
     return B2D_OK;
 }
 
+int b2d::check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n) {
+    if (palettes)
+        for (size_t i = 0; i < n; i++)
+            if (palettes[i] >= r->pal_count[levels ? levels[i] : 0u])
+                return fail(B2D_ERR_INVALID_ARG, "frame palette out of range (>= the palette count of the frame's level)");
+    return B2D_OK;
+}
+
 int b2d::check_slots_free(const b2d_renderer *r, size_t batches) {
     for (size_t k = 0; k < batches && k < 2; k++)
         if (!r->slot[(r->next_ticket + (int64_t)k) & 1].rastered)
@@ -618,6 +626,8 @@ int b2d_scene_create_dynamic(const b2d_archive *a, int level_index, const b2d_dy
         s->level = Level::load(*a->wad, level_index);
         s->blob = compile_scene(s->level, td, dyn_list(dyn, n_dyn));
         fill_scene_info(s.get());
+        s->palettes = td.palettes;
+        if (s->palettes.empty()) s->palettes.push_back({});
         *out = s.release();
         return B2D_OK;
     });
@@ -685,7 +695,26 @@ int b2d_scene_create_from_lumps_dynamic(const b2d_level_lumps *lv, const b2d_tex
         }
         s->blob = compile_scene(s->level, td, dyn_list(dyn, n_dyn));
         fill_scene_info(s.get());
+        s->palettes.assign(1, td.palettes.empty() ? std::array<uint8_t, 768>{} : td.palettes[0]);
         *out = s.release();
+        return B2D_OK;
+    });
+}
+
+int b2d_scene_num_palettes(const b2d_scene *s) {
+    if (!s) return fail(B2D_ERR_INVALID_ARG, "null scene");
+    return (int)s->palettes.size();
+}
+
+int b2d_scene_set_palettes(b2d_scene *s, const uint8_t *playpal, size_t n_palettes) {
+    if (!s || !playpal || n_palettes == 0) return fail(B2D_ERR_INVALID_ARG, "null argument or no palettes");
+    if (n_palettes > (size_t)INT32_MAX / 768) return fail(B2D_ERR_INVALID_ARG, "too many palettes");
+    if (std::memcmp(playpal, s->palettes[0].data(), 768) != 0)
+        return fail(B2D_ERR_INVALID_ARG, "palette 0 differs from the palette the scene was made with");
+    return guarded([&] {
+        std::vector<std::array<uint8_t, 768>> p(n_palettes);
+        for (size_t i = 0; i < n_palettes; i++) std::memcpy(p[i].data(), playpal + 768 * i, 768);
+        s->palettes = std::move(p);
         return B2D_OK;
     });
 }
@@ -941,10 +970,16 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
         }
         words = std::max(words, (size_t)lv.layout.words);
     }
-    // every level's palette side by side (b2d_palette_lut_levels_device): at most B2D_MAX_LEVELS x 1 KB
-    CU(allocate(r->d_palettes, r->lv.size() * 256 * sizeof(uint32_t)));
-    for (size_t k = 0; k < r->lv.size(); k++)
-        CU(cudaMemcpy(r->d_palettes.get() + k * 256, r->lv[k].ds.palette, 256 * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
+    // every palette of every level in one colour table (K3-levels, K4), copied from the scenes now: 14 KB per PLAYPAL
+    std::vector<uint32_t> table;
+    for (size_t k = 0; k < n_levels; k++) {
+        r->pal_base.push_back((uint32_t)(table.size() / 256));
+        r->pal_count.push_back((uint32_t)scenes[k]->palettes.size());
+        for (const auto &p : scenes[k]->palettes)
+            for (int i = 0; i < 256; i++) table.push_back(palette_word(&p[(size_t)i * 3]));
+    }
+    CU(allocate(r->d_palettes, table.size() * sizeof(uint32_t)));
+    CU(cudaMemcpy(r->d_palettes.get(), table.data(), table.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     // each worklist slot's staging, for the largest batch: max_batch frames with a table set each, or a stale set per level
     const size_t sets = std::max((size_t)max_batch, r->lv.size());
     const size_t stage_bytes = StageLayout(r->lv.size(), sets, (size_t)max_batch, sets * words, true, true).end;
@@ -1273,10 +1308,12 @@ int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint3
     return render_host(r, poses, fr, n, index_fb, rgba_fb);
 }
 
-// The n frame levels of a call staged in `s` on `st`: into staging grown to hold them (created whole, or not at all; the
-// old buffers go once the last call's kernel has read them), or into the present staging once the previous call's copy
-// has read it and, on `st`, its kernel the device copy.  The caller records s.done after its kernel.
-static int stage_levels(LevelStaging &s, const uint32_t *levels, size_t n, cudaStream_t st) {
+// The colour-table indices of the n frames of a call (frame_table of its checked levels and palettes) staged in `s` on
+// `st`: into staging grown to hold them (created whole, or not at all; the old buffers go once the last call's kernel has
+// read them), or into the present staging once the previous call's copy has read it and, on `st`, its kernel the device
+// copy.  The caller records s.done after its kernel.
+static int stage_tables(const b2d_renderer *r, LevelStaging &s, const uint32_t *levels, const uint32_t *palettes, size_t n,
+                        cudaStream_t st) {
     if (s.cap < n) {
         LevelStaging g;
         g.cap = s.cap ? s.cap : 1024;
@@ -1291,7 +1328,7 @@ static int stage_levels(LevelStaging &s, const uint32_t *levels, size_t n, cudaS
         CU(cudaEventSynchronize(s.copied.get()));     // the previous call's copy has read the staging
         CU(cudaStreamWaitEvent(st, s.done.get(), 0));        // ... and its kernel the device copy
     }
-    std::memcpy(s.h.get(), levels, n * sizeof(uint32_t));
+    for (size_t i = 0; i < n; i++) s.h.get()[i] = frame_table(r, levels, palettes, i);
     CU(cudaMemcpyAsync(s.d.get(), s.h.get(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(s.copied.get(), st));
     return B2D_OK;
@@ -1313,7 +1350,7 @@ int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    if (int rc = stage_levels(r->lut_levels, levels, n_frames, st)) return rc;
+    if (int rc = stage_tables(r, r->lut_levels, levels, nullptr, n_frames, st)) return rc;
     CU(launch_palette_levels(r->d_palettes.get(), r->lut_levels.d.get(), d_index, d_rgba, n_frames, (size_t)r->view.W * r->view.H, st));
     CU(cudaEventRecord(r->lut_levels.done.get(), st));
     r->launches += 1;
@@ -1336,25 +1373,30 @@ int b2d_resolve_frame_bytes(const b2d_renderer *r, int factor, int format, size_
     return B2D_OK;
 }
 
-int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, int factor, int format,
-                       void *d_out, void *cuda_stream) {
+int b2d_resolve_palettes_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, const uint32_t *palettes,
+                                size_t n_frames, int factor, int format, void *d_out, void *cuda_stream) {
     if (!r || !d_index || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (int rc = check_resolve(r, factor, format)) return rc;
     if (levels)
         for (size_t i = 0; i < n_frames; i++)
             if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    if (int rc = check_palettes(r, levels, palettes, n_frames)) return rc;
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    const uint32_t *d_levels = nullptr;          // NULL levels: every frame through level 0's palette, nothing to stage
-    if (levels) {
-        if (int rc = stage_levels(r->resolve_levels, levels, n_frames, st)) return rc;
-        d_levels = r->resolve_levels.d.get();
-    }
-    CU(launch_resolve(r->d_palettes.get(), d_levels, d_index, d_out, n_frames, r->view.W, r->view.H, factor, format, st));
-    if (levels) CU(cudaEventRecord(r->resolve_levels.done.get(), st));
+    const bool staged = levels || palettes;      // neither: every frame through table 0 (level 0, palette 0), nothing to stage
+    if (staged)
+        if (int rc = stage_tables(r, r->resolve_levels, levels, palettes, n_frames, st)) return rc;
+    CU(launch_resolve(r->d_palettes.get(), staged ? r->resolve_levels.d.get() : nullptr, d_index, d_out, n_frames, r->view.W,
+                      r->view.H, factor, format, st));
+    if (staged) CU(cudaEventRecord(r->resolve_levels.done.get(), st));
     r->launches += 1;
     return B2D_OK;
+}
+
+int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, int factor, int format,
+                       void *d_out, void *cuda_stream) {
+    return b2d_resolve_palettes_device(r, d_index, levels, nullptr, n_frames, factor, format, d_out, cuda_stream);
 }
 
 int b2d_device_alloc(int device, size_t bytes, void **d_out) {

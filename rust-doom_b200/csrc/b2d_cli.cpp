@@ -13,7 +13,9 @@
 // b2d_render_sharded_levels_states with --world.
 // --supersample K (1..8) renders at K times the resolution with the same field of view and resolves every frame to
 // --resolution RGB on the device (b2d_resolve_device, each frame through its own level's palette) for --dump and --stream;
-// not with --world.
+// not with --world.  --palette P colours those frames through PLAYPAL palette P instead of palette 0
+// (b2d_resolve_palettes_device; 1..8 Doom's damage flash, 9..12 the bonus flash, 13 the radiation suit), through the
+// resolve at the --supersample factor (1 by default); not with --world.
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -70,10 +72,11 @@ void write_ppm_rgb(std::FILE *f, const uint8_t *rgb, int w, int h) {
     std::fwrite(rgb, 1, (size_t)w * h * 3, f);
 }
 
-// --supersample: render the n poses (levels: per-frame levels and states, else the renderer's own state) into device index
-// frames at the renderer's view, resolve them by `factor` to RGB8 and download them into `rgb` (n x (W/factor) x (H/factor) x 3)
+// --supersample / --palette: render the n poses (levels: per-frame levels and states, else the renderer's own state) into
+// device index frames at the renderer's view, resolve them by `factor` to RGB8 through palette `palette` of each frame's
+// level and download them into `rgb` (n x (W/factor) x (H/factor) x 3)
 int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, size_t max_batch,
-                        const uint32_t *levels, const b2d_frame_state *states, int factor, std::vector<uint8_t> &rgb) {
+                        const uint32_t *levels, const b2d_frame_state *states, int factor, int palette, std::vector<uint8_t> &rgb) {
     const size_t n = poses.size(), npix = (size_t)view.width * view.height;
     size_t frame_bytes = 0;
     if (b2d_resolve_frame_bytes(r, factor, B2D_RESOLVE_RGB8, &frame_bytes) != B2D_OK) return fail("resolve");
@@ -95,7 +98,9 @@ int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const
         for (size_t i = 0; i < n; i += max_batch)
             if (b2d_render_device(r, dp + i, std::min(max_batch, n - i), di + npix * i, nullptr, nullptr) != B2D_OK) return fail("render");
     }
-    if (b2d_resolve_device(r, di, levels, n, factor, B2D_RESOLVE_RGB8, d_rgb, nullptr) != B2D_OK) return fail("resolve");
+    const std::vector<uint32_t> palettes(n, (uint32_t)palette);
+    if (b2d_resolve_palettes_device(r, di, levels, palettes.data(), n, factor, B2D_RESOLVE_RGB8, d_rgb, nullptr) != B2D_OK)
+        return fail("resolve");
     int32_t bits = 0;
     if (b2d_renderer_status(r, &bits) != B2D_OK) return fail("status");
     if (bits) { std::fprintf(stderr, "Fatal error: frames incomplete (status %d)\n", bits); return 1; }
@@ -155,7 +160,7 @@ int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st
 // --levels: the look-around of every level of `set` from its start, nposes per level, pose i at tic tics + i
 int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
                      const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file,
-                     int supersample) {
+                     int supersample, int palette) {
     std::vector<b2d_scene *> scenes;
     struct Scenes {
         std::vector<b2d_scene *> &v;
@@ -172,6 +177,10 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
         b2d_scene_info info;
         b2d_scene_info_get(sc, &info);
         if (!info.has_start) { std::fprintf(stderr, "Fatal error: level %d has no player-1 start\n", set[k]); return 1; }
+        if (palette >= b2d_scene_num_palettes(sc)) {
+            std::fprintf(stderr, "--palette takes a palette index below %d\n", b2d_scene_num_palettes(sc));
+            return 2;
+        }
         for (size_t i = 0; i < per_level; i++) {        // look around from the spawn point
             b2d_pose &p = poses[k * per_level + i];
             p = info.start;
@@ -206,9 +215,12 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
     }
     std::vector<uint8_t> index, rgb;
     std::vector<uint32_t> rgba;
-    if (supersample > 1) {
-        if (int rc = render_supersampled(r, 0, view, poses, n < 64 ? n : 64, levels.data(), states.data(), supersample, rgb)) return rc;
-        std::printf("rendered %zu frame(s) %dx%d of %zu level(s), supersampled %dx\n", n, width, height, set.size(), supersample);
+    const bool resolved = supersample > 1 || palette > 0;
+    if (resolved) {
+        if (int rc = render_supersampled(r, 0, view, poses, n < 64 ? n : 64, levels.data(), states.data(), supersample, palette, rgb))
+            return rc;
+        std::printf("rendered %zu frame(s) %dx%d of %zu level(s), supersampled %dx, palette %d\n", n, width, height, set.size(),
+                    supersample, palette);
     } else {
         index.resize(npix * n);
         rgba.resize(npix * n);
@@ -217,7 +229,7 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
         std::printf("rendered %zu frame(s) %dx%d of %zu level(s)\n", n, width, height, set.size());
     }
     auto write_frame = [&](std::FILE *f, size_t i) {
-        if (supersample > 1) write_ppm_rgb(f, rgb.data() + npix * 3 * i, width, height);
+        if (resolved) write_ppm_rgb(f, rgb.data() + npix * 3 * i, width, height);
         else write_ppm(f, rgba.data() + npix * i, width, height);
     };
     if (!dump.empty()) {
@@ -243,7 +255,7 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
 
 int main(int argc, char **argv) {
     std::string iwad, dump, stream, command, id_file, levels_arg;
-    int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16, supersample = 1;
+    int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16, supersample = 1, palette = 0;
     double fov = 65.0;
     unsigned long tics = 0;
     bool with_levels = false;
@@ -272,6 +284,13 @@ int main(int argc, char **argv) {
         else if (a == "--chunk") chunk = std::atoi(next("--chunk"));
         else if (a == "--id-file") id_file = next("--id-file");
         else if (a == "--supersample") supersample = std::atoi(next("--supersample"));
+        else if (a == "--palette") {
+            const char *v = next("--palette");
+            char *end = nullptr;
+            const long p = std::strtol(v, &end, 10);
+            if (!*v || *end || p < 0 || p > 0x7FFFFFFF) { std::fprintf(stderr, "--palette takes a palette index\n"); return 2; }
+            palette = (int)p;
+        }
         else if (a == "list-levels" || a == "check") command = a;
         else { std::fprintf(stderr, "unknown argument %s\n", a.c_str()); return 2; }
     }
@@ -279,6 +298,7 @@ int main(int argc, char **argv) {
     if (nposes < 1) nposes = 1;
     if (supersample < 1 || supersample > 8) { std::fprintf(stderr, "--supersample takes a factor in 1..8\n"); return 2; }
     if (supersample > 1 && world > 0) { std::fprintf(stderr, "--supersample does not combine with --world\n"); return 2; }
+    if (palette > 0 && world > 0) { std::fprintf(stderr, "--palette does not combine with --world\n"); return 2; }
 
     b2d_archive *arch = nullptr;
     if (b2d_archive_open(iwad.c_str(), &arch) != B2D_OK) return fail("open");
@@ -315,7 +335,7 @@ int main(int argc, char **argv) {
             return 2;
         }
         const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file,
-                                        supersample);
+                                        supersample, palette);
         b2d_archive_close(arch);
         return rc;
     }
@@ -324,6 +344,10 @@ int main(int argc, char **argv) {
     b2d_scene_info info;
     b2d_scene_info_get(sc, &info);
     if (!info.has_start) { std::fprintf(stderr, "Fatal error: the level has no player-1 start\n"); return 1; }
+    if (palette >= b2d_scene_num_palettes(sc)) {
+        std::fprintf(stderr, "--palette takes a palette index below %d\n", b2d_scene_num_palettes(sc));
+        return 2;
+    }
     b2d_view view;
     if (b2d_view_init(&view, width * supersample, height * supersample, fov) != B2D_OK) return fail("view");
     b2d_renderer *r = nullptr;
@@ -334,10 +358,11 @@ int main(int argc, char **argv) {
     for (int i = 0; i < nposes; i++)          // look around from the spawn point
         poses[(size_t)i].angle = info.start.angle + (uint32_t)(((uint64_t)i << 32) / (uint64_t)nposes);
     const size_t npix = (size_t)width * height;
-    if (supersample > 1) {
+    if (supersample > 1 || palette > 0) {
         std::vector<uint8_t> rgb;
-        if (int rc = render_supersampled(r, 0, view, poses, nposes < 64 ? nposes : 64, nullptr, nullptr, supersample, rgb)) return rc;
-        std::printf("rendered %d frame(s) %dx%d, supersampled %dx\n", nposes, width, height, supersample);
+        if (int rc = render_supersampled(r, 0, view, poses, nposes < 64 ? nposes : 64, nullptr, nullptr, supersample, palette, rgb))
+            return rc;
+        std::printf("rendered %d frame(s) %dx%d, supersampled %dx, palette %d\n", nposes, width, height, supersample, palette);
         if (!dump.empty()) {
             std::FILE *f = std::fopen(dump.c_str(), "wb");
             if (!f) { std::perror(dump.c_str()); return 1; }

@@ -34,6 +34,11 @@ int build_states(const b2d_renderer *r, const b2d_frame_state *states, const uin
 // Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
 // per-frame-level walk (a b2d_renderer_create renderer may not); B2D_ERR_INVALID_ARG otherwise.
 int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n);
+// Per-frame palettes (HOST, nullable = palette 0): frame i's palette below the palette count of its level (levels[i],
+// nullable = level 0), the levels already checked; B2D_ERR_INVALID_ARG otherwise.
+int check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n);
+// The colour-table index of frame i, pal_base[levels[i]] + palettes[i] (either array nullable: 0), after the checks above.
+inline uint32_t frame_table(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t i);
 // A one-call render of `batches` batches walks the first into the next worklist slot and alternates slots from there: it
 // is refused (B2D_ERR_INVALID_ARG) before anything is enqueued while a slot it would use holds a walked, unrastered batch.
 int check_slots_free(const b2d_renderer *r, size_t batches);
@@ -95,6 +100,9 @@ struct b2d_scene {
     std::vector<uint8_t> blob;
     Level level;
     b2d_scene_info info;
+    // every palette the scene holds, at least one; palettes[0] is the one compiled into the blob (768 zero bytes when
+    // the scene was made without a PLAYPAL)
+    std::vector<std::array<uint8_t, 768>> palettes;
 };
 
 // A worklist slot: the BSP walk of batch k+1 may run (b2d_walk_device, another stream) while batch k is rastered.
@@ -128,8 +136,8 @@ struct HostStaging {
     std::array<DeviceBuf<uint32_t>, 2> rgba;              // created by the first call that asks for RGBA frames
 };
 
-// A call's frame levels on the device, with their pinned staging (stage_levels, b2d_api.cu): grown by a call with more
-// frames than they hold.
+// A call's frame colour-table indices on the device, with their pinned staging (stage_tables, b2d_api.cu): grown by a
+// call with more frames than they hold.
 struct LevelStaging {
     DeviceBuf<uint32_t> d;
     PinnedBuf<uint32_t> h;
@@ -183,8 +191,12 @@ struct b2d_renderer {
     std::unique_ptr<HostStaging> host;
     uint32_t tics = 0;
     Event masked_done;                                    // last raster that used the masked-entry arena
-    DeviceBuf<uint32_t> d_palettes;                       // every level's palette, [n_levels][256]
-    // the frame levels of a call of b2d_palette_lut_levels_device and of b2d_resolve_device, each call kind with its own
+    // every palette of every level as one colour table, [sum of the levels' palette counts][256]: level l's palette p is
+    // table pal_base[l] + p.  K3-levels and K4 read a table index per frame (stage_tables, b2d_api.cu).
+    DeviceBuf<uint32_t> d_palettes;
+    std::vector<uint32_t> pal_base, pal_count;
+    // the frame tables of a call of b2d_palette_lut_levels_device and of b2d_resolve_device / b2d_resolve_palettes_device,
+    // each call kind with its own
     LevelStaging lut_levels, resolve_levels;
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;
@@ -194,6 +206,10 @@ struct b2d_renderer {
 
     ~b2d_renderer() { cudaSetDevice(device); }            // the members are released on the renderer's device
 };
+
+inline uint32_t b2d::frame_table(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t i) {
+    return r->pal_base[levels ? levels[i] : 0u] + (palettes ? palettes[i] : 0u);
+}
 
 #define B2D_CU(call)                                             \
     do {                                                         \

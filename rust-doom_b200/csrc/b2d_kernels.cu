@@ -10,8 +10,8 @@
 //                        carry the light->colormap lookup; every pixel is written exactly once.
 //   b2d_prelight_*     : build those planes once per renderer (32 light rows x texels / flats).
 //   b2d_palette_kernel : index -> RGBA8 with the 256-entry palette in shared memory, 128-bit I/O;
-//   b2d_palette_levels_kernel the same with a palette per frame (a level set's frames).
-//   b2d_resolve_kernel : k x k box filter of index frames through a palette (or its luma) per frame into RGBA, RGB,
+//   b2d_palette_levels_kernel the same with a colour table per frame (a level set's frames).
+//   b2d_resolve_kernel : k x k box filter of index frames through a colour table (or its luma) per frame into RGBA, RGB,
 //                        planar RGB or grey frames at 1/k of the size (C17).
 //
 // There is no dense contraction anywhere on this path, so no tensor-core (wgmma) work: the
@@ -1048,15 +1048,16 @@ b2d_palette_kernel(const uint32_t *__restrict__ palette, const uint8_t *__restri
         rgba[p] = s_pal[index[p]];
 }
 
-// Kernel 3 with a palette per frame: `parts` CTAs per frame (blockIdx.x = frame * parts + part), each loading the palette of
-// its frame's level, palettes[levels[frame]], into shared memory and streaming a contiguous 1/parts of the frame.
+// Kernel 3 with a colour table per frame: `parts` CTAs per frame (blockIdx.x = frame * parts + part), each loading its
+// frame's table, palettes[tables[frame]] (a palette of the frame's level), into shared memory and streaming a contiguous
+// 1/parts of the frame.
 __global__ void __launch_bounds__(256)
-b2d_palette_levels_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__restrict__ levels,
+b2d_palette_levels_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__restrict__ tables,
                           const uint8_t *__restrict__ index, uint32_t *__restrict__ rgba, size_t npix, int parts) {
     __shared__ uint32_t s_pal[256];
     const size_t frame = blockIdx.x / parts;
     const int part = blockIdx.x % parts;
-    s_pal[threadIdx.x] = palettes[(size_t)levels[frame] * 256 + threadIdx.x];
+    s_pal[threadIdx.x] = palettes[(size_t)tables[frame] * 256 + threadIdx.x];
     __syncthreads();
     const uint8_t *in = index + frame * npix;
     uint32_t *out = rgba + frame * npix;
@@ -1175,7 +1176,8 @@ __device__ __forceinline__ void resolve_emit(uint8_t *o, size_t opix, int OW, in
     }
 }
 
-// `parts` CTAs per frame (blockIdx.x = frame * parts + part), each loading its frame's palette -- as {R | B << 16, G}, or
+// `parts` CTAs per frame (blockIdx.x = frame * parts + part), each loading its frame's colour table, palettes[tables[frame]]
+// (NULL tables: table 0) -- as {R | B << 16, G}, or
 // the luma Y = (77 R + 150 G + 29 B + 128) >> 8 for grey -- into shared memory and resolving a contiguous 1/parts of the
 // frame's work items (sums of up to 64 entries stay below 2^14, so R and B share a word).  Vector path (`vec`: W a
 // multiple of P * K and the index frames 16-byte aligned): an item is P = 16 / gcd(K, 16) output pixels of one output row,
@@ -1183,7 +1185,7 @@ __device__ __forceinline__ void resolve_emit(uint8_t *o, size_t opix, int OW, in
 // compile-time constant.  Otherwise an item is one output pixel, read byte by byte.  Stores: store_run.
 template <int K, int FMT>
 __global__ void __launch_bounds__(256)
-b2d_resolve_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__restrict__ levels, const uint8_t *__restrict__ index,
+b2d_resolve_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__restrict__ tables, const uint8_t *__restrict__ index,
                    uint8_t *__restrict__ out, int W, int H, int parts, bool vec) {
     constexpr int P = K == 1 ? 16 : K == 2 ? 8 : K == 4 ? 4 : K == 6 ? 8 : K == 8 ? 2 : 16;     // 16 / gcd(K, 16)
     constexpr int kBpp = FMT == kResolveRgba ? 4 : FMT == kResolveGray ? 1 : 3;
@@ -1191,7 +1193,7 @@ b2d_resolve_kernel(const uint32_t *__restrict__ palettes, const uint32_t *__rest
     const size_t frame = blockIdx.x / parts;
     const int part = blockIdx.x % parts;
     {
-        const uint32_t c = palettes[(size_t)(levels ? levels[frame] : 0u) * 256 + threadIdx.x];
+        const uint32_t c = palettes[(size_t)(tables ? tables[frame] : 0u) * 256 + threadIdx.x];
         const uint32_t R = c & 0xFF, G = (c >> 8) & 0xFF, B = (c >> 16) & 0xFF;
         s_tab[threadIdx.x] = FMT == kResolveGray ? make_uint2((77 * R + 150 * G + 29 * B + 128) >> 8, 0u) : make_uint2(R | (B << 16), G);
     }
@@ -1433,13 +1435,13 @@ cudaError_t launch_state_sets(const StateSrc *d_srcs, const StateSet *d_sets, co
     return cudaGetLastError();
 }
 
-cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, uint32_t *d_rgba,
+cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_tables, const uint8_t *d_index, uint32_t *d_rgba,
                                   size_t n_frames, size_t npix, cudaStream_t stream) {
     if (n_frames == 0 || npix == 0) return cudaSuccess;
     // ~32 KB of a frame's index bytes per CTA (8 128-bit loads per thread): 64 CTAs per 1080p frame
     const size_t parts = (npix + 32767) / 32768;
     if (n_frames * parts > 0x7FFFFFFFull) return cudaErrorInvalidValue;
-    b2d_palette_levels_kernel<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_levels, d_index, d_rgba, npix, (int)parts);
+    b2d_palette_levels_kernel<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_tables, d_index, d_rgba, npix, (int)parts);
     return cudaGetLastError();
 }
 
@@ -1456,7 +1458,7 @@ static ResolveFn resolve_kernel_of(int format) {
     }
 }
 
-cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, void *d_out,
+cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_tables, const uint8_t *d_index, void *d_out,
                            size_t n_frames, int W, int H, int factor, int format, cudaStream_t stream) {
     if (n_frames == 0) return cudaSuccess;
     ResolveFn fn = nullptr;
@@ -1477,7 +1479,7 @@ cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_levels,
     // ~32 KB of a frame's index bytes per CTA, as K3 per level
     const size_t parts = ((size_t)W * H + 32767) / 32768;
     if (n_frames * parts > 0x7FFFFFFFull) return cudaErrorInvalidValue;
-    fn<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_levels, d_index, static_cast<uint8_t *>(d_out), W, H,
+    fn<<<(unsigned)(n_frames * parts), 256, 0, stream>>>(d_palettes, d_tables, d_index, static_cast<uint8_t *>(d_out), W, H,
                                                          (int)parts, vec);
     return cudaGetLastError();
 }

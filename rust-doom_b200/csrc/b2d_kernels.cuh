@@ -129,12 +129,13 @@ cudaError_t launch_prelight_textures(const uint8_t *d_colormap, const uint8_t *d
 // Kernel 3: palette LUT on its own (index -> RGBA8), 16 pixels per thread.
 cudaError_t launch_palette(const uint32_t *d_palette, const uint8_t *d_index, uint32_t *d_rgba,
                            size_t n_pixels, cudaStream_t stream);
-// ... with a palette per frame: frame f of the n_frames contiguous npix-pixel frames through palettes[levels[f] * 256 ..].
-cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, uint32_t *d_rgba,
+// ... with a colour table per frame: frame f of the n_frames contiguous npix-pixel frames through
+// palettes[tables[f] * 256 ..] (the renderer's table layout: b2d_renderer::d_palettes).
+cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_tables, const uint8_t *d_index, uint32_t *d_rgba,
                                   size_t n_frames, size_t npix, cudaStream_t stream);
-// Kernel 4: C17 resolve of the n_frames contiguous W x H index frames at d_index, frame f through palettes[levels[f] * 256 ..]
-// (d_levels NULL: level 0), box-filtered by `factor` (1..8, dividing W and H) into d_out in B2D_RESOLVE_* `format`.
-cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_levels, const uint8_t *d_index, void *d_out,
+// Kernel 4: C17 resolve of the n_frames contiguous W x H index frames at d_index, frame f through palettes[tables[f] * 256 ..]
+// (d_tables NULL: table 0), box-filtered by `factor` (1..8, dividing W and H) into d_out in B2D_RESOLVE_* `format`.
+cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_tables, const uint8_t *d_index, void *d_out,
                            size_t n_frames, int W, int H, int factor, int format, cudaStream_t stream);
 
 }  // namespace b2d

@@ -544,10 +544,8 @@ std::vector<uint8_t> compile_scene(const Level &lv, const TextureDirectory &td, 
     for (size_t k = 0; k < td.colormaps.size() && k < 34; k++) std::memcpy(&colormap[k * 256], td.colormaps[k].data(), 256);
     std::vector<uint32_t> palette(256, 0xFF000000u);
     if (!td.palettes.empty())
-        for (int i = 0; i < 256; i++) {
-            const uint8_t *c = &td.palettes[0][(size_t)i * 3];
-            palette[(size_t)i] = (uint32_t)c[0] | ((uint32_t)c[1] << 8) | ((uint32_t)c[2] << 16) | 0xFF000000u;
-        }
+        for (int i = 0; i < 256; i++)
+            palette[(size_t)i] = palette_word(&td.palettes[0][(size_t)i * 3]);
 
     // player-1 start (visitor.rs:1010-1026; game/src/level.rs:757-762; player.rs:88 camera_height)
     int32_t has_start = 0, sx = 0, sy = 0, sz = 0, sang = 0;

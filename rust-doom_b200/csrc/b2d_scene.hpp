@@ -401,6 +401,11 @@ inline const char *expand_moves(const uint8_t *blob, const SectorMove *moves, si
     return nullptr;
 }
 
+// A PLAYPAL entry (R, G, B bytes) as the RGBA8 word the kernels read: R in the low byte, alpha 0xFF.
+inline uint32_t palette_word(const uint8_t *c) {
+    return (uint32_t)c[0] | ((uint32_t)c[1] << 8) | ((uint32_t)c[2] << 16) | 0xFF000000u;
+}
+
 std::vector<uint8_t> compile_scene(const Archive &wad, const TextureDirectory &tex, int level_index,
                                    const std::vector<DynRec> &dynamic = {});
 std::vector<uint8_t> compile_scene(const Level &level, const TextureDirectory &tex, const std::vector<DynRec> &dynamic = {});

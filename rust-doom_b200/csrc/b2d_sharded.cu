@@ -160,12 +160,12 @@ struct b2d_comm {
     DeviceBuf<int32_t> d_token;
     DeviceBuf<Pose> d_poses; PinnedBuf<Pose> h_poses;
     size_t poses_cap = 0;
-    // resolved calls (b2d_render_sharded*_resolved): the rank-local index frames of one chunk, which K4 reads, and the
-    // frame levels of the rank's block with their pinned staging, uploaded once per call next to the poses
+    // resolved calls (b2d_render_sharded*_resolved*): the rank-local index frames of one chunk, which K4 reads, and the
+    // frame colour-table indices of the rank's block with their pinned staging, uploaded once per call next to the poses
     DeviceBuf<uint8_t> d_stage;
     size_t stage_bytes = 0;
-    DeviceBuf<uint32_t> d_levels; PinnedBuf<uint32_t> h_levels;
-    size_t levels_cap = 0;
+    DeviceBuf<uint32_t> d_tables; PinnedBuf<uint32_t> h_tables;
+    size_t tables_cap = 0;
 };
 
 namespace {
@@ -390,11 +390,12 @@ int check_sharded(const b2d_renderer *r, const b2d_comm *c, const b2d_pose *pose
 }
 
 // The resolve step of a resolved sharded call: K4 by `factor` into `format`, frame_bytes bytes per resolved frame;
-// block_levels (HOST, nullable = level 0 on every frame) holds the level of each entry of this rank's padded block.
+// block_tables (HOST, nullable = table 0 on every frame) holds the colour-table index (frame_table) of each entry of this
+// rank's padded block.
 struct ShardResolve {
     int factor = 1, format = B2D_RESOLVE_RGBA8;
     size_t frame_bytes = 0;
-    const uint32_t *block_levels = nullptr;
+    const uint32_t *block_tables = nullptr;
 };
 
 // The chunk loop of the sharded calls, after their arguments have been checked (check_sharded and the caller's checks of
@@ -426,11 +427,11 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
         B2D_CU(allocate(c->d_stage, chunk * npix));
         c->stage_bytes = chunk * npix;
     }
-    if (do_resolve && res->block_levels && c->levels_cap < per) {
-        c->levels_cap = 0; c->d_levels.reset(); c->h_levels.reset();
-        B2D_CU(allocate(c->d_levels, per * sizeof(uint32_t)));
-        B2D_CU(allocate(c->h_levels, per * sizeof(uint32_t)));
-        c->levels_cap = per;
+    if (do_resolve && res->block_tables && c->tables_cap < per) {
+        c->tables_cap = 0; c->d_tables.reset(); c->h_tables.reset();
+        B2D_CU(allocate(c->d_tables, per * sizeof(uint32_t)));
+        B2D_CU(allocate(c->h_tables, per * sizeof(uint32_t)));
+        c->tables_cap = per;
     }
     // this rank's block of poses, padded by repeating the last pose of the list, on the device in one copy
     if (c->poses_cap < per) {
@@ -451,11 +452,11 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
     B2D_CU(event_create(poses_up));
     B2D_CU(cudaEventRecord(poses_up.get(), render_stream));
     B2D_CU(cudaStreamWaitEvent(walk_stream, poses_up.get(), 0));
-    const uint32_t *d_levels = nullptr;                                  // the resolve's frame levels; NULL: level 0
-    if (do_resolve && res->block_levels) {
-        std::memcpy(c->h_levels.get(), res->block_levels, per * sizeof(uint32_t));
-        B2D_CU(cudaMemcpyAsync(c->d_levels.get(), c->h_levels.get(), per * sizeof(uint32_t), cudaMemcpyHostToDevice, render_stream));
-        d_levels = c->d_levels.get();
+    const uint32_t *d_tables = nullptr;                                  // the resolve's frame tables; NULL: table 0
+    if (do_resolve && res->block_tables) {
+        std::memcpy(c->h_tables.get(), res->block_tables, per * sizeof(uint32_t));
+        B2D_CU(cudaMemcpyAsync(c->d_tables.get(), c->h_tables.get(), per * sizeof(uint32_t), cudaMemcpyHostToDevice, render_stream));
+        d_tables = c->d_tables.get();
     }
     // the BSP walk of chunk k+1 runs as a background grid on its own stream under the raster of chunk k
     auto walk = [&](size_t k, int64_t *ticket) {
@@ -495,7 +496,7 @@ int sharded_loop(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_t
             result = b2d::raster_batch(r, ticket, do_resolve ? c->d_stage.get() : slice, nullptr, render_stream);
             if (result != B2D_OK) break;
             if (do_resolve) {
-                B2D_CU(launch_resolve(r->d_palettes.get(), d_levels ? d_levels + first : nullptr, c->d_stage.get(), slice, cnt,
+                B2D_CU(launch_resolve(r->d_palettes.get(), d_tables ? d_tables + first : nullptr, c->d_stage.get(), slice, cnt,
                                       r->view.W, r->view.H, res->factor, res->format, render_stream));
                 r->launches += 1;
             }
@@ -563,9 +564,9 @@ int render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n
 }
 
 int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
-                                 const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves, size_t n_moves,
-                                 size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out,
-                                 ShardResolve *res) {
+                                 const uint32_t *palettes, const b2d_frame_state *states, size_t n_total,
+                                 const b2d_sector_move *moves, size_t n_moves, size_t chunk_frames, int mode, b2d_chunk_fn fn,
+                                 void *user, b2d_sharded_stats *stats_out, ShardResolve *res) {
     int rc = check_sharded(r, c, poses, mode);
     if (rc == B2D_OK && res) rc = b2d_resolve_frame_bytes(r, res->factor, res->format, &res->frame_bytes);
     if (rc != B2D_OK) return rc;
@@ -575,19 +576,21 @@ int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *p
     std::vector<size_t> starts;
     Frames all{levels};
     rc = b2d::check_levels(r, levels, n_total);
+    if (rc == B2D_OK) rc = b2d::check_palettes(r, levels, palettes, n_total);
     if (rc == B2D_OK) rc = b2d::build_states(r, states, nullptr, n_total, moves, n_moves, fs, starts, all);
     if (rc != B2D_OK || n_total == 0) return rc;
-    // this rank's block, padded like its poses by repeating the last entry (level and state with it); its states stay
-    // where build_states put them
+    // this rank's block, padded like its poses by repeating the last entry (level, palette and state with it); its
+    // states stay where build_states put them
     const size_t world = (size_t)c->world, rank = (size_t)c->rank, per = (n_total + world - 1) / world;
-    std::vector<uint32_t> block_levels(per);
+    std::vector<uint32_t> block_levels(per), block_tables(per);
     std::vector<size_t> block_starts(per);
     for (size_t i = 0; i < per; i++) {
         const size_t g = std::min(rank * per + i, n_total - 1);
         block_levels[i] = levels[g];
+        block_tables[i] = b2d::frame_table(r, levels, palettes, g);
         block_starts[i] = starts[g];
     }
-    if (res) res->block_levels = block_levels.data();
+    if (res) res->block_tables = block_tables.data();
     return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
                         Frames{block_levels.data(), fs.data(), block_starts.data()}, res);
 }
@@ -604,8 +607,8 @@ int b2d_render_sharded(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size
 int b2d_render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, const uint32_t *levels,
                                      const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves, size_t n_moves,
                                      size_t chunk_frames, int mode, b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
-    return render_sharded_levels_states(r, c, poses, levels, states, n_total, moves, n_moves, chunk_frames, mode, fn, user,
-                                        stats_out, nullptr);
+    return render_sharded_levels_states(r, c, poses, levels, nullptr, states, n_total, moves, n_moves, chunk_frames, mode, fn,
+                                        user, stats_out, nullptr);
 }
 
 int b2d_render_sharded_resolved(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses, size_t n_total, size_t chunk_frames,
@@ -619,10 +622,20 @@ int b2d_render_sharded_levels_states_resolved(b2d_renderer *r, b2d_comm *c, cons
                                               const b2d_frame_state *states, size_t n_total, const b2d_sector_move *moves,
                                               size_t n_moves, size_t chunk_frames, int factor, int format, int mode,
                                               b2d_chunk_fn fn, void *user, b2d_sharded_stats *stats_out) {
+    return b2d_render_sharded_levels_states_resolved_palettes(r, c, poses, levels, nullptr, states, n_total, moves, n_moves,
+                                                              chunk_frames, factor, format, mode, fn, user, stats_out);
+}
+
+int b2d_render_sharded_levels_states_resolved_palettes(b2d_renderer *r, b2d_comm *c, const b2d_pose *poses,
+                                                       const uint32_t *levels, const uint32_t *palettes,
+                                                       const b2d_frame_state *states, size_t n_total,
+                                                       const b2d_sector_move *moves, size_t n_moves, size_t chunk_frames,
+                                                       int factor, int format, int mode, b2d_chunk_fn fn, void *user,
+                                                       b2d_sharded_stats *stats_out) {
     ShardResolve res;
     res.factor = factor; res.format = format;
-    return render_sharded_levels_states(r, c, poses, levels, states, n_total, moves, n_moves, chunk_frames, mode, fn, user,
-                                        stats_out, &res);
+    return render_sharded_levels_states(r, c, poses, levels, palettes, states, n_total, moves, n_moves, chunk_frames, mode, fn,
+                                        user, stats_out, &res);
 }
 
 }  // extern "C"

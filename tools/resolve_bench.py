@@ -1,7 +1,7 @@
 """The resolve kernel K4 (b2d_resolve_device) against K3 per level (b2d_palette_lut_levels_device), and what 2x
 anti-aliasing costs per frame.
 
-    python tools/resolve_bench.py [--frames 1000] [--rounds 5] [--reps 5] [--out FILE.json]
+    python tools/resolve_bench.py [--frames 1000] [--rounds 5] [--reps 5] [--out FILE.json] [--palettes]
 
 Frames: the c2 fly-through (synthetic SYN_E1M1, seed 1, 1920x1080), rendered once on the device.  Each round times, for
 every factor in 1, 2, 4 and every format, `reps` resolve calls over all frames and, right after, `reps` K3-per-level calls
@@ -10,6 +10,11 @@ median over rounds of ms per call, and GB/s of bytes read plus written (K4: W*H 
 K3: 5 bytes per pixel).  Then the render alone at 1920x1080 and at 3840x2160 (plain b2d_render_device batches, events
 around the batches) and the 2x resolve of the 4K frames: the per-frame cost of 2x anti-aliasing.  The card's name, power
 limit and SM clock are read in the same run.
+
+--palettes times per-frame palettes instead: b2d_resolve_device against b2d_resolve_palettes_device with every frame on
+palette 0 and with seeded random palettes 0..13, the three calls alternated within each round, at 1080p grey k=2, 1080p
+planar RGB k=2, 1080p RGB k=1 and 4K RGB k=2 (the 4K frames rendered from the same poses).  Both calls stage one u32 per
+frame and run the same kernel, so the expectation is equal times within noise.
 """
 import argparse
 import json
@@ -59,12 +64,46 @@ def render_frames(b2d, scene, poses, w, h, batch):
     return r, idx, run
 
 
+def palette_rows(b2d, scene, poses, args):
+    """--palettes: ms per call of the three calls at each shape, median and spread over rounds"""
+    import torch
+    n = len(poses)
+    levels = np.zeros(n, np.uint32)
+    zero = np.zeros(n, np.uint32)
+    rand = np.random.default_rng(14).integers(0, 14, n).astype(np.uint32)
+    rows = []
+    for (w, h), k, fmt in (((W, H), 2, "gray"), ((W, H), 2, "rgb_planar"), ((W, H), 1, "rgb"), ((2 * W, 2 * H), 2, "rgb")):
+        r, idx, _ = render_frames(b2d, scene, poses, w, h, 250 if w == W else 125)
+        code = b2d.RESOLVE_FORMATS[fmt]
+        out = torch.empty(n * r.resolve_frame_bytes(k, code), dtype=torch.uint8, device="cuda")
+        calls = {"resolve_device": lambda: r.resolve_device(idx.data_ptr(), n, k, code, out.data_ptr(), levels),
+                 "palettes_0": lambda: r.resolve_device(idx.data_ptr(), n, k, code, out.data_ptr(), levels, palettes=zero),
+                 "palettes_random": lambda: r.resolve_device(idx.data_ptr(), n, k, code, out.data_ptr(), levels, palettes=rand)}
+        for fn in calls.values():
+            fn()
+        torch.cuda.synchronize()
+        t = {c: [] for c in calls}
+        for _ in range(args.rounds):
+            for c, fn in calls.items():
+                t[c].append(timed(fn, args.reps))
+        row = {"view": "%dx%d" % (w, h), "factor": k, "format": fmt}
+        for c in calls:
+            row[c] = {"ms": round(statistics.median(t[c]), 3), "ms_min": round(min(t[c]), 3), "ms_max": round(max(t[c]), 3)}
+        rows.append(row)
+        print("%s k=%d %-10s " % (row["view"], k, fmt) + "  ".join("%s %.3f ms (%.3f .. %.3f)" % (c, v["ms"], v["ms_min"], v["ms_max"])
+                                                                 for c, v in ((c, row[c]) for c in calls)))
+        del r, idx, out
+        torch.cuda.empty_cache()
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=1000)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--palettes", action="store_true", help="time per-frame palettes against b2d_resolve_device")
     args = ap.parse_args()
     import torch
     import rust_doom_b200 as b2d
@@ -73,6 +112,14 @@ def main():
     n = args.frames
     scene = b2d.Scene(b2d.Archive.from_bytes(synthwad.build_iwad(1, ("E1M1",))), 0)
     poses = P.flythrough_poses(scene, n, 2)
+    if args.palettes:
+        res = {"frames": n, "rounds": args.rounds, "reps": args.reps, "palettes": palette_rows(b2d, scene, poses, args)}
+        res.update(gpu_info())
+        print(json.dumps(res))
+        if args.out:
+            with open(args.out, "w") as f:
+                json.dump(res, f, indent=1)
+        return
     r, idx, render_1x = render_frames(b2d, scene, poses, W, H, 250)
     levels = np.zeros(n, np.uint32)
     out = torch.empty(n * W * H * 4, dtype=torch.uint8, device="cuda")
