@@ -839,6 +839,46 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
 // of 256; at 1920 columns every other CTA straddles two frames).
 constexpr int kRasterWarps = 8;
 
+// The CTA's draw queue (DESIGN.md §5).  Each warp's front-to-back clip pass turns its strip's draws into records instead
+// of drawing them; after a barrier every warp of the CTA pops records and draws them, so a CTA lasts about as long as its
+// average strip instead of its longest one.  A record is a header {meta, three warp-uniform arguments} and, per lane, the
+// packed window [ya, yb) -- for a wall piece also the texture column and iscale | light row << 24 (iscale <= 2^23).
+// meta = pool offset (words) | kind << 16 | visible << 17 | owner warp << 18.  Flat spans and the closing void fill are
+// plane records (void: not visible).  A record that does not fit is drawn by its owner at once, as without the queue.
+constexpr uint32_t kQueueWords = 6144;                 // per-lane record words per CTA (24 KB)
+constexpr uint32_t kQueueRecs = kQueueWords / 32;      // headers: every record has at least 32 per-lane words
+constexpr uint32_t kRecWall = 1u << 16, kRecVisible = 1u << 17;
+
+struct DrawQueue {
+    uint4 *head;                 // [kQueueRecs]
+    uint32_t *pool;              // [kQueueWords]
+    uint32_t *nrec, *nwords;     // records and words handed out (the words of a record that found no header are lost)
+};
+
+// warp-wide: append one record, or return false when it does not fit; a draw that no lane owns needs no record
+__device__ __forceinline__ bool queue_push(const DrawQueue &q, int lane, uint32_t meta, int32_t a, int32_t b, int32_t c,
+                                           int ya, int yb, int32_t ucol, uint32_t iscale_row) {
+    const bool act = ya < yb;
+    if (!__any_sync(kFull, act)) return true;
+    const bool wall = meta & kRecWall;
+    const uint32_t words = wall ? 96u : 32u;
+    uint32_t off = 0, i = kQueueRecs;
+    if (lane == 0) {
+        off = atomicAdd(q.nwords, words);
+        if (off + words <= kQueueWords) i = atomicAdd(q.nrec, 1u);
+    }
+    i = __shfl_sync(kFull, i, 0);
+    if (i >= kQueueRecs) return false;
+    off = __shfl_sync(kFull, off, 0);
+    q.pool[off + lane] = act ? (uint32_t)ya | ((uint32_t)yb << 16) : 0u;
+    if (wall) {
+        q.pool[off + 32 + lane] = (uint32_t)ucol;
+        q.pool[off + 64 + lane] = iscale_row;
+    }
+    if (lane == 0) q.head[i] = make_uint4(meta | off, (uint32_t)a, (uint32_t)b, (uint32_t)c);
+    return true;
+}
+
 template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels>
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
@@ -849,62 +889,77 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     __shared__ uint32_t s_pal[kRgba ? (kLevels ? 256 * kRasterWarps : 256) : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
     __shared__ uint32_t s_chunks[kRasterWarps][kMasked ? kMaskedCapMax / kMaskedChunk : 1];
+    // what a warp drawing another warp's record needs of its strip: per lane {plane direction, sky column, x}, and the frame
+    __shared__ int4 s_lanes[kRasterWarps][32];
+    __shared__ int s_frame[kRasterWarps];
+    __shared__ uint4 s_qhead[kQueueRecs];
+    __shared__ uint32_t s_qpool[kQueueWords];
+    __shared__ uint32_t s_qn[3];                  // records, words, records popped
+    // per-frame states or levels: each warp's copy of its frame's scene description (see below)
+    __shared__ DeviceScene s_scn[kStates || kLevels ? kRasterWarps : 1];
+    if (threadIdx.x < 3) s_qn[threadIdx.x] = 0;
     if (kRgba && !kLevels) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
         for (int i = threadIdx.x; i < 256; i += blockDim.x) s_pal[i] = sc.palette[i];
-        __syncthreads();
     }
+    __syncthreads();
 
-    const int lane = threadIdx.x & 31;
-    const long long gw = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (gw >= (long long)n * strips) return;
-    const int frame = (int)(gw / strips), strip = (int)(gw % strips);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long gw = (long long)blockIdx.x * (blockDim.x >> 5) + warp;
+    // The grid's last CTA may hold warps without a strip: they skip the clip pass but take part in every barrier and
+    // in the draw phase.
+    const bool has_strip = gw < (long long)n * strips;
+    const int frame = has_strip ? (int)(gw / strips) : 0, strip = has_strip ? (int)(gw % strips) : 0;
     const int W = kW ? kW : vw.W, H = vw.H;
     const int x0 = strip * 32, x = x0 + lane;
-    const bool inside = x < W;
+    const bool inside = has_strip && x < W;
+    const DrawQueue q{s_qhead, s_qpool, &s_qn[0], &s_qn[1]};
 
-    const FrameConst fc = frames[frame];
+    FrameConst fc{};
+    if (has_strip) fc = frames[frame];
     const DeviceScene *scp = &sc;
     if constexpr (kStates && !kLevels) {
         // per-frame states: this warp's copy of the scene description, its five state-dependent tables pointed into the
         // frame's arena slot (the walk passed the slot on in FrameConst::pad[0]); every table read below goes through it
-        __shared__ DeviceScene s_sc[kRasterWarps];
-        DeviceScene *d = &s_sc[threadIdx.x >> 5];
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(&sc);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(d);
-        for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
-        __syncwarp();
-        if (lane == 0) {
-            const uint8_t *tb = st.base + (size_t)(uint32_t)fc.pad[0] * st.slot_bytes;
-            d->tex = reinterpret_cast<const TexRec *>(tb);
-            d->sectors = reinterpret_cast<const SectorRec *>(tb + st.off_sectors);
-            d->segs = reinterpret_cast<const SegRec *>(tb + st.off_segs);
-            d->sprites = reinterpret_cast<const SpriteRec *>(tb + st.off_sprites);
-            d->mids = reinterpret_cast<const MidRec *>(tb + st.off_mids);
+        DeviceScene *d = &s_scn[warp];
+        if (has_strip) {
+            const uint32_t *src = reinterpret_cast<const uint32_t *>(&sc);
+            uint32_t *dst = reinterpret_cast<uint32_t *>(d);
+            for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
+            __syncwarp();
+            if (lane == 0) {
+                const uint8_t *tb = st.base + (size_t)(uint32_t)fc.pad[0] * st.slot_bytes;
+                d->tex = reinterpret_cast<const TexRec *>(tb);
+                d->sectors = reinterpret_cast<const SectorRec *>(tb + st.off_sectors);
+                d->segs = reinterpret_cast<const SegRec *>(tb + st.off_segs);
+                d->sprites = reinterpret_cast<const SpriteRec *>(tb + st.off_sprites);
+                d->mids = reinterpret_cast<const MidRec *>(tb + st.off_mids);
+            }
+            __syncwarp();
         }
-        __syncwarp();
         scp = d;
     }
     if constexpr (kLevels) {
         // per-frame levels: this warp's copy of the scene of the frame's level (the walk passed the level on in
         // FrameConst::pad[1]), and that level's palette
-        __shared__ DeviceScene s_lv[kRasterWarps];
-        DeviceScene *d = &s_lv[threadIdx.x >> 5];
-        const DeviceScene *lsrc = lt.scenes + (uint32_t)fc.pad[1];
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(lsrc);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(d);
-        for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
-        if (kRgba) {
-            const uint32_t *pal = lsrc->palette;
-            for (int i = lane; i < 256; i += 32) s_pal[256 * (threadIdx.x >> 5) + i] = pal[i];
-        }
-        __syncwarp();
-        if constexpr (kStates) {
-            // ... with per-frame states: its five state-dependent tables pointed at the frame's TableSet (FrameConst::pad[0])
-            if (lane == 0) {
-                const TableSet t = lt.sets[(uint32_t)fc.pad[0]];
-                d->tex = t.tex; d->sectors = t.sectors; d->segs = t.segs; d->sprites = t.sprites; d->mids = t.mids;
+        DeviceScene *d = &s_scn[warp];
+        if (has_strip) {
+            const DeviceScene *lsrc = lt.scenes + (uint32_t)fc.pad[1];
+            const uint32_t *src = reinterpret_cast<const uint32_t *>(lsrc);
+            uint32_t *dst = reinterpret_cast<uint32_t *>(d);
+            for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
+            if (kRgba) {
+                const uint32_t *pal = lsrc->palette;
+                for (int i = lane; i < 256; i += 32) s_pal[256 * warp + i] = pal[i];
             }
             __syncwarp();
+            if constexpr (kStates) {
+                // ... with per-frame states: its five state-dependent tables pointed at the frame's TableSet (FrameConst::pad[0])
+                if (lane == 0) {
+                    const TableSet t = lt.sets[(uint32_t)fc.pad[0]];
+                    d->tex = t.tex; d->sectors = t.sectors; d->segs = t.segs; d->sprites = t.sprites; d->mids = t.mids;
+                }
+                __syncwarp();
+            }
         }
         scp = d;
     }
@@ -912,22 +967,27 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     const DeviceScene &ls = kLevels ? ts : sc;     // the level's own fields (sky, masked-entry cap): = sc but per-frame levels
     RasterCtx c;
     c.sc = &ts;
-    c.pal_s = (uint32_t)__cvta_generic_to_shared(kLevels ? s_pal + 256 * (threadIdx.x >> 5) : s_pal);
-    c.rowz = s_rowz[threadIdx.x >> 5];
+    c.pal_s = (uint32_t)__cvta_generic_to_shared(kLevels ? s_pal + 256 * warp : s_pal);
+    c.rowz = s_rowz[warp];
+    c.W = W; c.H = H; c.x = x; c.lane = lane;
+    int mcount = 0;
+    uint32_t *chunks = s_chunks[warp];
+    asm("" : "+l"(chunks));        // a run-time value: propagated into masked_pass as a constant, it makes that pass spill more
+    const SegFrame *wl = work + (size_t)frame * stride;
+
+    if (has_strip) {
     c.dir = plane_dir(fc, vw, inside ? x : 0, ls.invF);
     c.fb = index_fb + (size_t)frame * W * H + (inside ? x : 0);
     c.rgba = kRgba ? rgba_fb + (size_t)frame * W * H + (inside ? x : 0) : nullptr;
-    c.W = W; c.H = H; c.x = x; c.lane = lane;
     c.skycol = 0;
     if (ls.sky_tex >= 0 && inside) c.skycol = umulhi32(sky_u32(x, vw, fc.pose.angle), ts.tex[ls.sky_tex].w);
+    s_lanes[warp][lane] = make_int4(c.dir.ax, c.dir.ay, (int)c.skycol, inside ? x : 0);
+    if (lane == 0) s_frame[warp] = frame;
 
     int ct = 0, cb = inside ? H : 0;              // open window [ct, cb) of this lane's column
-    uint32_t *chunks = s_chunks[threadIdx.x >> 5];
-    asm("" : "+l"(chunks));        // a run-time value: propagated into masked_pass as a constant, it makes that pass spill more
     const bool defer = kMasked && ls.masked_list != nullptr;
-    int mcount = 0;
-    const SegFrame *wl = work + (size_t)frame * stride;
     const int count = fc.count;
+    const uint32_t owner = (uint32_t)warp << 18;
     bool done = false;
 
     for (int k0 = 0; k0 < count && !done; k0 += 32) {
@@ -982,17 +1042,20 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
 #pragma unroll 1
             for (int pz = 0; pz < 2; pz++) {
                 const bool top = pz == 0;
-                draw_plane_warp<kRgba, kW>(c, fc, vw, ok ? (top ? ct : wr.y4) : 0, ok ? (top ? wr.y1 : yend) : 0,
-                                                    top ? fcl : ffl, top ? SF.ceil_flat : SF.floor_flat, SF.light,
-                                                    top ? ceil_vis : floor_vis);
+                const int ya = ok ? (top ? ct : wr.y4) : 0, yb = ok ? (top ? wr.y1 : yend) : 0;
+                const int32_t h = top ? fcl : ffl, flat = top ? SF.ceil_flat : SF.floor_flat;
+                const bool vis = top ? ceil_vis : floor_vis;
+                if (!queue_push(q, lane, owner | (vis ? kRecVisible : 0u), h, flat, SF.light, ya, yb, 0, 0u))
+                    draw_plane_warp<kRgba, kW>(c, fc, vw, ya, yb, h, flat, SF.light, vis);
             }
 #pragma unroll 1
             for (int pw = 0; pw < 2; pw++) {
                 const bool upper = pw == 0;            // piece A, then piece B
                 if (!wall_piece(upper, two, fcl, ffl, S.otop, S.obot)) continue;
-                draw_wall_warp<kRgba, kW>(c, fc, ok ? (upper ? wr.y1 : wr.y3) : 0, ok ? (upper ? wr.y2 : wr.y4) : 0,
-                                                   upper ? S.texA : S.texB, upper ? S.tA : S.tB, upper ? S.hA : S.hB,
-                                                   ucol, ce.iscale, row);
+                const int ya = ok ? (upper ? wr.y1 : wr.y3) : 0, yb = ok ? (upper ? wr.y2 : wr.y4) : 0;
+                const int32_t tex = upper ? S.texA : S.texB, tA = upper ? S.tA : S.tB, hA = upper ? S.hA : S.hB;
+                if (!queue_push(q, lane, owner | kRecWall, tex, tA, hA, ya, yb, ucol, (uint32_t)ce.iscale | ((uint32_t)row << 24)))
+                    draw_wall_warp<kRgba, kW>(c, fc, ya, yb, tex, tA, hA, ucol, ce.iscale, row);
             }
             if (ok) wall_window(two, wr, H, ct, cb);
             if (defer && two && S.mid >= 0) {
@@ -1009,10 +1072,47 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         }
     }
     // whatever is still open is void
-    fill_void_warp<kRgba, kW>(c, inside ? ct : 0, inside ? cb : 0);
-    if (kMasked && mcount > 0) {
-        __syncwarp();
-        masked_pass<kRgba, kW, kStates, kLevels>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
+    if (!queue_push(q, lane, owner, 0, 0, 0, inside ? ct : 0, inside ? cb : 0, 0, 0u))
+        fill_void_warp<kRgba, kW>(c, inside ? ct : 0, inside ? cb : 0);
+    }
+
+    // Draw phase: every warp of the CTA pops records until the queue is empty.  Order does not matter: the clip windows
+    // of a strip's draws are disjoint, so every byte is still written once.
+    __syncthreads();
+    const uint32_t nrec = min(s_qn[0], kQueueRecs);
+    for (;;) {
+        uint32_t i = 0;
+        if (lane == 0) i = atomicAdd(&s_qn[2], 1u);
+        i = __shfl_sync(kFull, i, 0);
+        if (i >= nrec) break;
+        const uint4 hd = s_qhead[i];
+        const uint32_t off = hd.x & 0xFFFFu, o = hd.x >> 18;
+        const int4 ln = s_lanes[o][lane];
+        const int f = s_frame[o];
+        const FrameConst fo = frames[f];
+        RasterCtx d;
+        d.sc = kStates || kLevels ? &s_scn[o] : &sc;      // the owner's scene description
+        d.pal_s = (uint32_t)__cvta_generic_to_shared(kLevels ? s_pal + 256 * o : s_pal);
+        d.rowz = s_rowz[warp];
+        d.dir = PlaneDir{ln.x, ln.y};
+        d.fb = index_fb + (size_t)f * W * H + ln.w;
+        d.rgba = kRgba ? rgba_fb + (size_t)f * W * H + ln.w : nullptr;
+        d.W = W; d.H = H; d.x = ln.w; d.lane = lane;
+        d.skycol = (uint32_t)ln.z;
+        const uint32_t win = s_qpool[off + lane];
+        const int ya = (int)(win & 0xFFFFu), yb = (int)(win >> 16);
+        if (hd.x & kRecWall) {
+            const uint32_t isr = s_qpool[off + 64 + lane];
+            draw_wall_warp<kRgba, kW>(d, fo, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int32_t)hd.w, (int32_t)s_qpool[off + 32 + lane],
+                                      (int32_t)(isr & 0xFFFFFFu), (int)(isr >> 24));
+        } else {
+            draw_plane_warp<kRgba, kW>(d, fo, vw, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int)hd.w, hd.x & kRecVisible);
+        }
+    }
+    if constexpr (kMasked) {
+        // the masked pass overwrites solid pixels of its own strip: every draw of the CTA must be done first
+        __syncthreads();
+        if (mcount > 0) masked_pass<kRgba, kW, kStates, kLevels>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
     }
 }
 
@@ -1307,9 +1407,9 @@ cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw
 // columns and at other widths).  The warps that write the sectors of the same 128-byte frame lines, and of the next lines
 // of the same rows, then start together on one SM and finish those lines close together in time, so fewer partly written
 // lines sit in L2.  Against four-warp CTAs (one line group) that is worth 3.8 % of the bench.py c2 step and 5.9 % at 4K,
-// although residency falls from 20 to 16 warps per SM and the slots of a CTA's finished warps idle until its slowest strip
-// is done.  The registers are left to the compiler (cap 128): 86 for the 1080p and 4K index-only kernels, i.e. 2 CTAs
-// = 16 warps per SM (DESIGN.md §6).
+// although residency falls from 20 to 16 warps per SM.  The CTA's draw queue shares the strips' draws among its warps, so
+// a finished strip's warp draws for its slower siblings instead of idling.  The registers are left to the compiler (cap
+// 128): 94 for the 1080p and 4K index-only kernels, i.e. 2 CTAs = 16 warps per SM (DESIGN.md §5, §6).
 // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
 template <bool kStates, bool kLevels>
 static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
