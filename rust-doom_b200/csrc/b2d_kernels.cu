@@ -849,8 +849,21 @@ constexpr uint32_t kQueueWords = 6144;                 // per-lane record words 
 constexpr uint32_t kQueueRecs = kQueueWords / 32;      // headers: every record has at least 32 per-lane words
 constexpr uint32_t kRecWall = 1u << 16, kRecVisible = 1u << 17;
 
+// The queue is drawn in row bands (DESIGN.md §5): a work item is (band, record) with the record's windows clipped to the
+// band, and items go out band by band, so the CTA's stores sweep down its frame rows and a 128-byte line is finished soon
+// after it is started.  Every pixel depends only on its absolute row, so clipping changes no byte.  kBandRows is a
+// multiple of 32: band starts fall on the flat spans' 32-row constant chunks and on the wall batches of 8 and 16 rows.
+// The item list holds kItemCap items {record | band << 8}; a CTA with more draws its records whole, in record order, and
+// so does a CTA with a deferred masked entry: its masked pass rewrites pixels of lines that banding has already finished
+// and streamed out of L2 (DESIGN.md §6).
+constexpr int kBandRows = 256;
+constexpr int kMaxBands = (2160 + kBandRows - 1) / kBandRows;   // b2d_view_init accepts at most 2160 rows
+constexpr uint32_t kItemCap = 1024;
+static_assert(kBandRows % 32 == 0 && kMaxBands <= 256 && kQueueRecs <= 256, "an item is record | band << 8 in 16 bits");
+
 struct DrawQueue {
     uint4 *head;                 // [kQueueRecs]
+    uint32_t *ext;               // [kQueueRecs] the record's warp extent y0 | y1 << 16 (min ya, max yb over active lanes)
     uint32_t *pool;              // [kQueueWords]
     uint32_t *nrec, *nwords;     // records and words handed out (the words of a record that found no header are lost)
 };
@@ -860,6 +873,8 @@ __device__ __forceinline__ bool queue_push(const DrawQueue &q, int lane, uint32_
                                            int ya, int yb, int32_t ucol, uint32_t iscale_row) {
     const bool act = ya < yb;
     if (!__any_sync(kFull, act)) return true;
+    const uint32_t y0 = __reduce_min_sync(kFull, act ? (uint32_t)ya : 0xFFFFu);
+    const uint32_t y1 = __reduce_max_sync(kFull, act ? (uint32_t)yb : 0u);
     const bool wall = meta & kRecWall;
     const uint32_t words = wall ? 96u : 32u;
     uint32_t off = 0, i = kQueueRecs;
@@ -875,7 +890,10 @@ __device__ __forceinline__ bool queue_push(const DrawQueue &q, int lane, uint32_
         q.pool[off + 32 + lane] = (uint32_t)ucol;
         q.pool[off + 64 + lane] = iscale_row;
     }
-    if (lane == 0) q.head[i] = make_uint4(meta | off, (uint32_t)a, (uint32_t)b, (uint32_t)c);
+    if (lane == 0) {
+        q.head[i] = make_uint4(meta | off, (uint32_t)a, (uint32_t)b, (uint32_t)c);
+        q.ext[i] = y0 | y1 << 16;
+    }
     return true;
 }
 
@@ -893,11 +911,15 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     __shared__ int4 s_lanes[kRasterWarps][32];
     __shared__ int s_frame[kRasterWarps];
     __shared__ uint4 s_qhead[kQueueRecs];
+    __shared__ uint32_t s_qext[kQueueRecs];
     __shared__ uint32_t s_qpool[kQueueWords];
-    __shared__ uint32_t s_qn[3];                  // records, words, records popped
+    __shared__ uint16_t s_items[kItemCap];       // band-major work items: record | band << 8
+    __shared__ uint32_t s_band[kMaxBands];       // items per band, then each band's next slot in s_items
+    __shared__ uint32_t s_qn[5];                  // records, words, items popped, items, a warp deferred masked entries
     // per-frame states or levels: each warp's copy of its frame's scene description (see below)
     __shared__ DeviceScene s_scn[kStates || kLevels ? kRasterWarps : 1];
-    if (threadIdx.x < 3) s_qn[threadIdx.x] = 0;
+    if (threadIdx.x < 5) s_qn[threadIdx.x] = 0;
+    for (int b = threadIdx.x; b < kMaxBands; b += blockDim.x) s_band[b] = 0;
     if (kRgba && !kLevels) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
         for (int i = threadIdx.x; i < 256; i += blockDim.x) s_pal[i] = sc.palette[i];
     }
@@ -912,7 +934,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     const int W = kW ? kW : vw.W, H = vw.H;
     const int x0 = strip * 32, x = x0 + lane;
     const bool inside = has_strip && x < W;
-    const DrawQueue q{s_qhead, s_qpool, &s_qn[0], &s_qn[1]};
+    const DrawQueue q{s_qhead, s_qext, s_qpool, &s_qn[0], &s_qn[1]};
 
     FrameConst fc{};
     if (has_strip) fc = frames[frame];
@@ -1076,15 +1098,64 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         fill_void_warp<kRgba, kW>(c, inside ? ct : 0, inside ? cb : 0);
     }
 
-    // Draw phase: every warp of the CTA pops records until the queue is empty.  Order does not matter: the clip windows
-    // of a strip's draws are disjoint, so every byte is still written once.
+    if (kMasked && mcount > 0 && lane == 0) s_qn[4] = 1;
+    // Draw phase: every warp of the CTA pops work items until the list is empty.  Correctness does not depend on the
+    // order: the clip windows of a strip's draws are disjoint, so every byte is still written once.
     __syncthreads();
     const uint32_t nrec = min(s_qn[0], kQueueRecs);
+    // the band-major item list, a counting sort: items per band, an exclusive scan, then each record scattered to its bands
+    for (uint32_t r = threadIdx.x; r < nrec; r += blockDim.x) {
+        const uint32_t e = s_qext[r];
+        for (uint32_t b = (e & 0xFFFFu) / kBandRows; b <= ((e >> 16) - 1u) / kBandRows; b++) atomicAdd(&s_band[b], 1u);
+    }
+    __syncthreads();
+    if (warp == 0) {
+        constexpr int kPer = (kMaxBands + 31) / 32;
+        uint32_t v[kPer], sum = 0;
+#pragma unroll
+        for (int k = 0; k < kPer; k++) {
+            const int b = lane * kPer + k;
+            v[k] = b < kMaxBands ? s_band[b] : 0u;
+            sum += v[k];
+        }
+        uint32_t incl = sum;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t u = __shfl_up_sync(kFull, incl, d);
+            if (lane >= d) incl += u;
+        }
+        uint32_t at = incl - sum;
+#pragma unroll
+        for (int k = 0; k < kPer; k++) {
+            const int b = lane * kPer + k;
+            if (b < kMaxBands) s_band[b] = at;
+            at += v[k];
+        }
+        if (lane == 31) s_qn[3] = incl;
+    }
+    __syncthreads();
+    const bool banded = s_qn[3] <= kItemCap && !(kMasked && s_qn[4]);
+    if (banded) {
+        for (uint32_t r = threadIdx.x; r < nrec; r += blockDim.x) {
+            const uint32_t e = s_qext[r];
+            for (uint32_t b = (e & 0xFFFFu) / kBandRows; b <= ((e >> 16) - 1u) / kBandRows; b++)
+                s_items[atomicAdd(&s_band[b], 1u)] = (uint16_t)(r | b << 8);
+        }
+        __syncthreads();
+    }
+    const uint32_t nitems = banded ? s_qn[3] : nrec;
     for (;;) {
         uint32_t i = 0;
         if (lane == 0) i = atomicAdd(&s_qn[2], 1u);
         i = __shfl_sync(kFull, i, 0);
-        if (i >= nrec) break;
+        if (i >= nitems) break;
+        int lo = 0, hi = H;
+        if (banded) {
+            const uint32_t it = s_items[i];
+            i = it & 0xFFu;
+            lo = (int)(it >> 8) * kBandRows;
+            hi = lo + kBandRows;
+        }
         const uint4 hd = s_qhead[i];
         const uint32_t off = hd.x & 0xFFFFu, o = hd.x >> 18;
         const int4 ln = s_lanes[o][lane];
@@ -1100,7 +1171,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         d.W = W; d.H = H; d.x = ln.w; d.lane = lane;
         d.skycol = (uint32_t)ln.z;
         const uint32_t win = s_qpool[off + lane];
-        const int ya = (int)(win & 0xFFFFu), yb = (int)(win >> 16);
+        const int ya = max((int)(win & 0xFFFFu), lo), yb = min((int)(win >> 16), hi);
         if (hd.x & kRecWall) {
             const uint32_t isr = s_qpool[off + 64 + lane];
             draw_wall_warp<kRgba, kW>(d, fo, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int32_t)hd.w, (int32_t)s_qpool[off + 32 + lane],
