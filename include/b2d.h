@@ -351,6 +351,39 @@ int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, cons
                                   const b2d_frame_state *states, size_t n, const b2d_sector_move *moves,
                                   size_t n_moves, void *cuda_stream, int64_t *ticket_out);
 
+/* The player's light effects per frame (Doom's R_SetupFrame reads them from the player; DESIGN.md C18).
+ * fixed_colormap: -1, or the COLORMAP row 0..32 that every wall, flat, masked-middle and sprite pixel of the frame goes
+ * through instead of the row its light and depth select; sky pixels stay on row 0.  Doom uses 32 (INVERSECOLORMAP) for
+ * the invulnerability sphere and 1 for the light-amplification visor; blinking as a power wears off is the host's choice.
+ * extralight: 0..2, the A_Light1 / A_Light2 weapon flashes: every light level is raised by that many of Doom's 16 steps
+ * (ignored under a fixed colormap).
+ *
+ * The _lights forms of the three level-set calls with per-frame states take `lights` (a HOST array, one entry per frame,
+ * right after `states`) and are otherwise those calls: frame i is frame i of the call without lights, lit as lights[i]
+ * says.  lights == NULL, or every entry {-1, 0}, gives the frames and launches of the call without lights.  Frames share a
+ * table set when their (level, compact state, extralight) are equal; a frame with extra light on a level without
+ * time-dependent content or dynamic sectors gets a set expanded from the level's rest state.  A batch with a fixed colormap
+ * rasters with the fixed-colormap variant of the raster, in the same launch.  The first call that asks for row 32 on a
+ * level builds that level's row-32 texel and flat planes on its stream (two more launches, once per level and renderer).
+ * fixed_colormap outside -1..32 and extralight > 2 are B2D_ERR_INVALID_ARG, detected before anything is enqueued, as are
+ * the refusals of the calls without lights.  The ticket of b2d_walk_device_levels_states_lights is rastered by
+ * b2d_raster_device; each frame's fixed colormap is staged with its levels, under the same wait. */
+typedef struct b2d_frame_light {
+    int32_t fixed_colormap;           /* -1, or a COLORMAP row 0..32 */
+    uint32_t extralight;              /* 0..2 */
+} b2d_frame_light;
+int b2d_render_levels_states_lights(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels,
+                                    const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
+                                    const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb);
+int b2d_render_device_levels_states_lights(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
+                                           const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
+                                           const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb,
+                                           uint32_t *d_rgba_fb, void *cuda_stream);
+int b2d_walk_device_levels_states_lights(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
+                                         const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
+                                         const b2d_sector_move *moves, size_t n_moves, void *cuda_stream,
+                                         int64_t *ticket_out);
+
 /* Kernel 3 with a palette per frame: frame f of the n_frames contiguous W x H index frames at d_index (W x H: the
  * renderer's view) goes through the palette of level levels[f] into d_rgba, as the RGBA output of b2d_render_levels
  * colours it; on a set of one level it is b2d_palette_lut_device over n_frames * W * H pixels.  For gathered frames of a

@@ -145,6 +145,18 @@ def _frame_states(tics, moves_per_pose, n: int):
     return states, arr, nm
 
 
+def _frame_lights(lights, n: int):
+    """b2d_frame_light array for n poses from (fixed_colormap, extralight) pairs, one per pose (a sequence or an (n, 2)
+    integer array); the values are checked by the library (fixed_colormap -1..32, extralight 0..2)."""
+    a = np.asarray(lights, dtype=np.int64).reshape(-1, 2) if n else np.zeros((0, 2), np.int64)
+    assert len(a) == n, "one (fixed_colormap, extralight) pair per pose"
+    if n and (a[:, 0].min() < -2 ** 31 or a[:, 0].max() >= 2 ** 31 or a[:, 1].min() < 0 or a[:, 1].max() >= 2 ** 32):
+        raise B2dError(ERR_INVALID_ARG, "frame light out of range")
+    rec = np.zeros(max(n, 1), dtype=[("fixed_colormap", "<i4"), ("extralight", "<u4")])
+    rec["fixed_colormap"][:n], rec["extralight"][:n] = a[:, 0], a[:, 1]
+    return (_lib.FrameLight * max(n, 1)).from_buffer_copy(rec.tobytes())
+
+
 class Scene:
     def __init__(self, archive: Optional[Archive], level_index: int = 0, _handle=None, dynamic=()):
         """`dynamic`: (sector, floor_min, floor_max, ceil_min, ceil_max) per sector that may move (b2d_scene_create_dynamic)"""
@@ -489,36 +501,53 @@ class Renderer:
         _check(_lib.load().b2d_walk_device_levels(self._h, poses_ptr, lv.ctypes.data, n, stream or None, ctypes.byref(t)))
         return int(t.value)
 
-    def render_levels_states(self, poses: np.ndarray, levels, tics, moves_per_pose=None, rgba: bool = False):
+    def render_levels_states(self, poses: np.ndarray, levels, tics, moves_per_pose=None, rgba: bool = False, lights=None):
         """b2d_render_levels_states: pose i rendered from level levels[i] at level time tics[i] with the sector moves
-        moves_per_pose[i] of that level (None = every pose at rest), without touching the renderer's own time and moves."""
+        moves_per_pose[i] of that level (None = every pose at rest), without touching the renderer's own time and moves.
+        `lights`: None, or one (fixed_colormap, extralight) pair per pose (b2d_render_levels_states_lights, DESIGN.md C18)."""
         poses = np.ascontiguousarray(poses, dtype=POSE_DTYPE)
         n = len(poses)
         lv = _levels_array(levels, n)
         states, arr, nm = _frame_states(tics, moves_per_pose, n)
         out_index = np.empty((n, self.height, self.width), dtype=np.uint8)
         out_rgba = np.empty((n, self.height, self.width), dtype=np.uint32) if rgba else None
-        _check(_lib.load().b2d_render_levels_states(self._h, poses.ctypes.data, lv.ctypes.data, states, n, arr, nm,
-                                                    out_index.ctypes.data, out_rgba.ctypes.data if rgba else None))
+        if lights is None:
+            _check(_lib.load().b2d_render_levels_states(self._h, poses.ctypes.data, lv.ctypes.data, states, n, arr, nm,
+                                                        out_index.ctypes.data, out_rgba.ctypes.data if rgba else None))
+        else:
+            _check(_lib.load().b2d_render_levels_states_lights(self._h, poses.ctypes.data, lv.ctypes.data, states,
+                                                               _frame_lights(lights, n), n, arr, nm, out_index.ctypes.data,
+                                                               out_rgba.ctypes.data if rgba else None))
         return (out_index, out_rgba) if rgba else out_index
 
     def render_device_levels_states(self, poses_ptr: int, levels, tics, n: int, index_ptr: int, rgba_ptr: int = 0,
-                                    moves_per_pose=None, stream: int = 0):
+                                    moves_per_pose=None, stream: int = 0, lights=None):
         """b2d_render_device_levels_states: device poses / frames, per-frame levels and states as in
-        render_levels_states; n may exceed max_batch."""
+        render_levels_states; n may exceed max_batch.  `lights` as in render_levels_states."""
         lv = _levels_array(levels, n)
         states, arr, nm = _frame_states(tics, moves_per_pose, n)
-        _check(_lib.load().b2d_render_device_levels_states(self._h, poses_ptr, lv.ctypes.data, states, n, arr, nm, index_ptr,
-                                                           rgba_ptr or None, stream or None))
+        if lights is None:
+            _check(_lib.load().b2d_render_device_levels_states(self._h, poses_ptr, lv.ctypes.data, states, n, arr, nm, index_ptr,
+                                                               rgba_ptr or None, stream or None))
+        else:
+            _check(_lib.load().b2d_render_device_levels_states_lights(self._h, poses_ptr, lv.ctypes.data, states,
+                                                                      _frame_lights(lights, n), n, arr, nm, index_ptr,
+                                                                      rgba_ptr or None, stream or None))
 
-    def walk_device_levels_states(self, poses_ptr: int, levels, tics, n: int, moves_per_pose=None, stream: int = 0) -> int:
+    def walk_device_levels_states(self, poses_ptr: int, levels, tics, n: int, moves_per_pose=None, stream: int = 0,
+                                  lights=None) -> int:
         """b2d_walk_device_levels_states: the walk of a batch (1..max_batch) with per-frame levels and states; returns the
-        ticket for raster_device."""
+        ticket for raster_device.  `lights` as in render_levels_states."""
         lv = _levels_array(levels, n)
         states, arr, nm = _frame_states(tics, moves_per_pose, n)
         t = ctypes.c_int64(-1)
-        _check(_lib.load().b2d_walk_device_levels_states(self._h, poses_ptr, lv.ctypes.data, states, n, arr, nm, stream or None,
-                                                         ctypes.byref(t)))
+        if lights is None:
+            _check(_lib.load().b2d_walk_device_levels_states(self._h, poses_ptr, lv.ctypes.data, states, n, arr, nm,
+                                                             stream or None, ctypes.byref(t)))
+        else:
+            _check(_lib.load().b2d_walk_device_levels_states_lights(self._h, poses_ptr, lv.ctypes.data, states,
+                                                                    _frame_lights(lights, n), n, arr, nm, stream or None,
+                                                                    ctypes.byref(t)))
         return int(t.value)
 
     def render_ptr(self, poses_ptr: int, n: int, index_ptr: int, rgba_ptr: int = 0):

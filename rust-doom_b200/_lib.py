@@ -40,6 +40,11 @@ class FrameState(ctypes.Structure):
     _fields_ = [("tics", ctypes.c_uint32), ("first_move", ctypes.c_uint32), ("n_moves", ctypes.c_uint32)]
 
 
+class FrameLight(ctypes.Structure):
+    """b2d_frame_light: fixed colormap (-1, or a COLORMAP row 0..32) and extra light (0..2) of a frame"""
+    _fields_ = [("fixed_colormap", ctypes.c_int32), ("extralight", ctypes.c_uint32)]
+
+
 EXPORTS = [
     "b2d_last_error", "b2d_archive_open", "b2d_archive_open_memory", "b2d_archive_open_files", "b2d_archive_open_memory_files", "b2d_archive_num_levels",
     "b2d_archive_level_name", "b2d_archive_close", "b2d_wad_name", "b2d_scene_create", "b2d_scene_create_from_lumps", "b2d_scene_create_dynamic",
@@ -59,6 +64,7 @@ EXPORTS = [
     "b2d_resolve_device", "b2d_resolve_frame_bytes", "b2d_render_sharded_resolved", "b2d_render_sharded_levels_states_resolved",
     "b2d_scene_num_palettes", "b2d_scene_set_palettes", "b2d_resolve_palettes_device",
     "b2d_render_sharded_levels_states_resolved_palettes",
+    "b2d_render_levels_states_lights", "b2d_render_device_levels_states_lights", "b2d_walk_device_levels_states_lights",
 ]
 
 COMM_ID_BYTES = 128
@@ -169,6 +175,12 @@ def load() -> ctypes.CDLL:
                                                   vp, vp, vp]
     L.b2d_walk_device_levels_states.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), cs, ctypes.POINTER(SectorMove), cs, vp,
                                                 ctypes.POINTER(ctypes.c_int64)]
+    L.b2d_render_levels_states_lights.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), ctypes.POINTER(FrameLight), cs,
+                                                  ctypes.POINTER(SectorMove), cs, vp, vp]
+    L.b2d_render_device_levels_states_lights.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), ctypes.POINTER(FrameLight),
+                                                         cs, ctypes.POINTER(SectorMove), cs, vp, vp, vp]
+    L.b2d_walk_device_levels_states_lights.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), ctypes.POINTER(FrameLight),
+                                                       cs, ctypes.POINTER(SectorMove), cs, vp, ctypes.POINTER(ctypes.c_int64)]
     L.b2d_palette_lut_device.argtypes = [vp, vp, vp, cs, vp]
     L.b2d_debug_worklist.argtypes = [vp, cs, vp, vp, cs]
     L.b2d_debug_state_slots.argtypes = [vp, cs, vp]

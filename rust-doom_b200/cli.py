@@ -25,7 +25,11 @@ block's palette colours, each frame through its own level's palette): an anti-al
 
 --palette P colours the dumped and streamed frames through PLAYPAL palette P of each frame's level instead of palette 0
 (b2d_resolve_palettes_device; in Doom 1..8 are the damage flash, 9..12 the bonus flash, 13 the radiation suit), through
-the resolve at the --supersample factor (1 by default).  With --levels too; not with --world."""
+the resolve at the --supersample factor (1 by default).  With --levels too; not with --world.
+
+--fixed-colormap R and --extralight E light every frame of --levels as a player with those effects (DESIGN.md C18,
+b2d_render_levels_states_lights): R = 32 is Doom's invulnerability (INVERSECOLORMAP), 1 its light-amplification visor;
+E = 1 or 2 its weapon flashes.  Not with --world."""
 from __future__ import annotations
 
 import argparse
@@ -183,13 +187,15 @@ def _main_levels(b2d, arch, set_, view, args, w, h) -> int:
     n = len(poses)
     if not args.world:
         r = b2d.Renderer.from_levels(scenes, view, device=args.device, max_batch=min(n, 64))
+        lights = [(args.fixed_colormap, args.extralight)] * n if (args.fixed_colormap, args.extralight) != (-1, 0) else None
         if args.supersample > 1 or args.palette:
-            rgb = resolve_rgb(r, r.render_levels_states(poses, levels, tics), args.supersample, levels, args.palette)
+            rgb = resolve_rgb(r, r.render_levels_states(poses, levels, tics, lights=lights), args.supersample, levels,
+                              args.palette)
             print("rendered %d frame(s) %dx%d of %d level(s), supersampled %dx, palette %d" % (n, w, h, len(set_), args.supersample,
                                                                                              args.palette))
             frame = lambda i: rgb[i]    # noqa: E731
         else:
-            rgba = r.render_levels_states(poses, levels, tics, rgba=True)[1]
+            rgba = r.render_levels_states(poses, levels, tics, rgba=True, lights=lights)[1]
             print("rendered %d frame(s) %dx%d of %d level(s)" % (n, w, h, len(set_)))
             frame = lambda i: rgba_to_rgb(rgba[i])    # noqa: E731
         if args.dump:
@@ -276,6 +282,9 @@ def main(argv=None) -> int:
                     help="render at K times the resolution (1..8) and resolve every K x K block to one output pixel")
     ap.add_argument("--palette", type=int, default=0,
                     help="colour the frames through PLAYPAL palette P (Doom: 1..8 damage, 9..12 bonus, 13 radiation suit)")
+    ap.add_argument("--fixed-colormap", type=int, default=-1,
+                    help="with --levels: light every frame through COLORMAP row R, -1..32 (32 invulnerability, 1 visor)")
+    ap.add_argument("--extralight", type=int, default=0, help="with --levels: raise every light by E (0..2) weapon-flash steps")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 
@@ -297,6 +306,16 @@ def main(argv=None) -> int:
     if args.palette and (args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1):
         print("--palette does not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
         return 2
+    if not -1 <= args.fixed_colormap <= 32 or not 0 <= args.extralight <= 2:
+        print("--fixed-colormap takes a row in -1..32 and --extralight a value in 0..2", file=sys.stderr)
+        return 2
+    if (args.fixed_colormap, args.extralight) != (-1, 0):
+        if args.levels is None:
+            print("--fixed-colormap and --extralight take --levels", file=sys.stderr)
+            return 2
+        if args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            print("--fixed-colormap and --extralight do not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
+            return 2
     try:
         arch = b2d.Archive.open(args.iwad) if args.iwad else b2d.Archive.from_bytes(synthwad.build_iwad(1, synthwad.E1_MAPS[:3]))
         if args.command == "list-levels":

@@ -167,15 +167,19 @@ struct StageLayout {
     size_t scenes = 0;         // with per-frame levels: the DeviceScene of every level
     size_t srcs, sets, descs;  // StateSrc of every level | TableSet of every set to expand, then, with per-frame states, of
                                // every level's blob tables | StateSet of every set to expand
-    size_t frame_level, frame_set, states, end;  // per frame: level | TableSet index (per-frame states) | the sets' states
-    StageLayout(size_t nlev, size_t nsets, size_t n, size_t state_words, bool per_frame, bool per_level) {
+    size_t frame_level, frame_set;  // per frame: level | TableSet index (per-frame states)
+    size_t frame_fixed, planes;     // with fixed colormaps: per frame its row | per level its FixedPlanes
+    size_t states, end;             // the sets' states
+    StageLayout(size_t nlev, size_t nsets, size_t n, size_t state_words, bool per_frame, bool per_level, bool fixed_rows = false) {
         auto up = [](size_t x) { return (x + 15) & ~(size_t)15; };
         srcs = up((per_level ? nlev : 0) * sizeof(DeviceScene));
         sets = up(srcs + nlev * sizeof(StateSrc));
         descs = up(sets + (nsets + (per_frame ? nlev : 0)) * sizeof(TableSet));
         frame_level = up(descs + nsets * sizeof(StateSet));
         frame_set = up(frame_level + (per_level ? 4 * n : 0));
-        states = up(frame_set + (per_frame ? 4 * n : 0));
+        frame_fixed = up(frame_set + (per_frame ? 4 * n : 0));
+        planes = up(frame_fixed + (fixed_rows ? 4 * n : 0));
+        states = up(planes + (fixed_rows ? nlev * sizeof(FixedPlanes) : 0));
         end = states + 4 * state_words;
     }
 };
@@ -218,12 +222,40 @@ int profiled(b2d_renderer *r, cudaStream_t stream, int kind, Launch launch) {
     return B2D_OK;
 }
 
-// A table set a batch expands: level `level` at the compact state `state` (host) into the tables at `tables`.
+// A table set a batch expands: level `level` at the compact state `state` (host) with extra light `extralight` into the
+// tables at `tables`.
 struct Expansion {
     uint32_t level;
     const uint32_t *state;
     uint8_t *tables;
+    uint32_t extralight;
 };
+
+// bytes of one level's state-dependent tables, [tex | sectors | segs | sprites | mids]
+size_t level_table_bytes(const LevelRes &lv) {
+    return lv.src.ntex * sizeof(TexRec) + lv.src.nsectors * sizeof(SectorRec) + lv.src.nsegs * sizeof(SegRec) +
+           lv.src.nsprites * sizeof(SpriteRec) + lv.src.nmids * sizeof(MidRec);
+}
+
+// Level `lv`'s row-32 planes (fixed colormap 32, DESIGN.md C18), built on `stream` by the first batch that needs them: the
+// group is created whole, or not at all.
+int ensure_row32(b2d_renderer *r, LevelRes &lv, cudaStream_t stream) {
+    if (lv.row32) return B2D_OK;
+    std::unique_ptr<LevelRes::Row32> g(new (std::nothrow) LevelRes::Row32());
+    if (!g) return fail(B2D_ERR_NO_MEMORY, "out of host memory");
+    const DeviceScene &d = lv.ds;
+    CU(allocate(g->texels, (size_t)d.lit_texel_stride + 256));
+    g->flats = alloc_aligned_4g(r->device, (size_t)d.lit_flat_stride + 256);
+    if (!g->flats) return fail(B2D_ERR_NO_MEMORY, "no 4 GiB aligned device memory for the row-32 flats");
+    CU(event_create(g->built));
+    const uint8_t *row = d.colormap + 32 * 256;
+    CU(launch_prelight_textures_row(row, d.texels, d.tex, d.ntex, g->texels.get(), stream));
+    CU(launch_prelight_row(row, d.flats, g->flats.get(), d.lit_flat_stride, stream));
+    CU(cudaEventRecord(g->built.get(), stream));
+    r->launches += (d.ntex > 0) + (d.lit_flat_stride > 0);
+    lv.row32 = std::move(g);
+    return B2D_OK;
+}
 
 // the state-dependent tables (level time `tics`, sector offsets), laid out [tex | sectors | segs | sprites | mids]
 size_t state_table_bytes(const uint8_t *blob) {
@@ -290,7 +322,7 @@ int b2d::build_states(const b2d_renderer *r, const b2d_frame_state *states, cons
                 for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
             }
             compact_state(lv.h_blob.data(), lv.layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
-                          fs.data() + starts[i]);
+                          fs.data() + starts[i], out.lights ? out.lights[i].extralight : 0u);
         }
         out.fs = fs.data();
         out.starts = !levels && r->lv[0].h_blob.empty() ? nullptr : starts.data();
@@ -304,6 +336,19 @@ int b2d::check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
         return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
     for (size_t i = 0; i < n; i++)
         if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    return B2D_OK;
+}
+
+int b2d::check_lights(const b2d_frame_light *&lights, size_t n) {
+    if (!lights) return B2D_OK;
+    bool any = false;
+    for (size_t i = 0; i < n; i++) {
+        if (lights[i].fixed_colormap < -1 || lights[i].fixed_colormap > 32)
+            return fail(B2D_ERR_INVALID_ARG, "frame fixed colormap out of range (-1 .. 32)");
+        if (lights[i].extralight > 2) return fail(B2D_ERR_INVALID_ARG, "frame extra light out of range (0 .. 2)");
+        any = any || lights[i].fixed_colormap != -1 || lights[i].extralight != 0;
+    }
+    if (!any) lights = nullptr;
     return B2D_OK;
 }
 
@@ -342,6 +387,19 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
     if (rc != B2D_OK) return rc;
     const size_t nlev = r->lv.size();
     auto level = [&](int f) { return per_level ? fr.levels[f] : 0u; };
+    // fixed colormaps (per-frame levels and states only): the row-32 planes of every level a frame asks for them on,
+    // built on this stream the first time, and awaited by this batch's walk (and so by its raster)
+    bool fixed_rows = false;
+    for (int f = 0; f < n && fr.lights && per_frame && per_level; f++) {
+        const int32_t row = fr.lights[f].fixed_colormap;
+        fixed_rows = fixed_rows || row >= 0;
+        if (row != 32) continue;
+        LevelRes &lv = r->lv[level(f)];
+        const bool built = lv.row32 != nullptr;
+        rc = ensure_row32(r, lv, stream);
+        if (rc != B2D_OK) return rc;
+        if (built) CU(cudaStreamWaitEvent(stream, lv.row32->built.get(), 0));
+    }
     std::vector<Expansion> plan;
     std::vector<uint32_t> frame_set;
     size_t state_words = 0;
@@ -351,18 +409,20 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
         seen.reserve((size_t)n);
         size_t aoff = 0;
         for (int f = 0; f < n; f++) {
-            const uint32_t k = level(f);
+            const uint32_t k = level(f), e = fr.lights ? fr.lights[f].extralight : 0u;
             const LevelRes &lv = r->lv[k];
-            if (lv.h_blob.empty()) {                  // no set: the frame reads its level's blob tables
+            if (lv.h_blob.empty() && e == 0) {        // no set: the frame reads its level's blob tables
                 frame_set[(size_t)f] = (uint32_t)-1;
                 continue;
             }
-            const uint32_t *w = fr.fs + fr.starts[f];
+            // a level without time-dependent content has one state, its rest state
+            const uint32_t *w = lv.h_blob.empty() ? lv.state.data() : fr.fs + fr.starts[f];
             std::string key(reinterpret_cast<const char *>(&k), 4);
+            key.append(reinterpret_cast<const char *>(&e), 4);
             key.append(reinterpret_cast<const char *>(w), 4 * lv.layout.words);
             auto it = seen.emplace(std::move(key), (uint32_t)plan.size());
             if (it.second) {
-                plan.push_back(Expansion{k, w, s.arena.get() + aoff});
+                plan.push_back(Expansion{k, w, s.arena.get() + aoff, e});
                 aoff += lv.state_tables.slot_bytes;
                 state_words += lv.layout.words;
             }
@@ -373,13 +433,13 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
             LevelRes &lv = r->lv[k];
             if (lv.slot[slot].tables && lv.slot[slot].state != lv.state &&
                 (per_level ? std::find(fr.levels, fr.levels + n, k) != fr.levels + n : k == 0)) {
-                plan.push_back(Expansion{k, lv.state.data(), lv.slot[slot].tables.get()});
+                plan.push_back(Expansion{k, lv.state.data(), lv.slot[slot].tables.get(), 0});
                 state_words += lv.layout.words;
             }
         }
     }
     const size_t nsets = plan.size();
-    const StageLayout L(nlev, nsets, (size_t)n, state_words, per_frame, per_level);
+    const StageLayout L(nlev, nsets, (size_t)n, state_words, per_frame, per_level, fixed_rows);
     const bool stage = per_level || nsets > 0;
     size_t records = 0;
     if (stage) {
@@ -400,7 +460,7 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
             const LevelRes &lv = r->lv[plan[k].level];
             sets[k] = table_set(plan[k].tables, lv.state_tables);
             // one launch numbers the records of all per-frame sets; a launch of its own per stale set starts at 0
-            descs[k] = StateSet{plan[k].level, (uint32_t)woff, per_frame ? (uint32_t)records : 0u, 0};
+            descs[k] = StateSet{plan[k].level, (uint32_t)woff, per_frame ? (uint32_t)records : 0u, plan[k].extralight};
             std::memcpy(words + woff, plan[k].state, 4 * lv.layout.words);
             woff += lv.layout.words;
             records += set_records(lv);
@@ -410,6 +470,12 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
         for (int f = 0; f < n && per_frame; f++)
             reinterpret_cast<uint32_t *>(h + L.frame_set)[f] =
                 frame_set[(size_t)f] == (uint32_t)-1 ? (uint32_t)(nsets + level(f)) : frame_set[(size_t)f];
+        for (int f = 0; f < n && fixed_rows; f++) reinterpret_cast<int32_t *>(h + L.frame_fixed)[f] = fr.lights[f].fixed_colormap;
+        for (size_t k = 0; k < nlev && fixed_rows; k++) {
+            const LevelRes &lv = r->lv[k];
+            reinterpret_cast<FixedPlanes *>(h + L.planes)[k] =
+                lv.row32 ? FixedPlanes{lv.row32->texels.get(), lv.row32->flats.get()} : FixedPlanes{nullptr, nullptr};
+        }
     }
     CU(cudaStreamWaitEvent(stream, s.raster_done.get(), 0));      // the raster that last read this slot
     const uint8_t *d = s.stage.get();
@@ -434,6 +500,9 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
     BatchTables t{};
     t.per_frame = per_frame;
     t.per_level = per_level;
+    t.fixed_rows = fixed_rows;
+    if (fixed_rows)
+        t.fixed = FixedTables{reinterpret_cast<const int32_t *>(d + L.frame_fixed), reinterpret_cast<const FixedPlanes *>(d + L.planes)};
     if (per_level)
         t.levels = LevelTables{reinterpret_cast<const DeviceScene *>(d + L.scenes), reinterpret_cast<const uint32_t *>(d + L.frame_level),
                                per_frame ? d_sets : nullptr};
@@ -830,20 +899,25 @@ int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
     d.invF = (uint32_t)(4294967296ULL / (uint64_t)view.F);
     if (d.nsegs + d.nsprites > 65535) return fail(B2D_ERR_INVALID_ARG, "level has more than 65535 segs + sprites");
     if (walk_smem_per_warp(d) > 227 * 1024) return fail(B2D_ERR_INVALID_ARG, "level too large for the BSP-walk kernel's shared memory");
-    if (scene_is_timed(s->blob.data())) {
-        lv.h_blob = s->blob;
+    {   // the state rule's inputs, on every level (a frame with extra light reads a table set on any level): the blob's
+        // rest-state sections, the two slot maps and the light side tables
+        const uint8_t *blob = s->blob.data();
         try {
-            lv.layout = state_layout(lv.h_blob.data());
+            lv.layout = state_layout(blob);
         } catch (const std::exception &ex) {
             return fail(B2D_ERR_INVALID_ARG, ex.what());
         }
-        const uint8_t *blob = lv.h_blob.data();
         const StateLayout &L = lv.layout;
-        const size_t words = L.words;
-        // the state rule reads the blob's rest-state sections and the two slot maps
-        CU(allocate(lv.d_slot_maps, 4 * (L.sector_slots.size() + L.mid_seg.size()) + 4));
-        CU(cudaMemcpy(lv.d_slot_maps.get(), L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(lv.d_slot_maps.get() + L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
+        std::vector<int16_t> steps;
+        std::vector<int8_t> contrast;
+        light_steps(blob, steps, contrast);
+        const size_t maps = L.sector_slots.size() + L.mid_seg.size();         // words
+        CU(allocate(lv.d_slot_maps, 4 * maps + 2 * steps.size() + contrast.size() + 4));
+        uint8_t *dm = reinterpret_cast<uint8_t *>(lv.d_slot_maps.get());
+        CU(cudaMemcpy(dm, L.sector_slots.data(), 4 * L.sector_slots.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(dm + 4 * L.sector_slots.size(), L.mid_seg.data(), 4 * L.mid_seg.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(dm + 4 * maps, steps.data(), 2 * steps.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(dm + 4 * maps + 2 * steps.size(), contrast.data(), contrast.size(), cudaMemcpyHostToDevice));
         StateSrc &src = lv.src = state_src(blob, L);
         auto on_device = [&](auto p) { return reinterpret_cast<decltype(p)>(db + (reinterpret_cast<const uint8_t *>(p) - blob)); };
         src.tex = on_device(src.tex); src.sectors = on_device(src.sectors); src.segs = on_device(src.segs);
@@ -851,18 +925,26 @@ int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
         src.flat_anim = on_device(src.flat_anim); src.segdyn = on_device(src.segdyn);
         src.sector_slots = lv.d_slot_maps.get();
         src.mid_seg = reinterpret_cast<const int32_t *>(lv.d_slot_maps.get() + L.sector_slots.size());
+        src.sector_steps = reinterpret_cast<const int16_t *>(dm + 4 * maps);
+        src.seg_contrast = reinterpret_cast<const int8_t *>(dm + 4 * maps + 2 * steps.size());
         StateTables &t = lv.state_tables;              // one table set: [tex | sectors | segs | sprites | mids], 256 B aligned
         t.slot_bytes = (uint32_t)((state_table_bytes(blob) + 255) & ~(size_t)255);
         t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
         t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
         t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
         t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
-        for (auto &sl : lv.slot) CU(allocate(sl.tables, t.slot_bytes));
-        // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306).  The
-        // pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic 0,
-        // expanded by one launch.
-        lv.state.assign(words, 0);
+        // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306)
+        lv.state.assign(L.words, 0);
         compact_state(blob, L, 0, nullptr, nullptr, lv.state.data());
+    }
+    if (scene_is_timed(s->blob.data())) {
+        lv.h_blob = s->blob;
+        const uint8_t *blob = lv.h_blob.data();
+        const size_t words = lv.layout.words;
+        const StateTables &t = lv.state_tables;
+        for (auto &sl : lv.slot) CU(allocate(sl.tables, t.slot_bytes));
+        // The pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic
+        // 0, expanded by one launch.
         const StageLayout S(1, 2, 0, words, false, false);
         const uint32_t records = (uint32_t)set_records(lv);
         std::vector<uint8_t> stage(S.end);
@@ -982,7 +1064,7 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
     CU(cudaMemcpy(r->d_palettes.get(), table.data(), table.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     // each worklist slot's staging, for the largest batch: max_batch frames with a table set each, or a stale set per level
     const size_t sets = std::max((size_t)max_batch, r->lv.size());
-    const size_t stage_bytes = StageLayout(r->lv.size(), sets, (size_t)max_batch, sets * words, true, true).end;
+    const size_t stage_bytes = StageLayout(r->lv.size(), sets, (size_t)max_batch, sets * words, true, true, true).end;
     for (WorkSlot &sl : r->slot) {
         CU(allocate(sl.stage, stage_bytes));
         CU(allocate(sl.h_stage, stage_bytes));
@@ -1194,6 +1276,41 @@ int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, cons
     return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
 }
 
+int b2d_render_device_levels_states_lights(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
+                                           const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
+                                           const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb,
+                                           uint32_t *d_rgba_fb, void *cuda_stream) {
+    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    Frames fr{levels};
+    int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = check_lights(lights, n);
+    fr.lights = lights;
+    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
+    if (rc != B2D_OK || n == 0) return rc;
+    CU(cudaSetDevice(r->device));
+    return enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int b2d_walk_device_levels_states_lights(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
+                                         const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
+                                         const b2d_sector_move *moves, size_t n_moves, void *cuda_stream,
+                                         int64_t *ticket_out) {
+    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    Frames fr{levels};
+    int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = check_lights(lights, n);
+    fr.lights = lights;
+    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
+    if (rc != B2D_OK) return rc;
+    CU(cudaSetDevice(r->device));
+    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
+}
+
 // Host poses in, host frames out: the n frames `fr` in batches of max_batch.
 static int render_host(b2d_renderer *r, const b2d_pose *poses, const Frames &fr, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
     if (n == 0) return B2D_OK;
@@ -1303,6 +1420,21 @@ int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint3
     std::vector<size_t> starts;
     Frames fr{levels};
     int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
+    if (rc != B2D_OK) return rc;
+    return render_host(r, poses, fr, n, index_fb, rgba_fb);
+}
+
+int b2d_render_levels_states_lights(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels,
+                                    const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
+                                    const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    Frames fr{levels};
+    int rc = check_levels(r, levels, n);
+    if (rc == B2D_OK) rc = check_lights(lights, n);
+    fr.lights = lights;
     if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
     if (rc != B2D_OK) return rc;
     return render_host(r, poses, fr, n, index_fb, rgba_fb);
@@ -1471,7 +1603,7 @@ int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capaci
     if (!per_frame && lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
     if (s.ticket < 0) return fail(B2D_ERR_INVALID_ARG, "no batch has been walked");
     if (set >= (per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
-    const size_t need = state_table_bytes(lv.h_blob.data());
+    const size_t need = level_table_bytes(lv);
     if (size_out) *size_out = need;
     if (!out) return B2D_OK;
     if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");

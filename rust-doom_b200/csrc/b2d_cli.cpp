@@ -15,7 +15,9 @@
 // --resolution RGB on the device (b2d_resolve_device, each frame through its own level's palette) for --dump and --stream;
 // not with --world.  --palette P colours those frames through PLAYPAL palette P instead of palette 0
 // (b2d_resolve_palettes_device; 1..8 Doom's damage flash, 9..12 the bonus flash, 13 the radiation suit), through the
-// resolve at the --supersample factor (1 by default); not with --world.
+// resolve at the --supersample factor (1 by default); not with --world.  --fixed-colormap R (-1..32) and --extralight E (0..2)
+// light every frame of --levels as a player with those effects (b2d_*_levels_states_lights, DESIGN.md C18: 32 Doom's
+// invulnerability, 1 its light-amplification visor, E its weapon flashes); not with --world.
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -76,7 +78,8 @@ void write_ppm_rgb(std::FILE *f, const uint8_t *rgb, int w, int h) {
 // device index frames at the renderer's view, resolve them by `factor` to RGB8 through palette `palette` of each frame's
 // level and download them into `rgb` (n x (W/factor) x (H/factor) x 3)
 int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, size_t max_batch,
-                        const uint32_t *levels, const b2d_frame_state *states, int factor, int palette, std::vector<uint8_t> &rgb) {
+                        const uint32_t *levels, const b2d_frame_state *states, const b2d_frame_light *lights, int factor,
+                        int palette, std::vector<uint8_t> &rgb) {
     const size_t n = poses.size(), npix = (size_t)view.width * view.height;
     size_t frame_bytes = 0;
     if (b2d_resolve_frame_bytes(r, factor, B2D_RESOLVE_RGB8, &frame_bytes) != B2D_OK) return fail("resolve");
@@ -93,7 +96,8 @@ int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const
     const b2d_pose *dp = static_cast<const b2d_pose *>(d_poses);
     uint8_t *di = static_cast<uint8_t *>(d_index);
     if (levels) {
-        if (b2d_render_device_levels_states(r, dp, levels, states, n, nullptr, 0, di, nullptr, nullptr) != B2D_OK) return fail("render");
+        if (b2d_render_device_levels_states_lights(r, dp, levels, states, lights, n, nullptr, 0, di, nullptr, nullptr) != B2D_OK)
+            return fail("render");
     } else {
         for (size_t i = 0; i < n; i += max_batch)
             if (b2d_render_device(r, dp + i, std::min(max_batch, n - i), di + npix * i, nullptr, nullptr) != B2D_OK) return fail("render");
@@ -160,7 +164,7 @@ int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st
 // --levels: the look-around of every level of `set` from its start, nposes per level, pose i at tic tics + i
 int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
                      const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file,
-                     int supersample, int palette) {
+                     int supersample, int palette, b2d_frame_light light) {
     std::vector<b2d_scene *> scenes;
     struct Scenes {
         std::vector<b2d_scene *> &v;
@@ -189,6 +193,8 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
         }
     }
     for (size_t i = 0; i < n; i++) states[i] = b2d_frame_state{tics + (uint32_t)i, 0, 0};
+    const std::vector<b2d_frame_light> light_v(n, light);
+    const b2d_frame_light *lights = light.fixed_colormap != -1 || light.extralight != 0 ? light_v.data() : nullptr;
     b2d_view view;
     if (b2d_view_init(&view, width * supersample, height * supersample, fov) != B2D_OK) return fail("view");
     b2d_renderer *r = nullptr;
@@ -217,14 +223,15 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
     std::vector<uint32_t> rgba;
     const bool resolved = supersample > 1 || palette > 0;
     if (resolved) {
-        if (int rc = render_supersampled(r, 0, view, poses, n < 64 ? n : 64, levels.data(), states.data(), supersample, palette, rgb))
+        if (int rc = render_supersampled(r, 0, view, poses, n < 64 ? n : 64, levels.data(), states.data(), lights, supersample, palette, rgb))
             return rc;
         std::printf("rendered %zu frame(s) %dx%d of %zu level(s), supersampled %dx, palette %d\n", n, width, height, set.size(),
                     supersample, palette);
     } else {
         index.resize(npix * n);
         rgba.resize(npix * n);
-        if (b2d_render_levels_states(r, poses.data(), levels.data(), states.data(), n, nullptr, 0, index.data(), rgba.data()) != B2D_OK)
+        if (b2d_render_levels_states_lights(r, poses.data(), levels.data(), states.data(), lights, n, nullptr, 0, index.data(),
+                                            rgba.data()) != B2D_OK)
             return fail("render");
         std::printf("rendered %zu frame(s) %dx%d of %zu level(s)\n", n, width, height, set.size());
     }
@@ -256,6 +263,7 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
 int main(int argc, char **argv) {
     std::string iwad, dump, stream, command, id_file, levels_arg;
     int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16, supersample = 1, palette = 0;
+    b2d_frame_light light{-1, 0};
     double fov = 65.0;
     unsigned long tics = 0;
     bool with_levels = false;
@@ -291,6 +299,18 @@ int main(int argc, char **argv) {
             if (!*v || *end || p < 0 || p > 0x7FFFFFFF) { std::fprintf(stderr, "--palette takes a palette index\n"); return 2; }
             palette = (int)p;
         }
+        else if (a == "--fixed-colormap" || a == "--extralight") {
+            const char *v = next(a.c_str());
+            char *end = nullptr;
+            const long x = std::strtol(v, &end, 10);
+            const bool fixed = a == "--fixed-colormap";
+            if (!*v || *end || (fixed ? x < -1 || x > 32 : x < 0 || x > 2)) {
+                std::fprintf(stderr, fixed ? "--fixed-colormap takes a row in -1..32\n" : "--extralight takes a value in 0..2\n");
+                return 2;
+            }
+            if (fixed) light.fixed_colormap = (int32_t)x;
+            else light.extralight = (uint32_t)x;
+        }
         else if (a == "list-levels" || a == "check") command = a;
         else { std::fprintf(stderr, "unknown argument %s\n", a.c_str()); return 2; }
     }
@@ -299,6 +319,9 @@ int main(int argc, char **argv) {
     if (supersample < 1 || supersample > 8) { std::fprintf(stderr, "--supersample takes a factor in 1..8\n"); return 2; }
     if (supersample > 1 && world > 0) { std::fprintf(stderr, "--supersample does not combine with --world\n"); return 2; }
     if (palette > 0 && world > 0) { std::fprintf(stderr, "--palette does not combine with --world\n"); return 2; }
+    const bool lit = light.fixed_colormap != -1 || light.extralight != 0;
+    if (lit && world > 0) { std::fprintf(stderr, "--fixed-colormap and --extralight do not combine with --world\n"); return 2; }
+    if (lit && !with_levels) { std::fprintf(stderr, "--fixed-colormap and --extralight take --levels\n"); return 2; }
 
     b2d_archive *arch = nullptr;
     if (b2d_archive_open(iwad.c_str(), &arch) != B2D_OK) return fail("open");
@@ -335,7 +358,7 @@ int main(int argc, char **argv) {
             return 2;
         }
         const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file,
-                                        supersample, palette);
+                                        supersample, palette, light);
         b2d_archive_close(arch);
         return rc;
     }
@@ -360,7 +383,7 @@ int main(int argc, char **argv) {
     const size_t npix = (size_t)width * height;
     if (supersample > 1 || palette > 0) {
         std::vector<uint8_t> rgb;
-        if (int rc = render_supersampled(r, 0, view, poses, nposes < 64 ? nposes : 64, nullptr, nullptr, supersample, palette, rgb))
+        if (int rc = render_supersampled(r, 0, view, poses, nposes < 64 ? nposes : 64, nullptr, nullptr, nullptr, supersample, palette, rgb))
             return rc;
         std::printf("rendered %d frame(s) %dx%d, supersampled %dx, palette %d\n", nposes, width, height, supersample, palette);
         if (!dump.empty()) {

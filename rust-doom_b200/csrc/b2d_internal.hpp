@@ -18,22 +18,29 @@ int cuda_fail(cudaError_t e, const char *what);
 // The frames of a call, or of one batch of it (HOST arrays).  `levels`: the level of each frame, checked by check_levels
 // (nullptr: every frame on level 0).  `starts`: with per-frame states, frame i's compact state is fs[starts[i] ..] (its
 // level's layout.words words; none on a level without time-dependent content or dynamic sectors); nullptr: every level at
-// the renderer's own state, a plain batch.
+// the renderer's own state, a plain batch.  `lights`: with per-frame levels and states, each frame's fixed colormap and
+// extra light, checked by check_lights (nullptr: none, as when every frame is {-1, 0}).
 struct Frames {
     const uint32_t *levels = nullptr;
     const uint32_t *fs = nullptr;
     const size_t *starts = nullptr;
-    Frames from(size_t first) const { return {levels ? levels + first : nullptr, fs, starts ? starts + first : nullptr}; }
+    const b2d_frame_light *lights = nullptr;
+    Frames from(size_t first) const {
+        return {levels ? levels + first : nullptr, fs, starts ? starts + first : nullptr, lights ? lights + first : nullptr};
+    }
 };
 // The n per-frame states of a call on the frames of `out` (out.levels set by the caller), checked, and out.fs / out.starts
 // pointing into `fs` / `starts`: with `tics`, frame i at tics[i] with its level's current sector moves; else at
-// states[i] (its time and its range of `moves`).  With every frame on level 0 and a level 0 without time-dependent content
+// states[i] (its time and its range of `moves`), with out.lights[i]'s extra light if out.lights is set.  With every frame on level 0 and a level 0 without time-dependent content
 // or dynamic sectors, the call is a plain one (out.starts stays nullptr).  Nothing is enqueued.
 int build_states(const b2d_renderer *r, const b2d_frame_state *states, const uint32_t *tics, size_t n, const b2d_sector_move *moves,
                  size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts, Frames &out);
 // Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
 // per-frame-level walk (a b2d_renderer_create renderer may not); B2D_ERR_INVALID_ARG otherwise.
 int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n);
+// Per-frame light effects (HOST, nullable): fixed_colormap in -1..32 and extralight in 0..2; B2D_ERR_INVALID_ARG otherwise.
+// `lights` is set to nullptr when every frame is {-1, 0}, so that such a call is the call without lights.
+int check_lights(const b2d_frame_light *&lights, size_t n);
 // Per-frame palettes (HOST, nullable = palette 0): frame i's palette below the palette count of its level (levels[i],
 // nullable = level 0), the levels already checked; B2D_ERR_INVALID_ARG otherwise.
 int check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n);
@@ -157,20 +164,30 @@ struct LevelRes {
     Aligned4G d_lit_flats;
     DeviceBuf<uint8_t> d_walk_static;                     // node / subsector tables as the walk kernel's shared memory holds them
     DeviceScene ds{};
+    // The state rule's inputs, for every level: a frame with extra light (DESIGN.md C18) reads a table set expanded
+    // from a compact state on any level.
+    StateLayout layout;
+    std::vector<uint32_t> state;                          // the level's own compact state (set_time, set_*sector_moves)
+    DeviceBuf<uint32_t> d_slot_maps;                      // StateLayout::sector_slots, ::mid_seg, then the light side tables
+    StateSrc src{};                                       // device pointers into d_blob and d_slot_maps
+    StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
     // Scenes with time-dependent content or dynamic sectors (DESIGN.md §3 "State arena"); the rest stays empty.  The
     // device blob is never written after creation: the state rule reads its rest-state sections, and every batch reads
     // its five state-dependent tables from a table set expanded on the device from a compact state.
     std::vector<uint8_t> h_blob;                          // host copy of the scene
-    StateLayout layout;
-    std::vector<uint32_t> state;                          // the level's own compact state (set_time, set_*sector_moves)
-    DeviceBuf<uint32_t> d_slot_maps;                      // StateLayout::sector_slots, then ::mid_seg
-    StateSrc src{};                                       // device pointers into d_blob and d_slot_maps
-    StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
     // per worklist slot: the table set the slot's batches read and the compact state it was expanded from
     struct Slot {
         DeviceBuf<uint8_t> tables;
         std::vector<uint32_t> state;
     } slot[2];
+    // Fixed colormap 32 (C18): the row-32 texel and flat planes, built whole by the first call that asks for them on this
+    // level, on that call's stream (`built` follows the build; every batch that reads them waits for it).
+    struct Row32 {
+        DeviceBuf<uint8_t> texels;
+        Aligned4G flats;
+        Event built;
+    };
+    std::unique_ptr<Row32> row32;
 };
 
 struct b2d_renderer {

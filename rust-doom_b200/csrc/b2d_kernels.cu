@@ -420,8 +420,16 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t a) {
     return v;
 }
 
+// A frame's fixed colormap (kFixed raster variant, FixedTables): COLORMAP row `row` (-1: none) and the row-32 planes
+// of its level.
+struct FixedWarp {
+    const uint8_t *texels, *flats;
+    int row;
+};
+
 struct RasterCtx {
     const DeviceScene *sc;
+    FixedWarp fix;             // kFixed variant only
     uint32_t pal_s;            // ... of the palette (rgba only)
     uint2 *rowz;               // this warp's 32-entry staging of per-row plane constants {depth Q8, plane offset / 64}
     PlaneDir dir;              // direction of this lane's column ray (Q18), for the flat texel
@@ -507,7 +515,7 @@ __device__ __forceinline__ void draw_sky_warp(const RasterCtx &c, int ya, int yb
     }
 }
 
-template <bool kRgba, int kW>
+template <bool kRgba, int kW, bool kFixed = false>
 __device__ __forceinline__ void draw_plane_warp(const RasterCtx &c, const FrameConst &fc, const View &vw,
                                                 int ya, int yb, int32_t h, int32_t flat, int lightb,
                                                 bool visible) {
@@ -518,7 +526,13 @@ __device__ __forceinline__ void draw_plane_warp(const RasterCtx &c, const FrameC
     if (flat < 0 || flat >= sc.nflats) { fill_void_warp<kRgba, kW>(c, ya, yb); return; }
     // the pre-lit flats start at a multiple of 4 GiB (b2d_api.cu alloc_aligned_4g): a texel's address is {high word,
     // 32-bit offset} -- no 64-bit add per pixel
-    const uint64_t px_hi = reinterpret_cast<uint64_t>(sc.lit_flats) & 0xFFFFFFFF00000000ull;   // low word is zero: tell the compiler
+    const uint8_t *lit_flats = sc.lit_flats;
+    int fixed_row = -1;
+    if constexpr (kFixed) {      // a fixed colormap: every row of the plane on one pre-lit plane (row 32: the level's own)
+        lit_flats = c.fix.row == 32 ? c.fix.flats : lit_flats;
+        fixed_row = c.fix.row == 32 ? 0 : c.fix.row;
+    }
+    const uint64_t px_hi = reinterpret_cast<uint64_t>(lit_flats) & 0xFFFFFFFF00000000ull;   // low word is zero: tell the compiler
     const uint32_t habs = plane_habs(h, fc.pose.z);
     bool act = ya < yb;
     int y0 = __reduce_min_sync(kFull, act ? ya : 0x7FFFFFFF);
@@ -537,7 +551,7 @@ __device__ __forceinline__ void draw_plane_warp(const RasterCtx &c, const FrameC
             const PlaneRow pr = plane_row(habs, sc.yslope[yy]);
             // plane + flat offset / 64: the texel offset is then two instructions, LEA.HI (cm6 + (U >> 26)) and a funnel
             // shift ((.) << 6 | V >> 26)
-            c.rowz[c.lane] = make_uint2(pr.z8q, (sc.lit_flat_stride >> 6) * (uint32_t)light_row(lightb, pr.z8) + 64u * (uint32_t)flat);
+            c.rowz[c.lane] = make_uint2(pr.z8q, (sc.lit_flat_stride >> 6) * (uint32_t)(kFixed && fixed_row >= 0 ? fixed_row : light_row(lightb, pr.z8)) + 64u * (uint32_t)flat);
         }
         __syncwarp();
         const int rows = min(32, y1 - yc);
@@ -597,7 +611,8 @@ __device__ __forceinline__ void wall_fast_loop(const RasterCtx &c, const uint8_t
     }
 }
 
-template <bool kRgba, int kW>
+// `row`: the lane's light row; with a fixed colormap (kFixed) its row, 32 meaning the level's row-32 plane
+template <bool kRgba, int kW, bool kFixed = false>
 __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameConst &fc, int ya, int yb,
                                                int32_t tex, int32_t tA, int32_t hA, int32_t ucol,
                                                int32_t iscale, int row) {
@@ -608,6 +623,9 @@ __device__ __forceinline__ void draw_wall_warp(const RasterCtx &c, const FrameCo
     bool act = ya < yb;
     const uint32_t col = (uint32_t)floormod32(ucol, (int32_t)T.w);
     const uint8_t *pl = sc.lit_texels + (size_t)row * sc.lit_texel_stride + T.texel_off;   // this lane's light plane
+    if constexpr (kFixed) {
+        if (row == 32) pl = c.fix.texels + T.texel_off;
+    }
     const uint32_t tstep = (uint32_t)(iscale >> 4);
     int y0 = __reduce_min_sync(kFull, act ? ya : 0x7FFFFFFF);
     int y1 = __reduce_max_sync(kFull, act ? yb : 0);
@@ -720,11 +738,16 @@ __device__ __forceinline__ uint32_t *masked_push(const DeviceScene &sc, uint32_t
 // front-to-back walk reached it (the per-column silhouette of everything nearer).  Texels whose opacity plane
 // is 0 leave the pixel as the solid pass drew it (static.frag:21-22).  Kept out of line so that the
 // register allocation of the solid pass is not affected.  kStates and kLevels only give each raster variant its own copy
-// (one caller each, so that what the compiler propagates into it from its caller stays as it is).
-template <bool kRgba, int kW, bool kStates, bool kLevels>
+// (one caller each, so that what the compiler propagates into it from its caller stays as it is).  The kFixed variant
+// takes the frame's fixed colormap as two more arguments, its row-32 texel plane and its row (`fix`: empty in the others,
+// whose arguments stay as they are).
+template <bool kRgba, int kW, bool kStates, bool kLevels, typename... Fix>
 __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, int32_t pose_z, uint8_t *fb,
                                          uint32_t *rgba, uint32_t pal_s, int x, int lane,
-                                         const SegFrame *wl, const uint32_t *chunks, int count) {
+                                         const SegFrame *wl, const uint32_t *chunks, int count, Fix... fix) {
+    constexpr bool kFixed = sizeof...(Fix) != 0;
+    static_assert(sizeof...(Fix) == 0 || sizeof...(Fix) == 2, "the fixed colormap: the row-32 texel plane and the row");
+    struct { const uint8_t *texels; int row; } const fw{fix...};     // the row-32 texel plane and the row
     // everything arrives by value (or points at kernel parameters): taking the address of the solid pass's
     // register-resident context would force it into local memory
     RasterCtx c;
@@ -747,7 +770,7 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
             const int64_t scale = sprite_scale(vw, sp.cz);      // >= 1: the walk's sprite_setup accepted the sprite
             int32_t z8;
             scale_depth(vw, scale, iscale, z8);
-            row = light_row_sprite(P.light, z8);
+            row = kFixed && fw.row >= 0 ? fw.row : light_row_sprite(P.light, z8);
             tex = P.tex; tA = 0; hA = P.low + sh;
             if (ya < yb) {
                 clip_rows(P.low + sh, P.low, row_scale(scale), pose_z, c.H, ya, yb);
@@ -763,7 +786,7 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
                 clip_rows(M.high, M.low, ce.scale, pose_z, c.H, ya, yb);
                 ucol = wall_column(S.uoff, S.len_q12, ce.s24);
                 iscale = ce.iscale;
-                row = light_row(S.light, ce.z8);
+                row = kFixed && fw.row >= 0 ? fw.row : light_row(S.light, ce.z8);
             } else {
                 ya = yb = 0;
             }
@@ -780,6 +803,9 @@ __device__ __noinline__ void masked_pass(const DeviceScene &sc, const View &vw, 
         const bool inter = tex_interleaved(T);
         const bool has_mask = T.mask_off != 0xFFFFFFFFu;
         const uint8_t *pl = sc.lit_texels + (size_t)row * sc.lit_texel_stride + T.texel_off;
+        if constexpr (kFixed) {
+            if (row == 32) pl = fw.texels + T.texel_off;
+        }
         const uint8_t *pm = sc.lit_texels + (size_t)32 * sc.lit_texel_stride + T.texel_off;
         const uint32_t tstep = (uint32_t)(iscale >> 4);
         uint32_t t = (uint32_t)wall_tbase(tA, hA, pose_z, c.H, iscale) + (uint32_t)y0 * tstep;
@@ -897,12 +923,17 @@ __device__ __forceinline__ bool queue_push(const DrawQueue &q, int lane, uint32_
     return true;
 }
 
-template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels>
+// `Fixed`: empty, or FixedTables -- the fixed-colormap variant (kFixed, DESIGN.md C18; per-frame levels and states only),
+// whose frames may have a fixed colormap and which alone takes the appended parameter `fx`.  An empty pack leaves the
+// other variants' names, parameters and code as they are.
+template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels, typename... Fixed>
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st,
-                  const __grid_constant__ LevelTables lt) {
+                  const __grid_constant__ LevelTables lt, const Fixed... fx) {
+    constexpr bool kFixed = sizeof...(Fixed) != 0;
+    static_assert(!kFixed || (kStates && kLevels && sizeof...(Fixed) == 1), "fixed colormaps come with per-frame levels and states");
     // per-frame levels: a palette per warp (the warps of a CTA may draw frames of levels from different WADs)
     __shared__ uint32_t s_pal[kRgba ? (kLevels ? 256 * kRasterWarps : 256) : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
@@ -918,6 +949,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     __shared__ uint32_t s_qn[5];                  // records, words, items popped, items, a warp deferred masked entries
     // per-frame states or levels: each warp's copy of its frame's scene description (see below)
     __shared__ DeviceScene s_scn[kStates || kLevels ? kRasterWarps : 1];
+    __shared__ FixedWarp s_fix[kFixed ? kRasterWarps : 1];      // each warp's fixed colormap
     if (threadIdx.x < 5) s_qn[threadIdx.x] = 0;
     for (int b = threadIdx.x; b < kMaxBands; b += blockDim.x) s_band[b] = 0;
     if (kRgba && !kLevels) {   // the palette into shared memory (colours come pre-lit from global memory: no colormap here)
@@ -985,10 +1017,19 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         }
         scp = d;
     }
+    if constexpr (kFixed) {
+        if (has_strip && lane == 0) {
+            const FixedTables &t = (fx, ...);       // the one element of the pack
+            const FixedPlanes p = t.planes[(uint32_t)fc.pad[1]];
+            s_fix[warp] = FixedWarp{p.texels, p.flats, t.frame_fixed[frame]};
+        }
+        __syncwarp();
+    }
     const DeviceScene &ts = *scp;      // = sc without per-frame states or levels
     const DeviceScene &ls = kLevels ? ts : sc;     // the level's own fields (sky, masked-entry cap): = sc but per-frame levels
     RasterCtx c;
     c.sc = &ts;
+    if constexpr (kFixed) c.fix = s_fix[warp];
     c.pal_s = (uint32_t)__cvta_generic_to_shared(kLevels ? s_pal + 256 * warp : s_pal);
     c.rowz = s_rowz[warp];
     c.W = W; c.H = H; c.x = x; c.lane = lane;
@@ -1053,7 +1094,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             int yend = ct, row = 0;
             int32_t ucol = 0;
             if (ok) {
-                row = light_row(S.light, ce.z8);
+                row = kFixed && c.fix.row >= 0 ? c.fix.row : light_row(S.light, ce.z8);
                 ucol = wall_column(S.uoff, S.len_q12, ce.s24);
                 wr = wall_rows(fcl, ffl, two, S.otop, S.obot, ce.scale, fc.pose.z, H, ct, cb);
                 yend = cb;
@@ -1068,7 +1109,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
                 const int32_t h = top ? fcl : ffl, flat = top ? SF.ceil_flat : SF.floor_flat;
                 const bool vis = top ? ceil_vis : floor_vis;
                 if (!queue_push(q, lane, owner | (vis ? kRecVisible : 0u), h, flat, SF.light, ya, yb, 0, 0u))
-                    draw_plane_warp<kRgba, kW>(c, fc, vw, ya, yb, h, flat, SF.light, vis);
+                    draw_plane_warp<kRgba, kW, kFixed>(c, fc, vw, ya, yb, h, flat, SF.light, vis);
             }
 #pragma unroll 1
             for (int pw = 0; pw < 2; pw++) {
@@ -1077,7 +1118,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
                 const int ya = ok ? (upper ? wr.y1 : wr.y3) : 0, yb = ok ? (upper ? wr.y2 : wr.y4) : 0;
                 const int32_t tex = upper ? S.texA : S.texB, tA = upper ? S.tA : S.tB, hA = upper ? S.hA : S.hB;
                 if (!queue_push(q, lane, owner | kRecWall, tex, tA, hA, ya, yb, ucol, (uint32_t)ce.iscale | ((uint32_t)row << 24)))
-                    draw_wall_warp<kRgba, kW>(c, fc, ya, yb, tex, tA, hA, ucol, ce.iscale, row);
+                    draw_wall_warp<kRgba, kW, kFixed>(c, fc, ya, yb, tex, tA, hA, ucol, ce.iscale, row);
             }
             if (ok) wall_window(two, wr, H, ct, cb);
             if (defer && two && S.mid >= 0) {
@@ -1163,6 +1204,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         const FrameConst fo = frames[f];
         RasterCtx d;
         d.sc = kStates || kLevels ? &s_scn[o] : &sc;      // the owner's scene description
+        if constexpr (kFixed) d.fix = s_fix[o];
         d.pal_s = (uint32_t)__cvta_generic_to_shared(kLevels ? s_pal + 256 * o : s_pal);
         d.rowz = s_rowz[warp];
         d.dir = PlaneDir{ln.x, ln.y};
@@ -1174,16 +1216,20 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
         const int ya = max((int)(win & 0xFFFFu), lo), yb = min((int)(win >> 16), hi);
         if (hd.x & kRecWall) {
             const uint32_t isr = s_qpool[off + 64 + lane];
-            draw_wall_warp<kRgba, kW>(d, fo, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int32_t)hd.w, (int32_t)s_qpool[off + 32 + lane],
+            draw_wall_warp<kRgba, kW, kFixed>(d, fo, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int32_t)hd.w, (int32_t)s_qpool[off + 32 + lane],
                                       (int32_t)(isr & 0xFFFFFFu), (int)(isr >> 24));
         } else {
-            draw_plane_warp<kRgba, kW>(d, fo, vw, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int)hd.w, hd.x & kRecVisible);
+            draw_plane_warp<kRgba, kW, kFixed>(d, fo, vw, ya, yb, (int32_t)hd.y, (int32_t)hd.z, (int)hd.w, hd.x & kRecVisible);
         }
     }
     if constexpr (kMasked) {
         // the masked pass overwrites solid pixels of its own strip: every draw of the CTA must be done first
         __syncthreads();
-        if (mcount > 0) masked_pass<kRgba, kW, kStates, kLevels>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
+        if constexpr (kFixed) {
+            if (mcount > 0) masked_pass<kRgba, kW, kStates, kLevels>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount, c.fix.texels, c.fix.row);
+        } else {
+            if (mcount > 0) masked_pass<kRgba, kW, kStates, kLevels>(ts, vw, fc.pose.z, c.fb, c.rgba, c.pal_s, x, lane, wl, chunks, mcount);
+        }
     }
 }
 
@@ -1482,7 +1528,7 @@ cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw
 // a finished strip's warp draws for its slower siblings instead of idling.  The registers are left to the compiler (cap
 // 128): 94 for the 1080p and 4K index-only kernels, i.e. 2 CTAs = 16 warps per SM (DESIGN.md §5, §6).
 // The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
-template <bool kStates, bool kLevels>
+template <bool kStates, bool kLevels, bool kFixed>
 static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
                              const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
                              cudaStream_t stream) {
@@ -1490,8 +1536,13 @@ static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, 
     const int strips = (vw.W + 31) / 32;
     const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
 #define B2D_RASTER_GO(RGBA, KW) do { \
+    if constexpr (kFixed) { \
+    if (masked) b2d_raster_kernel<RGBA, KW, true, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels, t.fixed); \
+    else b2d_raster_kernel<RGBA, KW, false, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels, t.fixed); \
+    } else { \
     if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels); \
     else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels); \
+    } \
     } while (0)
     if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
     else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
@@ -1501,11 +1552,14 @@ static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, 
     return cudaGetLastError();
 }
 
-// Per-frame states take the kStates variant of each shape; the frames are the same pixel for pixel.
+// Per-frame states take the kStates variant of each shape; the frames are the same pixel for pixel.  A batch of per-frame
+// levels and states with a fixed colormap takes the kFixed variant.
 cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
                           int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream) {
-    auto go = t.per_level ? (t.per_frame ? raster_go<true, true> : raster_go<false, true>)
-                          : (t.per_frame ? raster_go<true, false> : raster_go<false, false>);
+    if (t.fixed_rows && !(t.per_level && t.per_frame)) return cudaErrorInvalidValue;
+    auto go = t.per_level ? (t.per_frame ? (t.fixed_rows ? raster_go<true, true, true> : raster_go<true, true, false>)
+                                         : raster_go<false, true, false>)
+                          : (t.per_frame ? raster_go<true, false, false> : raster_go<false, false, false>);
     return go(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream);
 }
 
@@ -1547,6 +1601,50 @@ b2d_prelight_tex_kernel(const uint8_t *__restrict__ colormap, const uint8_t *__r
 }
 }  // namespace
 
+namespace {
+// one more pre-lit plane, of one COLORMAP row: flats (row-major) and textures (one CTA per texture, in the planes' layout)
+__global__ void __launch_bounds__(256)
+b2d_prelight_row_kernel(const uint8_t *__restrict__ row, const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, size_t n) {
+    __shared__ uint8_t cm[256];
+    cm[threadIdx.x] = row[threadIdx.x];
+    __syncthreads();
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = cm[src[i]];
+}
+
+__global__ void __launch_bounds__(256)
+b2d_prelight_tex_row_kernel(const uint8_t *__restrict__ row, const uint8_t *__restrict__ texels, const TexRec *__restrict__ tex,
+                            int ntex, uint8_t *__restrict__ dst) {
+    __shared__ uint8_t cm[256];
+    cm[threadIdx.x] = row[threadIdx.x];
+    __syncthreads();
+    for (int ti = blockIdx.x; ti < ntex; ti += gridDim.x) {
+        const TexRec T = tex[ti];
+        const bool inter = tex_interleaved(T);
+        const uint32_t n = T.w * T.h;
+        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+            const uint32_t r = i / T.w, col = i - r * T.w;
+            dst[T.texel_off + lit_index(inter, T.w, r, col)] = cm[texels[T.texel_off + i]];
+        }
+    }
+}
+}  // namespace
+
+cudaError_t launch_prelight_row(const uint8_t *d_row, const uint8_t *d_src, uint8_t *d_dst, size_t n, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    int blocks = (int)((n + 255) / 256);
+    if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+    b2d_prelight_row_kernel<<<blocks, 256, 0, stream>>>(d_row, d_src, d_dst, n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_prelight_textures_row(const uint8_t *d_row, const uint8_t *d_texels, const TexRec *d_tex, int ntex,
+                                         uint8_t *d_dst, cudaStream_t stream) {
+    if (ntex <= 0) return cudaSuccess;
+    const int cap = device_sms() * 8;
+    b2d_prelight_tex_row_kernel<<<ntex < cap ? ntex : cap, 256, 0, stream>>>(d_row, d_texels, d_tex, ntex, d_dst);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_prelight_textures(const uint8_t *d_colormap, const uint8_t *d_texels, const TexRec *d_tex, int ntex,
                                      uint8_t *d_dst, size_t stride, cudaStream_t stream) {
     if (ntex <= 0) return cudaSuccess;
@@ -1581,7 +1679,8 @@ b2d_state_sets_kernel(const StateSrc *__restrict__ srcs, const StateSet *__restr
         const StateSet S = sets[lo];
         const StateSrc &src = srcs[S.level];
         const TableSet o = out[lo];
-        const StateIn st = state_in(states + S.state, src.ndyn);
+        StateIn st = state_in(states + S.state, src.ndyn);
+        st.extra = S.extralight;
         uint32_t i = g - S.first;
         if (i < src.ntex) { const_cast<TexRec *>(o.tex)[i] = tex_at(src, st, i); continue; }
         i -= src.ntex;

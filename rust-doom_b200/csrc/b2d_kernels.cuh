@@ -78,9 +78,21 @@ struct LevelTables {
 
 // One table set to expand (launch_state_sets): level `level`'s rule at the compact state at word `state` of the launch's
 // states, into the tables of its TableSet.  `first`: the set's first record in the launch's numbering of all its records
-// (the record counts of the sets before it, summed).
+// (the record counts of the sets before it, summed).  `extralight`: the player's extra light, 0..2 (DESIGN.md C18).
 struct StateSet {
-    uint32_t level, state, first, pad;
+    uint32_t level, state, first, extralight;
+};
+
+// Fixed colormaps (b2d_*_levels_states_lights, DESIGN.md C18): the kFixed raster variant lights every wall, flat and
+// masked pixel of frame i through COLORMAP row frame_fixed[i] (-1: by light and depth, as without it).  Rows 0..31 are
+// the level's pre-lit planes; row 32 is planes[level of the frame], built for a level by the first call that asks for it.
+struct FixedPlanes {
+    const uint8_t *texels;       // row 32 of every texture, in the layout of a pre-lit texture plane
+    const uint8_t *flats;        // row 32 of every flat, at an address that is a multiple of 4 GiB (as the pre-lit flats)
+};
+struct FixedTables {
+    const int32_t *frame_fixed;
+    const FixedPlanes *planes;   // per level
 };
 
 // Bytes of dynamic shared memory the BSP-walk kernel needs per frame (= per CTA) for this scene.
@@ -94,11 +106,14 @@ constexpr size_t kWalkSmemMax = 227 * 1024;      // the largest shared-memory op
 // every frame reads `scene` (level 0 as the batch's worklist slot reads it); with them, the scenes of `levels` (and `scene`
 // is not read).  With per-frame states the five state-dependent tables come from `states` (level 0's slot layout; with
 // per-frame levels, only its frame_slot is read, into `levels.sets`).
+// With fixed colormaps (`fixed_rows`: some frame of the batch has one), the raster reads `fixed` (per-frame levels and
+// states only).
 struct BatchTables {
     DeviceScene scene;
     StateTables states;
     LevelTables levels;
-    bool per_frame, per_level;
+    FixedTables fixed;
+    bool per_frame, per_level, fixed_rows;
 };
 
 // Kernel 1: front-to-back BSP walk, one CTA per frame.  Writes frames[i] and up to `stride` worklist entries per frame at
@@ -125,6 +140,12 @@ cudaError_t launch_prelight(const uint8_t *d_colormap, const uint8_t *d_src, uin
 // Textures: 32 pre-lit planes (+ opacity plane 32) of every texture of the table, in its per-texture layout.
 cudaError_t launch_prelight_textures(const uint8_t *d_colormap, const uint8_t *d_texels, const TexRec *d_tex, int ntex,
                                      uint8_t *d_dst, size_t stride, cudaStream_t stream);
+
+// One more pre-lit plane, of COLORMAP row `d_row` (256 bytes): the flats (dst[i] = row[src[i]], i < n) and the textures
+// (in the per-texture layout of the planes above).  For fixed colormap 32 (FixedPlanes).
+cudaError_t launch_prelight_row(const uint8_t *d_row, const uint8_t *d_src, uint8_t *d_dst, size_t n, cudaStream_t stream);
+cudaError_t launch_prelight_textures_row(const uint8_t *d_row, const uint8_t *d_texels, const TexRec *d_tex, int ntex,
+                                         uint8_t *d_dst, cudaStream_t stream);
 
 // Kernel 3: palette LUT on its own (index -> RGBA8), 16 pixels per thread.
 cudaError_t launch_palette(const uint32_t *d_palette, const uint8_t *d_index, uint32_t *d_rgba,

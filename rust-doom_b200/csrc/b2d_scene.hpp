@@ -79,7 +79,8 @@ constexpr int32_t kFlatSky = -1, kFlatMissing = -2, kTexNone = -1;
 // Light level of a sector at `tics` (game/src/lights.rs:26-66), float32 operation by operation (volatile keeps
 // every intermediate a rounded float32: no x87 excess precision, no fused multiply-add).  The sine of the random
 // effect's hash is the correctly rounded float32 sine: double-precision sine, rounded once (DESIGN.md C15).
-inline uint8_t light_byte_at(const LightRec &L, uint32_t tics) {
+// `extralight` (0..2, DESIGN.md C18): the player's extra light adds f32(2 e) / f32(31) to the level before the clamp.
+inline uint8_t light_byte_at(const LightRec &L, uint32_t tics, uint32_t extralight = 0) {
     volatile float time = (float)tics / 35.0f;
     volatile float v = L.level;
     auto fract = [](float x) -> float { volatile float f = std::floor(x); volatile float r = x - f; return r; };
@@ -109,6 +110,10 @@ inline uint8_t light_byte_at(const LightRec &L, uint32_t tics) {
         volatile float s3 = L.sync * 3.5435f;
         volatile float ph = ts + s3;
         v = fract(ph) < L.duration ? L.alt : L.level;
+    }
+    if (extralight) {
+        volatile float x = (float)(2 * extralight) / 31.0f;
+        v = v + x;
     }
     if (v < 0.0f) v = 0.0f; else if (v > 1.0f) v = 1.0f;
     volatile float scaled = v * 255.0f;
@@ -154,6 +159,10 @@ struct StateSrc {
     const uint32_t *sector_slots;   // per sector: light slot (low 16 bits) | dynamic slot << 16; kNoSlot = none
     const int32_t *mid_seg;         // per masked middle: the seg that owns it (each has exactly one), -1 = none
     uint32_t ntex, nflats, nanim, nsectors, nsegs, nsprites, nmids, ndyn;
+    // Extra light (C18; read only by a state with extra light): per sector its static light in steps of 1/31
+    // (light >> 3, light_steps), then per seg its fake contrast (-1, 0, +1; 0 in front of a light effect)
+    const int16_t *sector_steps;
+    const int8_t *seg_contrast;
 };
 
 // One compact state as the per-record functions read it.
@@ -161,10 +170,12 @@ struct StateIn {
     uint32_t tics, moved;
     const int32_t *off;             // floor, ceiling offset per dynamic slot
     const uint8_t *light;           // light byte per light slot
+    uint32_t extra;                 // the player's extra light, 0..2 (C18): the light bytes of the state already hold it
 };
 
 B2D_HD StateIn state_in(const uint32_t *words, uint32_t ndyn) {
     StateIn s;
+    s.extra = 0;
     s.tics = words[0];
     s.moved = words[1];
     s.off = reinterpret_cast<const int32_t *>(words + 2);
@@ -194,6 +205,34 @@ B2D_HD int32_t ceil_off_of(const StateSrc &s, const StateIn &st, uint32_t f) {
     return d == kNoSlot ? 0 : st.off[2 * d + 1];
 }
 
+// The static light byte of `steps` (a sector's light >> 3, plus 2 per step of extra light) with fake contrast `contrast`:
+// light_byte's float32 sequence (C12, C18), rounded operation by operation on the device as on the host.
+B2D_HD uint8_t light_byte_steps(int32_t steps, int contrast) {
+#ifdef __CUDA_ARCH__
+    float level = __fdiv_rn((float)steps, 31.0f);
+    if (contrast) {
+        level = __fadd_rn(level, contrast > 0 ? 2.0f / 31.0f : -2.0f / 31.0f);
+        level = level > 1.0f ? 1.0f : (level < 0.0f ? 0.0f : level);
+    }
+    level = level > 1.0f ? 1.0f : (level < 0.0f ? 0.0f : level);
+    return (uint8_t)(int)__fmul_rn(level, 255.0f);
+#else
+    volatile float level = (float)steps / 31.0f;
+    if (contrast) {
+        volatile float c = contrast > 0 ? 2.0f / 31.0f : -2.0f / 31.0f;
+        level = level + c;
+        if (level > 1.0f) level = 1.0f; else if (level < 0.0f) level = 0.0f;
+    }
+    if (level > 1.0f) level = 1.0f; else if (level < 0.0f) level = 0.0f;
+    volatile float scaled = level * 255.0f;
+    return (uint8_t)(int)scaled;
+#endif
+}
+// the static light byte of sector f (no light effect) raised by the state's extra light
+B2D_HD int32_t extra_light_of(const StateSrc &s, const StateIn &st, uint32_t f, int contrast) {
+    return light_byte_steps((int32_t)s.sector_steps[f] + 2 * (int32_t)st.extra, contrast);
+}
+
 // Level time (C14): every frame name of an animation group shows group frame (tics/8) mod n.
 B2D_HD TexRec tex_at(const StateSrc &s, const StateIn &st, uint32_t i) {
     const int32_t j = anim_now(s, st.tics, (int32_t)s.tex[i].anim_first, s.tex[i].anim_nk, (int32_t)i);
@@ -211,6 +250,7 @@ B2D_HD SectorRec sector_at(const StateSrc &s, const StateIn &st, uint32_t i) {
     r.floor_flat = flat_now(s, st.tics, r.floor_flat);
     r.ceil_flat = flat_now(s, st.tics, r.ceil_flat);
     if (has_light_slot(s, i)) r.light = light_of(s, st, i);
+    else if (st.extra) r.light = extra_light_of(s, st, i, 0);
     if (st.moved) {
         r.floor += floor_off_of(s, st, i);
         r.ceil += ceil_off_of(s, st, i);
@@ -227,6 +267,7 @@ B2D_HD SegRec seg_at(const StateSrc &s, const StateIn &st, uint32_t i) {
     const uint32_t f = (uint32_t)S.front;
     if (f >= s.nsectors) return S;
     if (has_light_slot(s, f)) S.light = light_of(s, st, f);
+    else if (st.extra) S.light = extra_light_of(s, st, f, s.seg_contrast[i]);
     if (!st.moved) return S;
     const SegDynRec D = s.segdyn[i];
     const int32_t fo = floor_off_of(s, st, f), co = ceil_off_of(s, st, f);
@@ -253,6 +294,7 @@ B2D_HD SpriteRec sprite_at(const StateSrc &s, const StateIn &st, uint32_t i) {
     const uint32_t f = (uint32_t)P.sector;
     if (f >= s.nsectors) return P;
     if (has_light_slot(s, f)) P.light = light_of(s, st, f);
+    else if (st.extra) P.light = extra_light_of(s, st, f, 0);
     if (st.moved) P.low += P.hanging ? ceil_off_of(s, st, f) : floor_off_of(s, st, f);
     return P;
 }
@@ -317,9 +359,10 @@ inline uint32_t state_tics(const StateLayout &L, uint32_t tics) {
     return 0;
 }
 
-// The compact state of level time `tics` with `floor_off` / `ceil_off` (nullptr, or one offset per sector) into out[words].
+// The compact state of level time `tics` with `floor_off` / `ceil_off` (nullptr, or one offset per sector) into out[words];
+// its light bytes with the player's `extralight` (C18).
 inline void compact_state(const uint8_t *blob, const StateLayout &L, uint32_t tics, const int32_t *floor_off,
-                          const int32_t *ceil_off, uint32_t *out) {
+                          const int32_t *ceil_off, uint32_t *out, uint32_t extralight = 0) {
     const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
     const LightRec *lights = reinterpret_cast<const LightRec *>(blob + h[H_OFF_LIGHTS]);
     for (uint32_t w = 0; w < L.words; w++) out[w] = 0;
@@ -332,7 +375,27 @@ inline void compact_state(const uint8_t *blob, const StateLayout &L, uint32_t ti
         }
     }
     uint8_t *light = reinterpret_cast<uint8_t *>(out + 2 + 2 * L.dyn_sectors.size());
-    for (size_t k = 0; k < L.light_sectors.size(); k++) light[k] = light_byte_at(lights[L.light_sectors[k]], tics);
+    for (size_t k = 0; k < L.light_sectors.size(); k++) light[k] = light_byte_at(lights[L.light_sectors[k]], tics, extralight);
+}
+
+// The side tables of StateSrc::sector_steps / seg_contrast, derived from the blob: a sector's lights record holds
+// (light >> 3) / 31 whatever its effect, and a seg's contrast follows from its vertices as compile_scene derives it
+// (visitor.rs:887-901: +1 for a wall along the map's x axis, -1 along its y axis, none in front of a light effect).
+inline void light_steps(const uint8_t *blob, std::vector<int16_t> &sector_steps, std::vector<int8_t> &seg_contrast) {
+    const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
+    const LightRec *lights = reinterpret_cast<const LightRec *>(blob + h[H_OFF_LIGHTS]);
+    const SegRec *segs = reinterpret_cast<const SegRec *>(blob + h[H_OFF_SEGS]);
+    const int32_t *verts = reinterpret_cast<const int32_t *>(blob + h[H_OFF_VERTS]);
+    sector_steps.assign(h[H_NSECTORS], 0);
+    for (uint32_t i = 0; i < h[H_NSECTORS]; i++) sector_steps[i] = (int16_t)std::lrint((double)lights[i].level * 31.0);
+    seg_contrast.assign(h[H_NSEGS], 0);
+    for (uint32_t i = 0; i < h[H_NSEGS]; i++) {
+        const SegRec &S = segs[i];
+        if ((S.flags & kSegInvalid) || (uint32_t)S.front >= h[H_NSECTORS] || lights[S.front].kind != kLightNone) continue;
+        if ((uint32_t)S.v1 >= h[H_NVERTS] || (uint32_t)S.v2 >= h[H_NVERTS]) continue;
+        const int64_t dx = (int64_t)verts[2 * S.v2] - verts[2 * S.v1], dy = (int64_t)verts[2 * S.v2 + 1] - verts[2 * S.v1 + 1];
+        seg_contrast[i] = dy == 0 ? 1 : (dx == 0 ? -1 : 0);
+    }
 }
 
 inline StateSrc state_src(const uint8_t *blob, const StateLayout &L) {
@@ -350,6 +413,7 @@ inline StateSrc state_src(const uint8_t *blob, const StateLayout &L) {
     s.mid_seg = L.mid_seg.data();
     s.ntex = h[H_NTEX]; s.nflats = h[H_NFLATS]; s.nanim = h[H_NANIM]; s.nsectors = h[H_NSECTORS];
     s.nsegs = h[H_NSEGS]; s.nsprites = h[H_NSPRITES]; s.nmids = h[H_NMIDS]; s.ndyn = (uint32_t)L.dyn_sectors.size();
+    s.sector_steps = nullptr; s.seg_contrast = nullptr;     // the caller's, when it expands states with extra light
     return s;
 }
 
