@@ -147,13 +147,34 @@ int ensure_slot(const b2d_renderer *r, WorkSlot &s) {
     return B2D_OK;
 }
 
+// The layout of one table set of a level, [tex | sectors | segs | sprites | mids] (b2d_scene_tables_at's), from its five
+// record counts: the byte offsets of the sections after the first, the set's bytes, and `slot`, those rounded up to 256
+// (the space a set takes in an arena or as a worklist slot's own set).
+struct SetLayout {
+    size_t sectors, segs, sprites, mids, bytes, slot;
+    SetLayout(size_t ntex, size_t nsectors, size_t nsegs, size_t nsprites, size_t nmids)
+        : sectors(ntex * sizeof(TexRec)), segs(sectors + nsectors * sizeof(SectorRec)), sprites(segs + nsegs * sizeof(SegRec)),
+          mids(sprites + nsprites * sizeof(SpriteRec)), bytes(mids + nmids * sizeof(MidRec)), slot((bytes + 255) & ~(size_t)255) {}
+    explicit SetLayout(const StateSrc &s) : SetLayout(s.ntex, s.nsectors, s.nsegs, s.nsprites, s.nmids) {}
+    explicit SetLayout(const uint8_t *blob)      // a scene blob's, from its header
+        : SetLayout(hdr(blob)[H_NTEX], hdr(blob)[H_NSECTORS], hdr(blob)[H_NSEGS], hdr(blob)[H_NSPRITES], hdr(blob)[H_NMIDS]) {}
+    // the five tables of the set at `base`
+    TableSet at(const uint8_t *base) const {
+        return TableSet{reinterpret_cast<const TexRec *>(base), reinterpret_cast<const SectorRec *>(base + sectors),
+                        reinterpret_cast<const SegRec *>(base + segs), reinterpret_cast<const SpriteRec *>(base + sprites),
+                        reinterpret_cast<const MidRec *>(base + mids)};
+    }
+  private:
+    static const uint32_t *hdr(const uint8_t *blob) { return reinterpret_cast<const uint32_t *>(blob); }
+};
+
 // Per-frame states: the two worklist slots' arenas of max_batch table sets, allocated together by the first such call.  A
-// set takes its level's slot_bytes; the arena is sized by the largest of the levels, so that it holds max_batch sets of
-// any mix of levels (b2d_render_levels_states) as well as max_batch sets of level 0 (b2d_render_states).
+// set takes its level's SetLayout::slot; the arena is sized by the largest of the levels, so that it holds max_batch sets
+// of any mix of levels.
 int ensure_states(b2d_renderer *r) {
     if (r->slot[0].arena) return B2D_OK;
     size_t slot_bytes = 0;
-    for (const LevelRes &lv : r->lv) slot_bytes = std::max(slot_bytes, (size_t)lv.state_tables.slot_bytes);
+    for (const LevelRes &lv : r->lv) slot_bytes = std::max(slot_bytes, SetLayout(lv.src).slot);
     DeviceBuf<uint8_t> arena[2];
     for (auto &a : arena) CU(allocate(a, (size_t)r->max_batch * slot_bytes));
     for (int i = 0; i < 2; i++) r->slot[i].arena = std::move(arena[i]);
@@ -184,13 +205,6 @@ struct StageLayout {
     }
 };
 
-// the five tables of the table set at `set`, laid out as `t` says
-TableSet table_set(const uint8_t *set, const StateTables &t) {
-    return TableSet{reinterpret_cast<const TexRec *>(set), reinterpret_cast<const SectorRec *>(set + t.off_sectors),
-                    reinterpret_cast<const SegRec *>(set + t.off_segs), reinterpret_cast<const SpriteRec *>(set + t.off_sprites),
-                    reinterpret_cast<const MidRec *>(set + t.off_mids)};
-}
-
 // records of one table set of a level (the threads of its expansion)
 size_t set_records(const LevelRes &lv) { return (size_t)lv.src.ntex + lv.src.nsectors + lv.src.nsegs + lv.src.nsprites + lv.src.nmids; }
 
@@ -199,7 +213,7 @@ size_t set_records(const LevelRes &lv) { return (size_t)lv.src.ntex + lv.src.nse
 DeviceScene slot_scene(const LevelRes &lv, int slot) {
     DeviceScene d = lv.ds;
     if (const uint8_t *set = lv.slot[slot].tables.get()) {
-        const TableSet t = table_set(set, lv.state_tables);
+        const TableSet t = SetLayout(lv.src).at(set);
         d.tex = t.tex; d.sectors = t.sectors; d.segs = t.segs; d.sprites = t.sprites; d.mids = t.mids;
     }
     return d;
@@ -231,12 +245,6 @@ struct Expansion {
     uint32_t extralight;
 };
 
-// bytes of one level's state-dependent tables, [tex | sectors | segs | sprites | mids]
-size_t level_table_bytes(const LevelRes &lv) {
-    return lv.src.ntex * sizeof(TexRec) + lv.src.nsectors * sizeof(SectorRec) + lv.src.nsegs * sizeof(SegRec) +
-           lv.src.nsprites * sizeof(SpriteRec) + lv.src.nmids * sizeof(MidRec);
-}
-
 // Level `lv`'s row-32 planes (fixed colormap 32, DESIGN.md C18), built on `stream` by the first batch that needs them: the
 // group is created whole, or not at all.
 int ensure_row32(b2d_renderer *r, LevelRes &lv, cudaStream_t stream) {
@@ -257,21 +265,12 @@ int ensure_row32(b2d_renderer *r, LevelRes &lv, cudaStream_t stream) {
     return B2D_OK;
 }
 
-// the state-dependent tables (level time `tics`, sector offsets), laid out [tex | sectors | segs | sprites | mids]
-size_t state_table_bytes(const uint8_t *blob) {
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
-    return h[H_NTEX] * sizeof(TexRec) + h[H_NSECTORS] * sizeof(SectorRec) + h[H_NSEGS] * sizeof(SegRec) +
-           h[H_NSPRITES] * sizeof(SpriteRec) + h[H_NMIDS] * sizeof(MidRec);
-}
-
+// the state-dependent tables (level time `tics`, sector offsets) as a table set at `out` (SetLayout(blob))
 void state_tables(const uint8_t *blob, uint32_t tics, const int32_t *floor_off, const int32_t *ceil_off, uint8_t *out) {
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
-    TexRec *tex = reinterpret_cast<TexRec *>(out);
-    SectorRec *sectors = reinterpret_cast<SectorRec *>(tex + h[H_NTEX]);
-    SegRec *segs = reinterpret_cast<SegRec *>(sectors + h[H_NSECTORS]);
-    SpriteRec *sprites = reinterpret_cast<SpriteRec *>(segs + h[H_NSEGS]);
-    MidRec *mids = reinterpret_cast<MidRec *>(sprites + h[H_NSPRITES]);
-    scene_at_time(blob, tics, tex, sectors, segs, sprites, mids, floor_off, ceil_off);
+    const SetLayout L(blob);
+    scene_at_time(blob, tics, reinterpret_cast<TexRec *>(out), reinterpret_cast<SectorRec *>(out + L.sectors),
+                  reinterpret_cast<SegRec *>(out + L.segs), reinterpret_cast<SpriteRec *>(out + L.sprites),
+                  reinterpret_cast<MidRec *>(out + L.mids), floor_off, ceil_off);
 }
 
 // The compact state of level time `tics` with the level's current sector moves into out[layout.words] (out is not
@@ -281,11 +280,39 @@ void state_at(const LevelRes &lv, uint32_t tics, uint32_t *out) {
     std::copy(lv.state.begin() + 1, lv.state.begin() + 2 + 2 * (ptrdiff_t)lv.layout.dyn_sectors.size(), out + 1);
 }
 
+// Per-frame palettes (HOST, nullable = palette 0): frame i's palette below the palette count of its level (levels[i],
+// nullable = level 0), the levels already checked; B2D_ERR_INVALID_ARG otherwise.
+int check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n) {
+    if (palettes)
+        for (size_t i = 0; i < n; i++)
+            if (palettes[i] >= r->pal_count[levels ? levels[i] : 0u])
+                return fail(B2D_ERR_INVALID_ARG, "frame palette out of range (>= the palette count of the frame's level)");
+    return B2D_OK;
+}
+
 }  // namespace
 
-int b2d::build_states(const b2d_renderer *r, const b2d_frame_state *states, const uint32_t *tics, size_t n,
-                      const b2d_sector_move *moves, size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts,
-                      Frames &out) {
+int b2d::CallFrames::prepare(const b2d_renderer *r, size_t n) {
+    if (takes & kFrameLevels) {
+        if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
+        if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
+            return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
+        for (size_t i = 0; i < n; i++)
+            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    }
+    if (int rc = check_palettes(r, levels, palettes, n)) return rc;
+    if (lights) {
+        bool any = false;
+        for (size_t i = 0; i < n; i++) {
+            if (lights[i].fixed_colormap < -1 || lights[i].fixed_colormap > 32)
+                return fail(B2D_ERR_INVALID_ARG, "frame fixed colormap out of range (-1 .. 32)");
+            if (lights[i].extralight > 2) return fail(B2D_ERR_INVALID_ARG, "frame extra light out of range (0 .. 2)");
+            any = any || lights[i].fixed_colormap != -1 || lights[i].extralight != 0;
+        }
+        if (!any) lights = nullptr;
+    }
+    frames = Frames{levels, nullptr, nullptr, lights};
+    if (!(takes & kFrameStates) && !tics) return B2D_OK;
     if (!tics) {
         if (!states || (n_moves && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
         for (size_t i = 0; i < n; i++)
@@ -293,7 +320,6 @@ int b2d::build_states(const b2d_renderer *r, const b2d_frame_state *states, cons
                 return fail(B2D_ERR_INVALID_ARG, "a frame's move range runs past the end of the move list");
     }
     return guarded([&] {
-        const uint32_t *levels = out.levels;
         size_t total = 0;
         starts.assign(n, 0);
         for (size_t i = 0; i < n; i++) {
@@ -322,42 +348,12 @@ int b2d::build_states(const b2d_renderer *r, const b2d_frame_state *states, cons
                 for (size_t k = 0; k < fo.size() && !moved; k++) moved = fo[k] != 0 || co[k] != 0;    // all zero: at rest
             }
             compact_state(lv.h_blob.data(), lv.layout, states[i].tics, moved ? fo.data() : nullptr, moved ? co.data() : nullptr,
-                          fs.data() + starts[i], out.lights ? out.lights[i].extralight : 0u);
+                          fs.data() + starts[i], lights ? lights[i].extralight : 0u);
         }
-        out.fs = fs.data();
-        out.starts = !levels && r->lv[0].h_blob.empty() ? nullptr : starts.data();
+        frames.fs = fs.data();
+        frames.starts = !levels && r->lv[0].h_blob.empty() ? nullptr : starts.data();
         return B2D_OK;
     });
-}
-
-int b2d::check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
-    if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
-    if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
-        return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
-    for (size_t i = 0; i < n; i++)
-        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
-    return B2D_OK;
-}
-
-int b2d::check_lights(const b2d_frame_light *&lights, size_t n) {
-    if (!lights) return B2D_OK;
-    bool any = false;
-    for (size_t i = 0; i < n; i++) {
-        if (lights[i].fixed_colormap < -1 || lights[i].fixed_colormap > 32)
-            return fail(B2D_ERR_INVALID_ARG, "frame fixed colormap out of range (-1 .. 32)");
-        if (lights[i].extralight > 2) return fail(B2D_ERR_INVALID_ARG, "frame extra light out of range (0 .. 2)");
-        any = any || lights[i].fixed_colormap != -1 || lights[i].extralight != 0;
-    }
-    if (!any) lights = nullptr;
-    return B2D_OK;
-}
-
-int b2d::check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n) {
-    if (palettes)
-        for (size_t i = 0; i < n; i++)
-            if (palettes[i] >= r->pal_count[levels ? levels[i] : 0u])
-                return fail(B2D_ERR_INVALID_ARG, "frame palette out of range (>= the palette count of the frame's level)");
-    return B2D_OK;
 }
 
 int b2d::check_slots_free(const b2d_renderer *r, size_t batches) {
@@ -371,8 +367,7 @@ int b2d::check_slots_free(const b2d_renderer *r, size_t batches) {
 // awaited through an event, so a caller may run walks and rasters on two streams and have the walk of batch k+1 overlap the
 // raster of batch k.  The batch's table sets are expanded on `stream` first.  With per-frame states: frames whose (level,
 // compact state) are equal share a set; sets are numbered in order of first appearance and packed into the slot's arena,
-// each at its level's slot_bytes (level 0's sets at level 0's stride, as the per-frame-state kernels without per-frame
-// levels read them), and one launch expands them all.  Without: the slot's own table set of each timed level the batch
+// and one launch expands them all.  Without: the slot's own table set of each timed level the batch
 // uses is re-expanded, one launch per level, when the level's state differs from the one the set holds, so the walk and
 // the raster of a ticket read one state whatever is set in between.  What the batch stages (StageLayout) goes to the device
 // in one copy; a plain batch at an unchanged state stages nothing and does not wait on the host.
@@ -423,7 +418,7 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
             auto it = seen.emplace(std::move(key), (uint32_t)plan.size());
             if (it.second) {
                 plan.push_back(Expansion{k, w, s.arena.get() + aoff, e});
-                aoff += lv.state_tables.slot_bytes;
+                aoff += SetLayout(lv.src).slot;
                 state_words += lv.layout.words;
             }
             frame_set[(size_t)f] = it.first->second;
@@ -458,7 +453,7 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
         size_t woff = 0;
         for (size_t k = 0; k < nsets; k++) {
             const LevelRes &lv = r->lv[plan[k].level];
-            sets[k] = table_set(plan[k].tables, lv.state_tables);
+            sets[k] = SetLayout(lv.src).at(plan[k].tables);
             // one launch numbers the records of all per-frame sets; a launch of its own per stale set starts at 0
             descs[k] = StateSet{plan[k].level, (uint32_t)woff, per_frame ? (uint32_t)records : 0u, plan[k].extralight};
             std::memcpy(words + woff, plan[k].state, 4 * lv.layout.words);
@@ -503,18 +498,10 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
     t.fixed_rows = fixed_rows;
     if (fixed_rows)
         t.fixed = FixedTables{reinterpret_cast<const int32_t *>(d + L.frame_fixed), reinterpret_cast<const FixedPlanes *>(d + L.planes)};
-    if (per_level)
-        t.levels = LevelTables{reinterpret_cast<const DeviceScene *>(d + L.scenes), reinterpret_cast<const uint32_t *>(d + L.frame_level),
-                               per_frame ? d_sets : nullptr};
-    else
-        t.scene = slot_scene(r->lv[0], slot);
-    if (per_frame) {
-        if (!per_level) {
-            t.states = r->lv[0].state_tables;
-            t.states.base = s.arena.get();
-        }
-        t.states.frame_slot = reinterpret_cast<const uint32_t *>(d + L.frame_set);
-    }
+    if (!per_level) t.scene = slot_scene(r->lv[0], slot);
+    t.levels = LevelTables{per_level ? reinterpret_cast<const DeviceScene *>(d + L.scenes) : nullptr,
+                           per_level ? reinterpret_cast<const uint32_t *>(d + L.frame_level) : nullptr,
+                           per_frame ? d_sets : nullptr, per_frame ? reinterpret_cast<const uint32_t *>(d + L.frame_set) : nullptr};
     rc = profiled(r, stream, 0, [&] {
         return launch_walk(t, r->walk_smem, r->view, d_poses, n, s.frames.get(), s.work.get(), r->stride, stream, background);
     });
@@ -713,7 +700,7 @@ int b2d_scene_create_from_lumps(const b2d_level_lumps *lv, const b2d_textures *t
 int b2d_scene_tables_at(const b2d_scene *s, uint32_t tics, const b2d_sector_move *moves, size_t n_moves, void *out,
                         size_t capacity, size_t *size_out) {
     if (!s || (n_moves && !moves)) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    const size_t need = state_table_bytes(s->blob.data());
+    const size_t need = SetLayout(s->blob.data()).bytes;
     if (size_out) *size_out = need;
     if (!out) return B2D_OK;
     if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");
@@ -927,12 +914,6 @@ int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
         src.mid_seg = reinterpret_cast<const int32_t *>(lv.d_slot_maps.get() + L.sector_slots.size());
         src.sector_steps = reinterpret_cast<const int16_t *>(dm + 4 * maps);
         src.seg_contrast = reinterpret_cast<const int8_t *>(dm + 4 * maps + 2 * steps.size());
-        StateTables &t = lv.state_tables;              // one table set: [tex | sectors | segs | sprites | mids], 256 B aligned
-        t.slot_bytes = (uint32_t)((state_table_bytes(blob) + 255) & ~(size_t)255);
-        t.off_sectors = (uint32_t)(h[H_NTEX] * sizeof(TexRec));
-        t.off_segs = t.off_sectors + (uint32_t)(h[H_NSECTORS] * sizeof(SectorRec));
-        t.off_sprites = t.off_segs + (uint32_t)(h[H_NSEGS] * sizeof(SegRec));
-        t.off_mids = t.off_sprites + (uint32_t)(h[H_NSPRITES] * sizeof(SpriteRec));
         // tic 0 is a time like any other: a frame name with k > 0 shows its group's frame 0 (tex.rs:260, 302-306)
         lv.state.assign(L.words, 0);
         compact_state(blob, L, 0, nullptr, nullptr, lv.state.data());
@@ -941,8 +922,8 @@ int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
         lv.h_blob = s->blob;
         const uint8_t *blob = lv.h_blob.data();
         const size_t words = lv.layout.words;
-        const StateTables &t = lv.state_tables;
-        for (auto &sl : lv.slot) CU(allocate(sl.tables, t.slot_bytes));
+        const SetLayout t(lv.src);
+        for (auto &sl : lv.slot) CU(allocate(sl.tables, t.slot));
         // The pre-lit planes above were built from the blob's own (per-image) records; both slots' table sets start at tic
         // 0, expanded by one launch.
         const StageLayout S(1, 2, 0, words, false, false);
@@ -950,7 +931,7 @@ int create_level(b2d_renderer *r, LevelRes &lv, const b2d_scene *s) {
         std::vector<uint8_t> stage(S.end);
         *reinterpret_cast<StateSrc *>(stage.data() + S.srcs) = lv.src;
         for (uint32_t k = 0; k < 2; k++) {
-            reinterpret_cast<TableSet *>(stage.data() + S.sets)[k] = table_set(lv.slot[k].tables.get(), t);
+            reinterpret_cast<TableSet *>(stage.data() + S.sets)[k] = t.at(lv.slot[k].tables.get());
             reinterpret_cast<StateSet *>(stage.data() + S.descs)[k] = StateSet{0, 0, k * records, 0};
             lv.slot[k].state = lv.state;
         }
@@ -1159,31 +1140,43 @@ int b2d_render_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, uint8_
                           static_cast<cudaStream_t>(cuda_stream));
 }
 
-// walk + raster of the n frames `fr` (device poses) in batches of max_batch on `st`
-static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, const Frames &fr, size_t n, uint8_t *d_index_fb,
-                           uint32_t *d_rgba_fb, cudaStream_t st) {
-    int rc = check_slots_free(r, batch_count(r, n));
+// b2d_render_device_*: the null checks, then walk + raster of the n frames `c` describes (device poses), prepared, in
+// batches of max_batch on `cuda_stream`
+static int enqueue_batches(b2d_renderer *r, const b2d_pose *d_poses, CallFrames c, size_t n, uint8_t *d_index_fb,
+                           uint32_t *d_rgba_fb, void *cuda_stream) {
+    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    int rc = c.prepare(r, n);
+    if (rc != B2D_OK || n == 0) return rc;
+    CU(cudaSetDevice(r->device));
+    rc = check_slots_free(r, batch_count(r, n));
     if (rc != B2D_OK) return rc;
     const size_t npix = (size_t)r->view.W * r->view.H;
     for (size_t i = 0; i < n; i += (size_t)r->max_batch) {
         const size_t cnt = n - i < (size_t)r->max_batch ? n - i : (size_t)r->max_batch;
-        rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, fr.from(i), (int)cnt, d_index_fb + i * npix,
-                            d_rgba_fb ? d_rgba_fb + i * npix : nullptr, st);
+        rc = enqueue_frames(r, reinterpret_cast<const Pose *>(d_poses) + i, c.frames.from(i), (int)cnt, d_index_fb + i * npix,
+                            d_rgba_fb ? d_rgba_fb + i * npix : nullptr, static_cast<cudaStream_t>(cuda_stream));
         if (rc != B2D_OK) return rc;
     }
     return B2D_OK;
+}
+
+// b2d_walk_device*: the null checks and 1 <= n <= max_batch, then the walk of the n frames `c` describes (device poses),
+// prepared, as one batch in a background grid on `cuda_stream`
+static int walk_device(b2d_renderer *r, const b2d_pose *d_poses, CallFrames c, size_t n, void *cuda_stream, int64_t *ticket_out) {
+    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
+    if (int rc = c.prepare(r, n)) return rc;
+    CU(cudaSetDevice(r->device));
+    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), c.frames, (int)n, static_cast<cudaStream_t>(cuda_stream), true,
+                      ticket_out);
 }
 
 int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *tics, size_t n, uint8_t *d_index_fb,
                             uint32_t *d_rgba_fb, void *cuda_stream) {
     if (!r || !d_poses || !d_index_fb || !tics) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0) return B2D_OK;
-    CU(cudaSetDevice(r->device));
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr;
-    int rc = build_states(r, nullptr, tics, n, nullptr, 0, fs, starts, fr);
-    if (rc == B2D_OK) rc = enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+    int rc = check_slots_free(r, batch_count(r, n));                       // refused before the states are built
+    if (rc == B2D_OK) rc = enqueue_batches(r, d_poses, CallFrames(tics), n, d_index_fb, d_rgba_fb, cuda_stream);
     if (rc != B2D_OK) return rc;
     return b2d_renderer_set_time(r, tics[n - 1]);                          // the renderer is left at the last pose's time
 }
@@ -1191,35 +1184,17 @@ int b2d_render_device_timed(b2d_renderer *r, const b2d_pose *d_poses, const uint
 int b2d_render_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
                              const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb, uint32_t *d_rgba_fb,
                              void *cuda_stream) {
-    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr;
-    int rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK || n == 0) return rc;
-    CU(cudaSetDevice(r->device));
-    return enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+    return enqueue_batches(r, d_poses, CallFrames(kFrameStates, nullptr, states, moves, n_moves), n, d_index_fb, d_rgba_fb,
+                           cuda_stream);
 }
 
 int b2d_walk_device_states(b2d_renderer *r, const b2d_pose *d_poses, const b2d_frame_state *states, size_t n,
                            const b2d_sector_move *moves, size_t n_moves, void *cuda_stream, int64_t *ticket_out) {
-    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr;
-    int rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    CU(cudaSetDevice(r->device));
-    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
+    return walk_device(r, d_poses, CallFrames(kFrameStates, nullptr, states, moves, n_moves), n, cuda_stream, ticket_out);
 }
 
 int b2d_walk_device(b2d_renderer *r, const b2d_pose *d_poses, size_t n, void *cuda_stream, int64_t *ticket_out) {
-    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
-    CU(cudaSetDevice(r->device));
-    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), Frames{}, (int)n, static_cast<cudaStream_t>(cuda_stream), true,
-                      ticket_out);
+    return walk_device(r, d_poses, CallFrames(), n, cuda_stream, ticket_out);
 }
 
 int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint32_t *d_rgba_fb, void *cuda_stream) {
@@ -1230,89 +1205,48 @@ int b2d_raster_device(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint
 
 int b2d_render_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, uint8_t *d_index_fb,
                              uint32_t *d_rgba_fb, void *cuda_stream) {
-    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    const int rc = check_levels(r, levels, n);
-    if (rc != B2D_OK || n == 0) return rc;
-    CU(cudaSetDevice(r->device));
-    return enqueue_batches(r, d_poses, Frames{levels}, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+    return enqueue_batches(r, d_poses, CallFrames(kFrameLevels, levels), n, d_index_fb, d_rgba_fb, cuda_stream);
 }
 
 int b2d_walk_device_levels(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n, void *cuda_stream,
                            int64_t *ticket_out) {
-    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
-    const int rc = check_levels(r, levels, n);
-    if (rc != B2D_OK) return rc;
-    CU(cudaSetDevice(r->device));
-    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), Frames{levels}, (int)n, static_cast<cudaStream_t>(cuda_stream),
-                      true, ticket_out);
+    return walk_device(r, d_poses, CallFrames(kFrameLevels, levels), n, cuda_stream, ticket_out);
 }
 
 int b2d_render_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
                                     size_t n, const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb,
                                     uint32_t *d_rgba_fb, void *cuda_stream) {
-    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr{levels};
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK || n == 0) return rc;
-    CU(cudaSetDevice(r->device));
-    return enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+    return enqueue_batches(r, d_poses, CallFrames(kFrameLevels | kFrameStates, levels, states, moves, n_moves), n, d_index_fb,
+                           d_rgba_fb, cuda_stream);
 }
 
 int b2d_walk_device_levels_states(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
                                   size_t n, const b2d_sector_move *moves, size_t n_moves, void *cuda_stream, int64_t *ticket_out) {
-    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr{levels};
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    CU(cudaSetDevice(r->device));
-    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
+    return walk_device(r, d_poses, CallFrames(kFrameLevels | kFrameStates, levels, states, moves, n_moves), n, cuda_stream,
+                       ticket_out);
 }
 
 int b2d_render_device_levels_states_lights(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
                                            const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
                                            const b2d_sector_move *moves, size_t n_moves, uint8_t *d_index_fb,
                                            uint32_t *d_rgba_fb, void *cuda_stream) {
-    if (!r || !d_poses || !d_index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr{levels};
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK) rc = check_lights(lights, n);
-    fr.lights = lights;
-    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK || n == 0) return rc;
-    CU(cudaSetDevice(r->device));
-    return enqueue_batches(r, d_poses, fr, n, d_index_fb, d_rgba_fb, static_cast<cudaStream_t>(cuda_stream));
+    return enqueue_batches(r, d_poses, CallFrames(kFrameLevels | kFrameStates, levels, states, moves, n_moves, lights), n,
+                           d_index_fb, d_rgba_fb, cuda_stream);
 }
 
 int b2d_walk_device_levels_states_lights(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels,
                                          const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
                                          const b2d_sector_move *moves, size_t n_moves, void *cuda_stream,
                                          int64_t *ticket_out) {
-    if (!r || !d_poses || !ticket_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (n == 0 || n > (size_t)r->max_batch) return fail(B2D_ERR_INVALID_ARG, "n must be in 1..max_batch");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr{levels};
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK) rc = check_lights(lights, n);
-    fr.lights = lights;
-    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    CU(cudaSetDevice(r->device));
-    return walk_batch(r, reinterpret_cast<const Pose *>(d_poses), fr, (int)n, static_cast<cudaStream_t>(cuda_stream), true, ticket_out);
+    return walk_device(r, d_poses, CallFrames(kFrameLevels | kFrameStates, levels, states, moves, n_moves, lights), n, cuda_stream,
+                       ticket_out);
 }
 
-// Host poses in, host frames out: the n frames `fr` in batches of max_batch.
-static int render_host(b2d_renderer *r, const b2d_pose *poses, const Frames &fr, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
+// b2d_render*: the null checks, then host poses in, host frames out: the n frames `c` describes, prepared, in batches of
+// max_batch.
+static int render_host(b2d_renderer *r, const b2d_pose *poses, CallFrames c, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
+    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (int rc = c.prepare(r, n)) return rc;
     if (n == 0) return B2D_OK;
     if (check_slots_free(r, batch_count(r, n)) != B2D_OK) return B2D_ERR_INVALID_ARG;
     CU(cudaSetDevice(r->device));
@@ -1348,7 +1282,7 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, const Frames &fr,
         std::memcpy(hp, poses + done, sizeof(Pose) * (size_t)cnt);
         cudaStream_t rs = hs.render_stream.get(), cs = hs.copy_stream[buf].get();
         CU(cudaMemcpyAsync(r->d_poses.get(), hp, sizeof(Pose) * (size_t)cnt, cudaMemcpyHostToDevice, rs));
-        int rc = enqueue_frames(r, r->d_poses.get(), fr.from(done), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs);
+        int rc = enqueue_frames(r, r->d_poses.get(), c.frames.from(done), cnt, hs.index[buf].get(), rgba_fb ? hs.rgba[buf].get() : nullptr, rs);
         if (rc != B2D_OK) return rc;
         CU(cudaEventRecord(hs.rendered[buf].get(), rs));
         CU(cudaStreamWaitEvent(cs, hs.rendered[buf].get(), 0));
@@ -1374,70 +1308,40 @@ static int render_host(b2d_renderer *r, const b2d_pose *poses, const Frames &fr,
 }
 
 int b2d_render(b2d_renderer *r, const b2d_pose *poses, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
-    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    return render_host(r, poses, Frames{}, n, index_fb, rgba_fb);
+    return render_host(r, poses, CallFrames(), n, index_fb, rgba_fb);
 }
 
 int b2d_render_timed(b2d_renderer *r, const b2d_pose *poses, const uint32_t *tics, size_t n, uint8_t *index_fb, uint32_t *rgba_fb) {
     if (!tics) return b2d_render(r, poses, n, index_fb, rgba_fb);
     if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (n == 0) return B2D_OK;
-    int rc = check_slots_free(r, batch_count(r, n));          // refused before the time changes as well
+    int rc = check_slots_free(r, batch_count(r, n));          // refused before the states are built and the time changes
     if (rc != B2D_OK) return rc;
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr;
-    rc = build_states(r, nullptr, tics, n, nullptr, 0, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    rc = render_host(r, poses, fr, n, index_fb, rgba_fb);
+    rc = render_host(r, poses, CallFrames(tics), n, index_fb, rgba_fb);
     const int trc = b2d_renderer_set_time(r, tics[n - 1]);                // the renderer is left at the last pose's time
     return rc != B2D_OK ? rc : trc;
 }
 
 int b2d_render_states(b2d_renderer *r, const b2d_pose *poses, const b2d_frame_state *states, size_t n,
                       const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
-    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr;
-    int rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    return render_host(r, poses, fr, n, index_fb, rgba_fb);
+    return render_host(r, poses, CallFrames(kFrameStates, nullptr, states, moves, n_moves), n, index_fb, rgba_fb);
 }
 
 int b2d_render_levels(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, size_t n, uint8_t *index_fb,
                       uint32_t *rgba_fb) {
-    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    int rc = check_levels(r, levels, n);
-    if (rc != B2D_OK) return rc;
-    return render_host(r, poses, Frames{levels}, n, index_fb, rgba_fb);
+    return render_host(r, poses, CallFrames(kFrameLevels, levels), n, index_fb, rgba_fb);
 }
 
 int b2d_render_levels_states(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels, const b2d_frame_state *states, size_t n,
                              const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
-    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr{levels};
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    return render_host(r, poses, fr, n, index_fb, rgba_fb);
+    return render_host(r, poses, CallFrames(kFrameLevels | kFrameStates, levels, states, moves, n_moves), n, index_fb, rgba_fb);
 }
 
 int b2d_render_levels_states_lights(b2d_renderer *r, const b2d_pose *poses, const uint32_t *levels,
                                     const b2d_frame_state *states, const b2d_frame_light *lights, size_t n,
                                     const b2d_sector_move *moves, size_t n_moves, uint8_t *index_fb, uint32_t *rgba_fb) {
-    if (!r || !poses || !index_fb) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames fr{levels};
-    int rc = check_levels(r, levels, n);
-    if (rc == B2D_OK) rc = check_lights(lights, n);
-    fr.lights = lights;
-    if (rc == B2D_OK) rc = build_states(r, states, nullptr, n, moves, n_moves, fs, starts, fr);
-    if (rc != B2D_OK) return rc;
-    return render_host(r, poses, fr, n, index_fb, rgba_fb);
+    return render_host(r, poses, CallFrames(kFrameLevels | kFrameStates, levels, states, moves, n_moves, lights), n, index_fb,
+                       rgba_fb);
 }
 
 // The colour-table indices of the n frames of a call (frame_table of its checked levels and palettes) staged in `s` on
@@ -1589,7 +1493,7 @@ int b2d_debug_state_slots(b2d_renderer *r, size_t n, uint32_t *slots_out) {
         return fail(B2D_ERR_INVALID_ARG, "the last walked batch has no per-frame states or fewer than n frames");
     CU(cudaSetDevice(r->device));
     CU(cudaDeviceSynchronize());
-    CU(cudaMemcpy(slots_out, s.tables.states.frame_slot, 4 * n, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(slots_out, s.tables.levels.frame_set, 4 * n, cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < n; i++)      // a frame on a level without a table set (TableSet index >= sets) has none
         if (slots_out[i] >= (uint32_t)s.sets) slots_out[i] = 0xFFFFFFFFu;
     return B2D_OK;
@@ -1603,7 +1507,7 @@ int b2d_debug_state_tables(b2d_renderer *r, size_t set, void *out, size_t capaci
     if (!per_frame && lv.h_blob.empty()) return fail(B2D_ERR_INVALID_ARG, "the scene has no time-dependent content or dynamic sectors");
     if (s.ticket < 0) return fail(B2D_ERR_INVALID_ARG, "no batch has been walked");
     if (set >= (per_frame ? (size_t)s.sets : 1)) return fail(B2D_ERR_INVALID_ARG, "table set out of range for the last walked batch");
-    const size_t need = level_table_bytes(lv);
+    const size_t need = SetLayout(lv.src).bytes;
     if (size_out) *size_out = need;
     if (!out) return B2D_OK;
     if (capacity < need) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the tables");

@@ -15,11 +15,11 @@
 namespace b2d {
 int fail(int code, const std::string &msg);            // sets the thread-local message, returns code
 int cuda_fail(cudaError_t e, const char *what);
-// The frames of a call, or of one batch of it (HOST arrays).  `levels`: the level of each frame, checked by check_levels
-// (nullptr: every frame on level 0).  `starts`: with per-frame states, frame i's compact state is fs[starts[i] ..] (its
-// level's layout.words words; none on a level without time-dependent content or dynamic sectors); nullptr: every level at
-// the renderer's own state, a plain batch.  `lights`: with per-frame levels and states, each frame's fixed colormap and
-// extra light, checked by check_lights (nullptr: none, as when every frame is {-1, 0}).
+// The frames of a call, or of one batch of it (HOST arrays, checked by CallFrames::prepare).  `levels`: the level of each
+// frame (nullptr: every frame on level 0).  `starts`: with per-frame states, frame i's compact state is fs[starts[i] ..]
+// (its level's layout.words words; none on a level without time-dependent content or dynamic sectors); nullptr: every
+// level at the renderer's own state, a plain batch.  `lights`: with per-frame levels and states, each frame's fixed
+// colormap and extra light (nullptr: none, as when every frame is {-1, 0}).
 struct Frames {
     const uint32_t *levels = nullptr;
     const uint32_t *fs = nullptr;
@@ -29,22 +29,40 @@ struct Frames {
         return {levels ? levels + first : nullptr, fs, starts ? starts + first : nullptr, lights ? lights + first : nullptr};
     }
 };
-// The n per-frame states of a call on the frames of `out` (out.levels set by the caller), checked, and out.fs / out.starts
-// pointing into `fs` / `starts`: with `tics`, frame i at tics[i] with its level's current sector moves; else at
-// states[i] (its time and its range of `moves`), with out.lights[i]'s extra light if out.lights is set.  With every frame on level 0 and a level 0 without time-dependent content
-// or dynamic sectors, the call is a plain one (out.starts stays nullptr).  Nothing is enqueued.
-int build_states(const b2d_renderer *r, const b2d_frame_state *states, const uint32_t *tics, size_t n, const b2d_sector_move *moves,
-                 size_t n_moves, std::vector<uint32_t> &fs, std::vector<size_t> &starts, Frames &out);
-// Per-frame levels: n HOST levels, each below the renderer's number of levels, and a renderer whose levels fit the
-// per-frame-level walk (a b2d_renderer_create renderer may not); B2D_ERR_INVALID_ARG otherwise.
-int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n);
-// Per-frame light effects (HOST, nullable): fixed_colormap in -1..32 and extralight in 0..2; B2D_ERR_INVALID_ARG otherwise.
-// `lights` is set to nullptr when every frame is {-1, 0}, so that such a call is the call without lights.
-int check_lights(const b2d_frame_light *&lights, size_t n);
-// Per-frame palettes (HOST, nullable = palette 0): frame i's palette below the palette count of its level (levels[i],
-// nullable = level 0), the levels already checked; B2D_ERR_INVALID_ARG otherwise.
-int check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n);
-// The colour-table index of frame i, pal_base[levels[i]] + palettes[i] (either array nullable: 0), after the checks above.
+// What a render, walk or sharded call says about its n frames (HOST arrays), and, once prepare() has checked it, its
+// `frames`, whose compact states live in `fs` / `starts`.  kFrameLevels: the call takes `levels`, a level each (refused if
+// null).  kFrameStates: the call takes `states`, a time and a range of `moves` each (refused if null); or `tics` (timed
+// calls), a time each with its level's current sector moves.  `palettes` and `lights` (nullable): a palette each, and a
+// fixed colormap and extra light each.
+constexpr unsigned kFrameLevels = 1, kFrameStates = 2;
+struct CallFrames {
+    CallFrames() = default;                  // no per-frame inputs: a plain call
+    CallFrames(unsigned takes, const uint32_t *levels, const b2d_frame_state *states = nullptr, const b2d_sector_move *moves = nullptr,
+               size_t n_moves = 0, const b2d_frame_light *lights = nullptr, const uint32_t *palettes = nullptr)
+        : takes(takes), levels(levels), states(states), moves(moves), n_moves(n_moves), lights(lights), palettes(palettes) {}
+    explicit CallFrames(const uint32_t *tics) : tics(tics) {}
+    // The checks, in this order, each B2D_ERR_INVALID_ARG with its message: the levels (each below the renderer's number
+    // of levels, on a renderer whose levels fit the per-frame-level walk -- a b2d_renderer_create renderer may not), the
+    // palettes (each below the palette count of its frame's level), the lights (fixed_colormap in -1..32, extralight in
+    // 0..2; lights of every frame {-1, 0} are dropped, so that such a call is the call without lights), the states (move
+    // ranges inside `moves`, moves of dynamic sectors).  Then the compact states: frame i's at fs[starts[i] ..] (none on a
+    // level without time-dependent content or dynamic sectors).  With every frame on level 0 and a level 0 without either,
+    // the call is a plain one (frames.starts stays nullptr).  Nothing is enqueued.
+    int prepare(const b2d_renderer *r, size_t n);
+
+    unsigned takes = 0;
+    const uint32_t *levels = nullptr;
+    const b2d_frame_state *states = nullptr;
+    const b2d_sector_move *moves = nullptr;
+    size_t n_moves = 0;
+    const b2d_frame_light *lights = nullptr;
+    const uint32_t *palettes = nullptr;
+    const uint32_t *tics = nullptr;
+    std::vector<uint32_t> fs;
+    std::vector<size_t> starts;
+    Frames frames;
+};
+// The colour-table index of frame i, pal_base[levels[i]] + palettes[i] (either array nullable: 0), the levels and palettes checked.
 inline uint32_t frame_table(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t i);
 // A one-call render of `batches` batches walks the first into the next worklist slot and alternates slots from there: it
 // is refused (B2D_ERR_INVALID_ARG) before anything is enqueued while a slot it would use holds a walked, unrastered batch.
@@ -122,7 +140,7 @@ struct WorkSlot {
     bool rastered = true;
     BatchTables tables{};                                 // what the batch's walk read and its raster reads
     // Per-frame states (b2d_render_states & co.): an arena of up to max_batch expanded table sets, allocated by the first
-    // such call; the batch's sets are packed into it, each at its level's slot_bytes
+    // such call; the batch's sets are packed into it
     DeviceBuf<uint8_t> arena;
     int sets = 0;                                         // table sets of the batch in the arena (distinct states)
     std::vector<uint32_t> set_level;                      // level of each table set
@@ -170,7 +188,6 @@ struct LevelRes {
     std::vector<uint32_t> state;                          // the level's own compact state (set_time, set_*sector_moves)
     DeviceBuf<uint32_t> d_slot_maps;                      // StateLayout::sector_slots, ::mid_seg, then the light side tables
     StateSrc src{};                                       // device pointers into d_blob and d_slot_maps
-    StateTables state_tables{};                           // slot size and section offsets (base / frame_slot per slot)
     // Scenes with time-dependent content or dynamic sectors (DESIGN.md §3 "State arena"); the rest stays empty.  The
     // device blob is never written after creation: the state rule reads its rest-state sections, and every batch reads
     // its five state-dependent tables from a table set expanded on the device from a compact state.

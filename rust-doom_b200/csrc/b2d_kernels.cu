@@ -120,23 +120,10 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity) {     
 // ------------------------------------------------------------------------------------------------
 // Kernel 1: BSP walk -> worklist
 // ------------------------------------------------------------------------------------------------
-// Per-frame states: the frame's table of kind T in its arena slot (tb = slot base), else the scene's one table.
-template <bool kStates, typename T>
-__device__ __forceinline__ const T *state_table(const T *plain, const uint8_t *tb, uint32_t off) {
-    return kStates ? reinterpret_cast<const T *>(tb + off) : plain;
-}
-// ... and with per-frame levels as well, the table of the frame's TableSet (`set`)
-template <bool kStates, bool kLevels, typename T>
-__device__ __forceinline__ const T *frame_table(const T *plain, const uint8_t *tb, uint32_t off, const T *set) {
-    if constexpr (kStates && kLevels) return set;
-    else return state_table<kStates>(plain, tb, off);
-}
-
 template <bool kStates, bool kLevels>
 __global__ void __launch_bounds__(128, 7)     // 7 CTAs/SM (72 registers): 924 frames resident on an H100's 132 SMs
 b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant__ View vw, const Pose *__restrict__ poses, int n,
-                FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride, const __grid_constant__ StateTables st,
-                const __grid_constant__ LevelTables lt) {
+                FrameConst *__restrict__ frames, SegFrame *__restrict__ work, int stride, const __grid_constant__ LevelTables lt) {
     // One CTA per frame.  The per-frame setup (steps 1-3) and the worklist records (step 5) are data-parallel and
     // use all 128 threads; the traversal itself (step 4) is sequential and runs in warp 0 with the lanes working
     // on the segs of a subsector / the words of the column mask.  The kernel is latency-bound (one frame = one
@@ -221,13 +208,11 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
     }
     FrameConst fc;
     frame_setup(poses[frame], fc);
-    uint32_t slot = 0;                  // per-frame states: this frame's slot of the arena
-    const uint8_t *tb = nullptr;
-    TableSet fs{};                      // ... and levels: this frame's tables (slot = its TableSet)
+    uint32_t set = 0;                   // per-frame states: this frame's table set, and its tables
+    TableSet fs{};
     if (kStates) {
-        slot = st.frame_slot[frame];
-        if constexpr (kLevels) fs = lt.sets[slot];
-        else tb = st.base + (size_t)slot * st.slot_bytes;
+        set = lt.frame_set[frame];
+        fs = lt.sets[set];
     }
 
     // 1. all vertices into view space (lane-parallel)
@@ -241,7 +226,7 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
 
     // 2. per-seg exact column interval + static/solid flags (lane-parallel, 64-bit setup)
     for (int i = tid; i < sc.nsegs; i += nthr) {
-        const SegRec &S = frame_table<kStates, kLevels>(sc.segs, tb, st.off_segs, fs.segs)[i];
+        const SegRec &S = (kStates ? fs.segs : sc.segs)[i];
         uint32_t packed = 0;
         int32_t flags = S.flags;
         if (!(flags & kSegInvalid)) {
@@ -266,11 +251,11 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
         if (kLevels) parity ^= 1u;
     }
     for (int i = tid; i < sc.nsprites; i += nthr) {          // decoration sprites: exact column interval
-        const SpriteRec &P = frame_table<kStates, kLevels>(sc.sprites, tb, st.off_sprites, fs.sprites)[i];
+        const SpriteRec &P = (kStates ? fs.sprites : sc.sprites)[i];
         SpriteFrame sp;
         uint32_t packed = 0;
         sp.cz = 0;
-        if (P.tex >= 0 && P.tex < sc.ntex && sprite_setup(fc, vw, P.x, P.y, (int32_t)frame_table<kStates, kLevels>(sc.tex, tb, 0u, fs.tex)[P.tex].w, sp))
+        if (P.tex >= 0 && P.tex < sc.ntex && sprite_setup(fc, vw, P.x, P.y, (int32_t)(kStates ? fs.tex : sc.tex)[P.tex].w, sp))
             packed = pack_range(sp.lo, sp.hi, kVisBit);
         sprr[i] = packed;
         sprz[i] = (int32_t)sp.cz;
@@ -383,14 +368,14 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
         SegFrame sf;
         if (si >= sc.nsegs) {
             const int pi = si - sc.nsegs;
-            const SpriteRec &P = frame_table<kStates, kLevels>(sc.sprites, tb, st.off_sprites, fs.sprites)[pi];
+            const SpriteRec &P = (kStates ? fs.sprites : sc.sprites)[pi];
             SpriteFrame sp;
-            sprite_setup(fc, vw, P.x, P.y, (int32_t)frame_table<kStates, kLevels>(sc.tex, tb, 0u, fs.tex)[P.tex].w, sp);
+            sprite_setup(fc, vw, P.x, P.y, (int32_t)(kStates ? fs.tex : sc.tex)[P.tex].w, sp);
             sprite_entry(pi, sp, sf);
             work[(size_t)frame * stride + k] = sf;
             continue;
         }
-        const SegRec &S = frame_table<kStates, kLevels>(sc.segs, tb, st.off_segs, fs.segs)[si];
+        const SegRec &S = (kStates ? fs.segs : sc.segs)[si];
         seg_frame_setup(vw, tx[S.v1], tz[S.v1], tx[S.v2], tz[S.v2], sf, false);
         sf.seg = si;
         work[(size_t)frame * stride + k] = sf;
@@ -400,9 +385,9 @@ b2d_walk_kernel(const __grid_constant__ DeviceScene scene, const __grid_constant
         fc.count = count;
         fc.status = status;
 #pragma unroll
-        for (int i = 0; i < 6; i++) fc.pad[i] = 0;
-        if (kStates) fc.pad[0] = (int32_t)slot;      // the raster reads the frame's tables from the same slot
-        if (kLevels) fc.pad[1] = (int32_t)resident;  // ... and the frame's scene from its level
+        for (int i = 0; i < 4; i++) fc.pad[i] = 0;
+        fc.set = kStates ? (int32_t)set : 0;           // the raster reads the frame's tables from the same set
+        fc.level = kLevels ? (int32_t)resident : 0;    // ... and the frame's scene from its level
         frames[frame] = fc;
     }
     __syncthreads();                              // the next frame of this CTA reuses the shared-memory tables
@@ -930,8 +915,8 @@ template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels, typename
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
-                  uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ StateTables st,
-                  const __grid_constant__ LevelTables lt, const Fixed... fx) {
+                  uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ LevelTables lt,
+                  const Fixed... fx) {
     constexpr bool kFixed = sizeof...(Fixed) != 0;
     static_assert(!kFixed || (kStates && kLevels && sizeof...(Fixed) == 1), "fixed colormaps come with per-frame levels and states");
     // per-frame levels: a palette per warp (the warps of a CTA may draw frames of levels from different WADs)
@@ -971,45 +956,25 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     FrameConst fc{};
     if (has_strip) fc = frames[frame];
     const DeviceScene *scp = &sc;
-    if constexpr (kStates && !kLevels) {
-        // per-frame states: this warp's copy of the scene description, its five state-dependent tables pointed into the
-        // frame's arena slot (the walk passed the slot on in FrameConst::pad[0]); every table read below goes through it
+    if constexpr (kStates || kLevels) {
+        // per-frame states or levels: this warp's copy of the scene description of its frame -- with per-frame levels, of
+        // the frame's level (the walk passed the level on in FrameConst::level), with that level's palette; with per-frame
+        // states, its five state-dependent tables pointed at the frame's TableSet (FrameConst::set).  Every table read
+        // below goes through it.
         DeviceScene *d = &s_scn[warp];
         if (has_strip) {
-            const uint32_t *src = reinterpret_cast<const uint32_t *>(&sc);
-            uint32_t *dst = reinterpret_cast<uint32_t *>(d);
-            for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
-            __syncwarp();
-            if (lane == 0) {
-                const uint8_t *tb = st.base + (size_t)(uint32_t)fc.pad[0] * st.slot_bytes;
-                d->tex = reinterpret_cast<const TexRec *>(tb);
-                d->sectors = reinterpret_cast<const SectorRec *>(tb + st.off_sectors);
-                d->segs = reinterpret_cast<const SegRec *>(tb + st.off_segs);
-                d->sprites = reinterpret_cast<const SpriteRec *>(tb + st.off_sprites);
-                d->mids = reinterpret_cast<const MidRec *>(tb + st.off_mids);
-            }
-            __syncwarp();
-        }
-        scp = d;
-    }
-    if constexpr (kLevels) {
-        // per-frame levels: this warp's copy of the scene of the frame's level (the walk passed the level on in
-        // FrameConst::pad[1]), and that level's palette
-        DeviceScene *d = &s_scn[warp];
-        if (has_strip) {
-            const DeviceScene *lsrc = lt.scenes + (uint32_t)fc.pad[1];
+            const DeviceScene *lsrc = kLevels ? lt.scenes + (uint32_t)fc.level : &sc;
             const uint32_t *src = reinterpret_cast<const uint32_t *>(lsrc);
             uint32_t *dst = reinterpret_cast<uint32_t *>(d);
             for (int i = lane; i < (int)(sizeof(DeviceScene) / 4); i += 32) dst[i] = src[i];
-            if (kRgba) {
+            if (kLevels && kRgba) {
                 const uint32_t *pal = lsrc->palette;
                 for (int i = lane; i < 256; i += 32) s_pal[256 * warp + i] = pal[i];
             }
             __syncwarp();
             if constexpr (kStates) {
-                // ... with per-frame states: its five state-dependent tables pointed at the frame's TableSet (FrameConst::pad[0])
                 if (lane == 0) {
-                    const TableSet t = lt.sets[(uint32_t)fc.pad[0]];
+                    const TableSet t = lt.sets[(uint32_t)fc.set];
                     d->tex = t.tex; d->sectors = t.sectors; d->segs = t.segs; d->sprites = t.sprites; d->mids = t.mids;
                 }
                 __syncwarp();
@@ -1020,7 +985,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     if constexpr (kFixed) {
         if (has_strip && lane == 0) {
             const FixedTables &t = (fx, ...);       // the one element of the pack
-            const FixedPlanes p = t.planes[(uint32_t)fc.pad[1]];
+            const FixedPlanes p = t.planes[(uint32_t)fc.level];
             s_fix[warp] = FixedWarp{p.texels, p.flats, t.frame_fixed[frame]};
         }
         __syncwarp();
@@ -1493,7 +1458,7 @@ static cudaError_t walk_go(const BatchTables &t, size_t smem, const View &vw, co
     const int sms = device_sms();
     const int blocks = (background && n > sms) ? sms : n, warps = 4;
     b2d_walk_kernel<kStates, kLevels><<<blocks, warps * 32, smem, stream>>>(t.scene, vw, d_poses, n, d_frames, d_work, stride,
-                                                                            t.states, t.levels);
+                                                                            t.levels);
     return cudaGetLastError();
 }
 
@@ -1537,11 +1502,11 @@ static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, 
     const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
 #define B2D_RASTER_GO(RGBA, KW) do { \
     if constexpr (kFixed) { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels, t.fixed); \
-    else b2d_raster_kernel<RGBA, KW, false, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels, t.fixed); \
+    if (masked) b2d_raster_kernel<RGBA, KW, true, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels, t.fixed); \
+    else b2d_raster_kernel<RGBA, KW, false, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels, t.fixed); \
     } else { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels); \
-    else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.states, t.levels); \
+    if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels); \
+    else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels); \
     } \
     } while (0)
     if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }

@@ -45,18 +45,9 @@ struct DeviceScene {
 
 constexpr int kMaskedChunk = 4;      // entries per arena chunk (528 bytes)
 
-// Per-frame states (b2d_render_states): the walk and raster variants that take it read the five state-dependent tables of
-// each frame from its slot of a state arena instead of DeviceScene::{tex, sectors, segs, sprites, mids}.  Slot s holds
-// [tex | sectors | segs | sprites | mids] at base + s * slot_bytes (the layout of b2d_scene_tables_at).
-struct StateTables {
-    const uint8_t *base;
-    const uint32_t *frame_slot;      // slot of each frame of the batch: read by the walk, passed on in FrameConst::pad[0]
-    uint32_t slot_bytes, off_sectors, off_segs, off_sprites, off_mids, pad;
-};
-
 // The five state-dependent tables of one level at one state: an expanded table set (in a state arena, or a level's own set of
 // a worklist slot), or, on a level without time-dependent content or dynamic sectors, its blob tables.  What a frame of a
-// batch with per-frame states and levels reads, and where launch_state_sets writes.
+// batch with per-frame states reads, and where launch_state_sets writes.
 struct TableSet {
     const TexRec *tex;
     const SectorRec *sectors;
@@ -67,13 +58,14 @@ struct TableSet {
 
 // Per-frame levels (b2d_render_levels): frame i of a batch is rendered from scenes[frame_level[i]], each the DeviceScene of
 // one level of the renderer as the batch's worklist slot reads it.  The walk copies the frame's scene into shared memory
-// and passes its level on in FrameConst::pad[1]; the raster reads the scene of that level.
-// With per-frame states as well (b2d_render_levels_states), frame i reads its five tables from sets[StateTables::frame_slot[i]]
-// (passed on in FrameConst::pad[0]) instead of its scene's; the other fields of StateTables are not read.
+// and passes its level on in FrameConst::level; the raster reads the scene of that level.
+// Per-frame states (b2d_render_states, b2d_render_levels_states), with or without per-frame levels: frame i reads its five
+// state-dependent tables from sets[frame_set[i]] (passed on in FrameConst::set) instead of its scene's.
 struct LevelTables {
     const DeviceScene *scenes;
     const uint32_t *frame_level;
     const TableSet *sets;
+    const uint32_t *frame_set;
 };
 
 // One table set to expand (launch_state_sets): level `level`'s rule at the compact state at word `state` of the launch's
@@ -104,13 +96,11 @@ constexpr size_t kWalkSmemMax = 227 * 1024;      // the largest shared-memory op
 
 // The tables a batch's walk and raster read, and which of their <kStates, kLevels> variants runs.  Without per-frame levels
 // every frame reads `scene` (level 0 as the batch's worklist slot reads it); with them, the scenes of `levels` (and `scene`
-// is not read).  With per-frame states the five state-dependent tables come from `states` (level 0's slot layout; with
-// per-frame levels, only its frame_slot is read, into `levels.sets`).
+// is not read).  With per-frame states the five state-dependent tables come from the table sets of `levels`.
 // With fixed colormaps (`fixed_rows`: some frame of the batch has one), the raster reads `fixed` (per-frame levels and
 // states only).
 struct BatchTables {
     DeviceScene scene;
-    StateTables states;
     LevelTables levels;
     FixedTables fixed;
     bool per_frame, per_level, fixed_rows;

@@ -33,7 +33,9 @@ struct FrameConst {
     int32_t px8, py8;          // camera position, Q8
     int32_t count;             // worklist length
     int32_t status;            // 0 ok, else kStatus* bits
-    int32_t pad[6];
+    int32_t set;               // per-frame states: the frame's TableSet (LevelTables::sets), else 0
+    int32_t level;             // per-frame levels: the frame's level (LevelTables::scenes), else 0
+    int32_t pad[4];
 };
 static_assert(sizeof(FrameConst) == 64, "FrameConst");
 

@@ -572,15 +572,11 @@ int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *p
     if (rc != B2D_OK) return rc;
     // the whole list, identical on every rank, is checked and its compact states built before anything else: every rank
     // then refuses the same input, before any collective
-    std::vector<uint32_t> fs;
-    std::vector<size_t> starts;
-    Frames all{levels};
-    rc = b2d::check_levels(r, levels, n_total);
-    if (rc == B2D_OK) rc = b2d::check_palettes(r, levels, palettes, n_total);
-    if (rc == B2D_OK) rc = b2d::build_states(r, states, nullptr, n_total, moves, n_moves, fs, starts, all);
+    CallFrames all(kFrameLevels | kFrameStates, levels, states, moves, n_moves, nullptr, palettes);
+    rc = all.prepare(r, n_total);
     if (rc != B2D_OK || n_total == 0) return rc;
     // this rank's block, padded like its poses by repeating the last entry (level, palette and state with it); its
-    // states stay where build_states put them
+    // states stay where prepare put them
     const size_t world = (size_t)c->world, rank = (size_t)c->rank, per = (n_total + world - 1) / world;
     std::vector<uint32_t> block_levels(per), block_tables(per);
     std::vector<size_t> block_starts(per);
@@ -588,11 +584,11 @@ int render_sharded_levels_states(b2d_renderer *r, b2d_comm *c, const b2d_pose *p
         const size_t g = std::min(rank * per + i, n_total - 1);
         block_levels[i] = levels[g];
         block_tables[i] = b2d::frame_table(r, levels, palettes, g);
-        block_starts[i] = starts[g];
+        block_starts[i] = all.starts[g];
     }
     if (res) res->block_tables = block_tables.data();
     return sharded_loop(r, c, poses, n_total, chunk_frames, mode, fn, user, stats_out,
-                        Frames{block_levels.data(), fs.data(), block_starts.data()}, res);
+                        Frames{block_levels.data(), all.fs.data(), block_starts.data()}, res);
 }
 
 }  // namespace

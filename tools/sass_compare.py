@@ -4,10 +4,12 @@
 
 Runs on a machine without a GPU (cuobjdump + c++filt).  Names are normalised so that a kernel that gained the per-frame
 state flag (`kStates`, DESIGN.md §5) is compared, in its `kStates = false` instantiation, with the kernel of the same name
-in the old build: the trailing `false` template argument and the appended `StateTables` parameter are dropped, and the
-hash of each anonymous namespace is ignored.  The per-frame level flag (`kLevels`) that follows it is dropped the same way
-in its `false` instantiations, with its appended `LevelTables` parameter.  Addresses and instruction encodings are
-dropped; the opcodes and operands are compared.  Exits 1 if any function of OLD is missing from NEW or differs.
+in the old build: the trailing `false` template argument is dropped, and the hash of each anonymous namespace is ignored.
+The per-frame level flag (`kLevels`) that follows it is dropped the same way in its `false` instantiations, with the
+appended `LevelTables` parameter.  Builds before per-frame states moved into `LevelTables` also took a `StateTables`
+parameter ahead of it; that is dropped wherever it stands, so their kernels pair with the later instantiations.
+Addresses are dropped; the opcodes and operands are compared.  Exits 1 if any function of OLD is missing from NEW or
+differs.
 """
 import re
 import subprocess
@@ -29,7 +31,7 @@ def functions(path):
     txt = re.sub(r"void (b2d::ANON::b2d_walk_kernel)<false>", r"\1", txt)
     txt = re.sub(r"(b2d_raster_kernel<[a-z]+, \d+, [a-z]+), false>", r"\1>", txt)
     txt = re.sub(r"(masked_pass<[a-z]+, \d+), false>", r"\1>", txt)
-    txt = re.sub(r", b2d::StateTables\)", ")", txt)
+    txt = re.sub(r", b2d::StateTables(?=[,)])", "", txt)
     out, cur = {}, None
     for line in txt.splitlines():
         m = re.match(r"\s*Function : (.*)", line)
