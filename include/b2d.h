@@ -174,6 +174,20 @@ int b2d_scene_info_get(const b2d_scene *s, b2d_scene_info *out);
  * call changes no existing renderer. */
 int b2d_scene_num_palettes(const b2d_scene *s);
 int b2d_scene_set_palettes(b2d_scene *s, const uint8_t *playpal, size_t n_palettes);
+/* The scene's automap table (DESIGN.md C19), built when the scene is created from its own LINEDEFS, SIDEDEFS, VERTEXES and
+ * SECTORS: one record per linedef whose two vertices exist, in LINEDEFS order, with Doom's AM_drawWalls colour at the
+ * level's rest heights, every line counted as mapped.  A line without a valid sidedef and sector on both sides is a wall
+ * (176); otherwise special 39 is 184, ML_SECRET 176, differing floors 64, differing ceilings 231, anything else 96 and
+ * drawn only under B2D_AUTOMAP_ALL_LINES; ML_DONTDRAW lines are drawn only under B2D_AUTOMAP_ALL_LINES.
+ * out = NULL: only *n_out is set; otherwise out must hold the *n_out records (B2D_ERR_INVALID_ARG if capacity is smaller). */
+typedef struct b2d_automap_line {
+    int32_t x0, y0, x1, y1;     /* vertex v1 and vertex v2, map units */
+    uint8_t colour;             /* palette index drawn normally, 0 = not drawn */
+    uint8_t colour_all;         /* palette index drawn under B2D_AUTOMAP_ALL_LINES */
+    uint16_t pad;
+    int32_t linedef;            /* index in LINEDEFS */
+} b2d_automap_line;
+int b2d_scene_automap_lines(const b2d_scene *s, b2d_automap_line *out, size_t capacity, size_t *n_out);
 /* Read-only access to the compiled "B2DS" blob (layout in DESIGN.md); valid until destroy. */
 const void *b2d_scene_blob(const b2d_scene *s, size_t *size_out);
 /* LevelWalker::sector_at (visitor.rs:1028-1060): sector id at a map position, -1 if outside. */
@@ -435,6 +449,25 @@ int b2d_resolve_frame_bytes(const b2d_renderer *r, int factor, int format, size_
  * every refusal of b2d_resolve_device, are B2D_ERR_INVALID_ARG, detected before anything is enqueued. */
 int b2d_resolve_palettes_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, const uint32_t *palettes,
                                 size_t n_frames, int factor, int format, void *d_out, void *cuda_stream);
+
+/* Kernel 5, Doom's automap (AM_Drawer; DESIGN.md C19): frame f of the n_frames contiguous W x H palette-index frames at
+ * d_out (W x H: the renderer's view) is the top-down line map of level levels[f] centred on d_poses[f] (device poses),
+ * at scale_q16 pixels per map unit in 16.16 (Doom's default 0.2 is 13107; 256 .. 64 << 16 accepted): the level's linedefs
+ * in the colours of b2d_scene_automap_lines, then the player arrow (209), then with B2D_AUTOMAP_THINGS its decoration
+ * things (112), later items over earlier ones, background 0.  B2D_AUTOMAP_ROTATE turns the map so the view direction
+ * points up; B2D_AUTOMAP_ALL_LINES draws every line (Doom's IDDT).  The frames are ordinary index frames:
+ * b2d_palette_lut_levels_device, b2d_resolve_device and b2d_resolve_palettes_device colour them.  `levels` is a HOST
+ * array, or NULL for level 0 on every frame (nothing is staged then), staged through pinned memory of this call's own with
+ * the waits of b2d_resolve_device.  The first call uploads every level's automap table on its stream; every later call,
+ * on any stream, waits on the device for that upload.  The call uses no worklist slot and no table set, is enqueued on
+ * `cuda_stream` and does not synchronise the device.  A NULL r, d_poses or d_out, unknown flag bits, a scale out of range,
+ * a level >= n_levels and more frames than one grid holds (n_frames * ceil(W/128) * ceil(H/32) > 2^31 - 1) are
+ * B2D_ERR_INVALID_ARG, detected before anything is enqueued; n_frames = 0 enqueues nothing. */
+#define B2D_AUTOMAP_ROTATE 1
+#define B2D_AUTOMAP_ALL_LINES 2
+#define B2D_AUTOMAP_THINGS 4
+int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n_frames, int32_t scale_q16,
+                       int flags, uint8_t *d_out, void *cuda_stream);
 
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the

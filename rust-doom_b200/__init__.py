@@ -232,6 +232,16 @@ class Scene:
         _check(_lib.load().b2d_scene_tables_at(self._h, tics, arr, n, buf, size.value, ctypes.byref(size)))
         return buf.raw[:size.value]
 
+    def automap_lines(self) -> np.ndarray:
+        """b2d_scene_automap_lines: the level's automap table (DESIGN.md C19) as a structured array with fields x0, y0, x1,
+        y1 (map units), colour, colour_all (palette indices, 0 = not drawn) and linedef, one record per linedef whose
+        vertices exist, in LINEDEFS order."""
+        n = ctypes.c_size_t()
+        _check(_lib.load().b2d_scene_automap_lines(self._h, None, 0, ctypes.byref(n)))
+        buf = (_lib.AutomapLine * max(n.value, 1))()
+        _check(_lib.load().b2d_scene_automap_lines(self._h, buf, n.value, ctypes.byref(n)))
+        return np.ctypeslib.as_array(buf)[:n.value].copy()
+
     @property
     def blob(self) -> bytes:
         n = ctypes.c_size_t()
@@ -331,6 +341,25 @@ MAX_LEVELS = 64                 # B2D_MAX_LEVELS
 RESOLVE_RGBA8, RESOLVE_RGB8, RESOLVE_RGB8_PLANAR, RESOLVE_GRAY8 = (_lib.RESOLVE_RGBA8, _lib.RESOLVE_RGB8, _lib.RESOLVE_RGB8_PLANAR,
                                                                    _lib.RESOLVE_GRAY8)
 RESOLVE_FORMATS = {"rgba": RESOLVE_RGBA8, "rgb": RESOLVE_RGB8, "rgb_planar": RESOLVE_RGB8_PLANAR, "gray": RESOLVE_GRAY8}
+
+
+AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS = _lib.AUTOMAP_ROTATE, _lib.AUTOMAP_ALL_LINES, _lib.AUTOMAP_THINGS
+AUTOMAP_FLAGS = {"rotate": AUTOMAP_ROTATE, "all": AUTOMAP_ALL_LINES, "things": AUTOMAP_THINGS}
+AUTOMAP_DEFAULT_SCALE_Q16 = 13107       # Doom's default automap scale, 0.2 pixels per map unit
+
+
+def automap_flags(flags) -> int:
+    """B2D_AUTOMAP_* bits from an int, or from names ("rotate", "all", "things") as a list or a comma-separated string"""
+    if isinstance(flags, int):
+        return flags
+    names = flags.split(",") if isinstance(flags, str) else list(flags)
+    out = 0
+    for name in (x.strip() for x in names):
+        if name:
+            if name not in AUTOMAP_FLAGS:
+                raise ValueError("unknown automap flag %r (rotate, all, things)" % name)
+            out |= AUTOMAP_FLAGS[name]
+    return out
 
 
 def _levels_array(levels, n: int) -> np.ndarray:
@@ -614,6 +643,34 @@ class Renderer:
         with torch.cuda.device(index.device):
             stream = torch.cuda.current_stream().cuda_stream
         self.resolve_device(index.data_ptr(), n, k, code, out.data_ptr(), levels, stream, palettes)
+        return out
+
+    def automap_device(self, poses_ptr: int, n: int, out_ptr: int, scale_q16: int = AUTOMAP_DEFAULT_SCALE_Q16,
+                       flags: int = 0, levels=None, stream: int = 0):
+        """b2d_automap_device: the automap (DESIGN.md C19) of the n device poses at poses_ptr into n contiguous W x H
+        palette-index frames at out_ptr, frame f of level levels[f] (host list; None = level 0), at scale_q16 pixels per map
+        unit in 16.16 (256 .. 64 << 16), flags an OR of AUTOMAP_ROTATE, AUTOMAP_ALL_LINES and AUTOMAP_THINGS."""
+        lv = None if levels is None else _levels_array(levels, n)
+        _check(_lib.load().b2d_automap_device(self._h, poses_ptr, None if lv is None else lv.ctypes.data, n, int(scale_q16),
+                                              int(flags), out_ptr, stream or None))
+
+    def automap(self, poses, levels=None, scale: float = 0.2, flags=0):
+        """The automaps of host or CUDA poses as a CUDA uint8 tensor [n, H, W] of palette indices, on the current torch
+        stream: `scale` in pixels per map unit (Doom's default 0.2), `flags` an int or names from "rotate", "all", "things".
+        Colour them with resolve() or palette_lut_levels_device like rendered frames."""
+        import torch
+        flags = automap_flags(flags)
+        dev = torch.device("cuda", self.device)
+        if isinstance(poses, torch.Tensor):
+            p = poses.to(dev).contiguous()
+        else:
+            arr = np.ascontiguousarray(poses)
+            p = torch.from_numpy(arr.view(np.uint8).reshape(-1)).to(dev)
+        n = p.numel() * p.element_size() // ctypes.sizeof(_lib.Pose)
+        out = torch.empty((n, self.height, self.width), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+        self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream)
         return out
 
     def worklist(self, n: int):

@@ -65,11 +65,19 @@ EXPORTS = [
     "b2d_scene_num_palettes", "b2d_scene_set_palettes", "b2d_resolve_palettes_device",
     "b2d_render_sharded_levels_states_resolved_palettes",
     "b2d_render_levels_states_lights", "b2d_render_device_levels_states_lights", "b2d_walk_device_levels_states_lights",
+    "b2d_scene_automap_lines", "b2d_automap_device",
 ]
 
 COMM_ID_BYTES = 128
 RESOLVE_RGBA8, RESOLVE_RGB8, RESOLVE_RGB8_PLANAR, RESOLVE_GRAY8 = 0, 1, 2, 3      # B2D_RESOLVE_*
 SHARD_RENDER_ONLY, SHARD_RENDER_GATHER, SHARD_GATHER_ONLY = 0, 1, 2
+AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS = 1, 2, 4      # B2D_AUTOMAP_*
+
+
+class AutomapLine(ctypes.Structure):
+    """b2d_automap_line: a linedef's endpoints (map units), colour drawn normally and under AUTOMAP_ALL_LINES, index"""
+    _fields_ = [("x0", ctypes.c_int32), ("y0", ctypes.c_int32), ("x1", ctypes.c_int32), ("y1", ctypes.c_int32),
+                ("colour", ctypes.c_uint8), ("colour_all", ctypes.c_uint8), ("pad", ctypes.c_uint16), ("linedef", ctypes.c_int32)]
 
 
 class ShardedStats(ctypes.Structure):
@@ -212,6 +220,8 @@ def load() -> ctypes.CDLL:
     L.b2d_scene_num_palettes.argtypes = [vp]
     L.b2d_scene_set_palettes.argtypes = [vp, vp, cs]
     L.b2d_resolve_palettes_device.argtypes = [vp, vp, vp, vp, cs, ci, ci, vp, vp]
+    L.b2d_scene_automap_lines.argtypes = [vp, ctypes.POINTER(AutomapLine), cs, ctypes.POINTER(cs)]
+    L.b2d_automap_device.argtypes = [vp, vp, vp, cs, ctypes.c_int32, ci, vp, vp]
     L.b2d_render_sharded_levels_states_resolved_palettes.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(FrameState), cs,
                                                                      ctypes.POINTER(SectorMove), cs, cs, ci, ci, ci, CHUNK_FN, vp,
                                                                      ctypes.POINTER(ShardedStats)]

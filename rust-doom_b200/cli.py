@@ -23,6 +23,11 @@ block to one pixel of the --resolution frame on the device (b2d_resolve_device, 
 block's palette colours, each frame through its own level's palette): an anti-aliased --dump and --stream.  Not with
 --world.
 
+--automap SCALE with --dump NAME.EXT also writes NAME.automap.EXT (NAME.automap.L.EXT per level with --levels): Doom's
+automap of the dumped pose at SCALE pixels per map unit (0.2 is Doom's default; b2d_automap_device, DESIGN.md C19),
+coloured through palette 0 of its level and resolved at the --supersample factor; --automap-flags rotate,all,things turns
+the map with the view, draws every line (IDDT) and draws the decoration things.  Not with --world.
+
 --palette P colours the dumped and streamed frames through PLAYPAL palette P of each frame's level instead of palette 0
 (b2d_resolve_palettes_device; in Doom 1..8 are the damage flash, 9..12 the bonus flash, 13 the radiation suit), through
 the resolve at the --supersample factor (1 by default).  With --levels too; not with --world.
@@ -141,6 +146,17 @@ def _write_image(path: str, rgb: np.ndarray):
         f.write(encode_png(rgb) if path.lower().endswith(".png") else encode_ppm(rgb))
 
 
+def _automap_name(dump: str, level=None) -> str:
+    stem, ext = os.path.splitext(dump)
+    return "%s.automap%s%s" % (stem, "" if level is None else ".%d" % level, ext or ".ppm")
+
+
+def automap_rgb(r, poses: np.ndarray, levels, scale: float, flags: str, factor: int) -> np.ndarray:
+    """(n, H, W, 3) uint8: the automaps of the poses (b2d_automap_device at the render size) through palette 0 of each
+    frame's level, resolved by `factor` as the rendered frames are"""
+    return r.resolve(r.automap(np.ascontiguousarray(poses), levels, scale, flags), factor, "rgb", levels).cpu().numpy()
+
+
 def resolve_rgb(r, index: np.ndarray, factor: int, levels=None, palette: int = 0) -> np.ndarray:
     """(n, H, W, 3) uint8: the host index frames of renderer r resolved by `factor` on its device through palette `palette`
     of each frame's level (b2d_resolve_device, b2d_resolve_palettes_device)"""
@@ -201,6 +217,11 @@ def _main_levels(b2d, arch, set_, view, args, w, h) -> int:
         if args.dump:
             for k, lvl in enumerate(set_):
                 _write_image(_dump_name(args.dump, lvl), frame(k * per_level))
+            if args.automap is not None:
+                firsts = np.arange(len(set_)) * per_level
+                am = automap_rgb(r, poses[firsts], list(range(len(set_))), args.automap, args.automap_flags, args.supersample)
+                for k, lvl in enumerate(set_):
+                    _write_image(_automap_name(args.dump, lvl), am[k])
         if args.stream:
             with open(args.stream, "wb") as f:
                 for i in range(n):
@@ -285,6 +306,10 @@ def main(argv=None) -> int:
     ap.add_argument("--fixed-colormap", type=int, default=-1,
                     help="with --levels: light every frame through COLORMAP row R, -1..32 (32 invulnerability, 1 visor)")
     ap.add_argument("--extralight", type=int, default=0, help="with --levels: raise every light by E (0..2) weapon-flash steps")
+    ap.add_argument("--automap", type=float, default=None, metavar="SCALE",
+                    help="with --dump: also write NAME.automap.EXT (NAME.automap.L.EXT with --levels), Doom's automap of "
+                         "the dumped pose at SCALE pixels per map unit (Doom's default: 0.2)")
+    ap.add_argument("--automap-flags", default="", help="with --automap: comma-separated rotate, all, things")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 
@@ -315,6 +340,18 @@ def main(argv=None) -> int:
             return 2
         if args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1:
             print("--fixed-colormap and --extralight do not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
+            return 2
+    if args.automap is not None:
+        if not 1.0 / 256 <= args.automap <= 64:
+            print("--automap takes a scale in pixels per map unit, 1/256 .. 64", file=sys.stderr)
+            return 2
+        try:
+            b2d.automap_flags(args.automap_flags)
+        except ValueError as e:
+            print("--automap-flags: %s" % e, file=sys.stderr)
+            return 2
+        if not args.dump or args.world or int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            print("--automap takes --dump and does not combine with sharded rendering (--world or torchrun)", file=sys.stderr)
             return 2
     try:
         arch = b2d.Archive.open(args.iwad) if args.iwad else b2d.Archive.from_bytes(synthwad.build_iwad(1, synthwad.E1_MAPS[:3]))
@@ -379,6 +416,8 @@ def main(argv=None) -> int:
             rgb0 = frame(0)
             with open(args.dump, "wb") as f:
                 f.write(encode_png(rgb0) if args.dump.lower().endswith(".png") else encode_ppm(rgb0))
+            if args.automap is not None:
+                _write_image(_automap_name(args.dump), automap_rgb(r, poses[:1], None, args.automap, args.automap_flags, ss)[0])
         if args.stream:
             with open(args.stream, "wb") as f:
                 for i in range(len(poses)):

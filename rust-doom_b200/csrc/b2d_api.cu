@@ -560,6 +560,37 @@ static int enqueue_frames(b2d_renderer *r, const Pose *d_poses, const Frames &fr
     return raster_batch(r, ticket, d_index, d_rgba, stream);
 }
 
+// The n words word(i) of a call staged in `s` on `st` (stage_tables: the colour-table indices of its frames, frame_table
+// of its checked levels and palettes; b2d_automap_device: its levels): into staging grown to hold them (created whole, or
+// not at all; the old buffers go once the last call's kernel has read them), or into the present staging once the
+// previous call's copy has read it and, on `st`, its kernel the device copy.  The caller records s.done after its kernel.
+template <typename Word>
+static int stage_words(LevelStaging &s, size_t n, cudaStream_t st, Word word) {
+    if (s.cap < n) {
+        LevelStaging g;
+        g.cap = s.cap ? s.cap : 1024;
+        while (g.cap < n) g.cap *= 2;
+        CU(allocate(g.d, g.cap * sizeof(uint32_t)));
+        CU(allocate(g.h, g.cap * sizeof(uint32_t)));
+        CU(event_create(g.copied));
+        CU(event_create(g.done));
+        if (s.done) CU(cudaEventSynchronize(s.done.get()));
+        s = std::move(g);
+    } else {
+        CU(cudaEventSynchronize(s.copied.get()));     // the previous call's copy has read the staging
+        CU(cudaStreamWaitEvent(st, s.done.get(), 0));        // ... and its kernel the device copy
+    }
+    for (size_t i = 0; i < n; i++) s.h.get()[i] = word(i);
+    CU(cudaMemcpyAsync(s.d.get(), s.h.get(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(s.copied.get(), st));
+    return B2D_OK;
+}
+
+static int stage_tables(const b2d_renderer *r, LevelStaging &s, const uint32_t *levels, const uint32_t *palettes, size_t n,
+                        cudaStream_t st) {
+    return stage_words(s, n, st, [&](size_t i) { return frame_table(r, levels, palettes, i); });
+}
+
 extern "C" {
 
 const char *b2d_last_error(void) { return g_error.c_str(); }
@@ -681,6 +712,7 @@ int b2d_scene_create_dynamic(const b2d_archive *a, int level_index, const b2d_dy
         TextureDirectory td = TextureDirectory::load(*a->wad);
         s->level = Level::load(*a->wad, level_index);
         s->blob = compile_scene(s->level, td, dyn_list(dyn, n_dyn));
+        s->automap = automap_lines(s->level);
         fill_scene_info(s.get());
         s->palettes = td.palettes;
         if (s->palettes.empty()) s->palettes.push_back({});
@@ -750,6 +782,7 @@ int b2d_scene_create_from_lumps_dynamic(const b2d_level_lumps *lv, const b2d_tex
             std::memcpy(td.palettes[0].data(), tex->palette, 768);
         }
         s->blob = compile_scene(s->level, td, dyn_list(dyn, n_dyn));
+        s->automap = automap_lines(s->level);
         fill_scene_info(s.get());
         s->palettes.assign(1, td.palettes.empty() ? std::array<uint8_t, 768>{} : td.palettes[0]);
         *out = s.release();
@@ -773,6 +806,20 @@ int b2d_scene_set_palettes(b2d_scene *s, const uint8_t *playpal, size_t n_palett
         s->palettes = std::move(p);
         return B2D_OK;
     });
+}
+
+static_assert(sizeof(b2d_automap_line) == sizeof(AutomapLine) && offsetof(b2d_automap_line, colour) == offsetof(AutomapLine, colour) &&
+                  offsetof(b2d_automap_line, linedef) == offsetof(AutomapLine, linedef), "b2d_automap_line");
+static_assert(B2D_AUTOMAP_ROTATE == kAutomapRotate && B2D_AUTOMAP_ALL_LINES == kAutomapAllLines && B2D_AUTOMAP_THINGS == kAutomapThings,
+              "automap flags");
+
+int b2d_scene_automap_lines(const b2d_scene *s, b2d_automap_line *out, size_t capacity, size_t *n_out) {
+    if (!s || !n_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    *n_out = s->automap.size();
+    if (!out) return B2D_OK;
+    if (capacity < s->automap.size()) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the automap lines");
+    if (!s->automap.empty()) std::memcpy(out, s->automap.data(), s->automap.size() * sizeof(AutomapLine));
+    return B2D_OK;
 }
 
 int b2d_scene_info_get(const b2d_scene *s, b2d_scene_info *out) {
@@ -1033,6 +1080,20 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
         }
         words = std::max(words, (size_t)lv.layout.words);
     }
+    // the automap's items of every level (host copies; the device tables come with the first automap call)
+    rc = guarded([&] {
+        for (size_t k = 0; k < n_levels; k++) {
+            const uint32_t *h = reinterpret_cast<const uint32_t *>(scenes[k]->blob.data());
+            const SpriteRec *sp = reinterpret_cast<const SpriteRec *>(scenes[k]->blob.data() + h[H_OFF_SPRITES]);
+            r->lv[k].automap_lines = scenes[k]->automap;
+            for (uint32_t i = 0; i < h[H_NSPRITES]; i++) {
+                r->lv[k].automap_things.push_back(sp[i].x);
+                r->lv[k].automap_things.push_back(sp[i].y);
+            }
+        }
+        return B2D_OK;
+    });
+    if (rc != B2D_OK) return rc;
     // every palette of every level in one colour table (K3-levels, K4), copied from the scenes now: 14 KB per PLAYPAL
     std::vector<uint32_t> table;
     for (size_t k = 0; k < n_levels; k++) {
@@ -1344,32 +1405,6 @@ int b2d_render_levels_states_lights(b2d_renderer *r, const b2d_pose *poses, cons
                        rgba_fb);
 }
 
-// The colour-table indices of the n frames of a call (frame_table of its checked levels and palettes) staged in `s` on
-// `st`: into staging grown to hold them (created whole, or not at all; the old buffers go once the last call's kernel has
-// read them), or into the present staging once the previous call's copy has read it and, on `st`, its kernel the device
-// copy.  The caller records s.done after its kernel.
-static int stage_tables(const b2d_renderer *r, LevelStaging &s, const uint32_t *levels, const uint32_t *palettes, size_t n,
-                        cudaStream_t st) {
-    if (s.cap < n) {
-        LevelStaging g;
-        g.cap = s.cap ? s.cap : 1024;
-        while (g.cap < n) g.cap *= 2;
-        CU(allocate(g.d, g.cap * sizeof(uint32_t)));
-        CU(allocate(g.h, g.cap * sizeof(uint32_t)));
-        CU(event_create(g.copied));
-        CU(event_create(g.done));
-        if (s.done) CU(cudaEventSynchronize(s.done.get()));
-        s = std::move(g);
-    } else {
-        CU(cudaEventSynchronize(s.copied.get()));     // the previous call's copy has read the staging
-        CU(cudaStreamWaitEvent(st, s.done.get(), 0));        // ... and its kernel the device copy
-    }
-    for (size_t i = 0; i < n; i++) s.h.get()[i] = frame_table(r, levels, palettes, i);
-    CU(cudaMemcpyAsync(s.d.get(), s.h.get(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(s.copied.get(), st));
-    return B2D_OK;
-}
-
 int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_rgba, size_t n_pixels, void *cuda_stream) {
     if (!r || !d_index || !d_rgba) return fail(B2D_ERR_INVALID_ARG, "null argument");
     CU(cudaSetDevice(r->device));
@@ -1433,6 +1468,69 @@ int b2d_resolve_palettes_device(b2d_renderer *r, const uint8_t *d_index, const u
 int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, int factor, int format,
                        void *d_out, void *cuda_stream) {
     return b2d_resolve_palettes_device(r, d_index, levels, nullptr, n_frames, factor, format, d_out, cuda_stream);
+}
+
+// The automap tables of every level on the device, created whole (or not at all) by the first automap call and uploaded
+// on its stream `st`: the lines and things of each level in one buffer, then an AutomapLevel per level pointing into it,
+// copied from pinned memory the group keeps.  `built` follows the copies; every later call waits for it on its own stream.
+static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
+    auto a = std::make_unique<b2d_renderer::Automap>();
+    size_t items = 0;
+    std::vector<size_t> line_off, thing_off;
+    for (const LevelRes &lv : r->lv) {
+        line_off.push_back(items);
+        items += lv.automap_lines.size() * sizeof(AutomapLine);
+        thing_off.push_back(items);
+        items += lv.automap_things.size() * sizeof(int32_t);
+    }
+    items = (items + 15) & ~(size_t)15;                   // the AutomapLevel records follow, aligned
+    const size_t bytes = items + r->lv.size() * sizeof(AutomapLevel);
+    CU(allocate(a->d, bytes));
+    CU(allocate(a->h, bytes));
+    CU(event_create(a->built));
+    uint8_t *h = a->h.get(), *d = a->d.get();
+    std::vector<AutomapLevel> levels(r->lv.size());
+    for (size_t k = 0; k < r->lv.size(); k++) {
+        const LevelRes &lv = r->lv[k];
+        if (!lv.automap_lines.empty()) std::memcpy(h + line_off[k], lv.automap_lines.data(), lv.automap_lines.size() * sizeof(AutomapLine));
+        if (!lv.automap_things.empty()) std::memcpy(h + thing_off[k], lv.automap_things.data(), lv.automap_things.size() * sizeof(int32_t));
+        const AutomapLevel L{reinterpret_cast<const AutomapLine *>(d + line_off[k]), reinterpret_cast<const int32_t *>(d + thing_off[k]),
+                             (int32_t)lv.automap_lines.size(), (int32_t)(lv.automap_things.size() / 2)};
+        std::memcpy(h + items + k * sizeof(AutomapLevel), &L, sizeof L);
+    }
+    a->d_levels_off = items;
+    CU(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(a->built.get(), st));
+    r->automap = std::move(a);
+    return B2D_OK;
+}
+
+int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n_frames, int32_t scale_q16,
+                       int flags, uint8_t *d_out, void *cuda_stream) {
+    if (!r || !d_poses || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (flags & ~(B2D_AUTOMAP_ROTATE | B2D_AUTOMAP_ALL_LINES | B2D_AUTOMAP_THINGS)) return fail(B2D_ERR_INVALID_ARG, "unknown automap flags");
+    if (scale_q16 < kAutomapScaleMin || scale_q16 > kAutomapScaleMax)
+        return fail(B2D_ERR_INVALID_ARG, "automap scale out of range (256 .. 64 << 16, 16.16 pixels per map unit)");
+    if (levels)
+        for (size_t i = 0; i < n_frames; i++)
+            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    for (const LevelRes &lv : r->lv)      // the key of an item is (item + 1) << 8 | colour
+        if (lv.automap_lines.size() + kAutomapArrowSegs + kAutomapThingSegs * lv.automap_things.size() / 2 >= (1u << 24))
+            return fail(B2D_ERR_INVALID_ARG, "level has too many automap items (2^24)");
+    if (n_frames > 0x7FFFFFFFull / automap_tiles(r->view)) return fail(B2D_ERR_INVALID_ARG, "too many frames for one grid (2^31 - 1 tiles)");
+    if (n_frames == 0) return B2D_OK;
+    CU(cudaSetDevice(r->device));
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    if (r->automap) CU(cudaStreamWaitEvent(st, r->automap->built.get(), 0));      // the first call's upload
+    else if (int rc = guarded([&] { return ensure_automap(r, st); })) return rc;
+    if (levels)
+        if (int rc = stage_words(r->automap_levels, n_frames, st, [&](size_t i) { return levels[i]; })) return rc;
+    const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->d_levels_off);
+    CU(launch_automap(d_levels, levels ? r->automap_levels.d.get() : nullptr, reinterpret_cast<const Pose *>(d_poses),
+                      n_frames, r->view, scale_q16, flags, d_out, st));
+    if (levels) CU(cudaEventRecord(r->automap_levels.done.get(), st));
+    r->launches += 1;
+    return B2D_OK;
 }
 
 int b2d_device_alloc(int device, size_t bytes, void **d_out) {

@@ -18,6 +18,11 @@
 // resolve at the --supersample factor (1 by default); not with --world.  --fixed-colormap R (-1..32) and --extralight E (0..2)
 // light every frame of --levels as a player with those effects (b2d_*_levels_states_lights, DESIGN.md C18: 32 Doom's
 // invulnerability, 1 its light-amplification visor, E its weapon flashes); not with --world.
+// --automap SCALE (pixels per map unit, 0.2 is Doom's default) with --dump NAME.ppm also writes NAME.automap.ppm (with
+// --levels NAME.automap.L.ppm): Doom's automap of the dumped pose (b2d_automap_device, DESIGN.md C19) through palette 0 of
+// its level, resolved at the --supersample factor; --automap-flags rotate,all,things turns the map with the view, draws
+// every line and draws the decoration things.  Not with --world.
+#include <cmath>
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -113,6 +118,44 @@ int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const
     return 0;
 }
 
+// --automap: the automaps of `poses` (levels: each pose's level, nullptr: level 0) at the renderer's view, coloured through
+// palette 0 of each frame's level and resolved by `factor` to RGB8 (b2d_automap_device, b2d_resolve_device), frame k written
+// to names[k]
+int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, const uint32_t *levels,
+                   int32_t scale_q16, int flags, int factor, const std::vector<std::string> &names) {
+    const size_t n = poses.size(), npix = (size_t)view.width * view.height;
+    size_t frame_bytes = 0;
+    if (b2d_resolve_frame_bytes(r, factor, B2D_RESOLVE_RGB8, &frame_bytes) != B2D_OK) return fail("resolve");
+    void *d_poses = nullptr, *d_index = nullptr, *d_rgb = nullptr;
+    struct Bufs {
+        int device;
+        void **p[3];
+        ~Bufs() { for (void **q : p) if (*q) b2d_device_free(device, *q); }
+    } owner{device, {&d_poses, &d_index, &d_rgb}};
+    if (b2d_device_alloc(device, sizeof(b2d_pose) * n, &d_poses) != B2D_OK || b2d_device_alloc(device, npix * n, &d_index) != B2D_OK ||
+        b2d_device_alloc(device, frame_bytes * n, &d_rgb) != B2D_OK)
+        return fail("device memory");
+    if (b2d_device_upload(device, d_poses, poses.data(), sizeof(b2d_pose) * n) != B2D_OK) return fail("upload");
+    uint8_t *di = static_cast<uint8_t *>(d_index);
+    if (b2d_automap_device(r, static_cast<const b2d_pose *>(d_poses), levels, n, scale_q16, flags, di, nullptr) != B2D_OK)
+        return fail("automap");
+    if (b2d_resolve_device(r, di, levels, n, factor, B2D_RESOLVE_RGB8, d_rgb, nullptr) != B2D_OK) return fail("resolve");
+    std::vector<uint8_t> rgb(frame_bytes * n);
+    if (b2d_device_download(device, rgb.data(), d_rgb, rgb.size()) != B2D_OK) return fail("download");
+    for (size_t k = 0; k < n; k++) {
+        std::FILE *f = std::fopen(names[k].c_str(), "wb");
+        if (!f) { std::perror(names[k].c_str()); return 1; }
+        write_ppm_rgb(f, rgb.data() + frame_bytes * k, view.width / factor, view.height / factor);
+        std::fclose(f);
+    }
+    return 0;
+}
+
+// the --dump name without its .ppm extension
+std::string dump_stem(const std::string &dump) {
+    return dump.size() > 4 && dump.compare(dump.size() - 4, 4, ".ppm") == 0 ? dump.substr(0, dump.size() - 4) : dump;
+}
+
 // b2d_render_sharded consumer: per-frame checksums of every gathered chunk into a device table (the table lives in device memory
 // obtained through b2d_device_alloc: the CLI itself links no CUDA library)
 struct ShardSink {
@@ -164,7 +207,7 @@ int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st
 // --levels: the look-around of every level of `set` from its start, nposes per level, pose i at tic tics + i
 int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
                      const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file,
-                     int supersample, int palette, b2d_frame_light light) {
+                     int supersample, int palette, b2d_frame_light light, int32_t automap_scale, int automap_flags) {
     std::vector<b2d_scene *> scenes;
     struct Scenes {
         std::vector<b2d_scene *> &v;
@@ -240,13 +283,24 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
         else write_ppm(f, rgba.data() + npix * i, width, height);
     };
     if (!dump.empty()) {
-        const std::string stem = dump.size() > 4 && dump.compare(dump.size() - 4, 4, ".ppm") == 0 ? dump.substr(0, dump.size() - 4) : dump;
+        const std::string stem = dump_stem(dump);
         for (size_t k = 0; k < set.size(); k++) {
             const std::string name = stem + "." + std::to_string(set[k]) + ".ppm";
             std::FILE *f = std::fopen(name.c_str(), "wb");
             if (!f) { std::perror(name.c_str()); return 1; }
             write_frame(f, k * per_level);
             std::fclose(f);
+        }
+        if (automap_scale) {
+            std::vector<b2d_pose> firsts;
+            std::vector<uint32_t> first_levels;
+            std::vector<std::string> names;
+            for (size_t k = 0; k < set.size(); k++) {
+                firsts.push_back(poses[k * per_level]);
+                first_levels.push_back((uint32_t)k);
+                names.push_back(stem + ".automap." + std::to_string(set[k]) + ".ppm");
+            }
+            if (int rc = write_automaps(r, 0, view, firsts, first_levels.data(), automap_scale, automap_flags, supersample, names)) return rc;
         }
     }
     if (!stream.empty()) {
@@ -263,6 +317,8 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
 int main(int argc, char **argv) {
     std::string iwad, dump, stream, command, id_file, levels_arg;
     int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16, supersample = 1, palette = 0;
+    int32_t automap_scale = 0;        // 0: no --automap
+    int automap_flags = 0;
     b2d_frame_light light{-1, 0};
     double fov = 65.0;
     unsigned long tics = 0;
@@ -311,6 +367,28 @@ int main(int argc, char **argv) {
             if (fixed) light.fixed_colormap = (int32_t)x;
             else light.extralight = (uint32_t)x;
         }
+        else if (a == "--automap") {
+            const char *v = next("--automap");
+            char *end = nullptr;
+            const double x = std::strtod(v, &end);
+            if (!*v || *end || !(x >= 1.0 / 256 && x <= 64)) {
+                std::fprintf(stderr, "--automap takes a scale in pixels per map unit, 1/256 .. 64\n");
+                return 2;
+            }
+            automap_scale = (int32_t)std::lround(x * 65536);
+        } else if (a == "--automap-flags") {
+            std::string v = next("--automap-flags");
+            size_t at = 0;
+            while (at <= v.size()) {
+                const size_t comma = std::min(v.find(',', at), v.size());
+                const std::string name = v.substr(at, comma - at);
+                if (name == "rotate") automap_flags |= B2D_AUTOMAP_ROTATE;
+                else if (name == "all") automap_flags |= B2D_AUTOMAP_ALL_LINES;
+                else if (name == "things") automap_flags |= B2D_AUTOMAP_THINGS;
+                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things\n"); return 2; }
+                at = comma + 1;
+            }
+        }
         else if (a == "list-levels" || a == "check") command = a;
         else { std::fprintf(stderr, "unknown argument %s\n", a.c_str()); return 2; }
     }
@@ -322,6 +400,7 @@ int main(int argc, char **argv) {
     const bool lit = light.fixed_colormap != -1 || light.extralight != 0;
     if (lit && world > 0) { std::fprintf(stderr, "--fixed-colormap and --extralight do not combine with --world\n"); return 2; }
     if (lit && !with_levels) { std::fprintf(stderr, "--fixed-colormap and --extralight take --levels\n"); return 2; }
+    if (automap_scale && (dump.empty() || world > 0)) { std::fprintf(stderr, "--automap takes --dump and does not combine with --world\n"); return 2; }
 
     b2d_archive *arch = nullptr;
     if (b2d_archive_open(iwad.c_str(), &arch) != B2D_OK) return fail("open");
@@ -358,7 +437,7 @@ int main(int argc, char **argv) {
             return 2;
         }
         const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file,
-                                        supersample, palette, light);
+                                        supersample, palette, light, automap_scale, automap_flags);
         b2d_archive_close(arch);
         return rc;
     }
@@ -392,6 +471,10 @@ int main(int argc, char **argv) {
             write_ppm_rgb(f, rgb.data(), width, height);
             std::fclose(f);
         }
+        if (automap_scale && !dump.empty())
+            if (int rc = write_automaps(r, 0, view, {poses[0]}, nullptr, automap_scale, automap_flags, supersample,
+                                        {dump_stem(dump) + ".automap.ppm"}))
+                return rc;
         if (!stream.empty()) {
             std::FILE *f = std::fopen(stream.c_str(), "wb");
             if (!f) { std::perror(stream.c_str()); return 1; }
@@ -430,6 +513,9 @@ int main(int argc, char **argv) {
         write_ppm(f, rgba.data(), width, height);
         std::fclose(f);
     }
+    if (automap_scale && !dump.empty())
+        if (int rc = write_automaps(r, 0, view, {poses[0]}, nullptr, automap_scale, automap_flags, 1, {dump_stem(dump) + ".automap.ppm"}))
+            return rc;
     if (!stream.empty()) {
         std::FILE *f = std::fopen(stream.c_str(), "wb");
         if (!f) { std::perror(stream.c_str()); return 1; }

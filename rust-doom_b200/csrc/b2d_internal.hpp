@@ -128,6 +128,7 @@ struct b2d_scene {
     // every palette the scene holds, at least one; palettes[0] is the one compiled into the blob (768 zero bytes when
     // the scene was made without a PLAYPAL)
     std::vector<std::array<uint8_t, 768>> palettes;
+    std::vector<AutomapLine> automap;                     // automap_lines(level), built at creation
 };
 
 // A worklist slot: the BSP walk of batch k+1 may run (b2d_walk_device, another stream) while batch k is rastered.
@@ -205,6 +206,10 @@ struct LevelRes {
         Event built;
     };
     std::unique_ptr<Row32> row32;
+    // The automap's items (DESIGN.md C19), host copies taken at creation: the scene's automap table and the x, y of the
+    // blob's sprites.  Uploaded by the first b2d_automap_device call (b2d_renderer::automap).
+    std::vector<AutomapLine> automap_lines;
+    std::vector<int32_t> automap_things;
 };
 
 struct b2d_renderer {
@@ -232,6 +237,17 @@ struct b2d_renderer {
     // the frame tables of a call of b2d_palette_lut_levels_device and of b2d_resolve_device / b2d_resolve_palettes_device,
     // each call kind with its own
     LevelStaging lut_levels, resolve_levels;
+    // The automap tables of every level on the device, created whole by the first b2d_automap_device call: the lines and
+    // things of each level, then one AutomapLevel per level (at d_levels_off) pointing into them, uploaded from the pinned
+    // copy `h` on that call's stream; `built` follows the upload.  With the call's own level staging.
+    struct Automap {
+        DeviceBuf<uint8_t> d;
+        PinnedBuf<uint8_t> h;
+        size_t d_levels_off = 0;
+        Event built;
+    };
+    std::unique_ptr<Automap> automap;
+    LevelStaging automap_levels;
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;
     bool profiling = false;

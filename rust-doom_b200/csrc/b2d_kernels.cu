@@ -1730,4 +1730,69 @@ cudaError_t launch_palette(const uint32_t *d_palette, const uint8_t *d_index, ui
     return cudaGetLastError();
 }
 
+namespace {
+constexpr int kAutomapTileW = 128, kAutomapTileH = 32;
+
+// Kernel 5, the automap (C19): one CTA per (frame, 128 x 32 tile).  The tile is a u32 key per pixel in shared memory:
+// every thread takes items of the frame's level in turn, transforms it, and draws its pixels inside the tile with
+// atomicMax of ((item + 1) << 8 | colour), so the last item in draw order wins whatever the schedule; 0 is the
+// background, colour 0.  The key's low byte is then written out: 16 bytes per thread, a whole 128-byte line per tile row,
+// when the tile is full-width and rows start 16-byte aligned; byte by byte otherwise.
+__global__ void __launch_bounds__(256)
+b2d_automap_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level, const Pose *__restrict__ poses,
+                   View vw, int32_t scale, int flags, uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec) {
+    __shared__ uint32_t keys[kAutomapTileH * kAutomapTileW];
+    const size_t frame = blockIdx.x / tiles;
+    const int tile = blockIdx.x - (int)(frame * tiles);
+    const int tx0 = (tile % tiles_x) * kAutomapTileW, ty0 = (tile / tiles_x) * kAutomapTileH;
+    const int tx1 = min(tx0 + kAutomapTileW, vw.W), ty1 = min(ty0 + kAutomapTileH, vw.H);
+    for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) keys[k] = 0;
+    const AutomapLevel L = levels[frame_level ? frame_level[frame] : 0];
+    const AutomapFrame f = automap_frame(poses[frame], vw, scale, flags);
+    __syncthreads();
+    const int n = automap_items(L, flags);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        int64_t e[4];
+        const uint32_t colour = automap_item(f, L, flags, i, e);
+        if (!colour) continue;
+        const uint32_t key = ((uint32_t)(i + 1) << 8) | colour;
+        automap_line(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1,
+                     [&](int32_t x, int32_t y) { atomicMax(&keys[(y - ty0) * kAutomapTileW + (x - tx0)], key); });
+    }
+    __syncthreads();
+    uint8_t *dst = out + frame * (size_t)vw.W * vw.H;
+    if (vec && tx1 - tx0 == kAutomapTileW) {
+        const int r = threadIdx.x >> 3, c = (threadIdx.x & 7) * 16;     // 8 threads per 128-byte row
+        if (ty0 + r < ty1) {
+            const uint32_t *k = &keys[r * kAutomapTileW + c];
+            uint32_t w[4];
+            for (int q = 0; q < 4; q++)
+                w[q] = (k[4 * q] & 0xFF) | (k[4 * q + 1] & 0xFF) << 8 | (k[4 * q + 2] & 0xFF) << 16 | (k[4 * q + 3] & 0xFF) << 24;
+            *reinterpret_cast<uint4 *>(dst + (size_t)(ty0 + r) * vw.W + tx0 + c) = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+    } else {
+        for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) {
+            const int x = tx0 + (k % kAutomapTileW), y = ty0 + k / kAutomapTileW;
+            if (x < tx1 && y < ty1) dst[(size_t)y * vw.W + x] = (uint8_t)keys[k];
+        }
+    }
+}
+}  // namespace
+
+size_t automap_tiles(const View &vw) {
+    return (size_t)((vw.W + kAutomapTileW - 1) / kAutomapTileW) * (size_t)((vw.H + kAutomapTileH - 1) / kAutomapTileH);
+}
+
+cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
+                           const View &vw, int32_t scale, int flags, uint8_t *d_out, cudaStream_t stream) {
+    if (n_frames == 0) return cudaSuccess;
+    const int tiles_x = (vw.W + kAutomapTileW - 1) / kAutomapTileW;
+    const int tiles = (int)automap_tiles(vw);
+    if (n_frames * (size_t)tiles > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
+    b2d_automap_kernel<<<(unsigned)(n_frames * tiles), 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags, d_out,
+                                                                         tiles_x, tiles, vec);
+    return cudaGetLastError();
+}
+
 }  // namespace b2d

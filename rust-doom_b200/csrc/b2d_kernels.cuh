@@ -148,5 +148,11 @@ cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_
 // (d_tables NULL: table 0), box-filtered by `factor` (1..8, dividing W and H) into d_out in B2D_RESOLVE_* `format`.
 cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_tables, const uint8_t *d_index, void *d_out,
                            size_t n_frames, int W, int H, int factor, int format, cudaStream_t stream);
+// Kernel 5's grid: CTAs (128 x 32 tiles) per frame of view vw.
+size_t automap_tiles(const View &vw);
+// Kernel 5: the C19 automap of n_frames poses into contiguous W x H index frames at d_out, frame f from the items of
+// levels[frame_level[f]] (d_frame_level NULL: level 0), `scale` and `flags` as checked by b2d_automap_device.
+cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
+                           const View &vw, int32_t scale, int flags, uint8_t *d_out, cudaStream_t stream);
 
 }  // namespace b2d

@@ -555,4 +555,153 @@ B2D_HD int32_t sprite_column(const SpriteFrame &sp, const View &vw, int x, int32
     return (int32_t)clampv<int64_t>(floordiv64(sp.cz * c2 - L, 256 * (int64_t)vw.F), 0, w - 1);
 }
 
+// ---- automap (DESIGN.md C19) -------------------------------------------------------------------
+// Flags (== B2D_AUTOMAP_*), the accepted scale range in pixels per map unit, Q16 (1/256 .. 64), and Doom's colours.
+constexpr int kAutomapRotate = 1, kAutomapAllLines = 2, kAutomapThings = 4;
+constexpr int32_t kAutomapScaleMin = 1 << 8, kAutomapScaleMax = 64 << 16;
+constexpr uint32_t kAutomapArrowColour = 209, kAutomapThingColour = 112;
+constexpr int32_t kAutomapArrowR = 8 * 16 * 65536 / 7;      // player_arrow's R: 8 * PLAYERRADIUS / 7, 16.16
+constexpr int kAutomapArrowSegs = 7, kAutomapThingSegs = 3;
+
+// One linedef of a level's automap table (b2d_automap_line): endpoints in map units, the colour drawn normally and under
+// kAutomapAllLines (0: not drawn), and the linedef's index.
+struct AutomapLine {
+    int32_t x0, y0, x1, y1;
+    uint8_t colour, colour_all;
+    uint16_t pad;
+    int32_t linedef;
+};
+static_assert(sizeof(AutomapLine) == 24, "AutomapLine");
+
+// A level's automap items: its linedef table and the positions (x, y in map units) of its decoration things in blob order.
+struct AutomapLevel {
+    const AutomapLine *lines;
+    const int32_t *things;
+    int32_t nlines, nthings;
+};
+
+// A frame's transform: centre (pose x, y in 16.16), the map rotation by 90 deg - angle (used with kAutomapRotate) and the
+// arrow's rotation (the pose angle, or 90 deg with kAutomapRotate), both Q30.
+struct AutomapFrame {
+    int64_t px, py;
+    int32_t c, s, ac, as;
+    int32_t scale, W, H;
+    bool rot;
+};
+B2D_HD AutomapFrame automap_frame(const Pose &p, const View &vw, int32_t scale, int flags) {
+    AutomapFrame f;
+    f.px = p.x; f.py = p.y;
+    f.rot = (flags & kAutomapRotate) != 0;
+    sincos_q30(0x40000000u - p.angle, f.c, f.s);
+    sincos_q30(f.rot ? 0x40000000u : p.angle, f.ac, f.as);
+    f.scale = scale; f.W = vw.W; f.H = vw.H;
+    return f;
+}
+
+// A 16.16 offset (dx, dy) from the frame's centre, rotated by (c, s) if `rot`, to Q8 screen coordinates (y down).
+// |dx|, |dy| <= 2^32 + 2^20 and |c|, |s| <= 2^30 with min(|c|, |s|) <= 2^29.5 keep the rotation below 2^63; the rotated
+// offset stays below 2^32.6 and, times scale <= 2^22, X and Y below 2^31 (C19).
+B2D_HD void automap_screen(const AutomapFrame &f, int64_t dx, int64_t dy, bool rot, int32_t c, int32_t s, int64_t &X, int64_t &Y) {
+    int64_t rx = dx, ry = dy;
+    if (rot) {
+        rx = (dx * c - dy * s) >> 30;
+        ry = (dx * s + dy * c) >> 30;
+    }
+    X = ((int64_t)f.W << 7) + ((rx * f.scale) >> 24);
+    Y = ((int64_t)f.H << 7) - ((ry * f.scale) >> 24);
+}
+// a map point in 16.16
+B2D_HD void automap_map(const AutomapFrame &f, int64_t mx, int64_t my, int64_t &X, int64_t &Y) {
+    automap_screen(f, mx - f.px, my - f.py, f.rot, f.c, f.s, X, Y);
+}
+
+// Items of a frame in draw order: the level's linedefs, the 7 segments of the player arrow, 3 segments per thing (with
+// kAutomapThings).
+B2D_HD int automap_items(const AutomapLevel &L, int flags) {
+    return L.nlines + kAutomapArrowSegs + ((flags & kAutomapThings) ? kAutomapThingSegs * L.nthings : 0);
+}
+// Item i's endpoints in Q8 screen coordinates (e[0], e[1]) - (e[2], e[3]) and its colour (0: not drawn).
+B2D_HD uint32_t automap_item(const AutomapFrame &f, const AutomapLevel &L, int flags, int i, int64_t e[4]) {
+    if (i < L.nlines) {
+        const AutomapLine l = L.lines[i];
+        const uint32_t colour = (flags & kAutomapAllLines) ? l.colour_all : l.colour;
+        automap_map(f, (int64_t)l.x0 * 65536, (int64_t)l.y0 * 65536, e[0], e[1]);
+        automap_map(f, (int64_t)l.x1 * 65536, (int64_t)l.y1 * 65536, e[2], e[3]);
+        return colour;
+    }
+    i -= L.nlines;
+    if (i < kAutomapArrowSegs) {          // player_arrow, in its own rotation about the centre
+        constexpr int32_t R = kAutomapArrowR;
+        const int32_t ax = i == 0 ? -R + R / 8 : i <= 2 ? R : i <= 4 ? -R + R / 8 : -R + 3 * R / 8;
+        const int32_t bx = i == 0 ? R : i <= 2 ? R - R / 2 : i <= 4 ? -R - R / 8 : -R + R / 8;
+        const int32_t by = i == 0 ? 0 : (i & 1) ? R / 4 : -(R / 4);
+        automap_screen(f, ax, 0, true, f.ac, f.as, e[0], e[1]);
+        automap_screen(f, bx, by, true, f.ac, f.as, e[2], e[3]);
+        return kAutomapArrowColour;
+    }
+    i -= kAutomapArrowSegs;
+    const int t = i / kAutomapThingSegs, k = i - t * kAutomapThingSegs;     // thintriangle_guy at size 16, angle 0
+    const int64_t tx = (int64_t)L.things[2 * t] * 65536, ty = (int64_t)L.things[2 * t + 1] * 65536;
+    const int32_t ax = k == 1 ? 1048576 : -524288, ay = k == 0 ? -734000 : k == 1 ? 0 : 734000;
+    const int32_t bx = k == 0 ? 1048576 : -524288, by = k == 0 ? 0 : k == 1 ? 734000 : -734000;
+    automap_map(f, tx + ax, ty + ay, e[0], e[1]);
+    automap_map(f, tx + bx, ty + by, e[2], e[3]);
+    return kAutomapThingColour;
+}
+
+// The pixels of the line (X0, Y0) - (X1, Y1) (Q8, |X|, |Y| < 2^31) inside the pixel rectangle [x0, x1) x [y0, y1), each
+// passed to plot(x, y) once.  Along the major axis (|dX| >= |dY|: X) every pixel whose centre lies in the endpoints'
+// range, inclusive; its minor coordinate is the floor of the exact interpolation at that centre.  A range without a
+// pixel centre draws the pixel holding (X0, Y0).  Pixels are independent, so the range is clamped to the rectangle, and
+// the part of it whose minor coordinate falls inside is found by bisection (the minor coordinate is monotone).
+template <typename Plot>
+B2D_HD void automap_line(int64_t X0, int64_t Y0, int64_t X1, int64_t Y1, int32_t x0, int32_t y0, int32_t x1, int32_t y1,
+                         Plot plot) {
+    if ((X0 < X1 ? X1 : X0) >> 8 < x0 || (X0 < X1 ? X0 : X1) >> 8 >= x1 || (Y0 < Y1 ? Y1 : Y0) >> 8 < y0 ||
+        (Y0 < Y1 ? Y0 : Y1) >> 8 >= y1)
+        return;                                             // the bounding box of every pixel the line draws misses
+    const bool xmaj = (X1 >= X0 ? X1 - X0 : X0 - X1) >= (Y1 >= Y0 ? Y1 - Y0 : Y0 - Y1);
+    int64_t M0 = xmaj ? X0 : Y0, m0 = xmaj ? Y0 : X0, M1 = xmaj ? X1 : Y1, m1 = xmaj ? Y1 : X1;
+    if (M1 < M0) {
+        int64_t t = M0; M0 = M1; M1 = t;
+        t = m0; m0 = m1; m1 = t;
+    }
+    int64_t lo = (M0 + 127) >> 8, hi = (M1 - 128) >> 8;    // pixels whose centre 256 i + 128 lies in [M0, M1]
+    if (lo > hi) {
+        const int64_t px = X0 >> 8, py = Y0 >> 8;
+        if (px >= x0 && px < x1 && py >= y0 && py < y1) plot((int32_t)px, (int32_t)py);
+        return;
+    }
+    const int32_t Mlo = xmaj ? x0 : y0, Mhi = xmaj ? x1 : y1, mlo = xmaj ? y0 : x0, mhi = xmaj ? y1 : x1;
+    if (lo < Mlo) lo = Mlo;
+    if (hi > Mhi - 1) hi = Mhi - 1;
+    if (lo > hi) return;
+    const uint64_t dM = (uint64_t)(M1 - M0);
+    const bool up = m1 >= m0;
+    const uint64_t dm = up ? (uint64_t)(m1 - m0) : (uint64_t)(m0 - m1);
+    auto minor = [&](int64_t i) -> int64_t {               // the minor pixel at major pixel i
+        if (dM == 0) return m0 >> 8;
+        const uint64_t p = (uint64_t)(256 * i + 128 - M0) * dm;     // <= dM * dm < 2^64
+        const uint64_t q = p / dM;
+        return (up ? m0 + (int64_t)q : m0 - (int64_t)q - (q * dM != p ? 1 : 0)) >> 8;
+    };
+    int64_t a = lo, b = hi + 1;                             // first pixel not before [mlo, mhi)
+    while (a < b) {
+        const int64_t mid = a + ((b - a) >> 1);
+        const int64_t j = minor(mid);
+        if (up ? j < mlo : j >= mhi) a = mid + 1; else b = mid;
+    }
+    const int64_t first = a;
+    b = hi + 1;                                             // first pixel past it
+    while (a < b) {
+        const int64_t mid = a + ((b - a) >> 1);
+        const int64_t j = minor(mid);
+        if (up ? j >= mhi : j < mlo) b = mid; else a = mid + 1;
+    }
+    for (int64_t i = first; i < a; i++) {
+        const int64_t j = minor(i);
+        if (xmaj) plot((int32_t)i, (int32_t)j); else plot((int32_t)j, (int32_t)i);
+    }
+}
+
 }  // namespace b2d

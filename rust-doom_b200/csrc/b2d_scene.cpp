@@ -600,4 +600,39 @@ std::vector<uint8_t> compile_scene(const Level &lv, const TextureDirectory &td, 
     return std::move(w.bytes);
 }
 
+std::vector<AutomapLine> automap_lines(const Level &lv) {
+    constexpr uint16_t kSecret = 0x20, kDontDraw = 0x80;         // ML_SECRET, ML_DONTDRAW
+    constexpr uint8_t kWall = 176, kTeleport = 184, kFloorStep = 64, kCeilStep = 231, kPlain = 96;
+    // the sector of sidedef `side`, or -1 when the sidedef or its sector does not exist
+    auto side_sector = [&](int side) -> int {
+        if (side < 0 || (size_t)side >= lv.sidedefs.size()) return -1;
+        const int sec = lv.sidedefs[(size_t)side].sector;
+        return (size_t)sec < lv.sectors.size() ? sec : -1;
+    };
+    std::vector<AutomapLine> out;
+    for (size_t i = 0; i < lv.linedefs.size(); i++) {
+        const Linedef &l = lv.linedefs[i];
+        if (l.v1 >= lv.vertices.size() || l.v2 >= lv.vertices.size()) continue;
+        const int front = side_sector(l.right), back = side_sector(l.left);
+        uint8_t c = kWall, all = kWall;
+        if (front >= 0 && back >= 0) {
+            const Sector &F = lv.sectors[(size_t)front], &B = lv.sectors[(size_t)back];
+            if (l.special == 39) c = kTeleport;
+            else if (l.flags & kSecret) c = kWall;
+            else if (F.floor != B.floor) c = kFloorStep;
+            else if (F.ceil != B.ceil) c = kCeilStep;
+            else c = 0;
+            all = c ? c : kPlain;
+        }
+        AutomapLine r{};
+        r.x0 = lv.vertices[l.v1].x; r.y0 = lv.vertices[l.v1].y;
+        r.x1 = lv.vertices[l.v2].x; r.y1 = lv.vertices[l.v2].y;
+        r.colour = (l.flags & kDontDraw) ? 0 : c;
+        r.colour_all = all;
+        r.linedef = (int32_t)i;
+        out.push_back(r);
+    }
+    return out;
+}
+
 }  // namespace b2d

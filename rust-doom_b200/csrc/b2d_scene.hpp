@@ -480,4 +480,8 @@ int sector_at(const Level &level, double x, double y, int *subsector_out = nullp
 // (light >> 3)/31 (+-2/31, clamped) * 255 truncated to u8, in the reference's float32 arithmetic.
 uint8_t light_byte(int16_t light, int contrast);
 
+// The level's automap table (DESIGN.md C19): a record per linedef whose vertices exist, in LINEDEFS order, coloured by
+// Doom's AM_drawWalls rule at the level's rest heights with every line counted as mapped.
+std::vector<AutomapLine> automap_lines(const Level &level);
+
 }  // namespace b2d
