@@ -469,6 +469,38 @@ int b2d_resolve_palettes_device(b2d_renderer *r, const uint8_t *d_index, const u
 int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n_frames, int32_t scale_q16,
                        int flags, uint8_t *d_out, void *cuda_stream);
 
+/* Doom's automap of the lines each frame has seen (AM_drawWalls with ML_MAPPED; DESIGN.md C20): b2d_automap_device with
+ * frame f's linedefs coloured by row f of d_seen (device memory, n_frames rows of b2d_renderer_seen_words uint32 words,
+ * as b2d_raster_device_seen writes them).  Under B2D_AUTOMAP_ALL_LINES a line has its all-lines colour, mapped or not;
+ * otherwise a mapped line has its normal colour (0: not drawn); otherwise, with B2D_AUTOMAP_ALLMAP (the computer area
+ * map), a line that is not ML_DONTDRAW is grey 99; otherwise it is not drawn.  The arrow and things are as in
+ * b2d_automap_device.  d_seen NULL counts every line as mapped: with flags below B2D_AUTOMAP_ALLMAP the frames are then
+ * byte-identical to b2d_automap_device's.  Levels are staged, the tables uploaded and the waits kept as in
+ * b2d_automap_device (the two calls share them).  Its refusals, unknown flag bits beyond B2D_AUTOMAP_ALLMAP and a d_seen
+ * that is not 4-byte aligned are B2D_ERR_INVALID_ARG, detected before anything is enqueued.  b2d_automap_device itself
+ * refuses B2D_AUTOMAP_ALLMAP. */
+#define B2D_AUTOMAP_ALLMAP 8
+int b2d_automap_seen_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const uint32_t *d_seen,
+                            size_t n_frames, int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream);
+
+/* Seen lines (Doom's ML_MAPPED; DESIGN.md C20).  A frame sees linedef l of its own level when a seg of l owns a column of
+ * the frame in the raster's front-to-back solid pass: the column lies in the seg's exact column interval, its clip window
+ * is still open and it passes the seg's column evaluation.  Sprites, masked middles and flats mark nothing; a shut door
+ * hides the lines behind it.  A row of seen lines is b2d_renderer_seen_words uint32 words (the largest
+ * ceil(n_linedefs / 32) of the renderer's levels, at least 1): bit l & 31 of word l >> 5 is linedef l, in LINEDEFS order,
+ * of the frame's level.
+ * b2d_raster_device_seen rasters a ticket of any walk form (b2d_walk_device and its _states, _levels, _levels_states and
+ * _levels_states_lights forms) like b2d_raster_device(r, ticket, d_index_fb, NULL, cuda_stream): the index frames are
+ * byte-identical, in the same single launch, with the same waits.  Frame f also ORs its seen lines into row f of d_seen
+ * (device memory, n x words uint32 for a ticket of n frames); bits already set stay set, so a caller that passes each
+ * agent's persistent row keeps Doom's sticky mapped set, and zeroing a row starts it again.  Frames with a status bit set
+ * (b2d_renderer_status) have unspecified seen lines, as their pixels are unspecified.  The first call uploads every
+ * level's seg -> linedef table on its stream; every later call, on any stream, waits on the device for that upload.  A
+ * NULL or not 4-byte aligned d_seen, and every refusal of b2d_raster_device, are B2D_ERR_INVALID_ARG, detected before
+ * anything is enqueued. */
+int b2d_renderer_seen_words(const b2d_renderer *r, uint32_t *words_out);
+int b2d_raster_device_seen(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint32_t *d_seen, void *cuda_stream);
+
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
  * per-frame `frame.finish()` of engine/src/renderer.rs:160-167.  One process per GPU.  NCCL (libnccl.so.2) is bound

@@ -344,12 +344,14 @@ RESOLVE_FORMATS = {"rgba": RESOLVE_RGBA8, "rgb": RESOLVE_RGB8, "rgb_planar": RES
 
 
 AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS = _lib.AUTOMAP_ROTATE, _lib.AUTOMAP_ALL_LINES, _lib.AUTOMAP_THINGS
-AUTOMAP_FLAGS = {"rotate": AUTOMAP_ROTATE, "all": AUTOMAP_ALL_LINES, "things": AUTOMAP_THINGS}
+AUTOMAP_ALLMAP = _lib.AUTOMAP_ALLMAP
+AUTOMAP_FLAGS = {"rotate": AUTOMAP_ROTATE, "all": AUTOMAP_ALL_LINES, "things": AUTOMAP_THINGS, "allmap": AUTOMAP_ALLMAP}
 AUTOMAP_DEFAULT_SCALE_Q16 = 13107       # Doom's default automap scale, 0.2 pixels per map unit
 
 
 def automap_flags(flags) -> int:
-    """B2D_AUTOMAP_* bits from an int, or from names ("rotate", "all", "things") as a list or a comma-separated string"""
+    """B2D_AUTOMAP_* bits from an int, or from names ("rotate", "all", "things", "allmap") as a list or a comma-separated
+    string"""
     if isinstance(flags, int):
         return flags
     names = flags.split(",") if isinstance(flags, str) else list(flags)
@@ -357,9 +359,19 @@ def automap_flags(flags) -> int:
     for name in (x.strip() for x in names):
         if name:
             if name not in AUTOMAP_FLAGS:
-                raise ValueError("unknown automap flag %r (rotate, all, things)" % name)
+                raise ValueError("unknown automap flag %r (rotate, all, things, allmap)" % name)
             out |= AUTOMAP_FLAGS[name]
     return out
+
+
+def seen_lines(row) -> np.ndarray:
+    """The linedef indices (ascending) whose bits are set in one row of seen lines (DESIGN.md C20): a numpy or torch
+    array of uint32 / int32 words, bit l & 31 of word l >> 5 for linedef l."""
+    if hasattr(row, "cpu"):
+        row = row.cpu().numpy()
+    words = np.ascontiguousarray(row).view(np.uint32).reshape(-1)
+    bits = np.unpackbits(words.view(np.uint8), bitorder="little")
+    return np.flatnonzero(bits).astype(np.int64)
 
 
 def _levels_array(levels, n: int) -> np.ndarray:
@@ -596,6 +608,63 @@ class Renderer:
     def raster_device(self, ticket: int, index_ptr: int, rgba_ptr: int = 0, stream: int = 0):
         _check(_lib.load().b2d_raster_device(self._h, ticket, index_ptr, rgba_ptr or None, stream or None))
 
+    @property
+    def seen_words(self) -> int:
+        """b2d_renderer_seen_words: uint32 words per row of seen lines (the largest ceil(n_linedefs / 32) of the levels)."""
+        w = ctypes.c_uint32()
+        _check(_lib.load().b2d_renderer_seen_words(self._h, ctypes.byref(w)))
+        return int(w.value)
+
+    def raster_device_seen(self, ticket: int, index_ptr: int, seen_ptr: int, stream: int = 0):
+        """b2d_raster_device_seen: raster_device of a ticket of any walk form into index frames only, and frame f's seen
+        lines (DESIGN.md C20) OR-ed into row f of the seen rows at seen_ptr (device, seen_words uint32 per row)."""
+        _check(_lib.load().b2d_raster_device_seen(self._h, ticket, index_ptr, seen_ptr, stream or None))
+
+    def render_seen(self, poses, levels=None, tics=None, moves_per_pose=None, lights=None, seen=None):
+        """Index frames and seen lines of host or CUDA poses, on the current torch stream: each batch of max_batch poses
+        walked by the walk its arguments ask for (plain; per-frame `tics` and `moves_per_pose`; per-frame `levels`; both;
+        `lights` with both, as in render_levels_states) and rastered by raster_device_seen.  Returns (uint8 tensor
+        [n, H, W], int32 tensor [n, seen_words]); with `seen` (a CUDA int32 tensor [n, seen_words]) the frames' seen lines
+        are OR-ed into it, and it is returned.  seen_lines() unpacks a row."""
+        import torch
+        if lights is not None and (levels is None or tics is None):
+            raise ValueError("lights come with per-frame levels and tics")
+        if moves_per_pose is not None and tics is None:
+            raise ValueError("moves_per_pose comes with per-frame tics")
+        dev = torch.device("cuda", self.device)
+        if isinstance(poses, torch.Tensor):
+            p = poses.to(dev).contiguous()
+        else:
+            p = torch.from_numpy(np.ascontiguousarray(poses, dtype=POSE_DTYPE).view(np.uint8).reshape(-1)).to(dev)
+        psize = ctypes.sizeof(_lib.Pose)
+        n = p.numel() * p.element_size() // psize
+        words = self.seen_words
+        if seen is None:
+            seen = torch.zeros((n, words), dtype=torch.int32, device=dev)
+        elif not (seen.is_cuda and seen.dtype == torch.int32 and tuple(seen.shape) == (n, words) and seen.is_contiguous()):
+            raise ValueError("seen must be a contiguous CUDA int32 tensor [%d, %d]" % (n, words))
+        out = torch.empty((n, self.height, self.width), dtype=torch.uint8, device=dev)
+        lv = None if levels is None else _levels_array(levels, n)
+        tc = None if tics is None else np.ascontiguousarray(tics, dtype=np.uint32)
+        npix = self.height * self.width
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+        for i in range(0, n, self.max_batch):
+            k = min(self.max_batch, n - i)
+            pp = p.data_ptr() + i * psize
+            mv = None if moves_per_pose is None else list(moves_per_pose)[i:i + k]
+            lt = None if lights is None else list(lights)[i:i + k]
+            if lv is None and tc is None:
+                ticket = self.walk_device(pp, k, stream)
+            elif lv is None:
+                ticket = self.walk_device_states(pp, tc[i:i + k], k, mv, stream)
+            elif tc is None:
+                ticket = self.walk_device_levels(pp, lv[i:i + k], k, stream)
+            else:
+                ticket = self.walk_device_levels_states(pp, lv[i:i + k], tc[i:i + k], k, mv, stream, lt)
+            self.raster_device_seen(ticket, out.data_ptr() + i * npix, seen.data_ptr() + i * words * 4, stream)
+        return out, seen
+
     def palette_lut_device(self, index_ptr: int, rgba_ptr: int, n_pixels: int, stream: int = 0):
         _check(_lib.load().b2d_palette_lut_device(self._h, index_ptr, rgba_ptr, n_pixels, stream or None))
 
@@ -646,18 +715,25 @@ class Renderer:
         return out
 
     def automap_device(self, poses_ptr: int, n: int, out_ptr: int, scale_q16: int = AUTOMAP_DEFAULT_SCALE_Q16,
-                       flags: int = 0, levels=None, stream: int = 0):
+                       flags: int = 0, levels=None, stream: int = 0, seen_ptr=None):
         """b2d_automap_device: the automap (DESIGN.md C19) of the n device poses at poses_ptr into n contiguous W x H
         palette-index frames at out_ptr, frame f of level levels[f] (host list; None = level 0), at scale_q16 pixels per map
-        unit in 16.16 (256 .. 64 << 16), flags an OR of AUTOMAP_ROTATE, AUTOMAP_ALL_LINES and AUTOMAP_THINGS."""
+        unit in 16.16 (256 .. 64 << 16), flags an OR of AUTOMAP_ROTATE, AUTOMAP_ALL_LINES and AUTOMAP_THINGS.  With
+        `seen_ptr` (device rows of seen lines, seen_words uint32 per frame) or AUTOMAP_ALLMAP in the flags it calls
+        b2d_automap_seen_device: frame f draws the lines row f has mapped (C20; seen_ptr None: every line)."""
         lv = None if levels is None else _levels_array(levels, n)
-        _check(_lib.load().b2d_automap_device(self._h, poses_ptr, None if lv is None else lv.ctypes.data, n, int(scale_q16),
-                                              int(flags), out_ptr, stream or None))
+        lvp = None if lv is None else lv.ctypes.data
+        if seen_ptr is not None or int(flags) & AUTOMAP_ALLMAP:
+            _check(_lib.load().b2d_automap_seen_device(self._h, poses_ptr, lvp, seen_ptr or None, n, int(scale_q16), int(flags),
+                                                       out_ptr, stream or None))
+        else:
+            _check(_lib.load().b2d_automap_device(self._h, poses_ptr, lvp, n, int(scale_q16), int(flags), out_ptr, stream or None))
 
-    def automap(self, poses, levels=None, scale: float = 0.2, flags=0):
+    def automap(self, poses, levels=None, scale: float = 0.2, flags=0, seen=None):
         """The automaps of host or CUDA poses as a CUDA uint8 tensor [n, H, W] of palette indices, on the current torch
-        stream: `scale` in pixels per map unit (Doom's default 0.2), `flags` an int or names from "rotate", "all", "things".
-        Colour them with resolve() or palette_lut_levels_device like rendered frames."""
+        stream: `scale` in pixels per map unit (Doom's default 0.2), `flags` an int or names from "rotate", "all", "things",
+        "allmap".  `seen`: a CUDA int32 tensor [n, seen_words] of seen lines (render_seen), whose mapped lines each frame
+        draws (automap_device's seen_ptr).  Colour them with resolve() or palette_lut_levels_device like rendered frames."""
         import torch
         flags = automap_flags(flags)
         dev = torch.device("cuda", self.device)
@@ -670,7 +746,12 @@ class Renderer:
         out = torch.empty((n, self.height, self.width), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream().cuda_stream
-        self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream)
+        seen_ptr = None
+        if seen is not None:
+            if not (seen.is_cuda and seen.dtype == torch.int32 and tuple(seen.shape) == (n, self.seen_words) and seen.is_contiguous()):
+                raise ValueError("seen must be a contiguous CUDA int32 tensor [%d, %d]" % (n, self.seen_words))
+            seen_ptr = seen.data_ptr()
+        self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream, seen_ptr)
         return out
 
     def worklist(self, n: int):

@@ -65,13 +65,13 @@ EXPORTS = [
     "b2d_scene_num_palettes", "b2d_scene_set_palettes", "b2d_resolve_palettes_device",
     "b2d_render_sharded_levels_states_resolved_palettes",
     "b2d_render_levels_states_lights", "b2d_render_device_levels_states_lights", "b2d_walk_device_levels_states_lights",
-    "b2d_scene_automap_lines", "b2d_automap_device",
+    "b2d_scene_automap_lines", "b2d_automap_device", "b2d_renderer_seen_words", "b2d_raster_device_seen", "b2d_automap_seen_device",
 ]
 
 COMM_ID_BYTES = 128
 RESOLVE_RGBA8, RESOLVE_RGB8, RESOLVE_RGB8_PLANAR, RESOLVE_GRAY8 = 0, 1, 2, 3      # B2D_RESOLVE_*
 SHARD_RENDER_ONLY, SHARD_RENDER_GATHER, SHARD_GATHER_ONLY = 0, 1, 2
-AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS = 1, 2, 4      # B2D_AUTOMAP_*
+AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS, AUTOMAP_ALLMAP = 1, 2, 4, 8      # B2D_AUTOMAP_*
 
 
 class AutomapLine(ctypes.Structure):
@@ -222,6 +222,10 @@ def load() -> ctypes.CDLL:
     L.b2d_resolve_palettes_device.argtypes = [vp, vp, vp, vp, cs, ci, ci, vp, vp]
     L.b2d_scene_automap_lines.argtypes = [vp, ctypes.POINTER(AutomapLine), cs, ctypes.POINTER(cs)]
     L.b2d_automap_device.argtypes = [vp, vp, vp, cs, ctypes.c_int32, ci, vp, vp]
+    L.b2d_renderer_seen_words.argtypes = [vp, ctypes.POINTER(ctypes.c_uint32)]
+    L.b2d_raster_device_seen.argtypes = [vp, ctypes.c_int64, vp, vp, vp]
+    L.b2d_raster_device_seen.restype = ctypes.c_int
+    L.b2d_automap_seen_device.argtypes = [vp, vp, vp, vp, cs, ctypes.c_int32, ci, vp, vp]
     L.b2d_render_sharded_levels_states_resolved_palettes.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(FrameState), cs,
                                                                      ctypes.POINTER(SectorMove), cs, cs, ci, ci, ci, CHUNK_FN, vp,
                                                                      ctypes.POINTER(ShardedStats)]

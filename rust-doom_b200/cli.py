@@ -26,7 +26,9 @@ block's palette colours, each frame through its own level's palette): an anti-al
 --automap SCALE with --dump NAME.EXT also writes NAME.automap.EXT (NAME.automap.L.EXT per level with --levels): Doom's
 automap of the dumped pose at SCALE pixels per map unit (0.2 is Doom's default; b2d_automap_device, DESIGN.md C19),
 coloured through palette 0 of its level and resolved at the --supersample factor; --automap-flags rotate,all,things turns
-the map with the view, draws every line (IDDT) and draws the decoration things.  Not with --world.
+the map with the view, draws every line (IDDT) and draws the decoration things; seen draws only the lines the run's
+frames of that level saw (Renderer.render_seen, DESIGN.md C20) and allmap adds the unseen ones in grey (the computer
+area map).  Not with --world.
 
 --palette P colours the dumped and streamed frames through PLAYPAL palette P of each frame's level instead of palette 0
 (b2d_resolve_palettes_device; in Doom 1..8 are the damage flash, 9..12 the bonus flash, 13 the radiation suit), through
@@ -151,10 +153,30 @@ def _automap_name(dump: str, level=None) -> str:
     return "%s.automap%s%s" % (stem, "" if level is None else ".%d" % level, ext or ".ppm")
 
 
-def automap_rgb(r, poses: np.ndarray, levels, scale: float, flags: str, factor: int) -> np.ndarray:
+def automap_flag_names(flags: str):
+    """(the B2D_AUTOMAP_* names of --automap-flags, whether it names `seen`); unknown names raise ValueError"""
+    names = [x.strip() for x in flags.split(",") if x.strip()]
+    rest = ",".join(x for x in names if x != "seen")
+    import rust_doom_b200 as b2d
+    b2d.automap_flags(rest)
+    return rest, "seen" in names
+
+
+def automap_rgb(r, poses: np.ndarray, levels, scale: float, flags: str, factor: int, run_poses=None, run_levels=None) -> np.ndarray:
     """(n, H, W, 3) uint8: the automaps of the poses (b2d_automap_device at the render size) through palette 0 of each
-    frame's level, resolved by `factor` as the rendered frames are"""
-    return r.resolve(r.automap(np.ascontiguousarray(poses), levels, scale, flags), factor, "rgb", levels).cpu().numpy()
+    frame's level, resolved by `factor` as the rendered frames are.  With `seen` in the flags, frame k draws the lines
+    that the run's frames (run_poses, of levels run_levels) of its level saw (Renderer.render_seen, OR-ed per level)."""
+    import torch
+    names, seen = automap_flag_names(flags)
+    rows = None
+    if seen:
+        kw = {} if run_levels is None else {"levels": list(run_levels)}
+        per_frame = r.render_seen(np.ascontiguousarray(run_poses), **kw)[1].cpu().numpy().view(np.uint32)
+        run_lv = np.zeros(len(per_frame), np.int64) if run_levels is None else np.asarray(run_levels)
+        lv = np.zeros(len(poses), np.int64) if levels is None else np.asarray(levels)
+        rows = np.stack([np.bitwise_or.reduce(per_frame[run_lv == l], axis=0) for l in lv])
+        rows = torch.from_numpy(rows.view(np.int32).copy()).cuda(r.device)
+    return r.resolve(r.automap(np.ascontiguousarray(poses), levels, scale, names, seen=rows), factor, "rgb", levels).cpu().numpy()
 
 
 def resolve_rgb(r, index: np.ndarray, factor: int, levels=None, palette: int = 0) -> np.ndarray:
@@ -219,7 +241,8 @@ def _main_levels(b2d, arch, set_, view, args, w, h) -> int:
                 _write_image(_dump_name(args.dump, lvl), frame(k * per_level))
             if args.automap is not None:
                 firsts = np.arange(len(set_)) * per_level
-                am = automap_rgb(r, poses[firsts], list(range(len(set_))), args.automap, args.automap_flags, args.supersample)
+                am = automap_rgb(r, poses[firsts], list(range(len(set_))), args.automap, args.automap_flags, args.supersample,
+                                 poses, levels)
                 for k, lvl in enumerate(set_):
                     _write_image(_automap_name(args.dump, lvl), am[k])
         if args.stream:
@@ -309,7 +332,8 @@ def main(argv=None) -> int:
     ap.add_argument("--automap", type=float, default=None, metavar="SCALE",
                     help="with --dump: also write NAME.automap.EXT (NAME.automap.L.EXT with --levels), Doom's automap of "
                          "the dumped pose at SCALE pixels per map unit (Doom's default: 0.2)")
-    ap.add_argument("--automap-flags", default="", help="with --automap: comma-separated rotate, all, things")
+    ap.add_argument("--automap-flags", default="", help="with --automap: comma-separated rotate, all, things, allmap (unseen lines in grey), "
+                         "seen (only the lines the run's frames saw)")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 
@@ -346,7 +370,7 @@ def main(argv=None) -> int:
             print("--automap takes a scale in pixels per map unit, 1/256 .. 64", file=sys.stderr)
             return 2
         try:
-            b2d.automap_flags(args.automap_flags)
+            automap_flag_names(args.automap_flags)
         except ValueError as e:
             print("--automap-flags: %s" % e, file=sys.stderr)
             return 2
@@ -417,7 +441,7 @@ def main(argv=None) -> int:
             with open(args.dump, "wb") as f:
                 f.write(encode_png(rgb0) if args.dump.lower().endswith(".png") else encode_ppm(rgb0))
             if args.automap is not None:
-                _write_image(_automap_name(args.dump), automap_rgb(r, poses[:1], None, args.automap, args.automap_flags, ss)[0])
+                _write_image(_automap_name(args.dump), automap_rgb(r, poses[:1], None, args.automap, args.automap_flags, ss, poses)[0])
         if args.stream:
             with open(args.stream, "wb") as f:
                 for i in range(len(poses)):

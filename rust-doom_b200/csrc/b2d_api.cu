@@ -524,7 +524,8 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
     return B2D_OK;
 }
 
-int b2d::raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream) {
+int b2d::raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
+                      const SeenTables *seen) {
     const int slot = (int)(ticket & 1);
     WorkSlot &s = r->slot[slot];
     if (ticket < 0 || s.ticket != ticket || s.rastered) return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
@@ -538,7 +539,8 @@ int b2d::raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_
     // masked content in a level the frames read: with per-frame levels, any level's
     const bool masked = r->d_masked && (s.tables.per_level || s.tables.scene.masked_list);
     const int rc = profiled(r, stream, 1, [&] {
-        return launch_raster(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba, stream);
+        return seen ? launch_raster_seen(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, *seen, stream)
+                    : launch_raster(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba, stream);
     });
     if (rc != B2D_OK) return rc;
     CU(cudaEventRecord(s.raster_done.get(), stream));
@@ -810,7 +812,8 @@ int b2d_scene_set_palettes(b2d_scene *s, const uint8_t *playpal, size_t n_palett
 
 static_assert(sizeof(b2d_automap_line) == sizeof(AutomapLine) && offsetof(b2d_automap_line, colour) == offsetof(AutomapLine, colour) &&
                   offsetof(b2d_automap_line, linedef) == offsetof(AutomapLine, linedef), "b2d_automap_line");
-static_assert(B2D_AUTOMAP_ROTATE == kAutomapRotate && B2D_AUTOMAP_ALL_LINES == kAutomapAllLines && B2D_AUTOMAP_THINGS == kAutomapThings,
+static_assert(B2D_AUTOMAP_ROTATE == kAutomapRotate && B2D_AUTOMAP_ALL_LINES == kAutomapAllLines && B2D_AUTOMAP_THINGS == kAutomapThings &&
+                  B2D_AUTOMAP_ALLMAP == kAutomapAllmap,
               "automap flags");
 
 int b2d_scene_automap_lines(const b2d_scene *s, b2d_automap_line *out, size_t capacity, size_t *n_out) {
@@ -1086,10 +1089,16 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
             const uint32_t *h = reinterpret_cast<const uint32_t *>(scenes[k]->blob.data());
             const SpriteRec *sp = reinterpret_cast<const SpriteRec *>(scenes[k]->blob.data() + h[H_OFF_SPRITES]);
             r->lv[k].automap_lines = scenes[k]->automap;
+            for (AutomapLine &l : r->lv[k].automap_lines)      // the device copy's don't-draw bit (the seen automap's ALLMAP rule)
+                if (scenes[k]->level.linedefs[(size_t)l.linedef].flags & 0x80) l.dev_flags = kAutomapDontDraw;
             for (uint32_t i = 0; i < h[H_NSPRITES]; i++) {
                 r->lv[k].automap_things.push_back(sp[i].x);
                 r->lv[k].automap_things.push_back(sp[i].y);
             }
+            // seen lines (C20): compiled segs are 1:1 with the SEGS lump
+            const Level &lvl = scenes[k]->level;
+            for (const Seg &sg : lvl.segs) r->lv[k].seg_line.push_back(sg.linedef < lvl.linedefs.size() ? (int32_t)sg.linedef : -1);
+            r->seen_words = std::max(r->seen_words, (uint32_t)((lvl.linedefs.size() + 31) / 32));
         }
         return B2D_OK;
     });
@@ -1505,10 +1514,57 @@ static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
     return B2D_OK;
 }
 
-int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n_frames, int32_t scale_q16,
-                       int flags, uint8_t *d_out, void *cuda_stream) {
+// The seg -> linedef tables of every level on the device, created whole (or not at all) by the first seen raster and
+// uploaded on its stream `st` from pinned memory the group keeps: the tables one after the other, then each level's offset
+// into them.  `built` follows the copy; every later call waits for it on its own stream.
+static int ensure_seen(b2d_renderer *r, cudaStream_t st) {
+    auto a = std::make_unique<b2d_renderer::Seen>();
+    std::vector<int32_t> words;
+    std::vector<uint32_t> off;
+    for (const LevelRes &lv : r->lv) {
+        off.push_back((uint32_t)words.size());
+        words.insert(words.end(), lv.seg_line.begin(), lv.seg_line.end());
+    }
+    a->d_off = words.size();
+    for (uint32_t o : off) words.push_back((int32_t)o);
+    CU(allocate(a->d, words.size() * sizeof(int32_t)));
+    CU(allocate(a->h, words.size() * sizeof(int32_t)));
+    CU(event_create(a->built));
+    std::memcpy(a->h.get(), words.data(), words.size() * sizeof(int32_t));
+    CU(cudaMemcpyAsync(a->d.get(), a->h.get(), words.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(a->built.get(), st));
+    r->seen = std::move(a);
+    return B2D_OK;
+}
+
+int b2d_renderer_seen_words(const b2d_renderer *r, uint32_t *words_out) {
+    if (!r || !words_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    *words_out = r->seen_words;
+    return B2D_OK;
+}
+
+int b2d_raster_device_seen(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint32_t *d_seen, void *cuda_stream) {
+    if (!r || !d_index_fb || !d_seen) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    if (reinterpret_cast<uintptr_t>(d_seen) & 3) return fail(B2D_ERR_INVALID_ARG, "seen rows not 4-byte aligned");
+    CU(cudaSetDevice(r->device));
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    const int slot = (int)(ticket & 1);
+    if (ticket < 0 || r->slot[slot].ticket != ticket || r->slot[slot].rastered)
+        return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
+    if (r->seen) CU(cudaStreamWaitEvent(st, r->seen->built.get(), 0));      // the first call's upload
+    else if (int rc = guarded([&] { return ensure_seen(r, st); })) return rc;
+    const SeenTables seen{d_seen, r->seen->d.get(), reinterpret_cast<const uint32_t *>(r->seen->d.get() + r->seen->d_off),
+                          r->seen_words};
+    return raster_batch(r, ticket, d_index_fb, nullptr, st, &seen);
+}
+
+// b2d_automap_device (seen_variant false: K5) and b2d_automap_seen_device (its seen variant, which also takes ALLMAP)
+static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const uint32_t *d_seen, size_t n_frames,
+                        int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream, bool seen_variant) {
     if (!r || !d_poses || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    if (flags & ~(B2D_AUTOMAP_ROTATE | B2D_AUTOMAP_ALL_LINES | B2D_AUTOMAP_THINGS)) return fail(B2D_ERR_INVALID_ARG, "unknown automap flags");
+    const int known = B2D_AUTOMAP_ROTATE | B2D_AUTOMAP_ALL_LINES | B2D_AUTOMAP_THINGS | (seen_variant ? B2D_AUTOMAP_ALLMAP : 0);
+    if (flags & ~known) return fail(B2D_ERR_INVALID_ARG, "unknown automap flags");
+    if (reinterpret_cast<uintptr_t>(d_seen) & 3) return fail(B2D_ERR_INVALID_ARG, "seen rows not 4-byte aligned");
     if (scale_q16 < kAutomapScaleMin || scale_q16 > kAutomapScaleMax)
         return fail(B2D_ERR_INVALID_ARG, "automap scale out of range (256 .. 64 << 16, 16.16 pixels per map unit)");
     if (levels)
@@ -1526,11 +1582,26 @@ int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t 
     if (levels)
         if (int rc = stage_words(r->automap_levels, n_frames, st, [&](size_t i) { return levels[i]; })) return rc;
     const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->d_levels_off);
-    CU(launch_automap(d_levels, levels ? r->automap_levels.d.get() : nullptr, reinterpret_cast<const Pose *>(d_poses),
-                      n_frames, r->view, scale_q16, flags, d_out, st));
+    const uint32_t *d_frame_level = levels ? r->automap_levels.d.get() : nullptr;
+    if (seen_variant)
+        CU(launch_automap_seen(d_levels, d_frame_level, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16,
+                               flags, d_seen, r->seen_words, d_out, st));
+    else
+        CU(launch_automap(d_levels, d_frame_level, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16, flags,
+                          d_out, st));
     if (levels) CU(cudaEventRecord(r->automap_levels.done.get(), st));
     r->launches += 1;
     return B2D_OK;
+}
+
+int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, size_t n_frames, int32_t scale_q16,
+                       int flags, uint8_t *d_out, void *cuda_stream) {
+    return automap_call(r, d_poses, levels, nullptr, n_frames, scale_q16, flags, d_out, cuda_stream, false);
+}
+
+int b2d_automap_seen_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const uint32_t *d_seen,
+                            size_t n_frames, int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream) {
+    return automap_call(r, d_poses, levels, d_seen, n_frames, scale_q16, flags, d_out, cuda_stream, true);
 }
 
 int b2d_device_alloc(int device, size_t bytes, void **d_out) {

@@ -21,7 +21,8 @@
 // --automap SCALE (pixels per map unit, 0.2 is Doom's default) with --dump NAME.ppm also writes NAME.automap.ppm (with
 // --levels NAME.automap.L.ppm): Doom's automap of the dumped pose (b2d_automap_device, DESIGN.md C19) through palette 0 of
 // its level, resolved at the --supersample factor; --automap-flags rotate,all,things turns the map with the view, draws
-// every line and draws the decoration things.  Not with --world.
+// every line and draws the decoration things; seen draws only the lines the run's frames of that level saw (b2d_raster_device_seen,
+// DESIGN.md C20), allmap adds the unseen ones in grey (the computer area map).  Not with --world.
 #include <cmath>
 #include <algorithm>
 #include <cstdint>
@@ -121,24 +122,34 @@ int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const
 // --automap: the automaps of `poses` (levels: each pose's level, nullptr: level 0) at the renderer's view, coloured through
 // palette 0 of each frame's level and resolved by `factor` to RGB8 (b2d_automap_device, b2d_resolve_device), frame k written
 // to names[k]
+// With `seen` (n rows of b2d_renderer_seen_words words) or B2D_AUTOMAP_ALLMAP, frame k draws the lines row k has mapped
+// (b2d_automap_seen_device).
 int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, const uint32_t *levels,
-                   int32_t scale_q16, int flags, int factor, const std::vector<std::string> &names) {
+                   int32_t scale_q16, int flags, int factor, const std::vector<std::string> &names,
+                   const std::vector<uint32_t> *seen = nullptr) {
     const size_t n = poses.size(), npix = (size_t)view.width * view.height;
     size_t frame_bytes = 0;
     if (b2d_resolve_frame_bytes(r, factor, B2D_RESOLVE_RGB8, &frame_bytes) != B2D_OK) return fail("resolve");
-    void *d_poses = nullptr, *d_index = nullptr, *d_rgb = nullptr;
+    void *d_poses = nullptr, *d_index = nullptr, *d_rgb = nullptr, *d_seen = nullptr;
     struct Bufs {
         int device;
-        void **p[3];
+        void **p[4];
         ~Bufs() { for (void **q : p) if (*q) b2d_device_free(device, *q); }
-    } owner{device, {&d_poses, &d_index, &d_rgb}};
+    } owner{device, {&d_poses, &d_index, &d_rgb, &d_seen}};
     if (b2d_device_alloc(device, sizeof(b2d_pose) * n, &d_poses) != B2D_OK || b2d_device_alloc(device, npix * n, &d_index) != B2D_OK ||
         b2d_device_alloc(device, frame_bytes * n, &d_rgb) != B2D_OK)
         return fail("device memory");
     if (b2d_device_upload(device, d_poses, poses.data(), sizeof(b2d_pose) * n) != B2D_OK) return fail("upload");
+    if (seen) {
+        if (b2d_device_alloc(device, seen->size() * sizeof(uint32_t), &d_seen) != B2D_OK) return fail("device memory");
+        if (b2d_device_upload(device, d_seen, seen->data(), seen->size() * sizeof(uint32_t)) != B2D_OK) return fail("upload");
+    }
     uint8_t *di = static_cast<uint8_t *>(d_index);
-    if (b2d_automap_device(r, static_cast<const b2d_pose *>(d_poses), levels, n, scale_q16, flags, di, nullptr) != B2D_OK)
-        return fail("automap");
+    const b2d_pose *dp = static_cast<const b2d_pose *>(d_poses);
+    const int rc = seen || (flags & B2D_AUTOMAP_ALLMAP)
+                       ? b2d_automap_seen_device(r, dp, levels, static_cast<const uint32_t *>(d_seen), n, scale_q16, flags, di, nullptr)
+                       : b2d_automap_device(r, dp, levels, n, scale_q16, flags, di, nullptr);
+    if (rc != B2D_OK) return fail("automap");
     if (b2d_resolve_device(r, di, levels, n, factor, B2D_RESOLVE_RGB8, d_rgb, nullptr) != B2D_OK) return fail("resolve");
     std::vector<uint8_t> rgb(frame_bytes * n);
     if (b2d_device_download(device, rgb.data(), d_rgb, rgb.size()) != B2D_OK) return fail("download");
@@ -149,6 +160,51 @@ int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std:
         std::fclose(f);
     }
     return 0;
+}
+
+// --automap-flags seen: the lines the run's frames saw (b2d_walk_device / b2d_walk_device_levels, then
+// b2d_raster_device_seen in batches of max_batch), OR-ed per level into rows[level * words ..] of n_levels rows
+int run_seen_rows(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, const uint32_t *levels,
+                  size_t n_levels, int max_batch, std::vector<uint32_t> &rows) {
+    uint32_t words = 0;
+    if (b2d_renderer_seen_words(r, &words) != B2D_OK) return fail("seen words");
+    const size_t n = poses.size(), npix = (size_t)view.width * view.height, mb = (size_t)max_batch;
+    void *d_poses = nullptr, *d_index = nullptr, *d_seen = nullptr;
+    struct Bufs {
+        int device;
+        void **p[3];
+        ~Bufs() { for (void **q : p) if (*q) b2d_device_free(device, *q); }
+    } owner{device, {&d_poses, &d_index, &d_seen}};
+    if (b2d_device_alloc(device, sizeof(b2d_pose) * n, &d_poses) != B2D_OK || b2d_device_alloc(device, npix * mb, &d_index) != B2D_OK ||
+        b2d_device_alloc(device, sizeof(uint32_t) * words * mb, &d_seen) != B2D_OK)
+        return fail("device memory");
+    if (b2d_device_upload(device, d_poses, poses.data(), sizeof(b2d_pose) * n) != B2D_OK) return fail("upload");
+    rows.assign(n_levels * words, 0u);
+    std::vector<uint32_t> batch(words * mb);
+    for (size_t i = 0; i < n; i += mb) {
+        const size_t k = std::min(mb, n - i);
+        std::fill(batch.begin(), batch.end(), 0u);
+        if (b2d_device_upload(device, d_seen, batch.data(), batch.size() * sizeof(uint32_t)) != B2D_OK) return fail("upload");
+        const b2d_pose *dp = static_cast<const b2d_pose *>(d_poses) + i;
+        int64_t ticket = -1;
+        const int rc = levels ? b2d_walk_device_levels(r, dp, levels + i, k, nullptr, &ticket) : b2d_walk_device(r, dp, k, nullptr, &ticket);
+        if (rc != B2D_OK) return fail("walk");
+        if (b2d_raster_device_seen(r, ticket, static_cast<uint8_t *>(d_index), static_cast<uint32_t *>(d_seen), nullptr) != B2D_OK)
+            return fail("seen raster");
+        if (b2d_device_download(device, batch.data(), d_seen, sizeof(uint32_t) * words * k) != B2D_OK) return fail("download");
+        for (size_t f = 0; f < k; f++)
+            for (uint32_t w = 0; w < words; w++) rows[(levels ? levels[i + f] : 0u) * words + w] |= batch[f * words + w];
+    }
+    return 0;
+}
+
+// --automap on one level: the automap of the run's first pose, with `seen` of the lines all its poses saw
+int write_run_automap(b2d_renderer *r, const b2d_view &view, const std::vector<b2d_pose> &poses, int max_batch, int32_t scale_q16,
+                      int flags, bool seen, int factor, const std::string &name) {
+    std::vector<uint32_t> rows;
+    if (seen)
+        if (int rc = run_seen_rows(r, 0, view, poses, nullptr, 1, max_batch, rows)) return rc;
+    return write_automaps(r, 0, view, {poses[0]}, nullptr, scale_q16, flags, factor, {name}, seen ? &rows : nullptr);
 }
 
 // the --dump name without its .ppm extension
@@ -207,7 +263,8 @@ int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st
 // --levels: the look-around of every level of `set` from its start, nposes per level, pose i at tic tics + i
 int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
                      const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file,
-                     int supersample, int palette, b2d_frame_light light, int32_t automap_scale, int automap_flags) {
+                     int supersample, int palette, b2d_frame_light light, int32_t automap_scale, int automap_flags,
+                     bool automap_seen) {
     std::vector<b2d_scene *> scenes;
     struct Scenes {
         std::vector<b2d_scene *> &v;
@@ -300,7 +357,13 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
                 first_levels.push_back((uint32_t)k);
                 names.push_back(stem + ".automap." + std::to_string(set[k]) + ".ppm");
             }
-            if (int rc = write_automaps(r, 0, view, firsts, first_levels.data(), automap_scale, automap_flags, supersample, names)) return rc;
+            std::vector<uint32_t> seen;
+            if (automap_seen) {
+                if (int rc = run_seen_rows(r, 0, view, poses, levels.data(), set.size(), n < 64 ? (int)n : 64, seen)) return rc;
+            }
+            if (int rc = write_automaps(r, 0, view, firsts, first_levels.data(), automap_scale, automap_flags, supersample, names,
+                                        automap_seen ? &seen : nullptr))
+                return rc;
         }
     }
     if (!stream.empty()) {
@@ -319,6 +382,7 @@ int main(int argc, char **argv) {
     int level = 0, width = 1280, height = 720, nposes = 1, rank = 0, world = 0, chunk = 16, supersample = 1, palette = 0;
     int32_t automap_scale = 0;        // 0: no --automap
     int automap_flags = 0;
+    bool automap_seen = false;        // --automap-flags seen: the automap shows the lines the run's frames saw
     b2d_frame_light light{-1, 0};
     double fov = 65.0;
     unsigned long tics = 0;
@@ -385,7 +449,9 @@ int main(int argc, char **argv) {
                 if (name == "rotate") automap_flags |= B2D_AUTOMAP_ROTATE;
                 else if (name == "all") automap_flags |= B2D_AUTOMAP_ALL_LINES;
                 else if (name == "things") automap_flags |= B2D_AUTOMAP_THINGS;
-                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things\n"); return 2; }
+                else if (name == "allmap") automap_flags |= B2D_AUTOMAP_ALLMAP;
+                else if (name == "seen") automap_seen = true;
+                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things, allmap, seen\n"); return 2; }
                 at = comma + 1;
             }
         }
@@ -437,7 +503,7 @@ int main(int argc, char **argv) {
             return 2;
         }
         const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file,
-                                        supersample, palette, light, automap_scale, automap_flags);
+                                        supersample, palette, light, automap_scale, automap_flags, automap_seen);
         b2d_archive_close(arch);
         return rc;
     }
@@ -472,8 +538,8 @@ int main(int argc, char **argv) {
             std::fclose(f);
         }
         if (automap_scale && !dump.empty())
-            if (int rc = write_automaps(r, 0, view, {poses[0]}, nullptr, automap_scale, automap_flags, supersample,
-                                        {dump_stem(dump) + ".automap.ppm"}))
+            if (int rc = write_run_automap(r, view, poses, nposes < 64 ? nposes : 64, automap_scale, automap_flags, automap_seen,
+                                           supersample, dump_stem(dump) + ".automap.ppm"))
                 return rc;
         if (!stream.empty()) {
             std::FILE *f = std::fopen(stream.c_str(), "wb");
@@ -514,7 +580,8 @@ int main(int argc, char **argv) {
         std::fclose(f);
     }
     if (automap_scale && !dump.empty())
-        if (int rc = write_automaps(r, 0, view, {poses[0]}, nullptr, automap_scale, automap_flags, 1, {dump_stem(dump) + ".automap.ppm"}))
+        if (int rc = write_run_automap(r, view, poses, nposes < 64 ? nposes : 64, automap_scale, automap_flags, automap_seen, 1,
+                                       dump_stem(dump) + ".automap.ppm"))
             return rc;
     if (!stream.empty()) {
         std::FILE *f = std::fopen(stream.c_str(), "wb");

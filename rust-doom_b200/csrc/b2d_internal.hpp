@@ -71,7 +71,9 @@ int check_slots_free(const b2d_renderer *r, size_t batches);
 // ticket (b2d_walk_device* / b2d_raster_device); neither is synchronised.
 int walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &frames, int n, cudaStream_t stream, bool background,
                int64_t *ticket_out);
-int raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream);
+// `seen`: the seen variant (b2d_raster_device_seen; index frames only), else nullptr
+int raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
+                 const SeenTables *seen = nullptr);
 
 // Owners of CUDA resources.  They release on the current device: ~b2d_renderer and b2d_comm_destroy select theirs first.
 struct DeviceFree { void operator()(void *p) const { cudaFree(p); } };
@@ -210,6 +212,9 @@ struct LevelRes {
     // blob's sprites.  Uploaded by the first b2d_automap_device call (b2d_renderer::automap).
     std::vector<AutomapLine> automap_lines;
     std::vector<int32_t> automap_things;
+    // Seen lines (DESIGN.md C20): the linedef of each seg of the level's SEGS lump (-1: none), built at creation and
+    // uploaded by the first b2d_raster_device_seen call (b2d_renderer::seen)
+    std::vector<int32_t> seg_line;
 };
 
 struct b2d_renderer {
@@ -248,6 +253,17 @@ struct b2d_renderer {
     };
     std::unique_ptr<Automap> automap;
     LevelStaging automap_levels;
+    // The seg -> linedef tables of every level on the device, created whole by the first b2d_raster_device_seen call:
+    // the tables one after the other, then each level's offset into them (at d_off), uploaded from the pinned copy `h`
+    // on that call's stream; `built` follows the upload.  `seen_words`: the length of a row of seen lines.
+    struct Seen {
+        DeviceBuf<int32_t> d;
+        PinnedBuf<int32_t> h;
+        size_t d_off = 0;
+        Event built;
+    };
+    std::unique_ptr<Seen> seen;
+    uint32_t seen_words = 1;
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;
     bool profiling = false;

@@ -16,6 +16,8 @@
 //
 // There is no dense contraction anywhere on this path, so no tensor-core (wgmma) work: the
 // kernels are integer/LSU/latency bound and are tuned against the HBM write roofline (DESIGN.md).
+#include <type_traits>
+
 #include "b2d_kernels.cuh"
 
 namespace b2d {
@@ -908,17 +910,28 @@ __device__ __forceinline__ bool queue_push(const DrawQueue &q, int lane, uint32_
     return true;
 }
 
-// `Fixed`: empty, or FixedTables -- the fixed-colormap variant (kFixed, DESIGN.md C18; per-frame levels and states only),
-// whose frames may have a fixed colormap and which alone takes the appended parameter `fx`.  An empty pack leaves the
-// other variants' names, parameters and code as they are.
-template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels, typename... Fixed>
+// the element of type T of a raster variant's appended tables
+template <typename T, typename A, typename... P>
+__device__ __forceinline__ const T &extra_tables(const A &a, const P &...p) {
+    if constexpr (std::is_same_v<T, A>) return a;
+    else return extra_tables<T>(p...);
+}
+
+// `Extra`: the variant's appended tables, each appended as a parameter of `fx` -- FixedTables for the fixed-colormap
+// variant (kFixed, DESIGN.md C18; per-frame levels and states only), whose frames may have a fixed colormap, then
+// SeenTables for the seen variant (kSeen, DESIGN.md C20; index frames only), which marks the lines each frame sees.  An
+// empty pack leaves the other variants' names, parameters and code as they are.
+template <bool kRgba, int kW, bool kMasked, bool kStates, bool kLevels, typename... Extra>
 __global__ void __launch_bounds__(32 * kRasterWarps, 16 / kRasterWarps)
 b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant__ View vw, const FrameConst *__restrict__ frames,
                   const SegFrame *__restrict__ work, int stride, int n, int strips,
                   uint8_t *__restrict__ index_fb, uint32_t *__restrict__ rgba_fb, const __grid_constant__ LevelTables lt,
-                  const Fixed... fx) {
-    constexpr bool kFixed = sizeof...(Fixed) != 0;
-    static_assert(!kFixed || (kStates && kLevels && sizeof...(Fixed) == 1), "fixed colormaps come with per-frame levels and states");
+                  const Extra... fx) {
+    constexpr bool kFixed = (std::is_same_v<Extra, FixedTables> || ...);
+    constexpr bool kSeen = (std::is_same_v<Extra, SeenTables> || ...);
+    static_assert(sizeof...(Extra) == (int)kFixed + (int)kSeen, "appended tables: FixedTables, SeenTables, each at most once");
+    static_assert(!kFixed || (kStates && kLevels), "fixed colormaps come with per-frame levels and states");
+    static_assert(!kSeen || !kRgba, "the seen variant draws index frames only");
     // per-frame levels: a palette per warp (the warps of a CTA may draw frames of levels from different WADs)
     __shared__ uint32_t s_pal[kRgba ? (kLevels ? 256 * kRasterWarps : 256) : 1];
     __shared__ uint2 s_rowz[kRasterWarps][32];
@@ -984,7 +997,7 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     }
     if constexpr (kFixed) {
         if (has_strip && lane == 0) {
-            const FixedTables &t = (fx, ...);       // the one element of the pack
+            const FixedTables &t = extra_tables<FixedTables>(fx...);
             const FixedPlanes p = t.planes[(uint32_t)fc.level];
             s_fix[warp] = FixedWarp{p.texels, p.flats, t.frame_fixed[frame]};
         }
@@ -1017,6 +1030,15 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
     const int count = fc.count;
     const uint32_t owner = (uint32_t)warp << 18;
     bool done = false;
+    // the seen variant: this frame's row of seen lines and its level's seg -> linedef table (lane 0 marks)
+    uint32_t *seen_row = nullptr;
+    const int32_t *seen_line = nullptr;
+    int32_t seen_last = -1;
+    if constexpr (kSeen) {
+        const SeenTables &st = extra_tables<SeenTables>(fx...);
+        seen_row = st.rows + (size_t)frame * st.words;
+        seen_line = st.seg_line + st.level_off[kLevels ? (uint32_t)fc.level : 0u];
+    }
 
     for (int k0 = 0; k0 < count && !done; k0 += 32) {
         int k = k0 + lane;
@@ -1047,6 +1069,17 @@ b2d_raster_kernel(const __grid_constant__ DeviceScene sc, const __grid_constant_
             ColumnEval ce = {0u, 1, 1, 0};
             bool ok = in && column_eval(sf, vw, x, ce);
             if (!__any_sync(kFull, ok)) continue;
+            if constexpr (kSeen) {
+                // C20: the seg owns a column of the frame.  Consecutive entries are often segs of one linedef: a warp
+                // marks a linedef once per run.
+                if (lane == 0) {
+                    const int32_t l = __ldg(seen_line + sf.seg);
+                    if (l >= 0 && l != seen_last) {
+                        atomicOr(seen_row + (l >> 5), 1u << (l & 31));
+                        seen_last = l;
+                    }
+                }
+            }
 
             const SegRec S = ts.segs[sf.seg];
             const SectorRec SF = ts.sectors[S.front];
@@ -1517,6 +1550,39 @@ static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, 
     return cudaGetLastError();
 }
 
+// The seen variant of raster_go (index frames only): FixedTables, when the batch has fixed colormaps, then SeenTables.
+template <bool kStates, bool kLevels, bool kFixed>
+static cudaError_t raster_seen_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
+                                  const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, const SeenTables &seen,
+                                  cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    const int strips = (vw.W + 31) / 32;
+    const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
+#define B2D_SEEN_GO(KW, MASKED) do { \
+    if constexpr (kFixed) \
+        b2d_raster_kernel<false, KW, MASKED, true, true, FixedTables, SeenTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, nullptr, t.levels, t.fixed, seen); \
+    else \
+        b2d_raster_kernel<false, KW, MASKED, kStates, kLevels, SeenTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, nullptr, t.levels, seen); \
+    } while (0)
+#define B2D_SEEN_W(KW) do { if (masked) B2D_SEEN_GO(KW, true); else B2D_SEEN_GO(KW, false); } while (0)
+    if (vw.W == 1920) B2D_SEEN_W(1920);
+    else if (vw.W == 3840) B2D_SEEN_W(3840);
+    else B2D_SEEN_W(0);
+#undef B2D_SEEN_W
+#undef B2D_SEEN_GO
+    return cudaGetLastError();
+}
+
+cudaError_t launch_raster_seen(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
+                               const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, const SeenTables &seen,
+                               cudaStream_t stream) {
+    if (t.fixed_rows && !(t.per_level && t.per_frame)) return cudaErrorInvalidValue;
+    auto go = t.per_level ? (t.per_frame ? (t.fixed_rows ? raster_seen_go<true, true, true> : raster_seen_go<true, true, false>)
+                                         : raster_seen_go<false, true, false>)
+                          : (t.per_frame ? raster_seen_go<true, false, false> : raster_seen_go<false, false, false>);
+    return go(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, seen, stream);
+}
+
 // Per-frame states take the kStates variant of each shape; the frames are the same pixel for pixel.  A batch of per-frame
 // levels and states with a fixed colormap takes the kFixed variant.
 cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
@@ -1777,6 +1843,51 @@ b2d_automap_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__re
         }
     }
 }
+
+// Kernel 5's seen variant (b2d_automap_seen_device, C20): the same tiles, with each line coloured by its frame's row of
+// seen lines (`seen` + frame * words; nullptr: every line mapped) and B2D_AUTOMAP_ALLMAP.  A kernel of its own, so that
+// K5's code stays as it is.
+__global__ void __launch_bounds__(256)
+b2d_automap_seen_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level,
+                        const Pose *__restrict__ poses, View vw, int32_t scale, int flags, uint8_t *__restrict__ out,
+                        int tiles_x, int tiles, bool vec, const uint32_t *__restrict__ seen, uint32_t words) {
+    __shared__ uint32_t keys[kAutomapTileH * kAutomapTileW];
+    const size_t frame = blockIdx.x / tiles;
+    const int tile = blockIdx.x - (int)(frame * tiles);
+    const int tx0 = (tile % tiles_x) * kAutomapTileW, ty0 = (tile / tiles_x) * kAutomapTileH;
+    const int tx1 = min(tx0 + kAutomapTileW, vw.W), ty1 = min(ty0 + kAutomapTileH, vw.H);
+    for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) keys[k] = 0;
+    const AutomapLevel L = levels[frame_level ? frame_level[frame] : 0];
+    const AutomapFrame f = automap_frame(poses[frame], vw, scale, flags);
+    const uint32_t *mapped = seen ? seen + frame * words : nullptr;
+    __syncthreads();
+    const int n = automap_items(L, flags);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        int64_t e[4];
+        const uint32_t colour = automap_seen_item(f, L, mapped, flags, i, e);
+        if (!colour) continue;
+        const uint32_t key = ((uint32_t)(i + 1) << 8) | colour;
+        automap_line(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1,
+                     [&](int32_t x, int32_t y) { atomicMax(&keys[(y - ty0) * kAutomapTileW + (x - tx0)], key); });
+    }
+    __syncthreads();
+    uint8_t *dst = out + frame * (size_t)vw.W * vw.H;
+    if (vec && tx1 - tx0 == kAutomapTileW) {
+        const int r = threadIdx.x >> 3, c = (threadIdx.x & 7) * 16;
+        if (ty0 + r < ty1) {
+            const uint32_t *k = &keys[r * kAutomapTileW + c];
+            uint32_t w[4];
+            for (int q = 0; q < 4; q++)
+                w[q] = (k[4 * q] & 0xFF) | (k[4 * q + 1] & 0xFF) << 8 | (k[4 * q + 2] & 0xFF) << 16 | (k[4 * q + 3] & 0xFF) << 24;
+            *reinterpret_cast<uint4 *>(dst + (size_t)(ty0 + r) * vw.W + tx0 + c) = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+    } else {
+        for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) {
+            const int x = tx0 + (k % kAutomapTileW), y = ty0 + k / kAutomapTileW;
+            if (x < tx1 && y < ty1) dst[(size_t)y * vw.W + x] = (uint8_t)keys[k];
+        }
+    }
+}
 }  // namespace
 
 size_t automap_tiles(const View &vw) {
@@ -1792,6 +1903,19 @@ cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame
     const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
     b2d_automap_kernel<<<(unsigned)(n_frames * tiles), 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags, d_out,
                                                                          tiles_x, tiles, vec);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_automap_seen(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
+                                const View &vw, int32_t scale, int flags, const uint32_t *d_seen, uint32_t words, uint8_t *d_out,
+                                cudaStream_t stream) {
+    if (n_frames == 0) return cudaSuccess;
+    const int tiles_x = (vw.W + kAutomapTileW - 1) / kAutomapTileW;
+    const int tiles = (int)automap_tiles(vw);
+    if (n_frames * (size_t)tiles > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
+    b2d_automap_seen_kernel<<<(unsigned)(n_frames * tiles), 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags,
+                                                                              d_out, tiles_x, tiles, vec, d_seen, words);
     return cudaGetLastError();
 }
 

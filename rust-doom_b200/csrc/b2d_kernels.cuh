@@ -87,6 +87,16 @@ struct FixedTables {
     const FixedPlanes *planes;   // per level
 };
 
+// Seen lines (b2d_raster_device_seen, DESIGN.md C20): the seen raster variant ORs bit l & 31 of word l >> 5 of row f of
+// `rows` (`words` words per row) for every linedef l of which a seg owns a column of frame f in the solid pass.
+// seg_line + level_off[level] is the level's seg -> linedef table (-1: no linedef).
+struct SeenTables {
+    uint32_t *rows;
+    const int32_t *seg_line;
+    const uint32_t *level_off;
+    uint32_t words;
+};
+
 // Bytes of dynamic shared memory the BSP-walk kernel needs per frame (= per CTA) for this scene.
 size_t walk_smem_per_warp(const DeviceScene &sc);
 // Static shared memory of the per-frame-level walk (its copy of the resident level's DeviceScene and the barrier words):
@@ -116,6 +126,10 @@ cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw
 // `masked`: some level the frames read has masked content (its masked_list is set).
 cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
                           int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream);
+// ... its seen variant: the same index frames (no RGBA), and each frame's seen lines OR-ed into its row of seen.rows.
+cudaError_t launch_raster_seen(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
+                               const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, const SeenTables &seen,
+                               cudaStream_t stream);
 
 // Expands the `nsets` table sets of a batch in one grid: set k by the rule of level sets[k].level (srcs[level]: device
 // pointers to that level's rest-state sections) into the tables of out[k].  `records`: the records of all sets together
@@ -154,5 +168,9 @@ size_t automap_tiles(const View &vw);
 // levels[frame_level[f]] (d_frame_level NULL: level 0), `scale` and `flags` as checked by b2d_automap_device.
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
                            const View &vw, int32_t scale, int flags, uint8_t *d_out, cudaStream_t stream);
+// ... its seen variant (C20): frame f's lines coloured by row f of d_seen (`words` per row; nullptr: every line mapped).
+cudaError_t launch_automap_seen(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
+                                const View &vw, int32_t scale, int flags, const uint32_t *d_seen, uint32_t words, uint8_t *d_out,
+                                cudaStream_t stream);
 
 }  // namespace b2d

@@ -562,13 +562,19 @@ constexpr int32_t kAutomapScaleMin = 1 << 8, kAutomapScaleMax = 64 << 16;
 constexpr uint32_t kAutomapArrowColour = 209, kAutomapThingColour = 112;
 constexpr int32_t kAutomapArrowR = 8 * 16 * 65536 / 7;      // player_arrow's R: 8 * PLAYERRADIUS / 7, 16.16
 constexpr int kAutomapArrowSegs = 7, kAutomapThingSegs = 3;
+// The seen automap (b2d_automap_seen_device, C20): B2D_AUTOMAP_ALLMAP, the computer area map's grey (GRAYS + 3), and the
+// device line table's don't-draw bit.
+constexpr int kAutomapAllmap = 8;
+constexpr uint32_t kAutomapAllmapColour = 99;
+constexpr uint16_t kAutomapDontDraw = 1;
 
 // One linedef of a level's automap table (b2d_automap_line): endpoints in map units, the colour drawn normally and under
-// kAutomapAllLines (0: not drawn), and the linedef's index.
+// kAutomapAllLines (0: not drawn), and the linedef's index.  `dev_flags` is 0 in the scene's table; the renderer's device
+// copy sets kAutomapDontDraw for an ML_DONTDRAW linedef (the seen automap's computer-area-map rule, C20).
 struct AutomapLine {
     int32_t x0, y0, x1, y1;
     uint8_t colour, colour_all;
-    uint16_t pad;
+    uint16_t dev_flags;
     int32_t linedef;
 };
 static_assert(sizeof(AutomapLine) == 24, "AutomapLine");
@@ -647,6 +653,25 @@ B2D_HD uint32_t automap_item(const AutomapFrame &f, const AutomapLevel &L, int f
     automap_map(f, tx + ax, ty + ay, e[0], e[1]);
     automap_map(f, tx + bx, ty + by, e[2], e[3]);
     return kAutomapThingColour;
+}
+
+// AM_drawWalls with mapped lines (C20): under kAutomapAllLines a line's all-lines colour, mapped or not; otherwise a mapped
+// line's normal colour (0: not drawn); otherwise, under kAutomapAllmap, grey 99 unless the line is ML_DONTDRAW; else 0.
+B2D_HD uint32_t automap_seen_colour(const AutomapLine &l, bool mapped, int flags) {
+    if (flags & kAutomapAllLines) return l.colour_all;
+    if (mapped) return l.colour;
+    if ((flags & kAutomapAllmap) && !(l.dev_flags & kAutomapDontDraw)) return kAutomapAllmapColour;
+    return 0;
+}
+// Item i as automap_item draws it, with the lines coloured by automap_seen_colour: `mapped` is the frame's row of seen
+// lines (bit l & 31 of word l >> 5 for linedef l), nullptr for every line mapped.
+B2D_HD uint32_t automap_seen_item(const AutomapFrame &f, const AutomapLevel &L, const uint32_t *mapped, int flags, int i,
+                                  int64_t e[4]) {
+    const uint32_t colour = automap_item(f, L, flags & ~kAutomapAllmap, i, e);
+    if (i >= L.nlines) return colour;
+    const AutomapLine &l = L.lines[i];
+    const uint32_t ld = (uint32_t)l.linedef;
+    return automap_seen_colour(l, mapped == nullptr || ((mapped[ld >> 5] >> (ld & 31)) & 1u), flags);
 }
 
 // The pixels of the line (X0, Y0) - (X1, Y1) (Q8, |X|, |Y| < 2^31) inside the pixel rectangle [x0, x1) x [y0, y1), each
