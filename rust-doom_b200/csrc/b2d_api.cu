@@ -280,6 +280,14 @@ void state_at(const LevelRes &lv, uint32_t tics, uint32_t *out) {
     std::copy(lv.state.begin() + 1, lv.state.begin() + 2 + 2 * (ptrdiff_t)lv.layout.dyn_sectors.size(), out + 1);
 }
 
+// Per-frame levels (HOST, nullable = level 0): each below the renderer's number of levels; B2D_ERR_INVALID_ARG otherwise.
+int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
+    if (levels)
+        for (size_t i = 0; i < n; i++)
+            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    return B2D_OK;
+}
+
 // Per-frame palettes (HOST, nullable = palette 0): frame i's palette below the palette count of its level (levels[i],
 // nullable = level 0), the levels already checked; B2D_ERR_INVALID_ARG otherwise.
 int check_palettes(const b2d_renderer *r, const uint32_t *levels, const uint32_t *palettes, size_t n) {
@@ -297,8 +305,7 @@ int b2d::CallFrames::prepare(const b2d_renderer *r, size_t n) {
         if (!levels) return fail(B2D_ERR_INVALID_ARG, "null level array");
         if (r->walk_smem + walk_levels_static_smem() > kWalkSmemMax)
             return fail(B2D_ERR_INVALID_ARG, "level too large for the per-frame-level BSP-walk kernel's shared memory");
-        for (size_t i = 0; i < n; i++)
-            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+        if (int rc = check_levels(r, levels, n)) return rc;
     }
     if (int rc = check_palettes(r, levels, palettes, n)) return rc;
     if (lights) {
@@ -524,11 +531,59 @@ int b2d::walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &fr, int 
     return B2D_OK;
 }
 
+// Creates the table group `g` whole (or not at all): `bytes` of device memory and of pinned memory, whose image
+// lay_out(h, d) writes (d: the device copy, which pointers in the image point into), uploaded on `st`; `built` follows the
+// upload.  `off`: where the image's per-level records start.
+template <typename LayOut>
+static int build_tables(std::unique_ptr<b2d_renderer::Tables> &g, size_t bytes, size_t off, cudaStream_t st, LayOut lay_out) {
+    auto a = std::make_unique<b2d_renderer::Tables>();
+    CU(allocate(a->d, bytes));
+    CU(allocate(a->h, bytes));
+    CU(event_create(a->built));
+    lay_out(a->h.get(), a->d.get());
+    a->off = off;
+    CU(cudaMemcpyAsync(a->d.get(), a->h.get(), bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(a->built.get(), st));
+    g = std::move(a);
+    return B2D_OK;
+}
+
+// The table group `g` of r for work enqueued on `st`: a wait for the first call's upload, or, at the first call,
+// build(r, st), which creates it with its upload on `st`.
+static int tables_on(b2d_renderer *r, const std::unique_ptr<b2d_renderer::Tables> &g, cudaStream_t st,
+                     int (*build)(b2d_renderer *, cudaStream_t)) {
+    if (!g) return guarded([&] { return build(r, st); });
+    CU(cudaStreamWaitEvent(st, g->built.get(), 0));
+    return B2D_OK;
+}
+
+// The seg -> linedef tables of every level (b2d_renderer::seen): the tables one after the other, then each level's
+// offset into them.
+static int ensure_seen(b2d_renderer *r, cudaStream_t st) {
+    std::vector<int32_t> words;
+    std::vector<uint32_t> off;
+    for (const LevelRes &lv : r->lv) {
+        off.push_back((uint32_t)words.size());
+        words.insert(words.end(), lv.seg_line.begin(), lv.seg_line.end());
+    }
+    const size_t tables = words.size() * sizeof(int32_t);
+    for (uint32_t o : off) words.push_back((int32_t)o);
+    const size_t bytes = words.size() * sizeof(int32_t);
+    return build_tables(r->seen, bytes, tables, st, [&](uint8_t *h, const uint8_t *) { std::memcpy(h, words.data(), bytes); });
+}
+
 int b2d::raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
-                      const SeenTables *seen) {
+                      uint32_t *d_seen) {
     const int slot = (int)(ticket & 1);
     WorkSlot &s = r->slot[slot];
     if (ticket < 0 || s.ticket != ticket || s.rastered) return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
+    SeenTables seen{};
+    if (d_seen) {
+        if (int rc = tables_on(r, r->seen, stream, ensure_seen)) return rc;
+        const uint8_t *d = r->seen->d.get();
+        seen = SeenTables{d_seen, reinterpret_cast<const int32_t *>(d), reinterpret_cast<const uint32_t *>(d + r->seen->off),
+                          r->seen_words};
+    }
     CU(cudaStreamWaitEvent(stream, s.walk_done.get(), 0));
     if (r->d_masked) {
         // one arena of deferred masked entries per renderer: rasters that use it run one after the other (each fills the
@@ -539,8 +594,8 @@ int b2d::raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_
     // masked content in a level the frames read: with per-frame levels, any level's
     const bool masked = r->d_masked && (s.tables.per_level || s.tables.scene.masked_list);
     const int rc = profiled(r, stream, 1, [&] {
-        return seen ? launch_raster_seen(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, *seen, stream)
-                    : launch_raster(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba, stream);
+        return launch_raster(s.tables, masked, r->view, s.frames.get(), s.work.get(), r->stride, s.n, d_index, d_rgba,
+                             d_seen ? &seen : nullptr, stream);
     });
     if (rc != B2D_OK) return rc;
     CU(cudaEventRecord(s.raster_done.get(), stream));
@@ -1425,8 +1480,7 @@ int b2d_palette_lut_device(b2d_renderer *r, const uint8_t *d_index, uint32_t *d_
 int b2d_palette_lut_levels_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *levels, size_t n_frames, uint32_t *d_rgba,
                                   void *cuda_stream) {
     if (!r || !d_index || !levels || !d_rgba) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    for (size_t i = 0; i < n_frames; i++)
-        if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    if (int rc = check_levels(r, levels, n_frames)) return rc;
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
@@ -1457,9 +1511,7 @@ int b2d_resolve_palettes_device(b2d_renderer *r, const uint8_t *d_index, const u
                                 size_t n_frames, int factor, int format, void *d_out, void *cuda_stream) {
     if (!r || !d_index || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (int rc = check_resolve(r, factor, format)) return rc;
-    if (levels)
-        for (size_t i = 0; i < n_frames; i++)
-            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    if (int rc = check_levels(r, levels, n_frames)) return rc;
     if (int rc = check_palettes(r, levels, palettes, n_frames)) return rc;
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
@@ -1479,11 +1531,9 @@ int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *
     return b2d_resolve_palettes_device(r, d_index, levels, nullptr, n_frames, factor, format, d_out, cuda_stream);
 }
 
-// The automap tables of every level on the device, created whole (or not at all) by the first automap call and uploaded
-// on its stream `st`: the lines and things of each level in one buffer, then an AutomapLevel per level pointing into it,
-// copied from pinned memory the group keeps.  `built` follows the copies; every later call waits for it on its own stream.
+// The automap tables of every level (b2d_renderer::automap): the lines and things of each level in one buffer, then an
+// AutomapLevel per level pointing into it.
 static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
-    auto a = std::make_unique<b2d_renderer::Automap>();
     size_t items = 0;
     std::vector<size_t> line_off, thing_off;
     for (const LevelRes &lv : r->lv) {
@@ -1493,48 +1543,16 @@ static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
         items += lv.automap_things.size() * sizeof(int32_t);
     }
     items = (items + 15) & ~(size_t)15;                   // the AutomapLevel records follow, aligned
-    const size_t bytes = items + r->lv.size() * sizeof(AutomapLevel);
-    CU(allocate(a->d, bytes));
-    CU(allocate(a->h, bytes));
-    CU(event_create(a->built));
-    uint8_t *h = a->h.get(), *d = a->d.get();
-    std::vector<AutomapLevel> levels(r->lv.size());
-    for (size_t k = 0; k < r->lv.size(); k++) {
-        const LevelRes &lv = r->lv[k];
-        if (!lv.automap_lines.empty()) std::memcpy(h + line_off[k], lv.automap_lines.data(), lv.automap_lines.size() * sizeof(AutomapLine));
-        if (!lv.automap_things.empty()) std::memcpy(h + thing_off[k], lv.automap_things.data(), lv.automap_things.size() * sizeof(int32_t));
-        const AutomapLevel L{reinterpret_cast<const AutomapLine *>(d + line_off[k]), reinterpret_cast<const int32_t *>(d + thing_off[k]),
-                             (int32_t)lv.automap_lines.size(), (int32_t)(lv.automap_things.size() / 2)};
-        std::memcpy(h + items + k * sizeof(AutomapLevel), &L, sizeof L);
-    }
-    a->d_levels_off = items;
-    CU(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(a->built.get(), st));
-    r->automap = std::move(a);
-    return B2D_OK;
-}
-
-// The seg -> linedef tables of every level on the device, created whole (or not at all) by the first seen raster and
-// uploaded on its stream `st` from pinned memory the group keeps: the tables one after the other, then each level's offset
-// into them.  `built` follows the copy; every later call waits for it on its own stream.
-static int ensure_seen(b2d_renderer *r, cudaStream_t st) {
-    auto a = std::make_unique<b2d_renderer::Seen>();
-    std::vector<int32_t> words;
-    std::vector<uint32_t> off;
-    for (const LevelRes &lv : r->lv) {
-        off.push_back((uint32_t)words.size());
-        words.insert(words.end(), lv.seg_line.begin(), lv.seg_line.end());
-    }
-    a->d_off = words.size();
-    for (uint32_t o : off) words.push_back((int32_t)o);
-    CU(allocate(a->d, words.size() * sizeof(int32_t)));
-    CU(allocate(a->h, words.size() * sizeof(int32_t)));
-    CU(event_create(a->built));
-    std::memcpy(a->h.get(), words.data(), words.size() * sizeof(int32_t));
-    CU(cudaMemcpyAsync(a->d.get(), a->h.get(), words.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(a->built.get(), st));
-    r->seen = std::move(a);
-    return B2D_OK;
+    return build_tables(r->automap, items + r->lv.size() * sizeof(AutomapLevel), items, st, [&](uint8_t *h, const uint8_t *d) {
+        for (size_t k = 0; k < r->lv.size(); k++) {
+            const LevelRes &lv = r->lv[k];
+            if (!lv.automap_lines.empty()) std::memcpy(h + line_off[k], lv.automap_lines.data(), lv.automap_lines.size() * sizeof(AutomapLine));
+            if (!lv.automap_things.empty()) std::memcpy(h + thing_off[k], lv.automap_things.data(), lv.automap_things.size() * sizeof(int32_t));
+            const AutomapLevel L{reinterpret_cast<const AutomapLine *>(d + line_off[k]), reinterpret_cast<const int32_t *>(d + thing_off[k]),
+                                 (int32_t)lv.automap_lines.size(), (int32_t)(lv.automap_things.size() / 2)};
+            std::memcpy(h + items + k * sizeof(AutomapLevel), &L, sizeof L);
+        }
+    });
 }
 
 int b2d_renderer_seen_words(const b2d_renderer *r, uint32_t *words_out) {
@@ -1547,15 +1565,7 @@ int b2d_raster_device_seen(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb,
     if (!r || !d_index_fb || !d_seen) return fail(B2D_ERR_INVALID_ARG, "null argument");
     if (reinterpret_cast<uintptr_t>(d_seen) & 3) return fail(B2D_ERR_INVALID_ARG, "seen rows not 4-byte aligned");
     CU(cudaSetDevice(r->device));
-    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    const int slot = (int)(ticket & 1);
-    if (ticket < 0 || r->slot[slot].ticket != ticket || r->slot[slot].rastered)
-        return fail(B2D_ERR_INVALID_ARG, "unknown or already rastered walk ticket");
-    if (r->seen) CU(cudaStreamWaitEvent(st, r->seen->built.get(), 0));      // the first call's upload
-    else if (int rc = guarded([&] { return ensure_seen(r, st); })) return rc;
-    const SeenTables seen{d_seen, r->seen->d.get(), reinterpret_cast<const uint32_t *>(r->seen->d.get() + r->seen->d_off),
-                          r->seen_words};
-    return raster_batch(r, ticket, d_index_fb, nullptr, st, &seen);
+    return raster_batch(r, ticket, d_index_fb, nullptr, static_cast<cudaStream_t>(cuda_stream), d_seen);
 }
 
 // b2d_automap_device (seen_variant false: K5) and b2d_automap_seen_device (its seen variant, which also takes ALLMAP)
@@ -1567,9 +1577,7 @@ static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t
     if (reinterpret_cast<uintptr_t>(d_seen) & 3) return fail(B2D_ERR_INVALID_ARG, "seen rows not 4-byte aligned");
     if (scale_q16 < kAutomapScaleMin || scale_q16 > kAutomapScaleMax)
         return fail(B2D_ERR_INVALID_ARG, "automap scale out of range (256 .. 64 << 16, 16.16 pixels per map unit)");
-    if (levels)
-        for (size_t i = 0; i < n_frames; i++)
-            if (levels[i] >= r->lv.size()) return fail(B2D_ERR_INVALID_ARG, "frame level out of range (>= the renderer's number of levels)");
+    if (int rc = check_levels(r, levels, n_frames)) return rc;
     for (const LevelRes &lv : r->lv)      // the key of an item is (item + 1) << 8 | colour
         if (lv.automap_lines.size() + kAutomapArrowSegs + kAutomapThingSegs * lv.automap_things.size() / 2 >= (1u << 24))
             return fail(B2D_ERR_INVALID_ARG, "level has too many automap items (2^24)");
@@ -1577,18 +1585,13 @@ static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    if (r->automap) CU(cudaStreamWaitEvent(st, r->automap->built.get(), 0));      // the first call's upload
-    else if (int rc = guarded([&] { return ensure_automap(r, st); })) return rc;
+    if (int rc = tables_on(r, r->automap, st, ensure_automap)) return rc;
     if (levels)
         if (int rc = stage_words(r->automap_levels, n_frames, st, [&](size_t i) { return levels[i]; })) return rc;
-    const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->d_levels_off);
+    const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->off);
     const uint32_t *d_frame_level = levels ? r->automap_levels.d.get() : nullptr;
-    if (seen_variant)
-        CU(launch_automap_seen(d_levels, d_frame_level, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16,
-                               flags, d_seen, r->seen_words, d_out, st));
-    else
-        CU(launch_automap(d_levels, d_frame_level, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16, flags,
-                          d_out, st));
+    CU(launch_automap(d_levels, d_frame_level, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16, flags,
+                      seen_variant, d_seen, r->seen_words, d_out, st));
     if (levels) CU(cudaEventRecord(r->automap_levels.done.get(), st));
     r->launches += 1;
     return B2D_OK;

@@ -71,9 +71,9 @@ int check_slots_free(const b2d_renderer *r, size_t batches);
 // ticket (b2d_walk_device* / b2d_raster_device); neither is synchronised.
 int walk_batch(b2d_renderer *r, const Pose *d_poses, const Frames &frames, int n, cudaStream_t stream, bool background,
                int64_t *ticket_out);
-// `seen`: the seen variant (b2d_raster_device_seen; index frames only), else nullptr
+// `d_seen`: the seen variant's rows of seen lines (b2d_raster_device_seen; index frames only), else nullptr
 int raster_batch(b2d_renderer *r, int64_t ticket, uint8_t *d_index, uint32_t *d_rgba, cudaStream_t stream,
-                 const SeenTables *seen = nullptr);
+                 uint32_t *d_seen = nullptr);
 
 // Owners of CUDA resources.  They release on the current device: ~b2d_renderer and b2d_comm_destroy select theirs first.
 struct DeviceFree { void operator()(void *p) const { cudaFree(p); } };
@@ -242,27 +242,22 @@ struct b2d_renderer {
     // the frame tables of a call of b2d_palette_lut_levels_device and of b2d_resolve_device / b2d_resolve_palettes_device,
     // each call kind with its own
     LevelStaging lut_levels, resolve_levels;
-    // The automap tables of every level on the device, created whole by the first b2d_automap_device call: the lines and
-    // things of each level, then one AutomapLevel per level (at d_levels_off) pointing into them, uploaded from the pinned
-    // copy `h` on that call's stream; `built` follows the upload.  With the call's own level staging.
-    struct Automap {
+    // A group of tables of every level on the device, created whole by the first call that reads them: the byte image `d`,
+    // uploaded from its pinned copy `h` on that call's stream (`built` follows the upload; every later call waits for it
+    // on its own stream).  `off`: where the image's per-level records start.
+    struct Tables {
         DeviceBuf<uint8_t> d;
         PinnedBuf<uint8_t> h;
-        size_t d_levels_off = 0;
+        size_t off = 0;
         Event built;
     };
-    std::unique_ptr<Automap> automap;
+    // The automap's (first b2d_automap_device call): the lines and things of each level, then one AutomapLevel per level
+    // pointing into them.  With the call's own level staging.
+    std::unique_ptr<Tables> automap;
     LevelStaging automap_levels;
-    // The seg -> linedef tables of every level on the device, created whole by the first b2d_raster_device_seen call:
-    // the tables one after the other, then each level's offset into them (at d_off), uploaded from the pinned copy `h`
-    // on that call's stream; `built` follows the upload.  `seen_words`: the length of a row of seen lines.
-    struct Seen {
-        DeviceBuf<int32_t> d;
-        PinnedBuf<int32_t> h;
-        size_t d_off = 0;
-        Event built;
-    };
-    std::unique_ptr<Seen> seen;
+    // The seen raster's (first b2d_raster_device_seen call): the seg -> linedef tables one after the other, then each
+    // level's offset into them.  `seen_words`: the length of a row of seen lines.
+    std::unique_ptr<Tables> seen;
     uint32_t seen_words = 1;
     DeviceBuf<uint32_t> d_masked_counter;
     int64_t launches = 0;

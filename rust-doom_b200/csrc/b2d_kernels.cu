@@ -1525,73 +1525,62 @@ cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw
 // although residency falls from 20 to 16 warps per SM.  The CTA's draw queue shares the strips' draws among its warps, so
 // a finished strip's warp draws for its slower siblings instead of idling.  The registers are left to the compiler (cap
 // 128): 94 for the 1080p and 4K index-only kernels, i.e. 2 CTAs = 16 warps per SM (DESIGN.md §5, §6).
-// The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).
-template <bool kStates, bool kLevels, bool kFixed>
+// The frame width is a compile-time constant for the benchmark resolutions (immediate store offsets).  `fx`: the variant's
+// appended tables (b2d_raster_kernel's `Extra`); a seen variant draws index frames only.
+template <bool kStates, bool kLevels, typename... Extra>
 static cudaError_t raster_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
                              const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
-                             cudaStream_t stream) {
+                             cudaStream_t stream, const Extra &...fx) {
+    constexpr bool kSeen = (std::is_same_v<Extra, SeenTables> || ...);
     if (n <= 0) return cudaSuccess;
     const int strips = (vw.W + 31) / 32;
     const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
-#define B2D_RASTER_GO(RGBA, KW) do { \
-    if constexpr (kFixed) { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels, t.fixed); \
-    else b2d_raster_kernel<RGBA, KW, false, true, true, FixedTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels, t.fixed); \
-    } else { \
-    if (masked) b2d_raster_kernel<RGBA, KW, true, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels); \
-    else b2d_raster_kernel<RGBA, KW, false, kStates, kLevels><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels); \
-    } \
-    } while (0)
-    if (d_rgba) { if (vw.W == 1920) B2D_RASTER_GO(true, 1920); else B2D_RASTER_GO(true, 0); }
-    else if (vw.W == 1920) B2D_RASTER_GO(false, 1920);
-    else if (vw.W == 3840) B2D_RASTER_GO(false, 3840);      // BASELINE.json's 4K configuration (index frames only)
-    else B2D_RASTER_GO(false, 0);
-#undef B2D_RASTER_GO
+    // the kernel of one frame shape; rgba and kw are std::integral_constant
+    const auto go = [&](auto rgba, auto kw) {
+        constexpr bool kRgba = decltype(rgba)::value;
+        constexpr int kW = decltype(kw)::value;
+        if (masked)
+            b2d_raster_kernel<kRgba, kW, true, kStates, kLevels, Extra...><<<nblocks, 32 * kRasterWarps, 0, stream>>>(
+                t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels, fx...);
+        else
+            b2d_raster_kernel<kRgba, kW, false, kStates, kLevels, Extra...><<<nblocks, 32 * kRasterWarps, 0, stream>>>(
+                t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, d_rgba, t.levels, fx...);
+    };
+    using Index = std::false_type;
+    using Rgba = std::true_type;
+    if (d_rgba) {
+        if constexpr (kSeen) return cudaErrorInvalidValue;
+        else if (vw.W == 1920) go(Rgba{}, std::integral_constant<int, 1920>{});
+        else go(Rgba{}, std::integral_constant<int, 0>{});
+    } else if (vw.W == 1920) go(Index{}, std::integral_constant<int, 1920>{});
+    else if (vw.W == 3840) go(Index{}, std::integral_constant<int, 3840>{});  // BASELINE.json's 4K configuration (index frames only)
+    else go(Index{}, std::integral_constant<int, 0>{});
     return cudaGetLastError();
 }
 
-// The seen variant of raster_go (index frames only): FixedTables, when the batch has fixed colormaps, then SeenTables.
+// The appended tables of a <kStates, kLevels> variant: FixedTables for kFixed, then SeenTables for a seen raster.
 template <bool kStates, bool kLevels, bool kFixed>
-static cudaError_t raster_seen_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
-                                  const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, const SeenTables &seen,
-                                  cudaStream_t stream) {
-    if (n <= 0) return cudaSuccess;
-    const int strips = (vw.W + 31) / 32;
-    const int nblocks = (int)(((long long)n * strips + kRasterWarps - 1) / kRasterWarps);
-#define B2D_SEEN_GO(KW, MASKED) do { \
-    if constexpr (kFixed) \
-        b2d_raster_kernel<false, KW, MASKED, true, true, FixedTables, SeenTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, nullptr, t.levels, t.fixed, seen); \
-    else \
-        b2d_raster_kernel<false, KW, MASKED, kStates, kLevels, SeenTables><<<nblocks, 32 * kRasterWarps, 0, stream>>>(t.scene, vw, d_frames, d_work, stride, n, strips, d_index_fb, nullptr, t.levels, seen); \
-    } while (0)
-#define B2D_SEEN_W(KW) do { if (masked) B2D_SEEN_GO(KW, true); else B2D_SEEN_GO(KW, false); } while (0)
-    if (vw.W == 1920) B2D_SEEN_W(1920);
-    else if (vw.W == 3840) B2D_SEEN_W(3840);
-    else B2D_SEEN_W(0);
-#undef B2D_SEEN_W
-#undef B2D_SEEN_GO
-    return cudaGetLastError();
-}
-
-cudaError_t launch_raster_seen(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
-                               const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, const SeenTables &seen,
-                               cudaStream_t stream) {
-    if (t.fixed_rows && !(t.per_level && t.per_frame)) return cudaErrorInvalidValue;
-    auto go = t.per_level ? (t.per_frame ? (t.fixed_rows ? raster_seen_go<true, true, true> : raster_seen_go<true, true, false>)
-                                         : raster_seen_go<false, true, false>)
-                          : (t.per_frame ? raster_seen_go<true, false, false> : raster_seen_go<false, false, false>);
-    return go(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, seen, stream);
+static cudaError_t raster_tables_go(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
+                                    const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba,
+                                    const SeenTables *seen, cudaStream_t stream) {
+    const auto go = [&](const auto &...fx) {
+        return seen ? raster_go<kStates, kLevels>(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, fx..., *seen)
+                    : raster_go<kStates, kLevels>(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream, fx...);
+    };
+    if constexpr (kFixed) return go(t.fixed);
+    else return go();
 }
 
 // Per-frame states take the kStates variant of each shape; the frames are the same pixel for pixel.  A batch of per-frame
 // levels and states with a fixed colormap takes the kFixed variant.
 cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
-                          int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream) {
+                          int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, const SeenTables *seen,
+                          cudaStream_t stream) {
     if (t.fixed_rows && !(t.per_level && t.per_frame)) return cudaErrorInvalidValue;
-    auto go = t.per_level ? (t.per_frame ? (t.fixed_rows ? raster_go<true, true, true> : raster_go<true, true, false>)
-                                         : raster_go<false, true, false>)
-                          : (t.per_frame ? raster_go<true, false, false> : raster_go<false, false, false>);
-    return go(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, stream);
+    auto go = t.per_level ? (t.per_frame ? (t.fixed_rows ? raster_tables_go<true, true, true> : raster_tables_go<true, true, false>)
+                                         : raster_tables_go<false, true, false>)
+                          : (t.per_frame ? raster_tables_go<true, false, false> : raster_tables_go<false, false, false>);
+    return go(t, masked, vw, d_frames, d_work, stride, n, d_index_fb, d_rgba, seen, stream);
 }
 
 namespace {
@@ -1804,9 +1793,14 @@ constexpr int kAutomapTileW = 128, kAutomapTileH = 32;
 // atomicMax of ((item + 1) << 8 | colour), so the last item in draw order wins whatever the schedule; 0 is the
 // background, colour 0.  The key's low byte is then written out: 16 bytes per thread, a whole 128-byte line per tile row,
 // when the tile is full-width and rows start 16-byte aligned; byte by byte otherwise.
-__global__ void __launch_bounds__(256)
-b2d_automap_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level, const Pose *__restrict__ poses,
-                   View vw, int32_t scale, int flags, uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec) {
+// kSeen, the seen variant (b2d_automap_seen_device, C20): each line is coloured by its frame's row of seen lines
+// (`seen` + frame * words; nullptr: every line mapped) and B2D_AUTOMAP_ALLMAP.  `vw` is taken by value: by reference,
+// the compiler schedules K5's item loop differently.
+template <bool kSeen>
+__device__ __forceinline__ void automap_tile(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level,
+                                             const Pose *__restrict__ poses, View vw, int32_t scale, int flags,
+                                             uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec,
+                                             const uint32_t *__restrict__ seen, uint32_t words) {
     __shared__ uint32_t keys[kAutomapTileH * kAutomapTileW];
     const size_t frame = blockIdx.x / tiles;
     const int tile = blockIdx.x - (int)(frame * tiles);
@@ -1815,11 +1809,12 @@ b2d_automap_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__re
     for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) keys[k] = 0;
     const AutomapLevel L = levels[frame_level ? frame_level[frame] : 0];
     const AutomapFrame f = automap_frame(poses[frame], vw, scale, flags);
+    const uint32_t *mapped = seen ? seen + frame * words : nullptr;
     __syncthreads();
     const int n = automap_items(L, flags);
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         int64_t e[4];
-        const uint32_t colour = automap_item(f, L, flags, i, e);
+        const uint32_t colour = kSeen ? automap_seen_item(f, L, mapped, flags, i, e) : automap_item(f, L, flags, i, e);
         if (!colour) continue;
         const uint32_t key = ((uint32_t)(i + 1) << 8) | colour;
         automap_line(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1,
@@ -1844,49 +1839,18 @@ b2d_automap_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__re
     }
 }
 
-// Kernel 5's seen variant (b2d_automap_seen_device, C20): the same tiles, with each line coloured by its frame's row of
-// seen lines (`seen` + frame * words; nullptr: every line mapped) and B2D_AUTOMAP_ALLMAP.  A kernel of its own, so that
-// K5's code stays as it is.
+__global__ void __launch_bounds__(256)
+b2d_automap_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level, const Pose *__restrict__ poses,
+                   View vw, int32_t scale, int flags, uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec) {
+    automap_tile<false>(levels, frame_level, poses, vw, scale, flags, out, tiles_x, tiles, vec, nullptr, 0);
+}
+
+// Kernel 5's seen variant: a kernel of its own, so that K5's code stays as it is.
 __global__ void __launch_bounds__(256)
 b2d_automap_seen_kernel(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level,
                         const Pose *__restrict__ poses, View vw, int32_t scale, int flags, uint8_t *__restrict__ out,
                         int tiles_x, int tiles, bool vec, const uint32_t *__restrict__ seen, uint32_t words) {
-    __shared__ uint32_t keys[kAutomapTileH * kAutomapTileW];
-    const size_t frame = blockIdx.x / tiles;
-    const int tile = blockIdx.x - (int)(frame * tiles);
-    const int tx0 = (tile % tiles_x) * kAutomapTileW, ty0 = (tile / tiles_x) * kAutomapTileH;
-    const int tx1 = min(tx0 + kAutomapTileW, vw.W), ty1 = min(ty0 + kAutomapTileH, vw.H);
-    for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) keys[k] = 0;
-    const AutomapLevel L = levels[frame_level ? frame_level[frame] : 0];
-    const AutomapFrame f = automap_frame(poses[frame], vw, scale, flags);
-    const uint32_t *mapped = seen ? seen + frame * words : nullptr;
-    __syncthreads();
-    const int n = automap_items(L, flags);
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        int64_t e[4];
-        const uint32_t colour = automap_seen_item(f, L, mapped, flags, i, e);
-        if (!colour) continue;
-        const uint32_t key = ((uint32_t)(i + 1) << 8) | colour;
-        automap_line(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1,
-                     [&](int32_t x, int32_t y) { atomicMax(&keys[(y - ty0) * kAutomapTileW + (x - tx0)], key); });
-    }
-    __syncthreads();
-    uint8_t *dst = out + frame * (size_t)vw.W * vw.H;
-    if (vec && tx1 - tx0 == kAutomapTileW) {
-        const int r = threadIdx.x >> 3, c = (threadIdx.x & 7) * 16;
-        if (ty0 + r < ty1) {
-            const uint32_t *k = &keys[r * kAutomapTileW + c];
-            uint32_t w[4];
-            for (int q = 0; q < 4; q++)
-                w[q] = (k[4 * q] & 0xFF) | (k[4 * q + 1] & 0xFF) << 8 | (k[4 * q + 2] & 0xFF) << 16 | (k[4 * q + 3] & 0xFF) << 24;
-            *reinterpret_cast<uint4 *>(dst + (size_t)(ty0 + r) * vw.W + tx0 + c) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-    } else {
-        for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) {
-            const int x = tx0 + (k % kAutomapTileW), y = ty0 + k / kAutomapTileW;
-            if (x < tx1 && y < ty1) dst[(size_t)y * vw.W + x] = (uint8_t)keys[k];
-        }
-    }
+    automap_tile<true>(levels, frame_level, poses, vw, scale, flags, out, tiles_x, tiles, vec, seen, words);
 }
 }  // namespace
 
@@ -1895,27 +1859,20 @@ size_t automap_tiles(const View &vw) {
 }
 
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
-                           const View &vw, int32_t scale, int flags, uint8_t *d_out, cudaStream_t stream) {
+                           const View &vw, int32_t scale, int flags, bool seen_variant, const uint32_t *d_seen, uint32_t words,
+                           uint8_t *d_out, cudaStream_t stream) {
     if (n_frames == 0) return cudaSuccess;
     const int tiles_x = (vw.W + kAutomapTileW - 1) / kAutomapTileW;
     const int tiles = (int)automap_tiles(vw);
     if (n_frames * (size_t)tiles > 0x7FFFFFFFull) return cudaErrorInvalidValue;
     const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
-    b2d_automap_kernel<<<(unsigned)(n_frames * tiles), 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags, d_out,
-                                                                         tiles_x, tiles, vec);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_automap_seen(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
-                                const View &vw, int32_t scale, int flags, const uint32_t *d_seen, uint32_t words, uint8_t *d_out,
-                                cudaStream_t stream) {
-    if (n_frames == 0) return cudaSuccess;
-    const int tiles_x = (vw.W + kAutomapTileW - 1) / kAutomapTileW;
-    const int tiles = (int)automap_tiles(vw);
-    if (n_frames * (size_t)tiles > 0x7FFFFFFFull) return cudaErrorInvalidValue;
-    const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
-    b2d_automap_seen_kernel<<<(unsigned)(n_frames * tiles), 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags,
-                                                                              d_out, tiles_x, tiles, vec, d_seen, words);
+    const unsigned blocks = (unsigned)(n_frames * tiles);
+    if (seen_variant)
+        b2d_automap_seen_kernel<<<blocks, 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags, d_out, tiles_x,
+                                                            tiles, vec, d_seen, words);
+    else
+        b2d_automap_kernel<<<blocks, 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags, d_out, tiles_x, tiles,
+                                                       vec);
     return cudaGetLastError();
 }
 

@@ -123,13 +123,12 @@ cudaError_t launch_walk(const BatchTables &t, size_t levels_smem, const View &vw
 
 // Kernel 2: wall-column / flat-span / sky rasteriser, one warp per (frame, 32-column strip), of the frames a walk of the same
 // tables wrote.  Writes every pixel of d_index_fb exactly once; if d_rgba != nullptr also the palette-mapped RGBA8.
-// `masked`: some level the frames read has masked content (its masked_list is set).
+// `masked`: some level the frames read has masked content (its masked_list is set).  `seen` (nullable): the seen variant,
+// which draws the same index frames (no RGBA: cudaErrorInvalidValue) and ORs each frame's seen lines into its row of
+// seen->rows.
 cudaError_t launch_raster(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames, const SegFrame *d_work,
-                          int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, cudaStream_t stream);
-// ... its seen variant: the same index frames (no RGBA), and each frame's seen lines OR-ed into its row of seen.rows.
-cudaError_t launch_raster_seen(const BatchTables &t, bool masked, const View &vw, const FrameConst *d_frames,
-                               const SegFrame *d_work, int stride, int n, uint8_t *d_index_fb, const SeenTables &seen,
-                               cudaStream_t stream);
+                          int stride, int n, uint8_t *d_index_fb, uint32_t *d_rgba, const SeenTables *seen,
+                          cudaStream_t stream);
 
 // Expands the `nsets` table sets of a batch in one grid: set k by the rule of level sets[k].level (srcs[level]: device
 // pointers to that level's rest-state sections) into the tables of out[k].  `records`: the records of all sets together
@@ -166,11 +165,10 @@ cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_tables,
 size_t automap_tiles(const View &vw);
 // Kernel 5: the C19 automap of n_frames poses into contiguous W x H index frames at d_out, frame f from the items of
 // levels[frame_level[f]] (d_frame_level NULL: level 0), `scale` and `flags` as checked by b2d_automap_device.
+// `seen_variant`: its seen variant (C20), frame f's lines coloured by row f of d_seen (`words` per row; nullptr: every
+// line mapped); d_seen and words are not read otherwise.
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
-                           const View &vw, int32_t scale, int flags, uint8_t *d_out, cudaStream_t stream);
-// ... its seen variant (C20): frame f's lines coloured by row f of d_seen (`words` per row; nullptr: every line mapped).
-cudaError_t launch_automap_seen(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
-                                const View &vw, int32_t scale, int flags, const uint32_t *d_seen, uint32_t words, uint8_t *d_out,
-                                cudaStream_t stream);
+                           const View &vw, int32_t scale, int flags, bool seen_variant, const uint32_t *d_seen, uint32_t words,
+                           uint8_t *d_out, cudaStream_t stream);
 
 }  // namespace b2d
