@@ -501,6 +501,42 @@ int b2d_automap_seen_device(b2d_renderer *r, const b2d_pose *d_poses, const uint
 int b2d_renderer_seen_words(const b2d_renderer *r, uint32_t *words_out);
 int b2d_raster_device_seen(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb, uint32_t *d_seen, void *cuda_stream);
 
+/* Doom's automap at each frame's own door and lift state, with other players' arrows (AM_drawWalls with live sector
+ * heights, AM_drawPlayers in a netgame; DESIGN.md C21): b2d_automap_seen_device, plus per frame
+ *  - a sector state, states[f] with moves[first_move .. first_move + n_moves) as b2d_walk_device_levels_states takes it
+ *    (tics are ignored: no automap colour depends on time).  A two-sided line that is neither special 39 nor ML_SECRET and
+ *    has a dynamic sector on a side gets its colour from its sectors' heights at that state: differing floors 64,
+ *    otherwise differing ceilings 231, otherwise not drawn (96 under B2D_AUTOMAP_ALL_LINES).  So a shut door's line is
+ *    yellow and a fully open one disappears; a lowered lift's line is brown.  The seen rule then applies unchanged.
+ *  - arrows arrows[arrow_ranges[f].first .. + n]: each is Doom's player arrow at (x, y) (16.16 map units, as b2d_pose)
+ *    pointing along `angle` (BAM), in palette index `colour` (1 .. 255), drawn after the frame's own arrow (209) and
+ *    before the things, in list order.  An arrow at the frame's own pose draws exactly the own arrow's pixels.  Listing
+ *    every player of a netgame, the viewer included, in Doom's player colours (green 112, grey 96, brown 64, red 176;
+ *    246 while invisible) gives Doom's co-op map; listing nobody gives deathmatch's.
+ * `levels`, `states`, `moves`, `arrow_ranges` and `arrows` are HOST arrays, each nullable: NULL levels is level 0 on every
+ * frame, NULL states every frame at rest, NULL arrow_ranges no arrows, and d_seen NULL every line mapped.  With every frame
+ * at rest and no arrows the frames are byte-identical to b2d_automap_seen_device(r, d_poses, levels, d_seen, ...)'s, and
+ * with d_seen NULL and flags below B2D_AUTOMAP_ALLMAP to b2d_automap_device's.  The per-frame inputs go to the device in
+ * one copy per call, through pinned staging of the call's own with the waits of b2d_automap_device's level staging;
+ * frames of equal level and sector offsets share one entry, and a call with no per-frame input stages nothing.  The
+ * tables upload with the first automap call of any kind.  Refusals, each B2D_ERR_INVALID_ARG and detected before anything
+ * is enqueued: every refusal of b2d_automap_seen_device; a move range past n_moves, a move of an undeclared sector or
+ * outside its range, moves on a level without dynamic sectors, a NULL moves with n_moves > 0; a NULL arrows with
+ * n_arrows > 0 (when arrow_ranges is given), an arrow range past n_arrows, an arrow colour of 0 or above 255; a frame whose
+ * lines + 7 + 7 * arrows + 3 * things items reach 2^24. */
+typedef struct b2d_automap_arrow {
+    int32_t x, y;               /* 16.16 map units */
+    uint32_t angle;             /* BAM */
+    uint32_t colour;            /* palette index, 1 .. 255 */
+} b2d_automap_arrow;
+typedef struct b2d_arrow_range {
+    uint32_t first, n;          /* arrows[first .. first + n) of the call's list */
+} b2d_arrow_range;
+int b2d_automap_states_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
+                              const b2d_sector_move *moves, size_t n_moves, const b2d_arrow_range *arrow_ranges,
+                              const b2d_automap_arrow *arrows, size_t n_arrows, const uint32_t *d_seen, size_t n_frames,
+                              int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream);
+
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the
  * per-frame `frame.finish()` of engine/src/renderer.rs:160-167.  One process per GPU.  NCCL (libnccl.so.2) is bound

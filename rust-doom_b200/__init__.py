@@ -145,6 +145,25 @@ def _frame_states(tics, moves_per_pose, n: int):
     return states, arr, nm
 
 
+def _frame_arrows(arrows, n: int):
+    """(b2d_arrow_range array, concatenated b2d_automap_arrow list, its length) for n frames: frame i's arrows arrows[i]
+    (an (k, 4) array or a list of (x, y, angle, colour): 16.16 map units, BAM, palette colour; None = none)"""
+    per = list(arrows)
+    assert len(per) == n, "one arrow list per frame"
+    ranges = (_lib.ArrowRange * max(n, 1))()
+    flat = []
+    for i in range(n):
+        a = [] if per[i] is None else np.asarray(per[i], dtype=np.int64).reshape(-1, 4).tolist()
+        ranges[i] = _lib.ArrowRange(len(flat), len(a))
+        flat += a
+    arr = (_lib.AutomapArrow * max(len(flat), 1))()
+    for k, (x, y, angle, colour) in enumerate(flat):
+        if not (-2 ** 31 <= x < 2 ** 31 and -2 ** 31 <= y < 2 ** 31 and 0 <= colour < 2 ** 32):
+            raise B2dError(ERR_INVALID_ARG, "automap arrow out of range")
+        arr[k] = _lib.AutomapArrow(int(x), int(y), int(angle) & 0xFFFFFFFF, int(colour))
+    return ranges, arr, len(flat)
+
+
 def _frame_lights(lights, n: int):
     """b2d_frame_light array for n poses from (fixed_colormap, extralight) pairs, one per pose (a sequence or an (n, 2)
     integer array); the values are checked by the library (fixed_colormap -1..32, extralight 0..2)."""
@@ -715,25 +734,37 @@ class Renderer:
         return out
 
     def automap_device(self, poses_ptr: int, n: int, out_ptr: int, scale_q16: int = AUTOMAP_DEFAULT_SCALE_Q16,
-                       flags: int = 0, levels=None, stream: int = 0, seen_ptr=None):
+                       flags: int = 0, levels=None, stream: int = 0, seen_ptr=None, moves_per_pose=None, arrows=None):
         """b2d_automap_device: the automap (DESIGN.md C19) of the n device poses at poses_ptr into n contiguous W x H
         palette-index frames at out_ptr, frame f of level levels[f] (host list; None = level 0), at scale_q16 pixels per map
         unit in 16.16 (256 .. 64 << 16), flags an OR of AUTOMAP_ROTATE, AUTOMAP_ALL_LINES and AUTOMAP_THINGS.  With
         `seen_ptr` (device rows of seen lines, seen_words uint32 per frame) or AUTOMAP_ALLMAP in the flags it calls
-        b2d_automap_seen_device: frame f draws the lines row f has mapped (C20; seen_ptr None: every line)."""
+        b2d_automap_seen_device: frame f draws the lines row f has mapped (C20; seen_ptr None: every line).  With
+        `moves_per_pose` (frame f's sector moves, a list of (sector, floor_offset, ceil_offset) as render_levels_states
+        takes them) or `arrows` (frame f's other players' arrows, (x, y, angle, colour) each), either None for none, it
+        calls b2d_automap_states_device (C21): the lines coloured at each frame's door and lift state, and the arrows
+        drawn after the frame's own."""
         lv = None if levels is None else _levels_array(levels, n)
         lvp = None if lv is None else lv.ctypes.data
-        if seen_ptr is not None or int(flags) & AUTOMAP_ALLMAP:
+        if moves_per_pose is not None or arrows is not None:
+            states, mv, nm = _frame_states(0, moves_per_pose, n) if moves_per_pose is not None else (None, None, 0)
+            ranges, arr, na = _frame_arrows(arrows, n) if arrows is not None else (None, None, 0)
+            _check(_lib.load().b2d_automap_states_device(self._h, poses_ptr, lvp, states, mv, nm, ranges, arr, na, seen_ptr or None,
+                                                         n, int(scale_q16), int(flags), out_ptr, stream or None))
+        elif seen_ptr is not None or int(flags) & AUTOMAP_ALLMAP:
             _check(_lib.load().b2d_automap_seen_device(self._h, poses_ptr, lvp, seen_ptr or None, n, int(scale_q16), int(flags),
                                                        out_ptr, stream or None))
         else:
             _check(_lib.load().b2d_automap_device(self._h, poses_ptr, lvp, n, int(scale_q16), int(flags), out_ptr, stream or None))
 
-    def automap(self, poses, levels=None, scale: float = 0.2, flags=0, seen=None):
+    def automap(self, poses, levels=None, scale: float = 0.2, flags=0, seen=None, moves_per_pose=None, arrows=None):
         """The automaps of host or CUDA poses as a CUDA uint8 tensor [n, H, W] of palette indices, on the current torch
         stream: `scale` in pixels per map unit (Doom's default 0.2), `flags` an int or names from "rotate", "all", "things",
         "allmap".  `seen`: a CUDA int32 tensor [n, seen_words] of seen lines (render_seen), whose mapped lines each frame
-        draws (automap_device's seen_ptr).  Colour them with resolve() or palette_lut_levels_device like rendered frames."""
+        draws (automap_device's seen_ptr).  `moves_per_pose`: each frame's sector moves, the lists render_levels_states
+        takes, so each door and lift line has its colour at that frame's state; `arrows`: per frame None or an array of
+        (x, y, angle, colour) rows, other players' arrows (DESIGN.md C21).  Colour the frames with resolve() or
+        palette_lut_levels_device like rendered frames."""
         import torch
         flags = automap_flags(flags)
         dev = torch.device("cuda", self.device)
@@ -751,7 +782,8 @@ class Renderer:
             if not (seen.is_cuda and seen.dtype == torch.int32 and tuple(seen.shape) == (n, self.seen_words) and seen.is_contiguous()):
                 raise ValueError("seen must be a contiguous CUDA int32 tensor [%d, %d]" % (n, self.seen_words))
             seen_ptr = seen.data_ptr()
-        self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream, seen_ptr)
+        self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream, seen_ptr,
+                            moves_per_pose, arrows)
         return out
 
     def worklist(self, n: int):

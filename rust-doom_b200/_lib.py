@@ -66,6 +66,7 @@ EXPORTS = [
     "b2d_render_sharded_levels_states_resolved_palettes",
     "b2d_render_levels_states_lights", "b2d_render_device_levels_states_lights", "b2d_walk_device_levels_states_lights",
     "b2d_scene_automap_lines", "b2d_automap_device", "b2d_renderer_seen_words", "b2d_raster_device_seen", "b2d_automap_seen_device",
+    "b2d_automap_states_device",
 ]
 
 COMM_ID_BYTES = 128
@@ -78,6 +79,16 @@ class AutomapLine(ctypes.Structure):
     """b2d_automap_line: a linedef's endpoints (map units), colour drawn normally and under AUTOMAP_ALL_LINES, index"""
     _fields_ = [("x0", ctypes.c_int32), ("y0", ctypes.c_int32), ("x1", ctypes.c_int32), ("y1", ctypes.c_int32),
                 ("colour", ctypes.c_uint8), ("colour_all", ctypes.c_uint8), ("pad", ctypes.c_uint16), ("linedef", ctypes.c_int32)]
+
+
+class AutomapArrow(ctypes.Structure):
+    """b2d_automap_arrow: another player's arrow, at (x, y) in 16.16 map units, angle in BAM, palette colour 1..255"""
+    _fields_ = [("x", ctypes.c_int32), ("y", ctypes.c_int32), ("angle", ctypes.c_uint32), ("colour", ctypes.c_uint32)]
+
+
+class ArrowRange(ctypes.Structure):
+    """b2d_arrow_range: arrows[first .. first + n) of the call's arrow list"""
+    _fields_ = [("first", ctypes.c_uint32), ("n", ctypes.c_uint32)]
 
 
 class ShardedStats(ctypes.Structure):
@@ -226,6 +237,9 @@ def load() -> ctypes.CDLL:
     L.b2d_raster_device_seen.argtypes = [vp, ctypes.c_int64, vp, vp, vp]
     L.b2d_raster_device_seen.restype = ctypes.c_int
     L.b2d_automap_seen_device.argtypes = [vp, vp, vp, vp, cs, ctypes.c_int32, ci, vp, vp]
+    L.b2d_automap_states_device.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), ctypes.POINTER(SectorMove), cs,
+                                            ctypes.POINTER(ArrowRange), ctypes.POINTER(AutomapArrow), cs, vp, cs, ctypes.c_int32,
+                                            ci, vp, vp]
     L.b2d_render_sharded_levels_states_resolved_palettes.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(FrameState), cs,
                                                                      ctypes.POINTER(SectorMove), cs, cs, ci, ci, ci, CHUNK_FN, vp,
                                                                      ctypes.POINTER(ShardedStats)]

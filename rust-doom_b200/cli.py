@@ -28,7 +28,8 @@ automap of the dumped pose at SCALE pixels per map unit (0.2 is Doom's default; 
 coloured through palette 0 of its level and resolved at the --supersample factor; --automap-flags rotate,all,things turns
 the map with the view, draws every line (IDDT) and draws the decoration things; seen draws only the lines the run's
 frames of that level saw (Renderer.render_seen, DESIGN.md C20) and allmap adds the unseen ones in grey (the computer
-area map).  Not with --world.
+area map); others draws the arrows of the run's first four poses of that level in Doom's co-op colours, the dumped pose's
+own in green 112 and the next three in 96, 64 and 176 (b2d_automap_states_device, DESIGN.md C21).  Not with --world.
 
 --palette P colours the dumped and streamed frames through PLAYPAL palette P of each frame's level instead of palette 0
 (b2d_resolve_palettes_device; in Doom 1..8 are the damage flash, 9..12 the bonus flash, 13 the radiation suit), through
@@ -153,21 +154,41 @@ def _automap_name(dump: str, level=None) -> str:
     return "%s.automap%s%s" % (stem, "" if level is None else ".%d" % level, ext or ".ppm")
 
 
-def automap_flag_names(flags: str):
-    """(the B2D_AUTOMAP_* names of --automap-flags, whether it names `seen`); unknown names raise ValueError"""
+# --automap-flags others: Doom's co-op player colours (green, grey, brown, red), the dumped pose's own first
+OTHER_COLOURS = (112, 96, 64, 176)
+
+
+def automap_flag_options(flags: str):
+    """(the B2D_AUTOMAP_* names of --automap-flags, whether it names `seen`, whether it names `others`); unknown names
+    raise ValueError"""
     names = [x.strip() for x in flags.split(",") if x.strip()]
-    rest = ",".join(x for x in names if x != "seen")
+    rest = ",".join(x for x in names if x not in ("seen", "others"))
     import rust_doom_b200 as b2d
     b2d.automap_flags(rest)
-    return rest, "seen" in names
+    return rest, "seen" in names, "others" in names
+
+
+def automap_flag_names(flags: str):
+    """(the B2D_AUTOMAP_* names of --automap-flags, whether it names `seen`); unknown names raise ValueError"""
+    return automap_flag_options(flags)[:2]
 
 
 def automap_rgb(r, poses: np.ndarray, levels, scale: float, flags: str, factor: int, run_poses=None, run_levels=None) -> np.ndarray:
     """(n, H, W, 3) uint8: the automaps of the poses (b2d_automap_device at the render size) through palette 0 of each
     frame's level, resolved by `factor` as the rendered frames are.  With `seen` in the flags, frame k draws the lines
-    that the run's frames (run_poses, of levels run_levels) of its level saw (Renderer.render_seen, OR-ed per level)."""
+    that the run's frames (run_poses, of levels run_levels) of its level saw (Renderer.render_seen, OR-ed per level).
+    With `others`, frame k (the first of the run's poses of its level) also draws the arrows of the first four run poses
+    of its level in OTHER_COLOURS, its own pose's in green (b2d_automap_states_device)."""
     import torch
-    names, seen = automap_flag_names(flags)
+    names, seen, others = automap_flag_options(flags)
+    arrows = None
+    if others:
+        run_lv = np.zeros(len(run_poses), np.int64) if run_levels is None else np.asarray(run_levels)
+        lv = np.zeros(len(poses), np.int64) if levels is None else np.asarray(levels)
+        arrows = []
+        for l in lv:
+            mine = np.asarray(run_poses)[run_lv == l][:len(OTHER_COLOURS)]
+            arrows.append([(int(p["x"]), int(p["y"]), int(p["angle"]), c) for p, c in zip(mine, OTHER_COLOURS)])
     rows = None
     if seen:
         kw = {} if run_levels is None else {"levels": list(run_levels)}
@@ -176,7 +197,8 @@ def automap_rgb(r, poses: np.ndarray, levels, scale: float, flags: str, factor: 
         lv = np.zeros(len(poses), np.int64) if levels is None else np.asarray(levels)
         rows = np.stack([np.bitwise_or.reduce(per_frame[run_lv == l], axis=0) for l in lv])
         rows = torch.from_numpy(rows.view(np.int32).copy()).cuda(r.device)
-    return r.resolve(r.automap(np.ascontiguousarray(poses), levels, scale, names, seen=rows), factor, "rgb", levels).cpu().numpy()
+    return r.resolve(r.automap(np.ascontiguousarray(poses), levels, scale, names, seen=rows, arrows=arrows), factor, "rgb",
+                     levels).cpu().numpy()
 
 
 def resolve_rgb(r, index: np.ndarray, factor: int, levels=None, palette: int = 0) -> np.ndarray:
@@ -333,7 +355,7 @@ def main(argv=None) -> int:
                     help="with --dump: also write NAME.automap.EXT (NAME.automap.L.EXT with --levels), Doom's automap of "
                          "the dumped pose at SCALE pixels per map unit (Doom's default: 0.2)")
     ap.add_argument("--automap-flags", default="", help="with --automap: comma-separated rotate, all, things, allmap (unseen lines in grey), "
-                         "seen (only the lines the run's frames saw)")
+                         "seen (only the lines the run's frames saw), others (the run's next three poses as team-mates' arrows)")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 

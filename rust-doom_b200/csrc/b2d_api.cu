@@ -280,6 +280,33 @@ void state_at(const LevelRes &lv, uint32_t tics, uint32_t *out) {
     std::copy(lv.state.begin() + 1, lv.state.begin() + 2 + 2 * (ptrdiff_t)lv.layout.dyn_sectors.size(), out + 1);
 }
 
+// The state automap's changeable lines (C21) of a level: each two-sided line that is neither special 39 nor ML_SECRET and
+// has a dynamic sector (layout's slots) on a side gets kAutomapChangeable in its device copy and, in dyn (one record per
+// line, left empty when no line changes), its sectors' rest heights and dynamic slots.
+void automap_dyn_lines(const Level &lv, const StateLayout &layout, std::vector<AutomapLine> &lines, std::vector<AutomapDynLine> &dyn) {
+    auto side_sector = [&](int side) -> int {            // as automap_lines finds a side's sector
+        if (side < 0 || (size_t)side >= lv.sidedefs.size()) return -1;
+        const int sec = lv.sidedefs[(size_t)side].sector;
+        return (size_t)sec < lv.sectors.size() ? sec : -1;
+    };
+    auto slot = [&](int sec) -> uint32_t {
+        const uint32_t d = (size_t)sec < layout.sector_slots.size() ? layout.sector_slots[(size_t)sec] >> 16 : kNoSlot;
+        return d == kNoSlot ? kAutomapNoSlot : d;
+    };
+    for (size_t i = 0; i < lines.size(); i++) {
+        const Linedef &l = lv.linedefs[(size_t)lines[i].linedef];
+        const int front = side_sector(l.right), back = side_sector(l.left);
+        if (front < 0 || back < 0 || l.special == 39 || (l.flags & 0x20)) continue;
+        const AutomapDynLine d{{lv.sectors[(size_t)front].floor, lv.sectors[(size_t)back].floor},
+                               {lv.sectors[(size_t)front].ceil, lv.sectors[(size_t)back].ceil},
+                               {slot(front), slot(back)}};
+        if (d.slot[0] == kAutomapNoSlot && d.slot[1] == kAutomapNoSlot) continue;
+        dyn.resize(lines.size(), AutomapDynLine{});
+        dyn[i] = d;
+        lines[i].dev_flags |= kAutomapChangeable;
+    }
+}
+
 // Per-frame levels (HOST, nullable = level 0): each below the renderer's number of levels; B2D_ERR_INVALID_ARG otherwise.
 int check_levels(const b2d_renderer *r, const uint32_t *levels, size_t n) {
     if (levels)
@@ -1146,6 +1173,7 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
             r->lv[k].automap_lines = scenes[k]->automap;
             for (AutomapLine &l : r->lv[k].automap_lines)      // the device copy's don't-draw bit (the seen automap's ALLMAP rule)
                 if (scenes[k]->level.linedefs[(size_t)l.linedef].flags & 0x80) l.dev_flags = kAutomapDontDraw;
+            automap_dyn_lines(scenes[k]->level, r->lv[k].layout, r->lv[k].automap_lines, r->lv[k].automap_dyn);
             for (uint32_t i = 0; i < h[H_NSPRITES]; i++) {
                 r->lv[k].automap_things.push_back(sp[i].x);
                 r->lv[k].automap_things.push_back(sp[i].y);
@@ -1532,10 +1560,12 @@ int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *
 }
 
 // The automap tables of every level (b2d_renderer::automap): the lines and things of each level in one buffer, then an
-// AutomapLevel per level pointing into it.
+// AutomapLevel per level pointing into it, then each level's AutomapDynLine table pointer (automap_dyn_records) and the
+// tables.
+static size_t automap_dyn_records(const b2d_renderer *r) { return r->automap->off + r->lv.size() * sizeof(AutomapLevel); }
 static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
     size_t items = 0;
-    std::vector<size_t> line_off, thing_off;
+    std::vector<size_t> line_off, thing_off, dyn_off;
     for (const LevelRes &lv : r->lv) {
         line_off.push_back(items);
         items += lv.automap_lines.size() * sizeof(AutomapLine);
@@ -1543,7 +1573,13 @@ static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
         items += lv.automap_things.size() * sizeof(int32_t);
     }
     items = (items + 15) & ~(size_t)15;                   // the AutomapLevel records follow, aligned
-    return build_tables(r->automap, items + r->lv.size() * sizeof(AutomapLevel), items, st, [&](uint8_t *h, const uint8_t *d) {
+    const size_t dyn_records = items + r->lv.size() * sizeof(AutomapLevel);     // 8-byte aligned
+    size_t bytes = dyn_records + r->lv.size() * sizeof(const AutomapDynLine *);
+    for (const LevelRes &lv : r->lv) {
+        dyn_off.push_back(bytes);
+        bytes += lv.automap_dyn.size() * sizeof(AutomapDynLine);
+    }
+    return build_tables(r->automap, bytes, items, st, [&](uint8_t *h, const uint8_t *d) {
         for (size_t k = 0; k < r->lv.size(); k++) {
             const LevelRes &lv = r->lv[k];
             if (!lv.automap_lines.empty()) std::memcpy(h + line_off[k], lv.automap_lines.data(), lv.automap_lines.size() * sizeof(AutomapLine));
@@ -1551,6 +1587,9 @@ static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
             const AutomapLevel L{reinterpret_cast<const AutomapLine *>(d + line_off[k]), reinterpret_cast<const int32_t *>(d + thing_off[k]),
                                  (int32_t)lv.automap_lines.size(), (int32_t)(lv.automap_things.size() / 2)};
             std::memcpy(h + items + k * sizeof(AutomapLevel), &L, sizeof L);
+            const AutomapDynLine *dyn = lv.automap_dyn.empty() ? nullptr : reinterpret_cast<const AutomapDynLine *>(d + dyn_off[k]);
+            std::memcpy(h + dyn_records + k * sizeof dyn, &dyn, sizeof dyn);
+            if (dyn) std::memcpy(h + dyn_off[k], lv.automap_dyn.data(), lv.automap_dyn.size() * sizeof(AutomapDynLine));
         }
     });
 }
@@ -1568,9 +1607,54 @@ int b2d_raster_device_seen(b2d_renderer *r, int64_t ticket, uint8_t *d_index_fb,
     return raster_batch(r, ticket, d_index_fb, nullptr, static_cast<cudaStream_t>(cuda_stream), d_seen);
 }
 
-// b2d_automap_device (seen_variant false: K5) and b2d_automap_seen_device (its seen variant, which also takes ALLMAP)
+static_assert(sizeof(b2d_automap_arrow) == sizeof(AutomapArrow) && offsetof(b2d_automap_arrow, colour) == offsetof(AutomapArrow, colour),
+              "b2d_automap_arrow");
+
+// What b2d_automap_states_device adds to the seen automap (HOST arrays, each nullable; C21).
+struct AutomapStates {
+    const b2d_frame_state *states;
+    const b2d_sector_move *moves;
+    size_t n_moves;
+    const b2d_arrow_range *ranges;
+    const b2d_automap_arrow *arrows;
+    size_t n_arrows;
+};
+
+// The state automap's per-frame inputs as one staged image of words: an AutomapFrameIn per frame, the arrows, then the
+// distinct sector offsets (2 words per dynamic slot of the level) of the moved frames, shared by frames of equal level and
+// offsets.  `c` holds the frames' compact states (CallFrames::prepare), whose words 2 .. 2 + 2 * ndyn are the offsets.
+static int automap_states_image(const b2d_renderer *r, const uint32_t *levels, const AutomapStates &a, const CallFrames &c,
+                                size_t n, std::vector<uint32_t> &img) {
+    return guarded([&] {
+        const size_t arrow_words = a.ranges ? 4 * a.n_arrows : 0, pool = 4 * n + arrow_words;
+        img.assign(pool, 0);
+        if (arrow_words) std::memcpy(img.data() + 4 * n, a.arrows, 4 * arrow_words);
+        std::unordered_map<std::string, uint32_t> seen;
+        for (size_t i = 0; i < n; i++) {
+            const uint32_t level = levels ? levels[i] : 0u;
+            const LevelRes &lv = r->lv[level];
+            const uint32_t ndyn = (uint32_t)lv.layout.dyn_sectors.size();
+            AutomapFrameIn in{level, kAutomapNoSlot, a.ranges ? a.ranges[i].first : 0u, a.ranges ? a.ranges[i].n : 0u};
+            if (a.states && !c.starts.empty() && !lv.h_blob.empty() && ndyn && c.fs[c.starts[i] + 1]) {      // moved
+                const uint32_t *w = c.fs.data() + c.starts[i] + 2;
+                std::string key(reinterpret_cast<const char *>(&level), 4);
+                key.append(reinterpret_cast<const char *>(w), 8 * ndyn);
+                auto it = seen.emplace(std::move(key), (uint32_t)(img.size() - pool));
+                if (it.second) img.insert(img.end(), w, w + 2 * ndyn);
+                in.off = it.first->second;
+            }
+            std::memcpy(img.data() + 4 * i, &in, sizeof in);
+        }
+        if (img.size() - pool >= kAutomapNoSlot) return fail(B2D_ERR_INVALID_ARG, "too many distinct sector states for one call");
+        return B2D_OK;
+    });
+}
+
+// b2d_automap_device (seen_variant false, states nullptr: K5), b2d_automap_seen_device (its seen variant, which also takes
+// ALLMAP) and b2d_automap_states_device (states: the state variant)
 static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const uint32_t *d_seen, size_t n_frames,
-                        int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream, bool seen_variant) {
+                        int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream, bool seen_variant,
+                        const AutomapStates *states = nullptr) {
     if (!r || !d_poses || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
     const int known = B2D_AUTOMAP_ROTATE | B2D_AUTOMAP_ALL_LINES | B2D_AUTOMAP_THINGS | (seen_variant ? B2D_AUTOMAP_ALLMAP : 0);
     if (flags & ~known) return fail(B2D_ERR_INVALID_ARG, "unknown automap flags");
@@ -1582,13 +1666,54 @@ static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t
         if (lv.automap_lines.size() + kAutomapArrowSegs + kAutomapThingSegs * lv.automap_things.size() / 2 >= (1u << 24))
             return fail(B2D_ERR_INVALID_ARG, "level has too many automap items (2^24)");
     if (n_frames > 0x7FFFFFFFull / automap_tiles(r->view)) return fail(B2D_ERR_INVALID_ARG, "too many frames for one grid (2^31 - 1 tiles)");
+    // the state variant: the states as the walk checks them (without its shared-memory limit: nothing is walked), then
+    // the arrows, then each frame's items
+    CallFrames c(kFrameStates, levels, states ? states->states : nullptr, states ? states->moves : nullptr, states ? states->n_moves : 0);
+    std::vector<uint32_t> img;
+    if (states) {
+        if (states->states)
+            if (int rc = c.prepare(r, n_frames)) return rc;
+        if (states->ranges) {
+            if (states->n_arrows && !states->arrows) return fail(B2D_ERR_INVALID_ARG, "null argument");
+            for (size_t k = 0; k < states->n_arrows; k++)
+                if (states->arrows[k].colour == 0 || states->arrows[k].colour > 255)
+                    return fail(B2D_ERR_INVALID_ARG, "automap arrow colour out of range (1 .. 255)");
+            for (size_t i = 0; i < n_frames; i++) {
+                const b2d_arrow_range &g = states->ranges[i];
+                if (g.first > states->n_arrows || g.n > states->n_arrows - g.first)
+                    return fail(B2D_ERR_INVALID_ARG, "a frame's arrow range runs past the end of the arrow list");
+                const LevelRes &lv = r->lv[levels ? levels[i] : 0];
+                if (lv.automap_lines.size() + kAutomapArrowSegs * (1 + (uint64_t)g.n) + kAutomapThingSegs * lv.automap_things.size() / 2 >=
+                    (1u << 24))
+                    return fail(B2D_ERR_INVALID_ARG, "a frame has too many automap items (2^24)");
+            }
+        }
+        if (int rc = automap_states_image(r, levels, *states, c, n_frames, img)) return rc;
+    }
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     if (int rc = tables_on(r, r->automap, st, ensure_automap)) return rc;
+    const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->off);
+    if (states) {
+        // nothing per frame (level 0, at rest, no arrows): nothing to stage
+        const bool staged = levels || c.frames.starts || states->ranges;
+        if (staged)
+            if (int rc = stage_words(r->automap_states, img.size(), st, [&](size_t i) { return img[i]; })) return rc;
+        const uint32_t *d = r->automap_states.d.get();
+        const size_t pool = 4 * n_frames + (states->ranges ? 4 * states->n_arrows : 0);
+        const AutomapStateTables t{reinterpret_cast<const AutomapDynLine *const *>(r->automap->d.get() + automap_dyn_records(r)),
+                                   staged ? reinterpret_cast<const AutomapFrameIn *>(d) : nullptr,
+                                   staged ? reinterpret_cast<const int32_t *>(d + pool) : nullptr,
+                                   staged ? reinterpret_cast<const AutomapArrow *>(d + 4 * n_frames) : nullptr};
+        CU(launch_automap(d_levels, nullptr, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16, flags, true,
+                          d_seen, r->seen_words, d_out, st, &t));
+        if (staged) CU(cudaEventRecord(r->automap_states.done.get(), st));
+        r->launches += 1;
+        return B2D_OK;
+    }
     if (levels)
         if (int rc = stage_words(r->automap_levels, n_frames, st, [&](size_t i) { return levels[i]; })) return rc;
-    const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->off);
     const uint32_t *d_frame_level = levels ? r->automap_levels.d.get() : nullptr;
     CU(launch_automap(d_levels, d_frame_level, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16, flags,
                       seen_variant, d_seen, r->seen_words, d_out, st));
@@ -1605,6 +1730,14 @@ int b2d_automap_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t 
 int b2d_automap_seen_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const uint32_t *d_seen,
                             size_t n_frames, int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream) {
     return automap_call(r, d_poses, levels, d_seen, n_frames, scale_q16, flags, d_out, cuda_stream, true);
+}
+
+int b2d_automap_states_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
+                              const b2d_sector_move *moves, size_t n_moves, const b2d_arrow_range *arrow_ranges,
+                              const b2d_automap_arrow *arrows, size_t n_arrows, const uint32_t *d_seen, size_t n_frames,
+                              int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream) {
+    const AutomapStates a{states, moves, n_moves, arrow_ranges, arrows, n_arrows};
+    return automap_call(r, d_poses, levels, d_seen, n_frames, scale_q16, flags, d_out, cuda_stream, true, &a);
 }
 
 int b2d_device_alloc(int device, size_t bytes, void **d_out) {

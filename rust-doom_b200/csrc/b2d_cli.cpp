@@ -22,7 +22,8 @@
 // --levels NAME.automap.L.ppm): Doom's automap of the dumped pose (b2d_automap_device, DESIGN.md C19) through palette 0 of
 // its level, resolved at the --supersample factor; --automap-flags rotate,all,things turns the map with the view, draws
 // every line and draws the decoration things; seen draws only the lines the run's frames of that level saw (b2d_raster_device_seen,
-// DESIGN.md C20), allmap adds the unseen ones in grey (the computer area map).  Not with --world.
+// DESIGN.md C20), allmap adds the unseen ones in grey (the computer area map), others draws the arrows of the run's first
+// four poses of that level in Doom's co-op colours 112, 96, 64, 176 (b2d_automap_states_device, C21).  Not with --world.
 #include <cmath>
 #include <algorithm>
 #include <cstdint>
@@ -123,10 +124,12 @@ int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const
 // palette 0 of each frame's level and resolved by `factor` to RGB8 (b2d_automap_device, b2d_resolve_device), frame k written
 // to names[k]
 // With `seen` (n rows of b2d_renderer_seen_words words) or B2D_AUTOMAP_ALLMAP, frame k draws the lines row k has mapped
-// (b2d_automap_seen_device).
+// (b2d_automap_seen_device).  With `ranges` (one per frame) into `arrows`, frame k also draws those arrows
+// (b2d_automap_states_device).
 int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, const uint32_t *levels,
                    int32_t scale_q16, int flags, int factor, const std::vector<std::string> &names,
-                   const std::vector<uint32_t> *seen = nullptr) {
+                   const std::vector<uint32_t> *seen = nullptr, const std::vector<b2d_arrow_range> *ranges = nullptr,
+                   const std::vector<b2d_automap_arrow> *arrows = nullptr) {
     const size_t n = poses.size(), npix = (size_t)view.width * view.height;
     size_t frame_bytes = 0;
     if (b2d_resolve_frame_bytes(r, factor, B2D_RESOLVE_RGB8, &frame_bytes) != B2D_OK) return fail("resolve");
@@ -146,9 +149,11 @@ int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std:
     }
     uint8_t *di = static_cast<uint8_t *>(d_index);
     const b2d_pose *dp = static_cast<const b2d_pose *>(d_poses);
-    const int rc = seen || (flags & B2D_AUTOMAP_ALLMAP)
-                       ? b2d_automap_seen_device(r, dp, levels, static_cast<const uint32_t *>(d_seen), n, scale_q16, flags, di, nullptr)
-                       : b2d_automap_device(r, dp, levels, n, scale_q16, flags, di, nullptr);
+    const uint32_t *ds = static_cast<const uint32_t *>(d_seen);
+    const int rc = ranges ? b2d_automap_states_device(r, dp, levels, nullptr, nullptr, 0, ranges->data(), arrows->data(), arrows->size(),
+                                                      ds, n, scale_q16, flags, di, nullptr)
+                   : seen || (flags & B2D_AUTOMAP_ALLMAP) ? b2d_automap_seen_device(r, dp, levels, ds, n, scale_q16, flags, di, nullptr)
+                                                          : b2d_automap_device(r, dp, levels, n, scale_q16, flags, di, nullptr);
     if (rc != B2D_OK) return fail("automap");
     if (b2d_resolve_device(r, di, levels, n, factor, B2D_RESOLVE_RGB8, d_rgb, nullptr) != B2D_OK) return fail("resolve");
     std::vector<uint8_t> rgb(frame_bytes * n);
@@ -198,13 +203,31 @@ int run_seen_rows(b2d_renderer *r, int device, const b2d_view &view, const std::
     return 0;
 }
 
-// --automap on one level: the automap of the run's first pose, with `seen` of the lines all its poses saw
+// --automap-flags others: for automap frame k, on level frame_levels[k], the arrows of the first four of the run's poses
+// (levels: each one's level, nullptr: level 0) on that level, in Doom's co-op colours: green, grey, brown, red
+void team_arrows(const std::vector<b2d_pose> &poses, const uint32_t *levels, const std::vector<uint32_t> &frame_levels,
+                 std::vector<b2d_arrow_range> &ranges, std::vector<b2d_automap_arrow> &arrows) {
+    static const uint32_t colours[4] = {112, 96, 64, 176};
+    for (uint32_t level : frame_levels) {
+        b2d_arrow_range g{(uint32_t)arrows.size(), 0};
+        for (size_t i = 0; i < poses.size() && g.n < 4; i++)
+            if ((levels ? levels[i] : 0u) == level) arrows.push_back({poses[i].x, poses[i].y, poses[i].angle, colours[g.n++]});
+        ranges.push_back(g);
+    }
+}
+
+// --automap on one level: the automap of the run's first pose, with `seen` of the lines all its poses saw and, with
+// `others`, its first four poses' arrows
 int write_run_automap(b2d_renderer *r, const b2d_view &view, const std::vector<b2d_pose> &poses, int max_batch, int32_t scale_q16,
-                      int flags, bool seen, int factor, const std::string &name) {
+                      int flags, bool seen, bool others, int factor, const std::string &name) {
     std::vector<uint32_t> rows;
     if (seen)
         if (int rc = run_seen_rows(r, 0, view, poses, nullptr, 1, max_batch, rows)) return rc;
-    return write_automaps(r, 0, view, {poses[0]}, nullptr, scale_q16, flags, factor, {name}, seen ? &rows : nullptr);
+    std::vector<b2d_arrow_range> ranges;
+    std::vector<b2d_automap_arrow> arrows;
+    if (others) team_arrows(poses, nullptr, {0u}, ranges, arrows);
+    return write_automaps(r, 0, view, {poses[0]}, nullptr, scale_q16, flags, factor, {name}, seen ? &rows : nullptr,
+                          others ? &ranges : nullptr, &arrows);
 }
 
 // the --dump name without its .ppm extension
@@ -264,7 +287,7 @@ int report_sharded(b2d_renderer *r, ShardSink &sink, const b2d_sharded_stats &st
 int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, int height, double fov, int nposes, uint32_t tics,
                      const std::string &dump, const std::string &stream, int world, int rank, int chunk, const std::string &id_file,
                      int supersample, int palette, b2d_frame_light light, int32_t automap_scale, int automap_flags,
-                     bool automap_seen) {
+                     bool automap_seen, bool automap_others) {
     std::vector<b2d_scene *> scenes;
     struct Scenes {
         std::vector<b2d_scene *> &v;
@@ -361,8 +384,11 @@ int render_level_set(b2d_archive *arch, const std::vector<int> &set, int width, 
             if (automap_seen) {
                 if (int rc = run_seen_rows(r, 0, view, poses, levels.data(), set.size(), n < 64 ? (int)n : 64, seen)) return rc;
             }
+            std::vector<b2d_arrow_range> ranges;
+            std::vector<b2d_automap_arrow> arrows;
+            if (automap_others) team_arrows(poses, levels.data(), first_levels, ranges, arrows);
             if (int rc = write_automaps(r, 0, view, firsts, first_levels.data(), automap_scale, automap_flags, supersample, names,
-                                        automap_seen ? &seen : nullptr))
+                                        automap_seen ? &seen : nullptr, automap_others ? &ranges : nullptr, &arrows))
                 return rc;
         }
     }
@@ -383,6 +409,7 @@ int main(int argc, char **argv) {
     int32_t automap_scale = 0;        // 0: no --automap
     int automap_flags = 0;
     bool automap_seen = false;        // --automap-flags seen: the automap shows the lines the run's frames saw
+    bool automap_others = false;      // --automap-flags others: ... and the run's first four poses as players' arrows
     b2d_frame_light light{-1, 0};
     double fov = 65.0;
     unsigned long tics = 0;
@@ -451,7 +478,8 @@ int main(int argc, char **argv) {
                 else if (name == "things") automap_flags |= B2D_AUTOMAP_THINGS;
                 else if (name == "allmap") automap_flags |= B2D_AUTOMAP_ALLMAP;
                 else if (name == "seen") automap_seen = true;
-                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things, allmap, seen\n"); return 2; }
+                else if (name == "others") automap_others = true;
+                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things, allmap, seen, others\n"); return 2; }
                 at = comma + 1;
             }
         }
@@ -503,7 +531,8 @@ int main(int argc, char **argv) {
             return 2;
         }
         const int rc = render_level_set(arch, set, width, height, fov, nposes, (uint32_t)tics, dump, stream, world, rank, chunk, id_file,
-                                        supersample, palette, light, automap_scale, automap_flags, automap_seen);
+                                        supersample, palette, light, automap_scale, automap_flags, automap_seen,
+                                        automap_others);
         b2d_archive_close(arch);
         return rc;
     }
@@ -539,7 +568,7 @@ int main(int argc, char **argv) {
         }
         if (automap_scale && !dump.empty())
             if (int rc = write_run_automap(r, view, poses, nposes < 64 ? nposes : 64, automap_scale, automap_flags, automap_seen,
-                                           supersample, dump_stem(dump) + ".automap.ppm"))
+                                           automap_others, supersample, dump_stem(dump) + ".automap.ppm"))
                 return rc;
         if (!stream.empty()) {
             std::FILE *f = std::fopen(stream.c_str(), "wb");
@@ -580,8 +609,8 @@ int main(int argc, char **argv) {
         std::fclose(f);
     }
     if (automap_scale && !dump.empty())
-        if (int rc = write_run_automap(r, view, poses, nposes < 64 ? nposes : 64, automap_scale, automap_flags, automap_seen, 1,
-                                       dump_stem(dump) + ".automap.ppm"))
+        if (int rc = write_run_automap(r, view, poses, nposes < 64 ? nposes : 64, automap_scale, automap_flags, automap_seen,
+                                       automap_others, 1, dump_stem(dump) + ".automap.ppm"))
             return rc;
     if (!stream.empty()) {
         std::FILE *f = std::fopen(stream.c_str(), "wb");

@@ -212,6 +212,9 @@ struct LevelRes {
     // blob's sprites.  Uploaded by the first b2d_automap_device call (b2d_renderer::automap).
     std::vector<AutomapLine> automap_lines;
     std::vector<int32_t> automap_things;
+    // The state automap's (C21): an AutomapDynLine per automap line, read for the lines whose device copy has the
+    // kAutomapChangeable bit; empty when the level has none.
+    std::vector<AutomapDynLine> automap_dyn;
     // Seen lines (DESIGN.md C20): the linedef of each seg of the level's SEGS lump (-1: none), built at creation and
     // uploaded by the first b2d_raster_device_seen call (b2d_renderer::seen)
     std::vector<int32_t> seg_line;
@@ -251,10 +254,11 @@ struct b2d_renderer {
         size_t off = 0;
         Event built;
     };
-    // The automap's (first b2d_automap_device call): the lines and things of each level, then one AutomapLevel per level
-    // pointing into them.  With the call's own level staging.
+    // The automap's (first automap call of any kind): the lines and things of each level, then one AutomapLevel per level
+    // pointing into them, then one AutomapDynLine table pointer per level and those tables (automap_dyn_records).  With
+    // b2d_automap_device's own level staging, and b2d_automap_states_device's own staging of its per-frame inputs.
     std::unique_ptr<Tables> automap;
-    LevelStaging automap_levels;
+    LevelStaging automap_levels, automap_states;
     // The seen raster's (first b2d_raster_device_seen call): the seg -> linedef tables one after the other, then each
     // level's offset into them.  `seen_words`: the length of a row of seen lines.
     std::unique_ptr<Tables> seen;

@@ -1796,25 +1796,39 @@ constexpr int kAutomapTileW = 128, kAutomapTileH = 32;
 // kSeen, the seen variant (b2d_automap_seen_device, C20): each line is coloured by its frame's row of seen lines
 // (`seen` + frame * words; nullptr: every line mapped) and B2D_AUTOMAP_ALLMAP.  `vw` is taken by value: by reference,
 // the compiler schedules K5's item loop differently.
-template <bool kSeen>
+// kState, the state variant (b2d_automap_states_device, C21): the seen variant with the frame's level, sector offsets and
+// arrows from `st` (automap_state_item).  The offsets are read only by changeable lines, in the item loop.
+template <bool kSeen, bool kState = false>
 __device__ __forceinline__ void automap_tile(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level,
                                              const Pose *__restrict__ poses, View vw, int32_t scale, int flags,
                                              uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec,
-                                             const uint32_t *__restrict__ seen, uint32_t words) {
+                                             const uint32_t *__restrict__ seen, uint32_t words,
+                                             const AutomapStateTables st = AutomapStateTables{}) {
     __shared__ uint32_t keys[kAutomapTileH * kAutomapTileW];
     const size_t frame = blockIdx.x / tiles;
     const int tile = blockIdx.x - (int)(frame * tiles);
     const int tx0 = (tile % tiles_x) * kAutomapTileW, ty0 = (tile / tiles_x) * kAutomapTileH;
     const int tx1 = min(tx0 + kAutomapTileW, vw.W), ty1 = min(ty0 + kAutomapTileH, vw.H);
     for (int k = threadIdx.x; k < kAutomapTileH * kAutomapTileW; k += blockDim.x) keys[k] = 0;
-    const AutomapLevel L = levels[frame_level ? frame_level[frame] : 0];
+    AutomapFrameIn in{0, kAutomapNoSlot, 0, 0};
+    if (kState && st.frames) in = st.frames[frame];
+    const AutomapLevel L = levels[kState ? in.level : frame_level ? frame_level[frame] : 0];
     const AutomapFrame f = automap_frame(poses[frame], vw, scale, flags);
     const uint32_t *mapped = seen ? seen + frame * words : nullptr;
+    AutomapStateFrame sf{nullptr, nullptr, 0, 0};
+    const AutomapDynLine *dyn = nullptr;
+    if (kState) {
+        sf = AutomapStateFrame{in.off == kAutomapNoSlot ? nullptr : st.off + in.off, st.arrows + in.arrow_first, in.n_arrows,
+                               poses[frame].angle};
+        dyn = st.dyn[in.level];
+    }
     __syncthreads();
-    const int n = automap_items(L, flags);
+    const int n = kState ? automap_state_items(L, sf, flags) : automap_items(L, flags);
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         int64_t e[4];
-        const uint32_t colour = kSeen ? automap_seen_item(f, L, mapped, flags, i, e) : automap_item(f, L, flags, i, e);
+        const uint32_t colour = kState  ? automap_state_item(f, L, dyn, sf, mapped, flags, i, e)
+                                : kSeen ? automap_seen_item(f, L, mapped, flags, i, e)
+                                        : automap_item(f, L, flags, i, e);
         if (!colour) continue;
         const uint32_t key = ((uint32_t)(i + 1) << 8) | colour;
         automap_line(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1,
@@ -1852,6 +1866,14 @@ b2d_automap_seen_kernel(const AutomapLevel *__restrict__ levels, const uint32_t 
                         int tiles_x, int tiles, bool vec, const uint32_t *__restrict__ seen, uint32_t words) {
     automap_tile<true>(levels, frame_level, poses, vw, scale, flags, out, tiles_x, tiles, vec, seen, words);
 }
+
+// Kernel 5's state variant (C21), also a kernel of its own.
+__global__ void __launch_bounds__(256)
+b2d_automap_states_kernel(const AutomapLevel *__restrict__ levels, const Pose *__restrict__ poses, View vw, int32_t scale,
+                          int flags, uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec, const uint32_t *__restrict__ seen,
+                          uint32_t words, const AutomapStateTables st) {
+    automap_tile<true, true>(levels, nullptr, poses, vw, scale, flags, out, tiles_x, tiles, vec, seen, words, st);
+}
 }  // namespace
 
 size_t automap_tiles(const View &vw) {
@@ -1860,14 +1882,17 @@ size_t automap_tiles(const View &vw) {
 
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
                            const View &vw, int32_t scale, int flags, bool seen_variant, const uint32_t *d_seen, uint32_t words,
-                           uint8_t *d_out, cudaStream_t stream) {
+                           uint8_t *d_out, cudaStream_t stream, const AutomapStateTables *states) {
     if (n_frames == 0) return cudaSuccess;
     const int tiles_x = (vw.W + kAutomapTileW - 1) / kAutomapTileW;
     const int tiles = (int)automap_tiles(vw);
     if (n_frames * (size_t)tiles > 0x7FFFFFFFull) return cudaErrorInvalidValue;
     const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
     const unsigned blocks = (unsigned)(n_frames * tiles);
-    if (seen_variant)
+    if (states)
+        b2d_automap_states_kernel<<<blocks, 256, 0, stream>>>(d_levels, d_poses, vw, scale, flags, d_out, tiles_x, tiles, vec,
+                                                              d_seen, words, *states);
+    else if (seen_variant)
         b2d_automap_seen_kernel<<<blocks, 256, 0, stream>>>(d_levels, d_frame_level, d_poses, vw, scale, flags, d_out, tiles_x,
                                                             tiles, vec, d_seen, words);
     else

@@ -161,14 +161,30 @@ cudaError_t launch_palette_levels(const uint32_t *d_palettes, const uint32_t *d_
 // (d_tables NULL: table 0), box-filtered by `factor` (1..8, dividing W and H) into d_out in B2D_RESOLVE_* `format`.
 cudaError_t launch_resolve(const uint32_t *d_palettes, const uint32_t *d_tables, const uint8_t *d_index, void *d_out,
                            size_t n_frames, int W, int H, int factor, int format, cudaStream_t stream);
+// A frame's inputs to the state variant, staged per call: its level, the word offset of its sector offsets (floor,
+// ceiling per dynamic slot of its level) in `off` (kAutomapNoSlot: at rest), and its arrows arrows[arrow_first ..
+// arrow_first + n_arrows).
+struct AutomapFrameIn {
+    uint32_t level, off, arrow_first, n_arrows;
+};
+// The state variant's tables: per level its AutomapDynLine table (nullptr: no changeable lines), then the call's staging
+// (frames: nullptr for every frame on level 0, at rest, without arrows).
+struct AutomapStateTables {
+    const AutomapDynLine *const *dyn;
+    const AutomapFrameIn *frames;
+    const int32_t *off;
+    const AutomapArrow *arrows;
+};
 // Kernel 5's grid: CTAs (128 x 32 tiles) per frame of view vw.
 size_t automap_tiles(const View &vw);
 // Kernel 5: the C19 automap of n_frames poses into contiguous W x H index frames at d_out, frame f from the items of
 // levels[frame_level[f]] (d_frame_level NULL: level 0), `scale` and `flags` as checked by b2d_automap_device.
 // `seen_variant`: its seen variant (C20), frame f's lines coloured by row f of d_seen (`words` per row; nullptr: every
-// line mapped); d_seen and words are not read otherwise.
+// line mapped); d_seen and words are not read otherwise.  `states` (nullable): the state variant (C21) instead, which
+// takes frame f's level from states->frames[f] (d_frame_level is not read), its sector offsets and arrows, and colours
+// its lines by row f of d_seen as the seen variant does.
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
                            const View &vw, int32_t scale, int flags, bool seen_variant, const uint32_t *d_seen, uint32_t words,
-                           uint8_t *d_out, cudaStream_t stream);
+                           uint8_t *d_out, cudaStream_t stream, const AutomapStateTables *states = nullptr);
 
 }  // namespace b2d

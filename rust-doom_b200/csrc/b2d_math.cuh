@@ -626,6 +626,13 @@ B2D_HD void automap_map(const AutomapFrame &f, int64_t mx, int64_t my, int64_t &
 B2D_HD int automap_items(const AutomapLevel &L, int flags) {
     return L.nlines + kAutomapArrowSegs + ((flags & kAutomapThings) ? kAutomapThingSegs * L.nthings : 0);
 }
+// Segment i (0..6) of player_arrow, (ax, 0) - (bx, by) in 16.16 offsets from the arrow's centre, pointing along +x.
+B2D_HD void automap_arrow_seg(int i, int32_t &ax, int32_t &bx, int32_t &by) {
+    constexpr int32_t R = kAutomapArrowR;
+    ax = i == 0 ? -R + R / 8 : i <= 2 ? R : i <= 4 ? -R + R / 8 : -R + 3 * R / 8;
+    bx = i == 0 ? R : i <= 2 ? R - R / 2 : i <= 4 ? -R - R / 8 : -R + R / 8;
+    by = i == 0 ? 0 : (i & 1) ? R / 4 : -(R / 4);
+}
 // Item i's endpoints in Q8 screen coordinates (e[0], e[1]) - (e[2], e[3]) and its colour (0: not drawn).
 B2D_HD uint32_t automap_item(const AutomapFrame &f, const AutomapLevel &L, int flags, int i, int64_t e[4]) {
     if (i < L.nlines) {
@@ -637,10 +644,8 @@ B2D_HD uint32_t automap_item(const AutomapFrame &f, const AutomapLevel &L, int f
     }
     i -= L.nlines;
     if (i < kAutomapArrowSegs) {          // player_arrow, in its own rotation about the centre
-        constexpr int32_t R = kAutomapArrowR;
-        const int32_t ax = i == 0 ? -R + R / 8 : i <= 2 ? R : i <= 4 ? -R + R / 8 : -R + 3 * R / 8;
-        const int32_t bx = i == 0 ? R : i <= 2 ? R - R / 2 : i <= 4 ? -R - R / 8 : -R + R / 8;
-        const int32_t by = i == 0 ? 0 : (i & 1) ? R / 4 : -(R / 4);
+        int32_t ax, bx, by;
+        automap_arrow_seg(i, ax, bx, by);
         automap_screen(f, ax, 0, true, f.ac, f.as, e[0], e[1]);
         automap_screen(f, bx, by, true, f.ac, f.as, e[2], e[3]);
         return kAutomapArrowColour;
@@ -670,6 +675,90 @@ B2D_HD uint32_t automap_seen_item(const AutomapFrame &f, const AutomapLevel &L, 
     const uint32_t colour = automap_item(f, L, flags & ~kAutomapAllmap, i, e);
     if (i >= L.nlines) return colour;
     const AutomapLine &l = L.lines[i];
+    const uint32_t ld = (uint32_t)l.linedef;
+    return automap_seen_colour(l, mapped == nullptr || ((mapped[ld >> 5] >> (ld & 31)) & 1u), flags);
+}
+
+// ---- the automap at the frame's state, with other players' arrows (b2d_automap_states_device, C21) ----------------------
+// The device line table's bit for a line whose colour can follow the frame's sector heights: two-sided, neither special 39
+// nor ML_SECRET, with a dynamic sector on at least one side.  Its AutomapDynLine (same index as the line) holds the rest
+// heights of its front [0] and back [1] sectors, from the SECTORS lump, and their dynamic slots (kAutomapNoSlot: none).
+constexpr uint16_t kAutomapChangeable = 2;
+constexpr uint32_t kAutomapNoSlot = 0xFFFFFFFFu;
+constexpr uint32_t kAutomapFloorStep = 64, kAutomapCeilStep = 231, kAutomapPlain = 96;
+struct AutomapDynLine {
+    int32_t floor[2], ceil[2];
+    uint32_t slot[2];
+};
+static_assert(sizeof(AutomapDynLine) == 24, "AutomapDynLine");
+// Another player's arrow (b2d_automap_arrow): position in 16.16 map units, angle in BAM, colour 1..255.
+struct AutomapArrow {
+    int32_t x, y;
+    uint32_t angle, colour;
+};
+static_assert(sizeof(AutomapArrow) == 16, "AutomapArrow");
+// What a frame adds to C20's inputs: its sector offsets (floor, ceiling per dynamic slot; nullptr: at rest), its arrows,
+// and its pose's angle (the arrows' rotation under kAutomapRotate).
+struct AutomapStateFrame {
+    const int32_t *off;
+    const AutomapArrow *arrows;
+    uint32_t n_arrows, pose_angle;
+};
+
+// A changeable line's colours at sector offsets `off`: C19's rule for a two-sided line that is neither a teleporter nor
+// secret, with each sector's rest heights plus its slot's offsets (ML_DONTDRAW: not drawn normally).
+B2D_HD void automap_state_colours(AutomapLine &l, const AutomapDynLine &d, const int32_t *off) {
+    int32_t fl[2], ce[2];
+    for (int k = 0; k < 2; k++) {
+        const bool dyn = d.slot[k] != kAutomapNoSlot;
+        fl[k] = d.floor[k] + (dyn ? off[2 * d.slot[k]] : 0);
+        ce[k] = d.ceil[k] + (dyn ? off[2 * d.slot[k] + 1] : 0);
+    }
+    const uint32_t c = fl[0] != fl[1] ? kAutomapFloorStep : ce[0] != ce[1] ? kAutomapCeilStep : 0u;
+    l.colour = (uint8_t)((l.dev_flags & kAutomapDontDraw) ? 0u : c);
+    l.colour_all = (uint8_t)(c ? c : kAutomapPlain);
+}
+
+// Items of a frame in draw order: the level's linedefs, the player arrow, 7 segments per arrow of the frame, the things.
+B2D_HD int automap_state_items(const AutomapLevel &L, const AutomapStateFrame &s, int flags) {
+    return automap_items(L, flags) + kAutomapArrowSegs * (int)s.n_arrows;
+}
+
+// Segment k of arrow `a`: its centre is its position through the frame's map transform; its shape is turned once by
+// sincos_q30 of the arrow's angle (north-up) or of angle + 90 deg - the pose's angle (kAutomapRotate), with the own
+// arrow's formula, scaled as automap_screen scales and added to the centre.  An arrow at the pose draws the own arrow.
+B2D_HD void automap_arrow(const AutomapFrame &f, const AutomapArrow &a, uint32_t pose_angle, int k, int64_t e[4]) {
+    int32_t c, s, ax, bx, by;
+    sincos_q30(f.rot ? a.angle + 0x40000000u - pose_angle : a.angle, c, s);
+    automap_arrow_seg(k, ax, bx, by);
+    int64_t X, Y;
+    automap_map(f, a.x, a.y, X, Y);
+    X -= (int64_t)f.W << 7;
+    Y -= (int64_t)f.H << 7;
+    automap_screen(f, ax, 0, true, c, s, e[0], e[1]);
+    automap_screen(f, bx, by, true, c, s, e[2], e[3]);
+    e[0] += X; e[1] += Y; e[2] += X; e[3] += Y;
+}
+
+// Item i as automap_seen_item draws it, with each changeable line coloured at the frame's offsets and the frame's arrows
+// after the own arrow.  `dyn`: the level's AutomapDynLine table (read only for changeable lines).  With s.off nullptr and
+// no arrows, automap_seen_item.
+B2D_HD uint32_t automap_state_item(const AutomapFrame &f, const AutomapLevel &L, const AutomapDynLine *dyn,
+                                   const AutomapStateFrame &s, const uint32_t *mapped, int flags, int i, int64_t e[4]) {
+    const int own_end = L.nlines + kAutomapArrowSegs;
+    if (i >= own_end) {
+        const int j = i - own_end;
+        if (j < kAutomapArrowSegs * (int)s.n_arrows) {
+            const int a = j / kAutomapArrowSegs;
+            automap_arrow(f, s.arrows[a], s.pose_angle, j - a * kAutomapArrowSegs, e);
+            return s.arrows[a].colour;
+        }
+        i -= kAutomapArrowSegs * (int)s.n_arrows;      // a thing
+    }
+    const uint32_t colour = automap_item(f, L, flags & ~kAutomapAllmap, i, e);
+    if (i >= L.nlines) return colour;
+    AutomapLine l = L.lines[i];
+    if (s.off && (l.dev_flags & kAutomapChangeable)) automap_state_colours(l, dyn[i], s.off);
     const uint32_t ld = (uint32_t)l.linedef;
     return automap_seen_colour(l, mapped == nullptr || ((mapped[ld >> 5] >> (ld & 31)) & 1u), flags);
 }
