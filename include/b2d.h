@@ -188,6 +188,13 @@ typedef struct b2d_automap_line {
     int32_t linedef;            /* index in LINEDEFS */
 } b2d_automap_line;
 int b2d_scene_automap_lines(const b2d_scene *s, b2d_automap_line *out, size_t capacity, size_t *n_out);
+/* The automap grid's origin (DESIGN.md C22), in map units: its lines lie at x = x + 128 j and y = y + 128 j.  An archive
+ * scene takes it from its level's BLOCKMAP header, the two int16 at the start of the lump at marker + 10 (ML_BLOCKMAP),
+ * when that lump is named BLOCKMAP and holds at least 8 bytes, and is (0, 0) otherwise; a scene from lumps starts at
+ * (0, 0), since b2d_level_lumps has no BLOCKMAP: a host that has the lump sets it.  The origin is not in the blob.
+ * Renderers copy it when they are created, as they copy palettes.  A NULL argument is B2D_ERR_INVALID_ARG. */
+int b2d_scene_automap_grid_origin(const b2d_scene *s, int32_t *x_out, int32_t *y_out);
+int b2d_scene_set_automap_grid_origin(b2d_scene *s, int32_t x, int32_t y);
 /* Read-only access to the compiled "B2DS" blob (layout in DESIGN.md); valid until destroy. */
 const void *b2d_scene_blob(const b2d_scene *s, size_t *size_out);
 /* LevelWalker::sector_at (visitor.rs:1028-1060): sector id at a map position, -1 if outside. */
@@ -536,6 +543,39 @@ int b2d_automap_states_device(b2d_renderer *r, const b2d_pose *d_poses, const ui
                               const b2d_sector_move *moves, size_t n_moves, const b2d_arrow_range *arrow_ranges,
                               const b2d_automap_arrow *arrows, size_t n_arrows, const uint32_t *d_seen, size_t n_frames,
                               int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream);
+
+/* Doom's automap with its grid and the players' numbered marks (AM_drawGrid, AM_drawMarks; DESIGN.md C22):
+ * b2d_automap_states_device, plus
+ *  - B2D_AUTOMAP_GRID (Doom's G key): under everything, in grey 104, the lines x = ox + 128 j and y = oy + 128 j of
+ *    every j whose line lies in [-32768, 32767] map units, each spanning that whole range, through the frame's map
+ *    transform (so they turn with the map under B2D_AUTOMAP_ROTATE).  (ox, oy) is the frame's level's grid origin
+ *    (b2d_scene_automap_grid_origin).  Unlike vanilla Doom, which skips the first line left of and below the origin,
+ *    every line of the lattice is drawn.
+ *  - marks marks[mark_ranges[f].first .. + n], over everything, in list order: each is digit `number` (0 .. 9) of the
+ *    frame's level, the patch AMMNUM<number>, magnified k = max(1, H / 200) times.  The mark's point (x, y; 16.16 map units,
+ *    as b2d_pose) goes through the frame's map transform to pixel (X >> 8, Y >> 8) of its Q8 position; the patch's top-left
+ *    corner is that pixel minus k (leftoffset, topoffset), and each opaque texel fills a k x k block with its palette
+ *    index (0 included).  A mark is drawn only when its whole k w x k h rectangle lies inside the frame, and not at all
+ *    when its level lacks the digit.  Under B2D_AUTOMAP_ROTATE the position turns with the map and the patch stays upright.
+ * Archive scenes take the digits from the lumps AMMNUM0 .. AMMNUM9 (a later lump wins; a lump that is not a picture is a
+ * missing digit), scenes from lumps from b2d_textures entries of those names, at offsets 0.  They upload with the first
+ * automap call of any kind.  `mark_ranges` and `marks` are HOST arrays, NULL mark_ranges no marks; the per-frame marks go
+ * to the device in the same single copy as the call's other per-frame inputs.  With B2D_AUTOMAP_GRID clear and no marks
+ * the frames are byte-identical to b2d_automap_states_device's, in as many launches.  Refusals, each B2D_ERR_INVALID_ARG
+ * and detected before anything is enqueued: every refusal of b2d_automap_states_device (but for B2D_AUTOMAP_GRID); flag
+ * bits above B2D_AUTOMAP_GRID; a NULL marks with n_marks > 0 (when mark_ranges is given), a mark range past n_marks, a
+ * mark number above 9; a frame whose lines + 7 + 7 * arrows + 3 * things + marks items reach 2^24.  The other automap
+ * calls refuse B2D_AUTOMAP_GRID. */
+#define B2D_AUTOMAP_GRID 16
+typedef struct b2d_automap_mark {
+    int32_t x, y;               /* 16.16 map units, as b2d_pose */
+    uint32_t number;            /* 0 .. 9: drawn with AMMNUM<number> */
+} b2d_automap_mark;
+int b2d_automap_marks_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
+                             const b2d_sector_move *moves, size_t n_moves, const b2d_arrow_range *arrow_ranges,
+                             const b2d_automap_arrow *arrows, size_t n_arrows, const uint32_t *d_seen, size_t n_frames,
+                             int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream, const b2d_arrow_range *mark_ranges,
+                             const b2d_automap_mark *marks, size_t n_marks);
 
 /* ---- multi-GPU: pose-sharded render with a chunked, overlapped all-gather of finished frames ------------------
  * The reference has no collective and no multi-device path (SURVEY.md 2); the hand-off this replaces is the

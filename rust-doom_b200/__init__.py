@@ -164,6 +164,25 @@ def _frame_arrows(arrows, n: int):
     return ranges, arr, len(flat)
 
 
+def _frame_marks(marks, n: int):
+    """(b2d_arrow_range array, concatenated b2d_automap_mark list, its length) for n frames: frame i's marks marks[i] (an
+    (k, 3) array or a list of (x, y, number): 16.16 map units, digit 0..9; None = none)"""
+    per = list(marks)
+    assert len(per) == n, "one mark list per frame"
+    ranges = (_lib.ArrowRange * max(n, 1))()
+    flat = []
+    for i in range(n):
+        m = [] if per[i] is None else np.asarray(per[i], dtype=np.int64).reshape(-1, 3).tolist()
+        ranges[i] = _lib.ArrowRange(len(flat), len(m))
+        flat += m
+    arr = (_lib.AutomapMark * max(len(flat), 1))()
+    for k, (x, y, number) in enumerate(flat):
+        if not (-2 ** 31 <= x < 2 ** 31 and -2 ** 31 <= y < 2 ** 31 and 0 <= number < 2 ** 32):
+            raise B2dError(ERR_INVALID_ARG, "automap mark out of range")
+        arr[k] = _lib.AutomapMark(int(x), int(y), int(number))
+    return ranges, arr, len(flat)
+
+
 def _frame_lights(lights, n: int):
     """b2d_frame_light array for n poses from (fixed_colormap, extralight) pairs, one per pose (a sequence or an (n, 2)
     integer array); the values are checked by the library (fixed_colormap -1..32, extralight 0..2)."""
@@ -240,6 +259,21 @@ class Scene:
             raise ValueError("a PLAYPAL is a positive multiple of 768 bytes")
         buf = ctypes.create_string_buffer(raw, len(raw))
         _check(_lib.load().b2d_scene_set_palettes(self._h, buf, len(raw) // 768))
+
+    @property
+    def automap_grid_origin(self):
+        """b2d_scene_automap_grid_origin: (x, y) in map units, where the automap grid's lines cross (DESIGN.md C22): the
+        level's BLOCKMAP origin for an archive scene, (0, 0) for a scene from lumps until set."""
+        x, y = ctypes.c_int32(), ctypes.c_int32()
+        _check(_lib.load().b2d_scene_automap_grid_origin(self._h, ctypes.byref(x), ctypes.byref(y)))
+        return x.value, y.value
+
+    def set_automap_grid_origin(self, x: int, y: int):
+        """b2d_scene_set_automap_grid_origin: the grid origin in map units, e.g. the first two int16 of the level's
+        BLOCKMAP lump.  Renderers created afterwards see it; existing ones do not."""
+        if not (-2 ** 31 <= int(x) < 2 ** 31 and -2 ** 31 <= int(y) < 2 ** 31):
+            raise ValueError("grid origin out of the int32 range")
+        _check(_lib.load().b2d_scene_set_automap_grid_origin(self._h, int(x), int(y)))
 
     def tables_at(self, tics: int = 0, moves=()) -> bytes:
         """b2d_scene_tables_at: the state-dependent tables [textures | sectors | segs | sprites | mids] at level time `tics`
@@ -363,14 +397,15 @@ RESOLVE_FORMATS = {"rgba": RESOLVE_RGBA8, "rgb": RESOLVE_RGB8, "rgb_planar": RES
 
 
 AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS = _lib.AUTOMAP_ROTATE, _lib.AUTOMAP_ALL_LINES, _lib.AUTOMAP_THINGS
-AUTOMAP_ALLMAP = _lib.AUTOMAP_ALLMAP
-AUTOMAP_FLAGS = {"rotate": AUTOMAP_ROTATE, "all": AUTOMAP_ALL_LINES, "things": AUTOMAP_THINGS, "allmap": AUTOMAP_ALLMAP}
+AUTOMAP_ALLMAP, AUTOMAP_GRID = _lib.AUTOMAP_ALLMAP, _lib.AUTOMAP_GRID
+AUTOMAP_FLAGS = {"rotate": AUTOMAP_ROTATE, "all": AUTOMAP_ALL_LINES, "things": AUTOMAP_THINGS, "allmap": AUTOMAP_ALLMAP,
+                 "grid": AUTOMAP_GRID}
 AUTOMAP_DEFAULT_SCALE_Q16 = 13107       # Doom's default automap scale, 0.2 pixels per map unit
 
 
 def automap_flags(flags) -> int:
-    """B2D_AUTOMAP_* bits from an int, or from names ("rotate", "all", "things", "allmap") as a list or a comma-separated
-    string"""
+    """B2D_AUTOMAP_* bits from an int, or from names ("rotate", "all", "things", "allmap", "grid") as a list or a
+    comma-separated string"""
     if isinstance(flags, int):
         return flags
     names = flags.split(",") if isinstance(flags, str) else list(flags)
@@ -378,7 +413,7 @@ def automap_flags(flags) -> int:
     for name in (x.strip() for x in names):
         if name:
             if name not in AUTOMAP_FLAGS:
-                raise ValueError("unknown automap flag %r (rotate, all, things, allmap)" % name)
+                raise ValueError("unknown automap flag %r (rotate, all, things, allmap, grid)" % name)
             out |= AUTOMAP_FLAGS[name]
     return out
 
@@ -757,14 +792,30 @@ class Renderer:
         else:
             _check(_lib.load().b2d_automap_device(self._h, poses_ptr, lvp, n, int(scale_q16), int(flags), out_ptr, stream or None))
 
-    def automap(self, poses, levels=None, scale: float = 0.2, flags=0, seen=None, moves_per_pose=None, arrows=None):
+    def automap_marks_device(self, poses_ptr: int, n: int, out_ptr: int, scale_q16: int = AUTOMAP_DEFAULT_SCALE_Q16,
+                             flags: int = 0, levels=None, stream: int = 0, seen_ptr=None, moves_per_pose=None, arrows=None,
+                             marks=None):
+        """b2d_automap_marks_device (DESIGN.md C22): automap_device's state automap, which also takes AUTOMAP_GRID (the
+        grid at the level's grid origin, under everything) and `marks`: per frame None or a list of (x, y, number) rows
+        (16.16 map units, digit 0..9), drawn over everything with the level's AMMNUM digit patches."""
+        lv = None if levels is None else _levels_array(levels, n)
+        lvp = None if lv is None else lv.ctypes.data
+        states, mv, nm = _frame_states(0, moves_per_pose, n) if moves_per_pose is not None else (None, None, 0)
+        ranges, arr, na = _frame_arrows(arrows, n) if arrows is not None else (None, None, 0)
+        mranges, marr, nmk = _frame_marks(marks, n) if marks is not None else (None, None, 0)
+        _check(_lib.load().b2d_automap_marks_device(self._h, poses_ptr, lvp, states, mv, nm, ranges, arr, na, seen_ptr or None, n,
+                                                    int(scale_q16), int(flags), out_ptr, stream or None, mranges, marr, nmk))
+
+    def automap(self, poses, levels=None, scale: float = 0.2, flags=0, seen=None, moves_per_pose=None, arrows=None,
+                marks=None):
         """The automaps of host or CUDA poses as a CUDA uint8 tensor [n, H, W] of palette indices, on the current torch
         stream: `scale` in pixels per map unit (Doom's default 0.2), `flags` an int or names from "rotate", "all", "things",
         "allmap".  `seen`: a CUDA int32 tensor [n, seen_words] of seen lines (render_seen), whose mapped lines each frame
         draws (automap_device's seen_ptr).  `moves_per_pose`: each frame's sector moves, the lists render_levels_states
         takes, so each door and lift line has its colour at that frame's state; `arrows`: per frame None or an array of
-        (x, y, angle, colour) rows, other players' arrows (DESIGN.md C21).  Colour the frames with resolve() or
-        palette_lut_levels_device like rendered frames."""
+        (x, y, angle, colour) rows, other players' arrows (DESIGN.md C21).  "grid" in `flags` draws the grid and `marks`
+        (per frame None or (x, y, number) rows) the numbered marks (C22, automap_marks_device).  Colour the frames with
+        resolve() or palette_lut_levels_device like rendered frames."""
         import torch
         flags = automap_flags(flags)
         dev = torch.device("cuda", self.device)
@@ -782,8 +833,12 @@ class Renderer:
             if not (seen.is_cuda and seen.dtype == torch.int32 and tuple(seen.shape) == (n, self.seen_words) and seen.is_contiguous()):
                 raise ValueError("seen must be a contiguous CUDA int32 tensor [%d, %d]" % (n, self.seen_words))
             seen_ptr = seen.data_ptr()
-        self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream, seen_ptr,
-                            moves_per_pose, arrows)
+        if flags & AUTOMAP_GRID or marks is not None:
+            self.automap_marks_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream,
+                                      seen_ptr, moves_per_pose, arrows, marks)
+        else:
+            self.automap_device(p.data_ptr(), n, out.data_ptr(), int(round(scale * 65536)), flags, levels, stream, seen_ptr,
+                                moves_per_pose, arrows)
         return out
 
     def worklist(self, n: int):

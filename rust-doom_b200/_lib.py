@@ -66,13 +66,13 @@ EXPORTS = [
     "b2d_render_sharded_levels_states_resolved_palettes",
     "b2d_render_levels_states_lights", "b2d_render_device_levels_states_lights", "b2d_walk_device_levels_states_lights",
     "b2d_scene_automap_lines", "b2d_automap_device", "b2d_renderer_seen_words", "b2d_raster_device_seen", "b2d_automap_seen_device",
-    "b2d_automap_states_device",
+    "b2d_automap_states_device", "b2d_scene_automap_grid_origin", "b2d_scene_set_automap_grid_origin", "b2d_automap_marks_device",
 ]
 
 COMM_ID_BYTES = 128
 RESOLVE_RGBA8, RESOLVE_RGB8, RESOLVE_RGB8_PLANAR, RESOLVE_GRAY8 = 0, 1, 2, 3      # B2D_RESOLVE_*
 SHARD_RENDER_ONLY, SHARD_RENDER_GATHER, SHARD_GATHER_ONLY = 0, 1, 2
-AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS, AUTOMAP_ALLMAP = 1, 2, 4, 8      # B2D_AUTOMAP_*
+AUTOMAP_ROTATE, AUTOMAP_ALL_LINES, AUTOMAP_THINGS, AUTOMAP_ALLMAP, AUTOMAP_GRID = 1, 2, 4, 8, 16      # B2D_AUTOMAP_*
 
 
 class AutomapLine(ctypes.Structure):
@@ -89,6 +89,11 @@ class AutomapArrow(ctypes.Structure):
 class ArrowRange(ctypes.Structure):
     """b2d_arrow_range: arrows[first .. first + n) of the call's arrow list"""
     _fields_ = [("first", ctypes.c_uint32), ("n", ctypes.c_uint32)]
+
+
+class AutomapMark(ctypes.Structure):
+    """b2d_automap_mark: a numbered mark at (x, y) in 16.16 map units, drawn with digit patch AMMNUM<number> (0..9)"""
+    _fields_ = [("x", ctypes.c_int32), ("y", ctypes.c_int32), ("number", ctypes.c_uint32)]
 
 
 class ShardedStats(ctypes.Structure):
@@ -240,6 +245,11 @@ def load() -> ctypes.CDLL:
     L.b2d_automap_states_device.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), ctypes.POINTER(SectorMove), cs,
                                             ctypes.POINTER(ArrowRange), ctypes.POINTER(AutomapArrow), cs, vp, cs, ctypes.c_int32,
                                             ci, vp, vp]
+    L.b2d_scene_automap_grid_origin.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]
+    L.b2d_scene_set_automap_grid_origin.argtypes = [vp, ctypes.c_int32, ctypes.c_int32]
+    L.b2d_automap_marks_device.argtypes = [vp, vp, vp, ctypes.POINTER(FrameState), ctypes.POINTER(SectorMove), cs,
+                                           ctypes.POINTER(ArrowRange), ctypes.POINTER(AutomapArrow), cs, vp, cs, ctypes.c_int32,
+                                           ci, vp, vp, ctypes.POINTER(ArrowRange), ctypes.POINTER(AutomapMark), cs]
     L.b2d_render_sharded_levels_states_resolved_palettes.argtypes = [vp, vp, vp, vp, vp, ctypes.POINTER(FrameState), cs,
                                                                      ctypes.POINTER(SectorMove), cs, cs, ci, ci, ci, CHUNK_FN, vp,
                                                                      ctypes.POINTER(ShardedStats)]

@@ -29,7 +29,8 @@ coloured through palette 0 of its level and resolved at the --supersample factor
 the map with the view, draws every line (IDDT) and draws the decoration things; seen draws only the lines the run's
 frames of that level saw (Renderer.render_seen, DESIGN.md C20) and allmap adds the unseen ones in grey (the computer
 area map); others draws the arrows of the run's first four poses of that level in Doom's co-op colours, the dumped pose's
-own in green 112 and the next three in 96, 64 and 176 (b2d_automap_states_device, DESIGN.md C21).  Not with --world.
+own in green 112 and the next three in 96, 64 and 176 (b2d_automap_states_device, DESIGN.md C21); grid draws Doom's
+grid at the level's BLOCKMAP origin under the map (b2d_automap_marks_device, DESIGN.md C22).  Not with --world.
 
 --palette P colours the dumped and streamed frames through PLAYPAL palette P of each frame's level instead of palette 0
 (b2d_resolve_palettes_device; in Doom 1..8 are the damage flash, 9..12 the bonus flash, 13 the radiation suit), through
@@ -355,7 +356,8 @@ def main(argv=None) -> int:
                     help="with --dump: also write NAME.automap.EXT (NAME.automap.L.EXT with --levels), Doom's automap of "
                          "the dumped pose at SCALE pixels per map unit (Doom's default: 0.2)")
     ap.add_argument("--automap-flags", default="", help="with --automap: comma-separated rotate, all, things, allmap (unseen lines in grey), "
-                         "seen (only the lines the run's frames saw), others (the run's next three poses as team-mates' arrows)")
+                         "seen (only the lines the run's frames saw), others (the run's next three poses as team-mates' arrows), "
+                         "grid (Doom's 128-unit grid)")
     ap.add_argument("command", nargs="?", choices=["check", "list-levels"], default=None)
     args = ap.parse_args(argv)
 

@@ -787,6 +787,37 @@ std::vector<DynRec> dyn_list(const b2d_dynamic_sector *dyn, size_t n) {
     }
     return v;
 }
+
+// The automap digit names AMMNUM0 .. AMMNUM9 (C22)
+Name digit_name(int d) {
+    char name[8] = {'A', 'M', 'M', 'N', 'U', 'M', (char)('0' + d), 0};
+    return make_name(reinterpret_cast<const uint8_t *>(name), 8);
+}
+
+// An archive scene's grid origin and digits (C22): the origin from the header of the lump at marker + 10 (ML_BLOCKMAP)
+// when it is named BLOCKMAP and holds at least 8 bytes inside the file, else (0, 0); each digit the picture of its lump
+// name (a later lump wins), offsets included, or missing when absent, outside the file or undecodable.  Neither fails
+// the scene: the level renders without them.
+void archive_marks(const Archive &wad, int level_index, b2d_scene *s) {
+    const int bm = wad.level_lump_index(level_index) + 10;
+    if ((size_t)bm < wad.num_lumps() && wad.lump(bm).name == make_name("BLOCKMAP") && wad.lump(bm).size >= 8) {
+        try {
+            const uint8_t *p = wad.lump_data(bm);
+            s->grid_origin[0] = (int16_t)(p[0] | p[1] << 8);
+            s->grid_origin[1] = (int16_t)(p[2] | p[3] << 8);
+        } catch (const WadError &) {
+        }
+    }
+    for (int d = 0; d < kAutomapDigits; d++) {
+        const int i = wad.find(digit_name(d));
+        if (i < 0 || wad.lump(i).size <= 0) continue;
+        try {
+            s->digits[(size_t)d] = Image::decode(wad.lump_data(i), (size_t)wad.lump(i).size);
+        } catch (const WadError &) {
+            s->digits[(size_t)d] = Image{};
+        }
+    }
+}
 }  // namespace
 
 int b2d_scene_create_dynamic(const b2d_archive *a, int level_index, const b2d_dynamic_sector *dyn, size_t n_dyn, b2d_scene **out) {
@@ -797,6 +828,7 @@ int b2d_scene_create_dynamic(const b2d_archive *a, int level_index, const b2d_dy
         s->level = Level::load(*a->wad, level_index);
         s->blob = compile_scene(s->level, td, dyn_list(dyn, n_dyn));
         s->automap = automap_lines(s->level);
+        archive_marks(*a->wad, level_index, s.get());
         fill_scene_info(s.get());
         s->palettes = td.palettes;
         if (s->palettes.empty()) s->palettes.push_back({});
@@ -867,6 +899,8 @@ int b2d_scene_create_from_lumps_dynamic(const b2d_level_lumps *lv, const b2d_tex
         }
         s->blob = compile_scene(s->level, td, dyn_list(dyn, n_dyn));
         s->automap = automap_lines(s->level);
+        for (int d = 0; d < kAutomapDigits; d++)      // the digits among the caller's images, at offsets 0 (C22)
+            if (const Image *im = td.texture(digit_name(d))) s->digits[(size_t)d] = *im;
         fill_scene_info(s.get());
         s->palettes.assign(1, td.palettes.empty() ? std::array<uint8_t, 768>{} : td.palettes[0]);
         *out = s.release();
@@ -904,6 +938,20 @@ int b2d_scene_automap_lines(const b2d_scene *s, b2d_automap_line *out, size_t ca
     if (!out) return B2D_OK;
     if (capacity < s->automap.size()) return fail(B2D_ERR_INVALID_ARG, "buffer too small for the automap lines");
     if (!s->automap.empty()) std::memcpy(out, s->automap.data(), s->automap.size() * sizeof(AutomapLine));
+    return B2D_OK;
+}
+
+int b2d_scene_automap_grid_origin(const b2d_scene *s, int32_t *x_out, int32_t *y_out) {
+    if (!s || !x_out || !y_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
+    *x_out = s->grid_origin[0];
+    *y_out = s->grid_origin[1];
+    return B2D_OK;
+}
+
+int b2d_scene_set_automap_grid_origin(b2d_scene *s, int32_t x, int32_t y) {
+    if (!s) return fail(B2D_ERR_INVALID_ARG, "null scene");
+    s->grid_origin[0] = x;
+    s->grid_origin[1] = y;
     return B2D_OK;
 }
 
@@ -1174,6 +1222,9 @@ static int create_renderer(const b2d_scene *const *scenes, size_t n_levels, cons
             for (AutomapLine &l : r->lv[k].automap_lines)      // the device copy's don't-draw bit (the seen automap's ALLMAP rule)
                 if (scenes[k]->level.linedefs[(size_t)l.linedef].flags & 0x80) l.dev_flags = kAutomapDontDraw;
             automap_dyn_lines(scenes[k]->level, r->lv[k].layout, r->lv[k].automap_lines, r->lv[k].automap_dyn);
+            r->lv[k].grid_origin[0] = scenes[k]->grid_origin[0];
+            r->lv[k].grid_origin[1] = scenes[k]->grid_origin[1];
+            r->lv[k].digits = scenes[k]->digits;
             for (uint32_t i = 0; i < h[H_NSPRITES]; i++) {
                 r->lv[k].automap_things.push_back(sp[i].x);
                 r->lv[k].automap_things.push_back(sp[i].y);
@@ -1561,11 +1612,17 @@ int b2d_resolve_device(b2d_renderer *r, const uint8_t *d_index, const uint32_t *
 
 // The automap tables of every level (b2d_renderer::automap): the lines and things of each level in one buffer, then an
 // AutomapLevel per level pointing into it, then each level's AutomapDynLine table pointer (automap_dyn_records) and the
-// tables.
+// tables, then an AutomapMarkLevel per level (automap_mark_records: the grid origin and digits, C22) and the digits' texels.
 static size_t automap_dyn_records(const b2d_renderer *r) { return r->automap->off + r->lv.size() * sizeof(AutomapLevel); }
+// `items`: where the AutomapLevel records start (b2d_renderer::Tables::off).
+static size_t automap_mark_records(const b2d_renderer *r, size_t items) {
+    size_t bytes = items + r->lv.size() * (sizeof(AutomapLevel) + sizeof(const AutomapDynLine *));
+    for (const LevelRes &lv : r->lv) bytes += lv.automap_dyn.size() * sizeof(AutomapDynLine);
+    return (bytes + 15) & ~(size_t)15;
+}
 static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
     size_t items = 0;
-    std::vector<size_t> line_off, thing_off, dyn_off;
+    std::vector<size_t> line_off, thing_off, dyn_off, digit_off;
     for (const LevelRes &lv : r->lv) {
         line_off.push_back(items);
         items += lv.automap_lines.size() * sizeof(AutomapLine);
@@ -1579,7 +1636,26 @@ static int ensure_automap(b2d_renderer *r, cudaStream_t st) {
         dyn_off.push_back(bytes);
         bytes += lv.automap_dyn.size() * sizeof(AutomapDynLine);
     }
+    const size_t mark_records = automap_mark_records(r, items);
+    bytes = mark_records + r->lv.size() * sizeof(AutomapMarkLevel);
+    for (const LevelRes &lv : r->lv)
+        for (const Image &im : lv.digits) {
+            digit_off.push_back(bytes);
+            bytes += im.px.size() * sizeof(uint16_t);
+        }
     return build_tables(r->automap, bytes, items, st, [&](uint8_t *h, const uint8_t *d) {
+        for (size_t k = 0; k < r->lv.size(); k++) {
+            const LevelRes &lv = r->lv[k];
+            AutomapMarkLevel m{lv.grid_origin[0], lv.grid_origin[1], {}};
+            for (int g = 0; g < kAutomapDigits; g++) {
+                const Image &im = lv.digits[(size_t)g];
+                const size_t at = digit_off[k * kAutomapDigits + (size_t)g];
+                if (im.px.empty()) continue;          // missing, or 0 x h / w x 0: nothing to draw
+                std::memcpy(h + at, im.px.data(), im.px.size() * sizeof(uint16_t));
+                m.digit[g] = AutomapDigit{reinterpret_cast<const uint16_t *>(d + at), im.w, im.h, im.xoff, im.yoff};
+            }
+            std::memcpy(h + mark_records + k * sizeof(AutomapMarkLevel), &m, sizeof m);
+        }
         for (size_t k = 0; k < r->lv.size(); k++) {
             const LevelRes &lv = r->lv[k];
             if (!lv.automap_lines.empty()) std::memcpy(h + line_off[k], lv.automap_lines.data(), lv.automap_lines.size() * sizeof(AutomapLine));
@@ -1650,13 +1726,26 @@ static int automap_states_image(const b2d_renderer *r, const uint32_t *levels, c
     });
 }
 
+static_assert(sizeof(b2d_automap_mark) == sizeof(AutomapMark) && offsetof(b2d_automap_mark, number) == offsetof(AutomapMark, number),
+              "b2d_automap_mark");
+static_assert(B2D_AUTOMAP_GRID == kAutomapGrid, "automap flags");
+
+// What b2d_automap_marks_device adds to the state automap (HOST arrays, nullable; C22).
+struct AutomapMarks {
+    const b2d_arrow_range *ranges;
+    const b2d_automap_mark *marks;
+    size_t n_marks;
+};
+
 // b2d_automap_device (seen_variant false, states nullptr: K5), b2d_automap_seen_device (its seen variant, which also takes
-// ALLMAP) and b2d_automap_states_device (states: the state variant)
+// ALLMAP), b2d_automap_states_device (states: the state variant) and b2d_automap_marks_device (states and marks: the
+// marks variant, which also takes GRID)
 static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const uint32_t *d_seen, size_t n_frames,
                         int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream, bool seen_variant,
-                        const AutomapStates *states = nullptr) {
+                        const AutomapStates *states = nullptr, const AutomapMarks *marks = nullptr) {
     if (!r || !d_poses || !d_out) return fail(B2D_ERR_INVALID_ARG, "null argument");
-    const int known = B2D_AUTOMAP_ROTATE | B2D_AUTOMAP_ALL_LINES | B2D_AUTOMAP_THINGS | (seen_variant ? B2D_AUTOMAP_ALLMAP : 0);
+    const int known = B2D_AUTOMAP_ROTATE | B2D_AUTOMAP_ALL_LINES | B2D_AUTOMAP_THINGS | (seen_variant ? B2D_AUTOMAP_ALLMAP : 0) |
+                      (marks ? B2D_AUTOMAP_GRID : 0);
     if (flags & ~known) return fail(B2D_ERR_INVALID_ARG, "unknown automap flags");
     if (reinterpret_cast<uintptr_t>(d_seen) & 3) return fail(B2D_ERR_INVALID_ARG, "seen rows not 4-byte aligned");
     if (scale_q16 < kAutomapScaleMin || scale_q16 > kAutomapScaleMax)
@@ -1688,7 +1777,33 @@ static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t
                     return fail(B2D_ERR_INVALID_ARG, "a frame has too many automap items (2^24)");
             }
         }
+        if (marks && marks->ranges) {
+            if (marks->n_marks && !marks->marks) return fail(B2D_ERR_INVALID_ARG, "null argument");
+            for (size_t k = 0; k < marks->n_marks; k++)
+                if (marks->marks[k].number > 9) return fail(B2D_ERR_INVALID_ARG, "automap mark number out of range (0 .. 9)");
+            for (size_t i = 0; i < n_frames; i++) {
+                const b2d_arrow_range &g = marks->ranges[i];
+                if (g.first > marks->n_marks || g.n > marks->n_marks - g.first)
+                    return fail(B2D_ERR_INVALID_ARG, "a frame's mark range runs past the end of the mark list");
+                const LevelRes &lv = r->lv[levels ? levels[i] : 0];
+                const uint64_t arrows = states->ranges ? states->ranges[i].n : 0;
+                if (lv.automap_lines.size() + kAutomapArrowSegs * (1 + arrows) + kAutomapThingSegs * lv.automap_things.size() / 2 + g.n >=
+                    (1u << 24))
+                    return fail(B2D_ERR_INVALID_ARG, "a frame has too many automap items (2^24)");
+            }
+        }
         if (int rc = automap_states_image(r, levels, *states, c, n_frames, img)) return rc;
+    }
+    // the marks variant's staging follows the state variant's: 2 words (first, n) per frame, then the marks
+    const size_t mark_at = img.size();
+    if (marks && marks->ranges) {
+        if (int rc = guarded([&] {
+                img.resize(mark_at + 2 * n_frames + 3 * marks->n_marks);
+                if (n_frames) std::memcpy(img.data() + mark_at, marks->ranges, 8 * n_frames);
+                if (marks->n_marks) std::memcpy(img.data() + mark_at + 2 * n_frames, marks->marks, 12 * marks->n_marks);
+                return B2D_OK;
+            }))
+            return rc;
     }
     if (n_frames == 0) return B2D_OK;
     CU(cudaSetDevice(r->device));
@@ -1697,7 +1812,8 @@ static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t
     const AutomapLevel *d_levels = reinterpret_cast<const AutomapLevel *>(r->automap->d.get() + r->automap->off);
     if (states) {
         // nothing per frame (level 0, at rest, no arrows): nothing to stage
-        const bool staged = levels || c.frames.starts || states->ranges;
+        const bool marked = marks && marks->ranges;
+        const bool staged = levels || c.frames.starts || states->ranges || marked;
         if (staged)
             if (int rc = stage_words(r->automap_states, img.size(), st, [&](size_t i) { return img[i]; })) return rc;
         const uint32_t *d = r->automap_states.d.get();
@@ -1706,8 +1822,11 @@ static int automap_call(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t
                                    staged ? reinterpret_cast<const AutomapFrameIn *>(d) : nullptr,
                                    staged ? reinterpret_cast<const int32_t *>(d + pool) : nullptr,
                                    staged ? reinterpret_cast<const AutomapArrow *>(d + 4 * n_frames) : nullptr};
+        const AutomapMarkTables m{
+            reinterpret_cast<const AutomapMarkLevel *>(r->automap->d.get() + automap_mark_records(r, r->automap->off)),
+            marked ? d + mark_at : nullptr, marked ? reinterpret_cast<const AutomapMark *>(d + mark_at + 2 * n_frames) : nullptr};
         CU(launch_automap(d_levels, nullptr, reinterpret_cast<const Pose *>(d_poses), n_frames, r->view, scale_q16, flags, true,
-                          d_seen, r->seen_words, d_out, st, &t));
+                          d_seen, r->seen_words, d_out, st, &t, marks ? &m : nullptr));
         if (staged) CU(cudaEventRecord(r->automap_states.done.get(), st));
         r->launches += 1;
         return B2D_OK;
@@ -1738,6 +1857,16 @@ int b2d_automap_states_device(b2d_renderer *r, const b2d_pose *d_poses, const ui
                               int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream) {
     const AutomapStates a{states, moves, n_moves, arrow_ranges, arrows, n_arrows};
     return automap_call(r, d_poses, levels, d_seen, n_frames, scale_q16, flags, d_out, cuda_stream, true, &a);
+}
+
+int b2d_automap_marks_device(b2d_renderer *r, const b2d_pose *d_poses, const uint32_t *levels, const b2d_frame_state *states,
+                             const b2d_sector_move *moves, size_t n_moves, const b2d_arrow_range *arrow_ranges,
+                             const b2d_automap_arrow *arrows, size_t n_arrows, const uint32_t *d_seen, size_t n_frames,
+                             int32_t scale_q16, int flags, uint8_t *d_out, void *cuda_stream, const b2d_arrow_range *mark_ranges,
+                             const b2d_automap_mark *marks, size_t n_marks) {
+    const AutomapStates a{states, moves, n_moves, arrow_ranges, arrows, n_arrows};
+    const AutomapMarks m{mark_ranges, marks, n_marks};
+    return automap_call(r, d_poses, levels, d_seen, n_frames, scale_q16, flags, d_out, cuda_stream, true, &a, &m);
 }
 
 int b2d_device_alloc(int device, size_t bytes, void **d_out) {

@@ -23,7 +23,8 @@
 // its level, resolved at the --supersample factor; --automap-flags rotate,all,things turns the map with the view, draws
 // every line and draws the decoration things; seen draws only the lines the run's frames of that level saw (b2d_raster_device_seen,
 // DESIGN.md C20), allmap adds the unseen ones in grey (the computer area map), others draws the arrows of the run's first
-// four poses of that level in Doom's co-op colours 112, 96, 64, 176 (b2d_automap_states_device, C21).  Not with --world.
+// four poses of that level in Doom's co-op colours 112, 96, 64, 176 (b2d_automap_states_device, C21), grid draws Doom's
+// grid at the level's BLOCKMAP origin under the map (b2d_automap_marks_device, C22).  Not with --world.
 #include <cmath>
 #include <algorithm>
 #include <cstdint>
@@ -125,7 +126,7 @@ int render_supersampled(b2d_renderer *r, int device, const b2d_view &view, const
 // to names[k]
 // With `seen` (n rows of b2d_renderer_seen_words words) or B2D_AUTOMAP_ALLMAP, frame k draws the lines row k has mapped
 // (b2d_automap_seen_device).  With `ranges` (one per frame) into `arrows`, frame k also draws those arrows
-// (b2d_automap_states_device).
+// (b2d_automap_states_device).  B2D_AUTOMAP_GRID draws the grid under the map (b2d_automap_marks_device).
 int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std::vector<b2d_pose> &poses, const uint32_t *levels,
                    int32_t scale_q16, int flags, int factor, const std::vector<std::string> &names,
                    const std::vector<uint32_t> *seen = nullptr, const std::vector<b2d_arrow_range> *ranges = nullptr,
@@ -150,7 +151,11 @@ int write_automaps(b2d_renderer *r, int device, const b2d_view &view, const std:
     uint8_t *di = static_cast<uint8_t *>(d_index);
     const b2d_pose *dp = static_cast<const b2d_pose *>(d_poses);
     const uint32_t *ds = static_cast<const uint32_t *>(d_seen);
-    const int rc = ranges ? b2d_automap_states_device(r, dp, levels, nullptr, nullptr, 0, ranges->data(), arrows->data(), arrows->size(),
+    const int rc = (flags & B2D_AUTOMAP_GRID)
+                       ? b2d_automap_marks_device(r, dp, levels, nullptr, nullptr, 0, ranges ? ranges->data() : nullptr,
+                                                  ranges ? arrows->data() : nullptr, ranges ? arrows->size() : 0, ds, n, scale_q16,
+                                                  flags, di, nullptr, nullptr, nullptr, 0)
+                   : ranges ? b2d_automap_states_device(r, dp, levels, nullptr, nullptr, 0, ranges->data(), arrows->data(), arrows->size(),
                                                       ds, n, scale_q16, flags, di, nullptr)
                    : seen || (flags & B2D_AUTOMAP_ALLMAP) ? b2d_automap_seen_device(r, dp, levels, ds, n, scale_q16, flags, di, nullptr)
                                                           : b2d_automap_device(r, dp, levels, n, scale_q16, flags, di, nullptr);
@@ -479,7 +484,8 @@ int main(int argc, char **argv) {
                 else if (name == "allmap") automap_flags |= B2D_AUTOMAP_ALLMAP;
                 else if (name == "seen") automap_seen = true;
                 else if (name == "others") automap_others = true;
-                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things, allmap, seen, others\n"); return 2; }
+                else if (name == "grid") automap_flags |= B2D_AUTOMAP_GRID;
+                else if (!name.empty()) { std::fprintf(stderr, "--automap-flags takes rotate, all, things, allmap, seen, others, grid\n"); return 2; }
                 at = comma + 1;
             }
         }

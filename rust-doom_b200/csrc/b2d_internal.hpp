@@ -131,6 +131,10 @@ struct b2d_scene {
     // the scene was made without a PLAYPAL)
     std::vector<std::array<uint8_t, 768>> palettes;
     std::vector<AutomapLine> automap;                     // automap_lines(level), built at creation
+    // The automap's grid origin (map units; the BLOCKMAP header's for an archive scene, else (0, 0) until set) and its
+    // digit patches AMMNUM0 .. AMMNUM9 (DESIGN.md C22); a digit with w == 0 is missing.
+    int32_t grid_origin[2] = {0, 0};
+    std::array<Image, kAutomapDigits> digits;
 };
 
 // A worklist slot: the BSP walk of batch k+1 may run (b2d_walk_device, another stream) while batch k is rastered.
@@ -215,6 +219,9 @@ struct LevelRes {
     // The state automap's (C21): an AutomapDynLine per automap line, read for the lines whose device copy has the
     // kAutomapChangeable bit; empty when the level has none.
     std::vector<AutomapDynLine> automap_dyn;
+    // The marks automap's (C22): the scene's grid origin and digit patches, copied at creation
+    int32_t grid_origin[2] = {0, 0};
+    std::array<Image, kAutomapDigits> digits;
     // Seen lines (DESIGN.md C20): the linedef of each seg of the level's SEGS lump (-1: none), built at creation and
     // uploaded by the first b2d_raster_device_seen call (b2d_renderer::seen)
     std::vector<int32_t> seg_line;

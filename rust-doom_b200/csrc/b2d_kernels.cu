@@ -1798,12 +1798,16 @@ constexpr int kAutomapTileW = 128, kAutomapTileH = 32;
 // the compiler schedules K5's item loop differently.
 // kState, the state variant (b2d_automap_states_device, C21): the seen variant with the frame's level, sector offsets and
 // arrows from `st` (automap_state_item).  The offsets are read only by changeable lines, in the item loop.
-template <bool kSeen, bool kState = false>
+// kMarks, the marks variant (b2d_automap_marks_device, C22): the state variant with, under kAutomapGrid, the grid lines
+// that can reach the tile (automap_grid_range) drawn with key 104, below every item's, and then the frame's marks, each
+// with a key above every item's and the last mark's highest; a mark's texels are drawn whatever their index, 0 included.
+template <bool kSeen, bool kState = false, bool kMarks = false>
 __device__ __forceinline__ void automap_tile(const AutomapLevel *__restrict__ levels, const uint32_t *__restrict__ frame_level,
                                              const Pose *__restrict__ poses, View vw, int32_t scale, int flags,
                                              uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec,
                                              const uint32_t *__restrict__ seen, uint32_t words,
-                                             const AutomapStateTables st = AutomapStateTables{}) {
+                                             const AutomapStateTables st = AutomapStateTables{},
+                                             const AutomapMarkTables mt = AutomapMarkTables{}) {
     __shared__ uint32_t keys[kAutomapTileH * kAutomapTileW];
     const size_t frame = blockIdx.x / tiles;
     const int tile = blockIdx.x - (int)(frame * tiles);
@@ -1833,6 +1837,48 @@ __device__ __forceinline__ void automap_tile(const AutomapLevel *__restrict__ le
         const uint32_t key = ((uint32_t)(i + 1) << 8) | colour;
         automap_line(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1,
                      [&](int32_t x, int32_t y) { atomicMax(&keys[(y - ty0) * kAutomapTileW + (x - tx0)], key); });
+    }
+    if (kMarks) {
+        const AutomapMarkLevel &ml = mt.levels[in.level];
+        if (flags & kAutomapGrid) {
+            const int32_t ox = ml.ox, oy = ml.oy;
+            int64_t a0, a1, b0, b1;
+            automap_grid_range(f, ox, true, tx0, ty0, tx1, ty1, a0, a1);
+            automap_grid_range(f, oy, false, tx0, ty0, tx1, ty1, b0, b1);
+            const int nv = a1 >= a0 ? (int)(a1 - a0 + 1) : 0, ng = nv + (b1 >= b0 ? (int)(b1 - b0 + 1) : 0);
+            const int lane = threadIdx.x & 31;
+            for (int g = threadIdx.x >> 5; g < ng; g += blockDim.x >> 5) {      // a warp per line, its lanes share the pixels
+                int64_t e[4];
+                const bool v = g < nv;
+                automap_grid_line(f, v ? ox : oy, v, v ? a0 + g : b0 + (g - nv), e);
+                AutomapSpan sp;
+                const int kind = automap_line_span(e[0], e[1], e[2], e[3], tx0, ty0, tx1, ty1, sp);
+                if (kind == 2 && lane == 0) atomicMax(&keys[(sp.py - ty0) * kAutomapTileW + (sp.px - tx0)], kAutomapGridColour);
+                if (kind == 1)
+                    for (int64_t i = sp.first + lane; i < sp.last; i += 32) {
+                        int32_t x, y;
+                        automap_span_pixel(sp, i, x, y);
+                        atomicMax(&keys[(y - ty0) * kAutomapTileW + (x - tx0)], kAutomapGridColour);
+                    }
+            }
+        }
+        const uint32_t first = mt.ranges ? mt.ranges[2 * frame] : 0u, nm = mt.ranges ? mt.ranges[2 * frame + 1] : 0u;
+        const int32_t k = automap_mark_k(vw.H);
+        for (uint32_t m = 0; m < nm; m++) {
+            const AutomapMark mk = mt.marks[first + m];
+            const AutomapDigit d = ml.digit[mk.number];
+            int32_t left, top;
+            if (!automap_mark_place(f, mk, d, k, left, top)) continue;
+            const int32_t x0 = max(left, tx0), x1 = min(left + k * d.w, tx1), y0 = max(top, ty0), y1 = min(top + k * d.h, ty1);
+            if (x0 >= x1 || y0 >= y1) continue;
+            const uint32_t key = (uint32_t)(n + m + 1) << 8;
+            const int w = x1 - x0, cnt = w * (y1 - y0);
+            for (int p = threadIdx.x; p < cnt; p += blockDim.x) {
+                const int32_t x = x0 + p % w, y = y0 + p / w;
+                const uint32_t t = automap_mark_texel(d, k, left, top, x, y);
+                if (!(t >> 8)) atomicMax(&keys[(y - ty0) * kAutomapTileW + (x - tx0)], key | t);
+            }
+        }
     }
     __syncthreads();
     uint8_t *dst = out + frame * (size_t)vw.W * vw.H;
@@ -1874,6 +1920,14 @@ b2d_automap_states_kernel(const AutomapLevel *__restrict__ levels, const Pose *_
                           uint32_t words, const AutomapStateTables st) {
     automap_tile<true, true>(levels, nullptr, poses, vw, scale, flags, out, tiles_x, tiles, vec, seen, words, st);
 }
+
+// Kernel 5's marks variant (C22), also a kernel of its own.
+__global__ void __launch_bounds__(256)
+b2d_automap_marks_kernel(const AutomapLevel *__restrict__ levels, const Pose *__restrict__ poses, View vw, int32_t scale,
+                         int flags, uint8_t *__restrict__ out, int tiles_x, int tiles, bool vec, const uint32_t *__restrict__ seen,
+                         uint32_t words, const AutomapStateTables st, const AutomapMarkTables mt) {
+    automap_tile<true, true, true>(levels, nullptr, poses, vw, scale, flags, out, tiles_x, tiles, vec, seen, words, st, mt);
+}
 }  // namespace
 
 size_t automap_tiles(const View &vw) {
@@ -1882,14 +1936,19 @@ size_t automap_tiles(const View &vw) {
 
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
                            const View &vw, int32_t scale, int flags, bool seen_variant, const uint32_t *d_seen, uint32_t words,
-                           uint8_t *d_out, cudaStream_t stream, const AutomapStateTables *states) {
+                           uint8_t *d_out, cudaStream_t stream, const AutomapStateTables *states,
+                           const AutomapMarkTables *marks) {
     if (n_frames == 0) return cudaSuccess;
     const int tiles_x = (vw.W + kAutomapTileW - 1) / kAutomapTileW;
     const int tiles = (int)automap_tiles(vw);
     if (n_frames * (size_t)tiles > 0x7FFFFFFFull) return cudaErrorInvalidValue;
     const bool vec = vw.W % 16 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0;
     const unsigned blocks = (unsigned)(n_frames * tiles);
-    if (states)
+    if (marks) {
+        if (!states) return cudaErrorInvalidValue;
+        b2d_automap_marks_kernel<<<blocks, 256, 0, stream>>>(d_levels, d_poses, vw, scale, flags, d_out, tiles_x, tiles, vec,
+                                                             d_seen, words, *states, *marks);
+    } else if (states)
         b2d_automap_states_kernel<<<blocks, 256, 0, stream>>>(d_levels, d_poses, vw, scale, flags, d_out, tiles_x, tiles, vec,
                                                               d_seen, words, *states);
     else if (seen_variant)

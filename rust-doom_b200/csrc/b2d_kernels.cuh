@@ -175,6 +175,13 @@ struct AutomapStateTables {
     const int32_t *off;
     const AutomapArrow *arrows;
 };
+// The marks variant's tables: per level its grid origin and digits, then the call's staging: 2 words per frame (first,
+// n) into `marks` (ranges nullptr: no marks).
+struct AutomapMarkTables {
+    const AutomapMarkLevel *levels;
+    const uint32_t *ranges;
+    const AutomapMark *marks;
+};
 // Kernel 5's grid: CTAs (128 x 32 tiles) per frame of view vw.
 size_t automap_tiles(const View &vw);
 // Kernel 5: the C19 automap of n_frames poses into contiguous W x H index frames at d_out, frame f from the items of
@@ -182,9 +189,11 @@ size_t automap_tiles(const View &vw);
 // `seen_variant`: its seen variant (C20), frame f's lines coloured by row f of d_seen (`words` per row; nullptr: every
 // line mapped); d_seen and words are not read otherwise.  `states` (nullable): the state variant (C21) instead, which
 // takes frame f's level from states->frames[f] (d_frame_level is not read), its sector offsets and arrows, and colours
-// its lines by row f of d_seen as the seen variant does.
+// its lines by row f of d_seen as the seen variant does.  `marks` (nullable, with `states`): the marks variant (C22),
+// the state variant with the grid under B2D_AUTOMAP_GRID and frame f's marks over everything.
 cudaError_t launch_automap(const AutomapLevel *d_levels, const uint32_t *d_frame_level, const Pose *d_poses, size_t n_frames,
                            const View &vw, int32_t scale, int flags, bool seen_variant, const uint32_t *d_seen, uint32_t words,
-                           uint8_t *d_out, cudaStream_t stream, const AutomapStateTables *states = nullptr);
+                           uint8_t *d_out, cudaStream_t stream, const AutomapStateTables *states = nullptr,
+                           const AutomapMarkTables *marks = nullptr);
 
 }  // namespace b2d

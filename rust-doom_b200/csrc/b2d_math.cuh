@@ -763,6 +763,94 @@ B2D_HD uint32_t automap_state_item(const AutomapFrame &f, const AutomapLevel &L,
     return automap_seen_colour(l, mapped == nullptr || ((mapped[ld >> 5] >> (ld & 31)) & 1u), flags);
 }
 
+// ---- the grid and the numbered marks (b2d_automap_marks_device, C22) ---------------------------------------------------
+// B2D_AUTOMAP_GRID; the grid's colour (GRIDCOLORS: GRAYS + GRAYSRANGE / 2) and spacing (MAPBLOCKUNITS), and the map range
+// its lines span and lie in.
+constexpr int kAutomapGrid = 16;
+constexpr uint32_t kAutomapGridColour = 104;
+constexpr int64_t kAutomapGridStep = 128, kAutomapGridMin = -32768, kAutomapGridMax = 32767;
+constexpr int kAutomapDigits = 10;
+// A digit patch (AMMNUM0 .. AMMNUM9): w x h row-major texels, a texel with a non-zero high byte transparent, and its
+// picture offsets.  px nullptr: the digit is missing and its marks are not drawn.
+struct AutomapDigit {
+    const uint16_t *px;
+    int32_t w, h, left, top;
+};
+static_assert(sizeof(AutomapDigit) == 24, "AutomapDigit");
+// A level's grid origin (the BLOCKMAP header's, map units) and its digits.
+struct AutomapMarkLevel {
+    int32_t ox, oy;
+    AutomapDigit digit[kAutomapDigits];
+};
+// A mark (b2d_automap_mark): position in 16.16 map units, digit 0 .. 9.
+struct AutomapMark {
+    int32_t x, y;
+    uint32_t number;
+};
+static_assert(sizeof(AutomapMark) == 12, "AutomapMark");
+
+B2D_HD int64_t automap_floordiv(int64_t a, int64_t b) {      // b > 0
+    const int64_t q = a / b;
+    return q - ((a % b != 0 && a < 0) ? 1 : 0);
+}
+// The lattice of one line family: every j whose line o + 128 j (map units) lies in [-32768, 32767].
+B2D_HD void automap_grid_lattice(int32_t o, int64_t &jlo, int64_t &jhi) {
+    jlo = -automap_floordiv((int64_t)o - kAutomapGridMin, kAutomapGridStep);
+    jhi = automap_floordiv(kAutomapGridMax - (int64_t)o, kAutomapGridStep);
+}
+// Grid line j of a family (vertical: constant map x = o + 128 j) from one end of the map range to the other, in Q8 screen
+// coordinates through the frame's map transform.  |d| <= 2^32 keeps C19's bound.
+B2D_HD void automap_grid_line(const AutomapFrame &f, int32_t o, bool vertical, int64_t j, int64_t e[4]) {
+    const int64_t at = ((int64_t)o + kAutomapGridStep * j) * 65536, lo = kAutomapGridMin * 65536, hi = kAutomapGridMax * 65536;
+    automap_map(f, vertical ? at : lo, vertical ? lo : at, e[0], e[1]);
+    automap_map(f, vertical ? at : hi, vertical ? hi : at, e[2], e[3]);
+}
+// The lattice indices [jlo, jhi] (empty when jlo > jhi) of one family whose lines can draw a pixel of the rectangle
+// [x0, x1) x [y0, y1).  Conservative: the rectangle, widened by 2 pixels on each side, is mapped back to map space by the
+// transpose of the frame's rotation (north-up: none), and its corners bound the map offset along the family's normal.
+// Rounding of the forward transform moves a line by a few Q8 units at most, and a drawn pixel's square meets the line.
+B2D_HD void automap_grid_range(const AutomapFrame &f, int32_t o, bool vertical, int32_t x0, int32_t y0, int32_t x1, int32_t y1,
+                               int64_t &jlo, int64_t &jhi) {
+    constexpr int64_t M = 512;
+    const int64_t u0 = (int64_t)x0 * 256 - M - ((int64_t)f.W << 7), u1 = (int64_t)x1 * 256 + M - ((int64_t)f.W << 7);
+    const int64_t v0 = ((int64_t)f.H << 7) - (int64_t)y1 * 256 - M, v1 = ((int64_t)f.H << 7) - (int64_t)y0 * 256 + M;
+    const int64_t c = f.rot ? f.c : (int64_t)1 << 30, s = f.rot ? f.s : 0;
+    const int64_t a = vertical ? c : -s, b = vertical ? s : c;      // the offset along the normal is (a u + b v) / (64 scale)
+    const int64_t au0 = a * u0, au1 = a * u1, bv0 = b * v0, bv1 = b * v1;
+    const int64_t lo = (au0 < au1 ? au0 : au1) + (bv0 < bv1 ? bv0 : bv1), hi = (au0 < au1 ? au1 : au0) + (bv0 < bv1 ? bv1 : bv0);
+    const int64_t div = 64 * (int64_t)f.scale, p = vertical ? f.px : f.py;
+    const int64_t dlo = automap_floordiv(lo, div) - 1 + p - (int64_t)o * 65536;
+    const int64_t dhi = -automap_floordiv(-hi, div) + 1 + p - (int64_t)o * 65536;
+    int64_t llo, lhi;
+    automap_grid_lattice(o, llo, lhi);
+    jlo = -automap_floordiv(-dlo, kAutomapGridStep * 65536);
+    jhi = automap_floordiv(dhi, kAutomapGridStep * 65536);
+    if (jlo < llo) jlo = llo;
+    if (jhi > lhi) jhi = lhi;
+}
+
+// The marks' magnification: Doom's patches are drawn for 200 lines.
+B2D_HD int32_t automap_mark_k(int32_t H) { return H / 200 > 1 ? H / 200 : 1; }
+// A mark's k w x k h rectangle: its point through the frame's map transform is pixel (X >> 8, Y >> 8), and the patch's
+// top-left corner is that pixel minus k (left, top).  False when the digit is missing or the rectangle is not wholly
+// inside the frame (Doom's fit test, at the patch's own size).
+B2D_HD bool automap_mark_place(const AutomapFrame &f, const AutomapMark &m, const AutomapDigit &d, int32_t k, int32_t &left,
+                               int32_t &top) {
+    if (!d.px) return false;
+    int64_t X, Y;
+    automap_map(f, m.x, m.y, X, Y);
+    const int64_t l = (X >> 8) - (int64_t)k * d.left, t = (Y >> 8) - (int64_t)k * d.top;
+    if (l < 0 || t < 0 || l + (int64_t)k * d.w > f.W || t + (int64_t)k * d.h > f.H) return false;
+    left = (int32_t)l;
+    top = (int32_t)t;
+    return true;
+}
+// The texel over pixel (x, y) of a mark placed at (left, top): its palette index in the low byte, transparent when the
+// high byte is not 0.
+B2D_HD uint32_t automap_mark_texel(const AutomapDigit &d, int32_t k, int32_t left, int32_t top, int32_t x, int32_t y) {
+    return d.px[(size_t)((y - top) / k) * (size_t)d.w + (size_t)((x - left) / k)];
+}
+
 // The pixels of the line (X0, Y0) - (X1, Y1) (Q8, |X|, |Y| < 2^31) inside the pixel rectangle [x0, x1) x [y0, y1), each
 // passed to plot(x, y) once.  Along the major axis (|dX| >= |dY|: X) every pixel whose centre lies in the endpoints'
 // range, inclusive; its minor coordinate is the floor of the exact interpolation at that centre.  A range without a
@@ -816,6 +904,70 @@ B2D_HD void automap_line(int64_t X0, int64_t Y0, int64_t X1, int64_t Y1, int32_t
         const int64_t j = minor(i);
         if (xmaj) plot((int32_t)i, (int32_t)j); else plot((int32_t)j, (int32_t)i);
     }
+}
+
+// automap_line's rule in two steps, so that the lanes of a warp can share one long line's pixels (the marks variant's
+// grid lines cross whole tiles): automap_line_span finds the major-axis pixels [first, last) the line draws inside the
+// rectangle (returns 1), or the one pixel (px, py) of a line without a pixel centre in its range when it lies inside
+// (returns 2), or nothing (0); automap_span_pixel gives the pixel at major index i.  The same pixels as automap_line.
+struct AutomapSpan {
+    int64_t M0, m0, first, last;
+    uint64_t dM, dm;
+    bool xmaj, up;
+    int32_t px, py;
+};
+B2D_HD int64_t automap_span_minor(const AutomapSpan &s, int64_t i) {
+    if (s.dM == 0) return s.m0 >> 8;
+    const uint64_t p = (uint64_t)(256 * i + 128 - s.M0) * s.dm;
+    const uint64_t q = p / s.dM;
+    return (s.up ? s.m0 + (int64_t)q : s.m0 - (int64_t)q - (q * s.dM != p ? 1 : 0)) >> 8;
+}
+B2D_HD void automap_span_pixel(const AutomapSpan &s, int64_t i, int32_t &x, int32_t &y) {
+    const int64_t j = automap_span_minor(s, i);
+    x = (int32_t)(s.xmaj ? i : j);
+    y = (int32_t)(s.xmaj ? j : i);
+}
+B2D_HD int automap_line_span(int64_t X0, int64_t Y0, int64_t X1, int64_t Y1, int32_t x0, int32_t y0, int32_t x1, int32_t y1,
+                             AutomapSpan &s) {
+    if ((X0 < X1 ? X1 : X0) >> 8 < x0 || (X0 < X1 ? X0 : X1) >> 8 >= x1 || (Y0 < Y1 ? Y1 : Y0) >> 8 < y0 ||
+        (Y0 < Y1 ? Y0 : Y1) >> 8 >= y1)
+        return 0;
+    s.xmaj = (X1 >= X0 ? X1 - X0 : X0 - X1) >= (Y1 >= Y0 ? Y1 - Y0 : Y0 - Y1);
+    int64_t M0 = s.xmaj ? X0 : Y0, m0 = s.xmaj ? Y0 : X0, M1 = s.xmaj ? X1 : Y1, m1 = s.xmaj ? Y1 : X1;
+    if (M1 < M0) {
+        int64_t t = M0; M0 = M1; M1 = t;
+        t = m0; m0 = m1; m1 = t;
+    }
+    int64_t lo = (M0 + 127) >> 8, hi = (M1 - 128) >> 8;
+    if (lo > hi) {
+        s.px = (int32_t)(X0 >> 8);
+        s.py = (int32_t)(Y0 >> 8);
+        return (X0 >> 8) >= x0 && (X0 >> 8) < x1 && (Y0 >> 8) >= y0 && (Y0 >> 8) < y1 ? 2 : 0;
+    }
+    const int32_t Mlo = s.xmaj ? x0 : y0, Mhi = s.xmaj ? x1 : y1, mlo = s.xmaj ? y0 : x0, mhi = s.xmaj ? y1 : x1;
+    if (lo < Mlo) lo = Mlo;
+    if (hi > Mhi - 1) hi = Mhi - 1;
+    if (lo > hi) return 0;
+    s.M0 = M0;
+    s.m0 = m0;
+    s.dM = (uint64_t)(M1 - M0);
+    s.up = m1 >= m0;
+    s.dm = s.up ? (uint64_t)(m1 - m0) : (uint64_t)(m0 - m1);
+    int64_t a = lo, b = hi + 1;                             // first pixel not before [mlo, mhi)
+    while (a < b) {
+        const int64_t mid = a + ((b - a) >> 1);
+        const int64_t j = automap_span_minor(s, mid);
+        if (s.up ? j < mlo : j >= mhi) a = mid + 1; else b = mid;
+    }
+    s.first = a;
+    b = hi + 1;                                             // first pixel past it
+    while (a < b) {
+        const int64_t mid = a + ((b - a) >> 1);
+        const int64_t j = automap_span_minor(s, mid);
+        if (s.up ? j >= mhi : j < mlo) b = mid; else a = mid + 1;
+    }
+    s.last = a;
+    return s.first < s.last ? 1 : 0;
 }
 
 }  // namespace b2d
